@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200-native SageAttention hot path.
+"""bench.py — headline benchmark of the H100-native (sm_90a) SageAttention hot path.
 
 Contract (one JSON line on stdout from rank 0):
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 N = 1  workload = BASELINE.json configs[1]: qk_int8_pv_fp8, hd=128, seq=8192, non-causal, B=4 H=32
        (the reference bench defaults, bench/bench_qk_int8_pv_fp8_cuda.py:22-24), bf16, synthetic randn.
@@ -14,6 +14,8 @@ N > 1  workload = configs[4]: sequence-parallel sageattn, hd=128, seq=32768, B=1
        INT8 K / FP8 V all-gathered over NCCL (sageattention_b200.parallel); total work fixed -> "scaling": "strong".
 --impl reference : the reference's own algorithm on the HOST cores (CPU port in oracle/, all torch threads) on a
        bounded sample of the same workload; rank 0 only.
+--dump-outputs DIR : after the timed steps, rank 0 writes what the last timed step returned — a fixed, seeded sample of rows of the
+       attention output — as DIR/<name>.npy (float32), so two builds can be compared output for output on identical inputs.
 """
 import argparse, json, os, subprocess, sys, threading, time
 
@@ -29,6 +31,8 @@ def parse():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-sweep", action="store_true", help="skip the context block (other configs, reference CUDA kernels on this GPU)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a seeded sample of the last timed step's output as DIR/<name>.npy (float32)")
     return ap.parse_args()
 
 
@@ -37,7 +41,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data sheet (dense)"
 
 
 class ClockSampler:
@@ -97,6 +101,21 @@ class ClockSampler:
                     reasons.add(name)
         return {"sm_mhz": sm[len(sm) // 2] if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": sorted(reasons), "samples": len(sm), "window_s": round(sum(b - a for a, b in self.windows), 3)}
+
+
+DUMP_ROWS = 16384   # rows of the [.., D] output written by --dump-outputs (8 MB at D = 128)
+
+
+def dump_outputs(dirname, o, rank):
+    """A fixed, seeded sample of rows of the output `o` (viewed as [-1, D]) and their row indices, as float32 .npy files."""
+    import numpy as np
+    import torch
+    os.makedirs(dirname, exist_ok=True)
+    flat = o.reshape(-1, o.shape[-1])
+    g = torch.Generator().manual_seed(0)
+    idx = torch.randperm(flat.shape[0], generator=g)[:DUMP_ROWS].sort().values
+    np.save(os.path.join(dirname, f"o_rank{rank}_rows.npy"), flat[idx.to(flat.device)].float().cpu().numpy())
+    np.save(os.path.join(dirname, f"o_rank{rank}_row_index.npy"), idx.to(torch.float32).numpy())
 
 
 def flops(B, H, Sq, Sk, D, causal=False):
@@ -202,7 +221,7 @@ def sweep_configs(dev, dtype):
             dense(f"hd128_s{S // 1024}k_{'causal' if causal else 'noncausal'}", 4, 32, S, 128, causal, n)
     dense("configs[2]_hd64_s32k_causal_per_thread", 4, 32, 32768, 64, True, 3)
     dense("hd64_s8k_noncausal", 4, 32, 8192, 64, False, 10)
-    # configs[3]: sageattn_varlen, GQA Hq=32 / Hkv=8, hd=128, sequence lengths 512..16384 shuffled with seed 0 (SURVEY 8d)
+    # configs[3]: sageattn_varlen, GQA Hq=32 / Hkv=8, hd=128, sequence lengths 512..16384 shuffled with seed 0
     lens = [512, 1024, 2048, 4096, 8192, 16384]
     g = torch.Generator().manual_seed(0)
     lens = [lens[i] for i in torch.randperm(len(lens), generator=g).tolist()]
@@ -221,10 +240,10 @@ def sweep_configs(dev, dtype):
 
 
 def reference_cuda_on_this_gpu(dev, dtype, B, H, S, D):
-    """Context only (BASELINE.md B4): the reference's OWN CUDA kernels (csrc/fused/fused.cu + the sm89 mma.sync attention
-    kernel, compiled unmodified for sm_100a by oracle/build_ref.py into oracle/_ref/) timed on this GPU at configs[1]:
-    kernel-only (reference convention, bench/bench_qk_int8_pv_fp8_cuda.py:66-104) and quantisation + kernel.  The reference's
-    sageattn() raises on sm_100 (core.py:157), so its two stages are called the way core.py:773-819 calls them."""
+    """Context only: the reference's OWN CUDA kernels (csrc/fused/fused.cu + the sm89 mma.sync attention
+    kernel, compiled unmodified for sm_90a by oracle/build_ref.py into oracle/_ref/, when built) timed on this GPU at configs[1]:
+    kernel-only (reference convention, bench/bench_qk_int8_pv_fp8_cuda.py:66-104) and quantisation + kernel, its two stages
+    called the way core.py:773-819 calls them."""
     import importlib.util
     import torch
 
@@ -259,7 +278,7 @@ def reference_cuda_on_this_gpu(dev, dtype, B, H, S, D):
     kms = _time_fn(kern, 5)
     cms = _time_fn(lambda: (quant(), kern()), 5)
     return {"what": "thu-ml/SageAttention sm89 kernel (qk_int8_sv_f8_accum_f16_fuse_v_scale_attn_inst_buf, mma.sync) + csrc/fused quantisers, "
-                    "unmodified sources compiled for sm_100a", "workload": "configs[1], per_warp quantisation",
+                    "unmodified sources compiled for sm_90a", "workload": "configs[1], per_warp quantisation",
             "kernel_tflops": fl / kms / 1e9, "quant_plus_kernel_tflops": fl / cms / 1e9, "kernel_ms": kms, "quant_plus_kernel_ms": cms}
 
 
@@ -280,12 +299,16 @@ def run_ours(args):
     D = 128
     dtype = torch.bfloat16
     torch.manual_seed(1234 + rank)
+    last = [None]   # output of the latest step
 
     if world == 1:
         B, H, S = 4, 32, 8192
         workload = WORKLOAD_N1
         q, k, v = (torch.randn(B, H, S, D, device=dev, dtype=dtype) for _ in range(3))
-        step = lambda: sab.sageattn(q, k, v, tensor_layout="HND", is_causal=False)
+
+        def step():
+            last[0] = sab.sageattn(q, k, v, tensor_layout="HND", is_causal=False)
+            return last[0]
         total_flops = flops(B, H, S, S, D)
         launches_per_step = 8  # k_mean(2) + quant q,k (2) + v stats(2) + v quant(1) + attention(1)
         scaling = "weak"
@@ -299,9 +322,9 @@ def run_ours(args):
         Sl = S // world
         workload = workload_sp(world)
         # per-rank shards shrink with N (32 MB per tensor at N=8): rotate over enough independent input sets that the
-        # bytes touched between two uses of the same set exceed twice the 126 MB L2 (timing rule: inputs larger than L2)
+        # bytes touched between two uses of the same set exceed twice the 50 MB L2 (timing rule: inputs larger than L2)
         per_set = 3 * B * H * Sl * D * 2
-        n_sets = max(1, -(-2 * 126 * 2 ** 20 // per_set))
+        n_sets = max(1, -(-2 * 50 * 2 ** 20 // per_set))
         sets = [tuple(torch.randn(B, H, Sl, D, device=dev, dtype=dtype) for _ in range(3)) for _ in range(n_sets)]
         q, k, v = sets[0]
         turn = [0]
@@ -309,7 +332,8 @@ def run_ours(args):
         def step():
             a, b, c = sets[turn[0] % n_sets]
             turn[0] += 1
-            return parallel.sageattn_sp(a, b, c, tensor_layout="HND", is_causal=False, fused_gather=fused_gather)
+            last[0] = parallel.sageattn_sp(a, b, c, tensor_layout="HND", is_causal=False, fused_gather=fused_gather)
+            return last[0]
         total_flops = flops(B, H, S, S, D)
         launches_per_step = 9
         scaling = "strong"
@@ -322,7 +346,7 @@ def run_ours(args):
         o = step()
     torch.cuda.synchronize()
 
-    # ---- value: device-resident inputs (each of q,k,v is >= 2x the 126 MB L2 at N=1: no flush needed)
+    # ---- value: device-resident inputs (each of q,k,v is >= 2x the 50 MB L2 at N=1: no flush needed)
     if world > 1:
         dist.barrier()
     torch.cuda.synchronize()
@@ -331,6 +355,8 @@ def run_ours(args):
     ms = time_events(step, args.steps)
     if sampler:
         sampler.end()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last[0], rank)
     t = torch.tensor([ms], device=dev)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -368,23 +394,13 @@ def run_ours(args):
         torch.cuda.synchronize()
         kms = time_events(kern, args.steps)
         achieved = total_flops / (kms * 1e-3) / 1e12
-        # 8-bit tensor peak: kind::i8 / kind::f8f6f4 issue at twice the bf16 rate (same UMMA cycles, K=32 vs 16);
-        # denominator = 2 x the MEASURED cuBLAS bf16 burst figure.
+        # 8-bit tensor peak: INT8 / FP8 wgmma issue at twice the bf16 rate (K=32 vs 16); denominator = 2 x the bf16 figure
         peak8 = 2.0 * pk["bf16_tflops"]
         roof = {"bound": "tensor", "achieved": achieved, "peak": peak8, "unit": "TFLOP/s", "frac": achieved / peak8,
-                "traffic": None, "kernel": "sab::sage_attn_alt_kernel<128,true,bf16> (SAB_ATTN_KERNEL=exact: sab::sage_attn_fwd_kernel; =q4: sab::sage_attn_q4_kernel)", "kernel_ms": kms,
-                "peak_source": f"2 x bf16_tflops ({pk['bf16_tflops']}) of {pk_src} MEASURED_PEAKS.json",
-                # the same tensor core measured directly this round (tools/microbench/mma_peak.cu, profiles/r02_mma_peak.txt): back-to-back
-                # tcgen05.mma on all SMs, operands in smem/TMEM — the instruction-issue ceiling, above what any real kernel sustains
-                "peak_mma_microbench": {"kind::i8": 4576.9, "kind::f8f6f4": 4467.2, "kind::f16 (bf16)": 2232.8, "unit": "TFLOP/s",
-                                        "frac_of_i8_f8_mean": achieved / (0.5 * (4576.9 + 4467.2)), "source": "profiles/r02_mma_peak.txt"},
+                "traffic": None, "kernel": "sab::sage_attn_fwd_kernel<128,true,bf16,false,false>", "kernel_ms": kms,
+                "peak_source": f"2 x bf16_tflops ({pk['bf16_tflops']}), {pk_src}",
                 "algorithmic_flops_per_launch": total_flops,
                 "algorithmic_hbm_bytes_per_launch": 5.0 * B * H * S * D}
-        import glob
-        trs = sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_attn_traffic.json")))   # newest round's ncu --set full capture
-        if trs:
-            roof["traffic"] = json.load(open(trs[-1])).get("dram_bytes_per_launch")
-            roof["traffic_source"] = os.path.relpath(trs[-1], ROOT)
 
         # ---- e2e: pinned host q,k,v -> H2D -> sageattn -> D2H of o, all inside the timed region
         qh, kh, vh = (torch.randn(B, H, S, D, dtype=dtype).pin_memory() for _ in range(3))
@@ -435,7 +451,7 @@ def run_ours(args):
     else:
         roof = {"bound": "tensor", "achieved": value, "peak": 2.0 * pk["bf16_tflops"] * world, "unit": "TFLOP/s",
                 "frac": value / (2.0 * pk["bf16_tflops"] * world), "traffic": None,
-                "peak_source": f"{world} x 2 x bf16_tflops of {pk_src} MEASURED_PEAKS.json (whole step incl. quant + all-gather)"}
+                "peak_source": f"{world} x 2 x bf16_tflops, {pk_src} (whole step incl. quant + all-gather)"}
         Sl = S // world
         qh, kh, vh = (torch.randn(B, H, Sl, D, dtype=dtype).pin_memory() for _ in range(3))
         oh = torch.empty(B, H, Sl, D, dtype=dtype).pin_memory()
@@ -492,8 +508,8 @@ def run_ours(args):
             "data": "synthetic randn, random-init (no datasets/checkpoints offline)",
             "config": {"workload": workload, "B": B, "H": H, "S": S, "D": D, "qk_quant_gran": "per_thread",
                        "pv_accum_dtype": "fp32+fp16", "smooth_k": True,
-                       "l2": ("inputs (3 x %d MB per rank) exceed the 126 MB L2; no flush" % (B * H * S * D * 2 // 2 ** 20)) if world == 1 else
-                             ("rotating over %d independent input sets of 3 x %d MB per rank (> 2 x the 126 MB L2 between reuses); no flush"
+                       "l2": ("inputs (3 x %d MB per rank) exceed the 50 MB L2; no flush" % (B * H * S * D * 2 // 2 ** 20)) if world == 1 else
+                             ("rotating over %d independent input sets of 3 x %d MB per rank (> 2 x the 50 MB L2 between reuses); no flush"
                               % (n_sets, B * H * (S // world) * D * 2 // 2 ** 20)),
                        "step": "full sageattn(): K-mean + INT8 quant Q/K + FP8 quant V + fused attention",
                        **({"kv_exchange": "peer copies + segment flags inside the attention launch" if fused_gather else
@@ -501,8 +517,8 @@ def run_ours(args):
             "roofline": roof, "e2e": e2e, "gpu_launches": launches_per_step * args.steps, "clocks": clocks,
             "cpu_baseline": cpu_baseline,
             "context": {"h100_published_kernel_tops_hd128_8k_noncausal": 900, "cached_kv": cached_kv,
-                        "configs": sweep, "reference_cuda_on_b200": ref_cuda, "single_gpu_same_workload": same_workload_1gpu,
-                        "note": "reference publishes kernel-only numbers on other hardware (BASELINE.md); no B200 number exists"},
+                        "configs": sweep, "reference_cuda_on_this_gpu": ref_cuda, "single_gpu_same_workload": same_workload_1gpu,
+                        "note": "the reference's published H100 figure is kernel-only (its sm90 wgmma kernel, not timed here); compare with roofline.achieved"},
         }
         print(json.dumps(line))
     if world > 1:

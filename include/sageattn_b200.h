@@ -1,10 +1,10 @@
 /*
- * sageattn_b200 — C ABI of the B200-native (sm_100a) SageAttention hot path.
+ * sageattn_b200 — C ABI of the H100-native (sm_90a) SageAttention hot path.
  *
  * Plain C: raw device pointers, sizes, element strides and a cudaStream_t (passed as void*).
  * No torch types.  Every entry point returns 0 on success or a negative sab_status; the message of
  * the last failure on the calling thread is available from sab_last_error().  Nothing is allocated
- * or retained by the library: the caller owns every buffer (the reference convention, SURVEY §8b).
+ * or retained by the library: the caller owns every buffer (the reference convention).
  *
  * Each function names the reference interface it replaces (paths relative to thu-ml/SageAttention):
  *   csrc/fused/fused.h:19-76            the eight `_fused` quantisation entry points
@@ -31,7 +31,7 @@ typedef enum {
   SAB_ERR_INVALID = -1,     /* bad argument (reference: TORCH_CHECK / std::invalid_argument) */
   SAB_ERR_UNSUPPORTED = -2, /* unsupported head_dim / dtype / granularity                     */
   SAB_ERR_CUDA = -3,        /* CUDA runtime / driver failure (launch, tensor-map encode)       */
-  SAB_ERR_ARCH = -4         /* device is not sm_100 (no fallback path exists)                  */
+  SAB_ERR_ARCH = -4         /* device is not sm_90 (no fallback path exists)                   */
 } sab_status;
 
 /* element types of the 16-bit inputs / outputs */
@@ -43,12 +43,12 @@ typedef enum {
 #define SAB_GRAN_PER_WARP 2
 #define SAB_GRAN_PER_THREAD 3
 
-/* rounding / epsilon semantics of the INT8 quantisers (SURVEY §7.3 item 5) */
+/* rounding / epsilon semantics of the INT8 quantisers */
 #define SAB_SEM_CUDA 0   /* csrc/fused/fused.cu:147-184: amax floored 1e-7, x*(127/amax), cvt.rni       */
 #define SAB_SEM_TRITON 1 /* triton/quant_per_block.py:41-45: scale=amax/127, x/scale, round-half-away    */
 
 const char* sab_last_error(void);
-/* 0 if the current device can run this library (compute capability 10.x), else SAB_ERR_ARCH. */
+/* 0 if the current device can run this library (compute capability 9.0), else SAB_ERR_ARCH. */
 int sab_check_device(void);
 int sab_version(void);
 
@@ -115,7 +115,7 @@ int sab_quant_per_block_int8_varlen(const void* x, int dtype, const void* mean, 
  *   v      : bhsd, `dtype`.
  *   v_fp8  : [B,H,D,S_pad] bytes, token-contiguous ("V transposed"), S_pad = ceil(S/128)*128, tokens
  *            >= S are written as 0.  Unlike the reference there is NO 16-token permutation: that is
- *            an mma.sync fragment artefact (fused.cu:287-291); tcgen05 reads V^T tiles directly.
+ *            an mma.sync fragment artefact (fused.cu:287-291); wgmma reads V^T tiles directly.
  *   v_scale: [B,H,D] fp32 = amax/scale_max;  v_fp8 = cvt.rn.satfinite.e4m3(v*(scale_max/amax)).
  *   v_mean : optional [B,H,D] fp32 (smooth_v): mean over tokens (denominator: S rounded up to 16,
  *            fused.cu:349,381), subtracted before quantisation.
@@ -131,7 +131,7 @@ int sab_per_channel_fp8(const void* v, int dtype, uint8_t* v_fp8, float* v_scale
                         const int32_t* cu_pad, int nseq, int max_seqlen, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Single-pass front-end (SURVEY section 8 f-1: "fuse quantisation into producers").  One launch each; a thread-block
+ * Single-pass front-end (quantisation fused into the statistics pass).  One launch each; a thread-block
  * cluster per (b,h) reduces the statistic through distributed shared memory and then quantises, so K / V
  * are read from HBM once (the second read hits L2) instead of twice:
  *  sab_k_smooth_quant_int8   = sab_k_mean + sab_quant_per_thread_int8(is_key) [SAB_GRAN_PER_THREAD] or
@@ -151,7 +151,7 @@ int sab_per_channel_fp8_fused(const void* v, int dtype, uint8_t* v_fp8, float* v
 
 /* ------------------------------------------------------------------------------------------------
  * Building blocks of the sequence-parallel path (no reference counterpart: the reference ships no SP
- * code, SURVEY §2.4; semantics chosen so that the sharded result equals the single-GPU one):
+ * code; semantics chosen so that the sharded result equals the single-GPU one):
  *  sab_channel_stats   : per-(b,h,d) fp32 sum / max / min over the LOCAL tokens (all-reduced by the host:
  *                        SUM for the global K mean, MAX/MIN for the global per-channel V range).
  *  sab_v_quant_with_amax: sab_per_channel_fp8 with the per-channel |max| supplied by the caller.
@@ -164,8 +164,8 @@ int sab_v_quant_with_amax(const void* v, int dtype, uint8_t* v_fp8, const float*
                           int64_t s_pad, float scale_max, void* workspace, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Fused attention: INT8 QK^T (tcgen05 kind::i8) -> fp32 online softmax -> FP8 P -> FP8 PV
- * (tcgen05 kind::f8f6f4, fp32 accumulation in tensor memory) -> fp16/bf16 O.
+ * Fused attention: INT8 QK^T (wgmma s8) -> fp32 online softmax -> FP8 P -> FP8 PV
+ * (wgmma e4m3, fp32 accumulation) -> fp16/bf16 O.
  * Replaces qk_int8_sv_f8_accum_{f32,f16}[_fuse_v_scale][_fuse_v_mean]_attn[_inst_buf]
  * (csrc/qattn/attn_cuda_sm89.h:19-104) and, with cu_seqlens, the Triton varlen launchers.
  *   q_int8 : bhsd int8 [B,Hq,Sq,D];  k_int8: bhsd int8 [B,Hkv,Skv,D];
@@ -201,14 +201,14 @@ int sab_qk_int8_sv_f8_attn(const int8_t* q_int8, const int8_t* k_int8, const uin
 
 /* ------------------------------------------------------------------------------------------------
  * FP16-PV variant: INT8 QK^T -> fp32 online softmax WITHOUT exponent offset -> FP16 P -> FP16 PV
- * (tcgen05 kind::f16, fp32 accumulation in tensor memory).  Replaces the Triton attention launchers
+ * (wgmma f16, fp32 accumulation).  Replaces the Triton attention launchers
  * `forward` of sageattention/triton/attn_qk_int8_per_block.py:130-183, attn_qk_int8_per_block_causal.py,
  * attn_qk_int8_block_varlen.py:123-150, attn_qk_int8_per_block_causal_varlen.py (the kernels behind
  * sageattn_qk_int8_pv_fp16_triton and sageattn_varlen).  Arguments as sab_qk_int8_sv_f8_attn except:
  *   v_f16t : [B,Hkv,D,s_pad] fp16 (token-contiguous, zero padded) from sab_v_transpose_f16;
  *   no v_scale / v_mean (V is not quantised); no sequence-parallel form.
  * sab_v_transpose_f16 replaces `v.to(torch.float16)` (sageattention/core.py:297-298) plus the K-major
- * re-layout tcgen05 needs; varlen form as sab_per_channel_fp8.
+ * re-layout the wgmma B operand needs; varlen form as sab_per_channel_fp8.
  * ---------------------------------------------------------------------------------------------- */
 int sab_v_transpose_f16(const void* v, int dtype, void* v_f16t, int B, int H, int S, int D, int64_t stride_b,
                         int64_t stride_h, int64_t stride_s, int64_t s_pad, const int32_t* cu_seqlens,

@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE ONLY: build the real reference CUDA kernels for sm_100a into oracle/_ref/.
+"""TEST INFRASTRUCTURE ONLY: build the real reference CUDA kernels for sm_90a into oracle/_ref/.
 
 Recipe (no reference build system is run; no reference source is copied):
   nvcc (flags of /root/reference/setup.py:52-61) on
@@ -6,7 +6,7 @@ Recipe (no reference build system is run; no reference source is copied):
     /root/reference/csrc/qattn/sm89_qk_int8_sv_f8_accum_f{16,32}_fuse_v_scale_attn_inst_buf.cu -> ref_qattn.so
     /root/reference/csrc/qattn/qk_int_sv_f16_cuda_sm80.cu                           -> ref_qattn80.so
   each linked with a small pybind TU of ours (ref_bind_*.cpp).
-Outputs go only to oracle/_ref/ (git-ignored, travels to the GPU box with gpurun).
+Outputs go only to oracle/_ref/ (git-ignored); tests/golden/make_reference_cuda_golden.py runs them.
 Usage: python oracle/build_ref.py   (needs /root/reference; ~4 min on 8 cores)
 """
 import os, subprocess, sys, sysconfig, concurrent.futures as cf
@@ -26,7 +26,7 @@ def _flags():
     nvcc = ["-O3", "-std=c++17", "-U__CUDA_NO_HALF_OPERATORS__", "-U__CUDA_NO_HALF_CONVERSIONS__",
             "-U__CUDA_NO_BFLOAT16_CONVERSIONS__", "-U__CUDA_NO_HALF2_OPERATORS__",
             "--use_fast_math", "--threads=4", "-diag-suppress=174", "--expt-relaxed-constexpr",
-            "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC"]
+            "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC"]
     cxx = ["-O3", "-std=c++17", "-fPIC"]
     libdir = ce.library_paths("cuda")
     link = ["-shared"] + [f"-L{p}" for p in libdir] + [f"-Wl,-rpath,{p}" for p in libdir] + \

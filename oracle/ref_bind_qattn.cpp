@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY (oracle/). Python binding for two *unmodified* reference sm89 attention
 // launchers (the ones sageattn_qk_int8_pv_fp8_cuda selects for pv_accum_dtype "fp32+fp16" and
-// "fp32+fp32", /root/reference/sageattention/core.py:816-819), compiled for sm_100a from the
+// "fp32+fp32", sageattention/core.py:816-819), compiled for sm_90a from the
 // sources where they lie under /root/reference (see build_ref.py).  Declarations come from
 // /root/reference/csrc/qattn/attn_cuda_sm89.h:68-104, #included by absolute path at build time.
 #include <torch/extension.h>

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE ONLY (oracle/). Python binding for the *unmodified* reference sm80 FP16-PV attention launchers
-// (the ones sageattn_qk_int8_pv_fp16_cuda selects, /root/reference/sageattention/core.py:601-617), compiled for sm_100a
+// (the ones sageattn_qk_int8_pv_fp16_cuda selects, sageattention/core.py:601-617), compiled for sm_90a
 // from the source where it lies under /root/reference (see build_ref.py).  Declarations come from
 // /root/reference/csrc/qattn/attn_cuda_sm80.h:19-65, #included by absolute path at build time.
 #include <torch/extension.h>

@@ -8,14 +8,14 @@ Every function cites the reference file:line (relative to /root/reference) that 
 
 Pinning status
 --------------
-* The reference ships NO tests / golden vectors (SURVEY.md §4), so parity is pinned against outputs
+* The reference ships NO tests / golden vectors, so parity is pinned against outputs
   of the reference code itself:
   - Triton-semantics functions (``quant_per_block_int8_triton``, ``quant_per_thread_int8_triton``,
     ``quant_per_block_int8_varlen_triton``, ``attn_int8_fp16_triton``) are checked bit-exact /
     to 2e-3 against the reference Triton kernels executed in this container under
     TRITON_INTERPRET=1; fixtures and generator: tests/golden/make_golden.py, tests/golden/*.npz.
   - CUDA-semantics functions (``quant_int8_cuda``, ``per_channel_fp8_cuda``, ``attn_int8_fp8_cuda``)
-    are checked on the GPU box against the real reference kernels built for sm_100a into
+    are checked on the GPU box against the real reference kernels built for sm_90a into
     oracle/_ref/ (oracle/build_ref.py) by tests/test_gpu_parity.py.
 """
 from __future__ import annotations
@@ -236,8 +236,8 @@ def attn_int8_fp8_cuda(q8, k8, v8, q_scale, k_scale, v_scale, *, qk_quant_gran="
     epilogue: O/d * v_scale -> out_dtype;  lse = log2(d) + m                  (…sm89.cuh:572-703)
     Causal uses top-left alignment (kv_idx > q_idx masked).
     `exp2_fn` (default torch.exp2) replaces the exponential of P only — used by tests/test_poly_exp_numerics.py to
-    quantify the opt-in FMA-pipe polynomial of the sm_100a kernel (csrc/ptx.cuh ex2_poly2) against this restatement.
-    `lazy_tau` (default None = the reference rule) restates the opt-in -DSAB_LAZY_RESCALE=tau build of the sm_100a kernel: the
+    quantify the opt-in FMA-pipe polynomial of the sm_90a kernel (csrc/ptx.cuh ex2_poly2) against this restatement.
+    `lazy_tau` (default None = the reference rule) restates the lazy running max of the sm_90a kernel: the
     running max only moves when it grew by more than tau (log2 units) and the exponent offset is 8.807 - tau."""
     B, Hq, Sq, D = q8.shape
     _, Hk, Sk, _ = k8.shape
@@ -375,7 +375,7 @@ def sageattn_qk_int8_pv_fp8_cuda(q, k, v, tensor_layout="HND", is_causal=False,
                                  pv_accum_dtype="fp32+fp16", smooth_k=True, smooth_v=False,
                                  return_lse=False, kv_tile=64, emulate_f16_accum=True, exp2_fn=None, lazy_tau=None):
     """sageattention/core.py:636-826 end to end (CPU).  emulate_f16_accum=False keeps the reference's V range
-    for "fp32+fp16" (2.25) but accumulates PV in fp32 — the B200 kernel's arithmetic (tcgen05 f32 accumulation)."""
+    for "fp32+fp16" (2.25) but accumulates PV in fp32 — the sm_90a kernel's arithmetic (fp32 accumulation)."""
     dtype = q.dtype
     q, k, v, hd_og = _pad_head_dim(q, k, v)
     if sm_scale is None:

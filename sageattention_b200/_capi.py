@@ -53,7 +53,7 @@ def lib():
         if not os.path.exists(_LIB_PATH):
             raise ImportError(
                 f"sageattention_b200: {_LIB_PATH} is missing. Build it with `python -m sageattention_b200.build` "
-                "(nvcc, sm_100a). There is no fallback implementation.")
+                "(nvcc, sm_90a). There is no fallback implementation.")
         _lib = ctypes.CDLL(_LIB_PATH)
         for name, (res, args) in EXPORTS.items():
             fn = getattr(_lib, name)

@@ -1,16 +1,16 @@
-"""Build the sm_100a CUDA library in-tree: sageattention_b200/lib/libsageattn_b200.so.
+"""Build the sm_90a CUDA library in-tree: sageattention_b200/lib/libsageattn_b200.so.
 
 One nvcc compile per source (in parallel) + one link, no torch headers (the boundary is a plain C ABI, include/sageattn_b200.h).
-nvcc cross-compiles without a GPU; the .so travels to the GPU box with the repo snapshot.
+nvcc cross-compiles without a GPU.
 """
 import os, subprocess, sys, hashlib
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libsageattn_b200.so")
-SOURCES = ["attn.cu", "attn_hd64.cu", "attn_alt.cu", "attn_q4.cu", "quant.cu", "capi.cu"]
+SOURCES = ["attn.cu", "quant.cu", "capi.cu"]
 HEADERS = ["ptx.cuh", "common.cuh", "attn_common.cuh", os.path.join("..", "..", "include", "sageattn_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 # per-source extra nvcc flags (none at present)
 EXTRA_FLAGS = {}
@@ -36,7 +36,7 @@ def build(force: bool = False, verbose: bool = False, defines=(), variant: str =
         return LIB
     os.makedirs(os.path.dirname(LIB), exist_ok=True)
     nvcc = os.environ.get("NVCC", "nvcc")
-    # variant objects go outside the repo: the gpurun snapshot (512 MiB cap) carries the .so files only
+    # variant objects go outside the repository tree
     objdir = os.path.join(os.path.dirname(LIB), "obj") if not variant else os.path.join("/tmp", "sab_obj_" + variant)
     os.makedirs(objdir, exist_ok=True)
 
@@ -52,7 +52,7 @@ def build(force: bool = False, verbose: bool = False, defines=(), variant: str =
     failed = [src for src, _, r in results if r.returncode != 0]
     link = None
     if not failed:
-        link = subprocess.run([nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "--shared", "-o", LIB] +
+        link = subprocess.run([nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "--shared", "-o", LIB] +
                               [obj for _, obj, _ in results], capture_output=True, text=True)
         log += link.stdout + link.stderr
     if verbose or failed or (link is not None and link.returncode != 0):

@@ -1,4 +1,4 @@
-"""Pre-quantised K/V for repeated attention calls (SURVEY §8 f-1: "accept pre-quantised/cached K,V across diffusion
+"""Pre-quantised K/V for repeated attention calls ("accept pre-quantised/cached K,V across diffusion
 steps or decode steps").
 
 `sageattn_qk_int8_pv_fp8_cuda` (sageattention/core.py:636-826) re-derives the K mean, the INT8 K and the FP8 V^T on every

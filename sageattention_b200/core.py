@@ -1,8 +1,8 @@
-"""Public API — drop-in for sageattention/core.py of thu-ml/SageAttention, backed by ONE sm_100a backend.
+"""Public API — drop-in for sageattention/core.py of thu-ml/SageAttention, backed by ONE sm_90a backend.
 
 Signatures and behaviour follow the reference (file:line cited per function); the bodies re-state the
 host logic (asserts, head-dim padding, K smoothing, LSE correction, output slicing) around the
-B200 kernels: fused quantisers (csrc/quant.cu) and the tcgen05 attention kernel (csrc/attn.cu).
+H100 kernels: fused quantisers (csrc/quant.cu) and the wgmma attention kernel (csrc/attn.cu).
 There is no arch dispatch, no Triton, no CPU fallback.
 """
 from typing import Any, Optional
@@ -58,12 +58,12 @@ def sageattn_qk_int8_pv_fp8_cuda(
 ) -> torch.Tensor:
     """INT8 QK^T + FP8 PV attention (reference: sageattention/core.py:636-826).
 
-    pv_accum_dtype keeps the reference vocabulary.  On B200 the PV product always accumulates in fp32
-    inside the tensor core (tcgen05 f32 accumulation is full-rate, so the reference's f16 first-level
+    pv_accum_dtype keeps the reference vocabulary.  The PV product always accumulates in fp32
+    (per 64-key tile in the tensor core, across tiles on the CUDA cores, so the reference's f16 first-level
     accumulator — a consumer-GPU speed trick — buys nothing); the option still selects the reference's V
     quantisation range: 2.25 for "fp32+fp16", 448 otherwise (core.py:805-807).  smooth_v is honoured
     only for "fp32" (core.py:797-803).  Unknown values raise (the reference silently returns an
-    uninitialised tensor, SURVEY §9 item 10)."""
+    uninitialised tensor)."""
     dtype = q.dtype
     _check_inputs(q, k, v)
     assert qk_quant_gran in ["per_warp", "per_thread"], "qk_quant_gran must be either 'per_warp' or 'per_thread'."
@@ -82,7 +82,7 @@ def sageattn_qk_int8_pv_fp8_cuda(
         sm_scale = head_dim_og ** -0.5
 
     # front-end: K mean (2 launches), Q / K quantisers, V statistics (2) + FP8 quantiser — 7 launches (reference: 6 + k.mean, core.py:773-809).
-    # The single-launch cluster variants (quant.smooth_quant_k, per_channel_fp8(fused=True)) exist but measured slower on B200.
+    # The single-launch cluster variants (quant.smooth_quant_k, per_channel_fp8(fused=True)) are opt-in.
     lse_correction = None
     km = k_mean(k, tensor_layout) if smooth_k else None
     if smooth_k and return_lse:
@@ -109,9 +109,10 @@ def sageattn_qk_int8_pv_fp8_cuda(
 
 def sageattn(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, tensor_layout: str = "HND", is_causal: bool = False,
              sm_scale: Optional[float] = None, return_lse: bool = False, **kwargs: Any):
-    """sageattention/core.py:79-157.  The reference dispatches on compute capability and raises on sm_100;
-    here the single B200 backend is used with the reference's sm89 defaults (per-thread INT8, FP8 PV,
-    "fp32+fp16" V range).  Unknown kwargs (attn_mask=, dropout_p=, scale=, ...) are accepted and ignored
+    """sageattention/core.py:79-157.  The reference dispatches on compute capability; on an H100 it calls its sm90 kernel with
+    pv_accum_dtype="fp32+fp32" (V range 448).  Here the single backend deliberately keeps the reference's sm89 defaults
+    (per-thread INT8, FP8 PV, "fp32+fp16" V range 2.25), so that sageattn() computes the same bytes on every GPU this library
+    has targeted; that is a documented difference from the reference's own sageattn() on an H100.  Unknown kwargs (attn_mask=, dropout_p=, scale=, ...) are accepted and ignored
     exactly like the reference so SDPA monkey-patches keep working (example/cogvideox_infer.py:35).
 
     The 2.25 V range of "fp32+fp16" exists in the reference to keep its fp16 PV accumulator from overflowing; this kernel
@@ -127,7 +128,7 @@ def sageattn_qk_int8_pv_fp8_cuda_sm90(q, k, v, tensor_layout: str = "HND", is_ca
                                       pv_accum_dtype: str = "fp32+fp32", smooth_k: bool = True, smooth_v: bool = False,
                                       return_lse: bool = False, **kwargs: Any):
     """API shell for sageattention/core.py:829-996 (Hopper entry point): same numerics contract, served by
-    the sm_100a kernel.  Only "fp32+fp32" exists in the reference for this entry (core.py:985-989)."""
+    the sm_90a kernel.  Only "fp32+fp32" exists in the reference for this entry (core.py:985-989)."""
     assert pv_accum_dtype == "fp32+fp32", "only 'fp32+fp32' is supported for the sm90 entry point"
     return sageattn_qk_int8_pv_fp8_cuda(q, k, v, tensor_layout=tensor_layout, is_causal=is_causal,
                                         qk_quant_gran=qk_quant_gran, sm_scale=sm_scale, pv_accum_dtype=pv_accum_dtype,
@@ -137,8 +138,8 @@ def sageattn_qk_int8_pv_fp8_cuda_sm90(q, k, v, tensor_layout: str = "HND", is_ca
 def sageattn_qk_int8_pv_fp16_triton(q, k, v, tensor_layout: str = "HND", quantization_backend: str = "triton",
                                     is_causal: bool = False, sm_scale: Optional[float] = None, smooth_k: bool = True,
                                     return_lse: bool = False, attn_mask: Optional[torch.Tensor] = None, **kwargs: Any):
-    """sageattention/core.py:160-331 on sm_100a: per-block INT8 quantisation with the Triton path's exact rounding
-    (bit-exact q/k/scales), sm_scale*log2e folded into q, then the FP16-PV kernel variant (tcgen05 kind::f16, P and
+    """sageattention/core.py:160-331 on sm_90a: per-block INT8 quantisation with the Triton path's exact rounding
+    (bit-exact q/k/scales), sm_scale*log2e folded into q, then the FP16-PV kernel variant (fp16 wgmma, P and
     V in fp16, softmax without exponent offset — the Triton kernel's numerics, triton/attn_qk_int8_per_block.py).
     attn_mask (bool, or the q dtype as an additive bias; broadcast to [B,Hq,Sq,Skv]; non-causal only) follows
     core.py:248-250, 310-325 and attn_qk_int8_per_block.py:33-52 — including the reference's convention that a float
@@ -191,11 +192,11 @@ def sageattn_qk_int8_pv_fp16_cuda(q, k, v, tensor_layout: str = "HND", is_causal
                                   qk_quant_gran: str = "per_thread", sm_scale: Optional[float] = None,
                                   pv_accum_dtype: str = "fp32", smooth_k: bool = True, smooth_v: bool = False,
                                   return_lse: bool = False, **kwargs: Any):
-    """sageattention/core.py:451-633 (INT8 QK^T + **FP16** PV) on sm_100a: V and P stay in fp16 — callers pick this entry
-    over the fp8 ones for accuracy — through the FP16-PV kernel variant (tcgen05 kind::f16, fp32 accumulation in TMEM).
+    """sageattention/core.py:451-633 (INT8 QK^T + **FP16** PV) on sm_90a: V and P stay in fp16 — callers pick this entry
+    over the fp8 ones for accuracy — through the FP16-PV kernel variant (fp16 wgmma, fp32 accumulation).
     Q/K quantisation is the reference's per-warp / per-thread INT8 (core.py:590-593; WARPQ is 32 for every mode here: the
     scale packing is internal to this call).  pv_accum_dtype keeps the reference vocabulary ("fp32", "fp16", "fp16+fp32",
-    core.py:601-617): the B200 tensor core always accumulates PV in fp32, i.e. every mode gets the accuracy of "fp32".
+    core.py:601-617): the kernel always accumulates PV in fp32, i.e. every mode gets the accuracy of "fp32".
     smooth_v exists in the reference only to protect the "fp16" accumulator from overflow (core.py:606-610); with fp32
     accumulation it has nothing to do, so it is accepted and ignored with the reference's warning."""
     dtype = q.dtype
@@ -221,7 +222,7 @@ def sageattn_qk_int8_pv_fp16_cuda(q, k, v, tensor_layout: str = "HND", is_causal
     k_int8, k_scale = quant_k_int8(k, km, qk_quant_gran, tensor_layout)
     gran = SAB_GRAN_PER_WARP if qk_quant_gran == "per_warp" else SAB_GRAN_PER_THREAD
     if smooth_v:
-        warnings.warn(f"pv_accum_dtype is '{pv_accum_dtype}' (fp32 accumulation on B200), smooth_v will be ignored.")
+        warnings.warn(f"pv_accum_dtype is '{pv_accum_dtype}' (fp32 accumulation on this backend), smooth_v will be ignored.")
     v_t = transpose_v_f16(v, tensor_layout=tensor_layout)       # `v.to(torch.float16)`, core.py:603
     o = torch.empty(q.size(), dtype=dtype, device=q.device)
     lse = ops.qk_int8_sv_f16_attn(q_int8, k_int8, v_t, o, q_scale, k_scale, _tensor_layout, 1 if is_causal else 0,
@@ -236,7 +237,7 @@ def sageattn_varlen(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu_seqlen
                     cu_seqlens_k: torch.Tensor, max_seqlen_q: int, max_seqlen_k: int, is_causal: bool = False,
                     sm_scale: Optional[float] = None, smooth_k: bool = True, **kwargs: Any) -> torch.Tensor:
     """sageattention/core.py:334-448: packed [T,H,D] tensors, per-block INT8 per sequence (Triton rounding,
-    bit-exact), K mean over all tokens of the batch (core.py:433), FP16 P and V (tcgen05 kind::f16) like the
+    bit-exact), K mean over all tokens of the batch (core.py:433), FP16 P and V (fp16 wgmma) like the
     reference's Triton varlen kernels."""
     dtype = q.dtype
     _check_inputs(q, k, v)

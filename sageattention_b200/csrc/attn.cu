@@ -1,65 +1,65 @@
-// Fused INT8-QK attention for sm_100a (B200): the EXACT-max kernel and the FP16-PV variants.
+// Fused INT8-QK attention for sm_90a (H100): INT8 QK^T -> fp32 online softmax -> FP8 (or FP16) P -> PV, all products on the
+// warpgroup tensor core (wgmma) with register accumulators.
 //
-// Serves (a) the FP16-PV numerics of the reference's Triton kernels (kPV16: sageattn_varlen, sageattn_qk_int8_pv_fp16_triton
-// incl. attn_mask, sageattn_qk_int8_pv_fp16_cuda) and (b) the INT8+FP8 path with the reference's exact running max
-// (SAB_ATTN_KERNEL=exact, debug dumps, head_dim 64 fallback); the product INT8+FP8 kernel at head_dim 128 is attn_alt.cu.
-// One CTA = one 128-row Q tile of one (batch, head).  384 threads, three warpgroups (setmaxnreg 112 / 80 / 48):
-//   warps 0-3  : softmax / epilogue — ONE THREAD PER Q ROW (TMEM lane == row): row max and row sum need no shuffles
-//   warps 4-7  : correction — rescale this row of O (TMEM) by alpha when the running max moved (alpha through shared memory)
-//   warp 8     : TMA producer (Q once; K and V^T 64-key tiles through an NS-deep mbarrier ring, swizzled smem)
-//   warp 9     : tcgen05.mma issuer (one elected lane) + TMEM allocator;  warps 10-11 idle (setmaxnreg is per warpgroup)
-// The softmax / MMA tile is 64 keys — the reference's CTA_K — so the running-max sequence, P (e4m3) and d are the
-// ones csrc/qattn/qk_int_sv_f8_cuda_sm89.cuh produces.  Tensor memory, 256 columns per CTA (two CTAs per SM):
-//   cols [0,64) / [64,128)  S(j) = Q K_j^T, int32 128x64, kind::i8, DOUBLE-BUFFERED on j&1: QK(j+1), QK(j+2) run on
-//                           the tensor core while the softmax warps work on S(j); P(j) (e4m3, 16 cols) overwrites
-//                           cols [0,16) of its S buffer and is the A operand (from TMEM) of the PV MMA
-//   cols [128,128+D)        O accumulator, fp32 128xD, kind::f8f6f4, B = V^T tile from smem
-// MMA order on the in-order tensor pipe:  QK(0) QK(1) | PV(0) QK(2) | PV(1) QK(3) | ...
-// Numerics follow the reference kernel (base-2 online softmax, -8.807 exponent offset so P fills (0,448], d from
-// un-rounded fp32 P, top-left causal alignment, rcp/lg2/ex2 .approx).  The one deliberate difference: PV accumulates
-// in fp32 inside the tensor core across tiles (the reference's f16 first-level accumulator is a consumer-GPU speed
-// trick; tcgen05 f32 accumulation is full rate).
+// Serves (a) the INT8+FP8 path (sageattn_qk_int8_pv_fp8_cuda and everything built on it) and (b) the FP16-PV numerics of the
+// reference's Triton kernels (kPV16: sageattn_varlen, sageattn_qk_int8_pv_fp16_triton incl. attn_mask,
+// sageattn_qk_int8_pv_fp16_cuda).  One CTA = one 128-row Q tile of one (batch, head), 384 threads:
+//   warps 0-3 / 4-7 : two consumer warpgroups, 64 Q rows each.  Per 64-key tile: S = Q K^T (wgmma s8, int32 accumulators in
+//                     registers), online softmax in registers, P (e4m3 or f16) handed to the PV wgmma as its register A operand,
+//                     O (fp32, 64 x D) accumulated in registers.  The two warpgroups run independently, so one's softmax overlaps
+//                     the other's tensor-core work.
+//   warp 8          : TMA producer (Q once; K and V^T 64-key tiles through a kStages-deep mbarrier ring, swizzled smem);
+//                     warps 9-11 only hand their registers over (setmaxnreg: 24 for the producer warpgroup, 240 for consumers).
+// The softmax / MMA tile is 64 keys — the reference's CTA_K — so the running-max sequence, P and d follow
+// csrc/qattn/qk_int_sv_f8_cuda_sm89.cuh: base-2 online softmax, -8.807 exponent offset so P fills (0,448], d from un-rounded fp32
+// P, top-left causal alignment, rcp/lg2/ex2 .approx.  FP8 PV is accumulated in two levels: each tile's product starts from zero in
+// the tensor core and is added to O in fp32 on the CUDA cores (Hopper's FP8 wgmma keeps fewer accumulator bits than fp32, so a
+// long accumulation inside the tensor core drifts; the reference's sm90 kernel does the same).  FP16 PV accumulates in place.
+// Running max of the INT8+FP8 path: LAZY by default (lazy_tau = 4 binades): the max moves only when an element of the tile would
+// overflow e4m3 (P > 448); when it moves, the new row maximum is placed tau binades below 448 (exponent offset 8.807 - tau), so O
+// is rarely rescaled.  P keeps e4m3's relative precision; it is a different rounding realisation than the reference kernel's (same
+// accuracy against exact attention, tests/test_gpu_parity.py).  SAB_ATTN_KERNEL=exact selects the reference's exact running max
+// (lazy_tau = 0): P, m and d are then the reference kernel's.
 #include <cstdlib>
 #include "attn_common.cuh"
 
 namespace sab {
 
-constexpr int kNumThreads = 384;  // warpgroups: 0-3 softmax, 4-7 correction, 8 TMA / 9 MMA / 10-11 idle (setmaxnreg is per warpgroup)
+constexpr int kConsumerWGs = 2;                           // 64 Q rows each
+constexpr int kNumThreads = (kConsumerWGs + 1) * 128;     // + the producer warpgroup (one TMA warp; setmaxnreg is per warpgroup)
+constexpr int kStages = 6;                                // K / V^T ring depth (64-key tiles)
+
+template <int D, bool kPV16>
+constexpr size_t attn_smem_bytes() {
+  return size_t(BM) * D + size_t(kStages) * (BN * D + BN * D * (kPV16 ? 2 : 1)) + (1 + 2 * kStages) * 8 + 1024;
+}
 
 // D: head dim (64 / 128).  kKT: per-thread K scales (4 per 64-key block) instead of 1.  OutT: __half / bf16.
-// kPV16: P and V in fp16 (tcgen05 kind::f16) with the Triton path's softmax (no exponent offset) — the numerics of the
-// reference's sageattn_qk_int8_pv_fp16_triton / sageattn_varlen kernels (triton/attn_qk_int8_per_block.py:22-128).
-// kMask (kPV16 only): attn_mask of sageattn_qk_int8_pv_fp16_triton — a bool mask marks elements like the out-of-range
-// keys (integer sentinel), an additive bias takes the float path `tile_bias` below.
-// kSeg: sequence-parallel form whose K/V segments arrive WHILE the kernel runs (peer copies on another stream): the TMA
-// producer polls one flag per (KV-head group, segment) before the first tile of a segment (AttnParams::seg_flags).
-template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false, bool kSeg = false>
-__global__ void __launch_bounds__(kNumThreads, 2)
+// kPV16: P and V in fp16 with the Triton path's softmax (no exponent offset) — the numerics of the reference's
+// sageattn_qk_int8_pv_fp16_triton / sageattn_varlen kernels (triton/attn_qk_int8_per_block.py:22-128).
+// kMask (kPV16 only): attn_mask of sageattn_qk_int8_pv_fp16_triton — a bool mask marks elements like the out-of-range keys
+// (integer sentinel), an additive bias takes the float path below.
+// Sequence-parallel fused gather (p.seg_flags != nullptr): K/V segments arrive WHILE the kernel runs (peer copies on another
+// stream); the TMA producer polls one flag per (KV-head group, segment) before the first tile of a segment.
+template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false>
+__global__ void __launch_bounds__(kNumThreads, 1)
 sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
-  // K / V^T ring: one slot = one 64-key tile (K tile 64 x D bytes + V^T tile D rows x 64 keys)
+                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnParams p) {
   constexpr uint32_t K_TILE = BN * D;
   constexpr uint32_t V_TILE = D * BN * (kPV16 ? 2 : 1);
-  constexpr int NS = kPV16 ? ((D == 128) ? 3 : 6) : ((D == 128) ? 5 : 10);
-  constexpr int SWQK = (D == 128) ? 128 : 64;   // swizzle span of the Q/K tiles (= row bytes)
+  constexpr int SWQK = D;                        // swizzle span of the Q/K tiles (= row bytes)
   constexpr int SWV = kPV16 ? 128 : 64;          // V^T rows: 64 keys = 64 B (fp8) / 128 B (fp16)
   constexpr uint32_t Q_BYTES = BM * D;
-  constexpr int PCOLS = kPV16 ? 32 : 16;         // TMEM columns of P (64 keys)
-  constexpr int NG = kKT ? 4 : 1;                // dequant-scale groups per 64-key tile
+  constexpr int NO = D / 2;                      // fp32 O accumulators per thread (64 x D over 128 threads)
 
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
   uint8_t* sK = sQ + Q_BYTES;
-  uint8_t* sV = sK + NS * K_TILE;
-  float* s_alpha = reinterpret_cast<float*>(sV + NS * V_TILE);   // [2][128] alpha(j): softmax -> correction warps
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_alpha + 2 * BM);
-  uint64_t* q_full = bars + 0;
-  uint64_t* s_full = bars + 1;    // [2] step(t) retired: S(t+2) ready in buffer t&1 AND PV(t) accumulated into O
-  uint64_t* p_full = bars + 3;    // [2] 256 arrivals: P(j) stored (softmax) + O rescaled (correction)
-  uint64_t* a_full = bars + 5;    // [2] 128 arrivals: alpha(j) published by the softmax warps
-  uint64_t* kv_full = bars + 7;   // [NS] TMA bytes landed (K + V^T tile)
-  uint64_t* kv_empty = kv_full + NS;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(kv_empty + NS);
+  uint8_t* sV = sK + kStages * K_TILE;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kStages * V_TILE);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = bars + 1;                  // [kStages] TMA bytes landed (K + V^T tile)
+  uint64_t* kv_empty = kv_full + kStages;        // [kStages] both consumer warpgroups finished with the slot
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -87,428 +87,337 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   int n_kv = (kv_len + BN - 1) / BN;                 // 64-key tiles
   if (p.causal) n_kv = min(n_kv, (p.causal_q_offset + (qt + 1) * BM + BN - 1) / BN);
 
-  // ---------------- one-time setup
-  if (warp == 8 && lane == 0) {
+  if (threadIdx.x == 0) {
     if ((smem_u32(smem) & 1023u) != 0) __trap();     // swizzled tiles need a 1 KB-aligned base
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
     mbar_init(q_full, 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(s_full + i, 1);
-      mbar_init(p_full + i, 256);
-      mbar_init(a_full + i, 128);
-    }
-    for (int i = 0; i < NS; ++i) {
+    for (int i = 0; i < kStages; ++i) {
       mbar_init(kv_full + i, 1);
-      mbar_init(kv_empty + i, 1);
+      mbar_init(kv_empty + i, kConsumerWGs);
     }
     fence_barrier_init();
   }
-  if (warp == 9) tmem_alloc<kTmemCols>(tmem_holder);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-  const uint32_t tO = tmem_base + 128;  // cols [128,128+D); S buffer b at cols [64b, 64b+64), P(b) at its first 16
-  // parity of the phase of s_full[t & 1] that completes when step(t-2) retires (S(t) ready / PV(t-2) accumulated)
-  auto s_parity = [](int t) { return uint32_t(t >> 1) & 1u; };
 
-  if (warp >= 8) {
-    setmaxnreg_dec_48();
-    if (warp == 8) {
-      // =============================== TMA producer ===============================
-      if (lane == 0 && n_kv > 0) {
-        mbar_expect_tx(q_full, Q_BYTES);
-        tma_load_4d(sQ, &tmQ, q_full, 0, q_off + qt * BM, h, tb);
-        [[maybe_unused]] int ready_seg = -1;
-        for (int j = 0; j < n_kv; ++j) {
-          const int s = j % NS;
-          const uint32_t ph = (j / NS) & 1;
-          int kc = k_off + j * BN, vc = v_off + j * BN, kb = tb;
-          if (p.kv_seg_len > 0) {  // all-gathered layout: segment-major
-            const int seg = (j * BN) / p.kv_seg_len;
-            kc = vc = j * BN - seg * p.kv_seg_len;
-            kb = seg * p.B + b;
-            if constexpr (kSeg) {
-              if (seg != ready_seg) {   // first tile of a segment: has the peer copy of this (head group, segment) landed?
-                const uint32_t* flag = p.seg_flags + (hk / p.seg_heads) * (p.Sk / p.kv_seg_len) + seg;
-                const long long t0 = clock64();
-                while (ld_acquire_sys_u32(flag) != p.seg_epoch) {
-                  __nanosleep(200);
-                  if (clock64() - t0 > (8ll << 30)) __trap();   // ~4 s: the copies never came; fail the launch instead of hanging the GPU
-                }
-                fence_proxy_async_all();
-                ready_seg = seg;
-              }
+  if (warp >= kConsumerWGs * 4) {
+    // =============================== TMA producer ===============================
+    setmaxnreg_dec<24>();
+    if (warp == kConsumerWGs * 4 && lane == 0 && n_kv > 0) {
+      tma_prefetch_desc(&tmQ);
+      tma_prefetch_desc(&tmK);
+      tma_prefetch_desc(&tmV);
+      mbar_expect_tx(q_full, Q_BYTES);
+      tma_load_4d(sQ, &tmQ, q_full, 0, q_off + qt * BM, h, tb);
+      int ready_seg = -1;
+      for (int j = 0; j < n_kv; ++j) {
+        const int s = j % kStages;
+        const uint32_t ph = (j / kStages) & 1;
+        int kc = k_off + j * BN, vc = v_off + j * BN, kb = tb;
+        if (p.kv_seg_len > 0) {  // all-gathered layout: segment-major
+          const int seg = (j * BN) / p.kv_seg_len;
+          kc = vc = j * BN - seg * p.kv_seg_len;
+          kb = seg * p.B + b;
+          if (p.seg_flags != nullptr && seg != ready_seg) {
+            // first tile of a segment: has the peer copy of this (head group, segment) landed?
+            const uint32_t* flag = p.seg_flags + (hk / p.seg_heads) * (p.Sk / p.kv_seg_len) + seg;
+            const long long t0 = clock64();
+            while (ld_acquire_sys_u32(flag) != p.seg_epoch) {
+              __nanosleep(200);
+              if (clock64() - t0 > (8ll << 30)) __trap();   // ~4 s: the copies never came; fail the launch instead of hanging
             }
+            fence_proxy_async_all();
+            ready_seg = seg;
           }
-          mbar_wait_wd(kv_empty + s, ph ^ 1);
-          mbar_expect_tx(kv_full + s, K_TILE + V_TILE);
-          tma_load_4d(sK + s * K_TILE, &tmK, kv_full + s, 0, kc, hk, kb);
-          tma_load_4d(sV + s * V_TILE, &tmV, kv_full + s, vc * (kPV16 ? 2 : 1), 0, hk, kb);   // byte coordinate
         }
-      }
-    } else if (warp == 9) {
-      // =============================== MMA issuer ===============================
-      // step(t) = PV(t) ; QK(t+2) ; commit -> s_full[t&1].   In-order tensor pipe:  QK0 QK1 | PV0 QK2 | PV1 QK3 | ...
-      if (n_kv > 0) {   // whole warp runs the loop (uniform control flow); one elected lane issues
-        constexpr uint32_t idesc_qk = make_idesc(2, 1, 1, BM, BN);  // s32 <- s8 x s8, 128 x 64
-        constexpr uint32_t idesc_pv = make_idesc(1, 0, 0, BM, D);   // f32 <- e4m3 x e4m3, 128 x D
-        const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-        const uint64_t dQ = make_smem_desc<SWQK>(smem_u32(sQ));
-        const uint64_t dK0 = make_smem_desc<SWQK>(smem_u32(sK));
-        const uint64_t dV0 = make_smem_desc<SWV>(smem_u32(sV));
-        auto issue_qk = [&](int t, bool wait_kv) {
-          const int st = t % NS;
-          if (wait_kv) {
-            mbar_wait_wd(kv_full + st, (t / NS) & 1);    // K(t) (and V^T(t)) landed
-            tc_fence_after();
-          }
-          const uint64_t dK = dK0 + uint64_t(st) * (K_TILE >> 4);
-          const uint32_t tS = tmem_u + (t & 1) * BN;
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < D / 32; ++k) umma_i8_ss(tS, dQ + 2 * k, dK + 2 * k, idesc_qk, k > 0);
-          }
-        };
-        mbar_wait_wd(q_full, 0);
-        issue_qk(0, true);
-        if (elect_one()) tc_commit(s_full + 0);
-        if (n_kv > 1) {
-          issue_qk(1, true);
-          if (elect_one()) tc_commit(s_full + 1);
-        }
-#ifdef SAB_TIMELINE
-        const bool tl_on = p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && lane == 0;
-        long long* tl = reinterpret_cast<long long*>(p.dbg) + 4096;
-#endif
-        for (int j = 0; j < n_kv; ++j) {
-          SAB_TL(8);
-          // K(j+2) comes from a slot filled several tiles ago: check it while P(j) is still being produced
-          if (j + 2 < n_kv) mbar_wait_wd(kv_full + (j + 2) % NS, ((j + 2) / NS) & 1);
-          mbar_wait_wd(p_full + (j & 1), (j >> 1) & 1);   // P(j) stored + O rescaled (also: S(j) fully consumed)
-          tc_fence_after();
-          SAB_TL(9);
-          const int st = j % NS;
-          const uint64_t dV = dV0 + uint64_t(st) * (V_TILE >> 4);
-          const uint32_t tP = tmem_u + (j & 1) * BN;
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < (kPV16 ? BN / 16 : BN / 32); ++k) {
-              if constexpr (kPV16) umma_f16_ts(tmem_u + 128, tP + 8 * k, dV + 2 * k, idesc_pv, (j > 0 || k > 0));
-              else umma_f8_ts(tmem_u + 128, tP + 8 * k, dV + 2 * k, idesc_pv, (j > 0 || k > 0));
-            }
-          }
-          SAB_TL(10);
-          if (j + 2 < n_kv) issue_qk(j + 2, false);        // reuses S buffer j&1 (after PV(j): in-order pipe)
-          if (elect_one()) {
-            tc_commit(s_full + (j & 1));
-            tc_commit(kv_empty + st);                      // slot j consumed once this step retires
-          }
-          SAB_TL(11);
-        }
+        mbar_wait_wd(kv_empty + s, ph ^ 1);
+        mbar_expect_tx(kv_full + s, K_TILE + V_TILE);
+        tma_load_4d(sK + s * K_TILE, &tmK, kv_full + s, 0, kc, hk, kb);
+        tma_load_4d(sV + s * V_TILE, &tmV, kv_full + s, vc * (kPV16 ? 2 : 1), 0, hk, kb);   // byte coordinate
       }
     }
-  } else if (warp >= 4) {
-    // =============================== correction: rescale O when the running max moved ===============================
-    // stays at the launch allocation (80 regs): 128 x (112 + 80 + 48) = 30720 = the CTA's register pool
-    const int row = (warp - 4) * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>((warp - 4) * 32) << 16;
-    for (int j = 0; j < n_kv; ++j) {
-      mbar_wait_wd(a_full + (j & 1), (j >> 1) & 1);
-      const float alpha = s_alpha[(j & 1) * BM + row];
-      if (j > 0 && __any_sync(0xffffffffu, alpha != 1.0f)) {
-        mbar_wait_wd(s_full + ((j + 1) & 1), s_parity(j + 1));   // step(j-1) retired: PV(j-1) is in O
-        tc_fence_after();
-        const uint64_t alpha2 = pack_f2(alpha, alpha);
-#pragma unroll
-        for (int ch = 0; ch < D / 32; ++ch) {
-          uint32_t r[32];
-          tmem_ld32(tO + lane_off + ch * 32, r);
-          tc_wait_ld();
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            float lo, hi;
-            unpack_f2(fmul2(pack_f2(__uint_as_float(r[i]), __uint_as_float(r[i + 1])), alpha2), lo, hi);
-            r[i] = __float_as_uint(lo);
-            r[i + 1] = __float_as_uint(hi);
-          }
-          tmem_st32(tO + lane_off + ch * 32, r);
-        }
-        tc_wait_st();
-      }
-      tc_fence_before();
-      mbar_arrive(p_full + (j & 1));
-    }
-  } else {
-    setmaxnreg_inc_112();
-    // =============================== softmax / epilogue ===============================
-    const int row = warp * 32 + lane;  // TMEM lane == Q row inside the tile
-    const uint32_t lane_off = static_cast<uint32_t>(warp * 32) << 16;
-    const int q_row = qt * BM + row;  // row index inside the sequence
-    const bool dump = p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0;
+    return;
+  }
 
+  // =============================== consumer warpgroups ===============================
+  setmaxnreg_inc<240>();
+  // wgmma accumulator layout (m64nN): warp w of the warpgroup owns rows 16w..16w+15; lane = 4 g + t holds rows 16w+g (registers
+  // 4i, 4i+1) and 16w+g+8 (4i+2, 4i+3) at columns 8i+2t, 8i+2t+1.  A row is spread over the 4 lanes of a quad.
+  const int wg = warp >> 2;
+  const int t = lane & 3;
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // rows row0 and row0 + 8 of the Q tile
+  int q_row[2];
+  float qss[2];
+  const float* qs_base = p.q_scale + (varlen ? int64_t(h) : (int64_t(b) * p.Hq + h) * p.qs_stride_bh);
+  const float* ks_base = p.k_scale + (varlen ? int64_t(hk) : (int64_t(b) * p.Hkv + hk) * p.ks_stride_bh);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int row = row0 + 8 * i;
+    q_row[i] = qt * BM + row;  // row index inside the sequence
     // per-row Q dequant scale (qk_int_sv_f8_cuda_sm89.cuh:98-114)
     int q_idx = (q_blk0 + qt) * p.q_mult;
     if (p.q_gran == SAB_GRAN_PER_WARP) q_idx += row >> 5;
     if (p.q_gran == SAB_GRAN_PER_THREAD) q_idx += (row >> 5) * 8 + (row & 7);
-    const float* qs_base = p.q_scale + (varlen ? int64_t(h) : (int64_t(b) * p.Hq + h) * p.qs_stride_bh);
-    const float* ks_base = p.k_scale + (varlen ? int64_t(hk) : (int64_t(b) * p.Hkv + hk) * p.ks_stride_bh);
-    const float qss = qs_base[int64_t(q_idx) * p.qs_stride_idx] * p.sm_scale_log2;
-
-    float m = kMaskValue;  // running max (log2 units, includes the -8.807 offset)
-    float d = 0.f;         // running sum of fp32 P
-#ifdef SAB_TIMELINE
-    const bool tl_on = p.dbg != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0;
-    long long* tl = reinterpret_cast<long long*>(p.dbg) + 4096;
-#endif
-
-    for (int j = 0; j < n_kv; ++j) {
-      const uint32_t tS = tmem_base + lane_off + (j & 1) * BN;
-      // dequant coefficient per scale group of this tile (…sm89.cuh:116-132, 255-257); tile j == 64-key block j
-      float coef[NG];
+    qss[i] = qs_base[int64_t(q_idx) * p.qs_stride_idx] * p.sm_scale_log2;
+  }
+  const float tau = p.lazy_tau;
+  float m[2] = {kMaskValue, kMaskValue};   // running max (log2 units, includes the -8.807 offset on the fp8 path)
+  float d[2] = {0.f, 0.f};                 // this thread's part of the running sum of fp32 P
+  float o[NO];
 #pragma unroll
-      for (int g = 0; g < NG; ++g) coef[g] = ks_base[int64_t((k_blk0 + j) * NG + g) * p.ks_stride_idx] * qss;
-      // number of visible keys of this tile for this row (OOB + causal, attn_utils.cuh:296-351)
-      int limit = kv_len - j * BN;
-      if (p.causal) limit = min(limit, p.causal_q_offset + q_row - j * BN + 1);
-      const bool masked_tile = (kv_len - j * BN < BN) || (p.causal && (j + 1) * BN > p.causal_q_offset + qt * BM + 1);
+  for (int i = 0; i < NO; ++i) o[i] = 0.f;
 
-      SAB_TL(0);
-      {
-        mbar_wait_wd(s_full + (j & 1), s_parity(j));
-        tc_fence_after();
-      }
-      SAB_TL(1);
-      uint32_t s[BN];
-      {
-        uint32_t (&lo)[32] = *reinterpret_cast<uint32_t (*)[32]>(&s[0]);
-        uint32_t (&hi)[32] = *reinterpret_cast<uint32_t (*)[32]>(&s[32]);
-        tmem_ld32(tS, lo);
-        tmem_ld32(tS + 32, hi);
-        tc_wait_ld();
-      }
-      SAB_TL(2);
-      if (dump && j == 0) {
+  const uint64_t dQ = make_wgmma_desc<SWQK>(smem_u32(sQ + wg * 64 * D));
+  const uint64_t dK0 = make_wgmma_desc<SWQK>(smem_u32(sK));
+  const uint64_t dV0 = make_wgmma_desc<SWV>(smem_u32(sV));
+  // P handed from the accumulator layout to the 8-bit A-operand layout (lane t of a quad holds keys 4t..4t+3 and 16+4t..16+4t+3
+  // of each 32-key chunk): two 16-bit pairs from lanes 2(t&1) and 2(t&1)+1 of the quad, from block 0 or 1 of the chunk
+  const int src0 = (lane & ~3) | ((t & 1) << 1);
+  const uint32_t psel = (t >> 1) ? 0x7632u : 0x5410u;
+
+  if (n_kv > 0) mbar_wait_wd(q_full, 0);
+  for (int j = 0; j < n_kv; ++j) {
+    const int st = j % kStages;
+    float coef[2];
+    {
+      // dequant coefficient (…sm89.cuh:116-132, 255-257); tile j == 64-key block j.  Per-thread K scales: the keys of lane t
+      // (8i+2t, 8i+2t+1) are all in scale group t.
+      const float ksv = ks_base[int64_t((k_blk0 + j) * (kKT ? 4 : 1) + (kKT ? t : 0)) * p.ks_stride_idx];
+      coef[0] = ksv * qss[0];
+      coef[1] = ksv * qss[1];
+    }
+    // number of visible keys of this tile per row (OOB + causal, attn_utils.cuh:296-351)
+    int limit[2];
 #pragma unroll
-        for (int i = 0; i < BN; ++i) p.dbg[row * BN + i] = int(s[i]);
-      }
+    for (int i = 0; i < 2; ++i) {
+      limit[i] = kv_len - j * BN;
+      if (p.causal) limit[i] = min(limit[i], p.causal_q_offset + q_row[i] - j * BN + 1);
+      if (kMask && q_row[i] >= q_len) limit[i] = 0;   // rows past the end: nothing visible, no mask bytes read
+    }
+    const bool masked_tile = kMask || (kv_len - j * BN < BN) || (p.causal && (j + 1) * BN > p.causal_q_offset + qt * BM + 1);
 
-      [[maybe_unused]] const char* mrow = nullptr;   // this row's 64 mask elements of tile j
-      if constexpr (kMask) {
-        const int64_t off = int64_t(b) * p.mask_sb + int64_t(h) * p.mask_sh + int64_t(q_row) * p.mask_sm + int64_t(j) * BN * p.mask_sn;
-        mrow = reinterpret_cast<const char*>(p.mask) + off * (p.mask_kind == 1 ? 1 : 2);
-        if (q_row >= q_len) limit = 0;   // rows past the end: nothing visible, no mask bytes read
+    mbar_wait_wd(kv_full + st, (j / kStages) & 1);
+    uint32_t s[32];
+    wgmma_fence();
+    {
+      const uint64_t dK = dK0 + uint64_t(st) * (K_TILE >> 4);
+#pragma unroll
+      for (int k = 0; k < D / 32; ++k) wgmma_qk_i8(s, dQ + 2 * k, dK + 2 * k, k > 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+
+    [[maybe_unused]] const char* mrow[2] = {nullptr, nullptr};   // this row's 64 mask elements of tile j
+    if constexpr (kMask) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int64_t off = int64_t(b) * p.mask_sb + int64_t(h) * p.mask_sh + int64_t(q_row[i]) * p.mask_sm + int64_t(j) * BN * p.mask_sn;
+        mrow[i] = reinterpret_cast<const char*>(p.mask) + off * (p.mask_kind == 1 ? 1 : 2);
         if (p.mask_kind == 1) {
 #pragma unroll
-          for (int i = 0; i < BN; ++i) {
-            if (i < limit && __ldg(reinterpret_cast<const uint8_t*>(mrow) + int64_t(i) * p.mask_sn) == 0) s[i] = uint32_t(kIntSentinel);
+          for (int c = 0; c < 16; ++c) {
+            const int key = 8 * (c >> 1) + 2 * t + (c & 1);
+            if (key < limit[i] && __ldg(reinterpret_cast<const uint8_t*>(mrow[i]) + int64_t(key) * p.mask_sn) == 0)
+              s[4 * (c >> 1) + 2 * i + (c & 1)] = uint32_t(kIntSentinel);
           }
         }
       }
+    }
 
-      auto tile = [&](auto masked_tag) {
-        constexpr bool MASKED = decltype(masked_tag)::value;
-        // ---- row max.  Scales are positive, so max_c(S_c*coef_g(c)) = max_g(coef_g * max_{c in g} S_c): integer
-        //      max per scale group (DPX 3-input max), one int->float conversion per group instead of per element.
-        if constexpr (MASKED) {
+    float e[32];           // P in fp32, same register order as S
+    float alpha[2];
+    auto tile = [&](auto masked_tag) {
+      constexpr bool MASKED = decltype(masked_tag)::value;
 #pragma unroll
-          for (int i = 0; i < BN; ++i)
-            if (i >= limit) s[i] = uint32_t(kIntSentinel);
-        }
-        float mx = kMaskValue;
+      for (int i = 0; i < 2; ++i) {
+        // ---- row max.  Scales are positive, so max_c(S_c*coef) = coef * max_c S_c: integer max, one conversion per row part
+        int v = kIntSentinel;
 #pragma unroll
-        for (int g = 0; g < NG; ++g) {
-          int v = kIntSentinel;
-          if constexpr (kKT) {
-#pragma unroll
-            for (int i8 = 0; i8 < BN; i8 += 8) v = __vimax3_s32(v, int(s[i8 + 2 * g]), int(s[i8 + 2 * g + 1]));
-          } else {
-            int v0 = kIntSentinel, v1 = kIntSentinel, v2 = kIntSentinel, v3 = kIntSentinel;   // 4 chains: ILP
-#pragma unroll
-            for (int i = 0; i < BN; i += 8) {
-              v0 = __vimax3_s32(v0, int(s[i]), int(s[i + 1]));
-              v1 = __vimax3_s32(v1, int(s[i + 2]), int(s[i + 3]));
-              v2 = __vimax3_s32(v2, int(s[i + 4]), int(s[i + 5]));
-              v3 = __vimax3_s32(v3, int(s[i + 6]), int(s[i + 7]));
-            }
-            v = max(max(v0, v1), max(v2, v3));
+        for (int c = 0; c < 16; ++c) {
+          const int idx = 4 * (c >> 1) + 2 * i + (c & 1);
+          if constexpr (MASKED) {
+            if (8 * (c >> 1) + 2 * t + (c & 1) >= limit[i]) s[idx] = uint32_t(kIntSentinel);
           }
-          float c = float(v) * coef[g];
-          if constexpr (MASKED) c = (v == kIntSentinel) ? kMaskValue : c;
-          mx = fmaxf(mx, c);
+          v = max(v, int(s[idx]));
         }
-        // fp8 P: update_mdo with the -log2(448) offset (attn_utils.cuh:377-396); fp16 P: plain running max (Triton path)
-        const float m_new = fmaxf(m, kPV16 ? mx : mx - kFp8Offset);
-        const float alpha = ex2_approx(m - m_new);
-        d *= alpha;
-        m = m_new;
-        // publish alpha: the correction warpgroup rescales this row of O (in TMEM) concurrently with the exponentials.
-        // Double-buffered: alpha(j+2) is written only after s_full(j+2), i.e. after the correction warp read alpha(j).
-        s_alpha[(j & 1) * BM + row] = alpha;
-        mbar_arrive(a_full + (j & 1));
+        float mx = float(v) * coef[i];
+        if constexpr (MASKED) mx = (v == kIntSentinel) ? kMaskValue : mx;
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        float m_new;
+        if constexpr (kPV16) {
+          m_new = fmaxf(m[i], mx);                             // plain running max (Triton path)
+        } else {
+          // update_mdo with the -log2(448) offset (attn_utils.cuh:377-396); lazy: move only by more than tau binades
+          const float m_true = fmaxf(m[i], mx - (kFp8Offset - tau));
+          m_new = (m_true - m[i] > tau) ? m_true : m[i];
+        }
+        alpha[i] = (m_new != m[i]) ? ex2_approx(m[i] - m_new) : 1.0f;
+        d[i] *= alpha[i];
+        m[i] = m_new;
+        // ---- P = exp2(S*coef - m_new); I2FP is exact (|S| < 2^24) and the FMA is the reference's fmaf(S, sm_scale', -m)
+        //      (attn_utils.cuh:450), so P is bit-identical to the reference kernel's at the same m
         const float nm = -m_new;
-        SAB_TL(3);
-
-        // ---- P = exp2(S*coef - m_new) -> e4m3 into TMEM (over the S buffer), d += sum(P).
-        // I2FP is exact (|S| < 2^24) and the FMA is the reference's fmaf(S, sm_scale', -m) (attn_utils.cuh:450), so P
-        // is bit-identical to the reference kernel's.  Packed fp32x2 math (FFMA2 / FADD2): elements (i, i+1) always
-        // share a scale group, so the dequant FMA and the row-sum accumulate issue once per PAIR.
-        uint64_t coef2[NG];
+        float sum = 0.f;
 #pragma unroll
-        for (int g = 0; g < NG; ++g) coef2[g] = pack_f2(coef[g], coef[g]);
-        const uint64_t nm2 = pack_f2(nm, nm);
-        uint64_t acc[4] = {0ull, 0ull, 0ull, 0ull};
-        uint32_t pk[PCOLS];
-#pragma unroll
-        for (int w = 0; w < BN / 4; ++w) {
-          float e[4];
-#pragma unroll
-          for (int u = 0; u < 4; u += 2) {
-            const int i = 4 * w + u;
-            const int g = kKT ? ((i & 7) >> 1) : 0;
-            const uint64_t f2 = pack_f2(__int2float_rn(int(s[i])), __int2float_rn(int(s[i + 1])));
-            float y0, y1;
-            unpack_f2(ffma2(f2, coef2[g], nm2), y0, y1);
-            e[u] = ex2_approx(y0);
-            e[u + 1] = ex2_approx(y1);
-            if constexpr (MASKED && kMask) {   // masked-out elements are not a prefix of the tile
-              e[u] = (int(s[i]) != kIntSentinel) ? e[u] : 0.f;
-              e[u + 1] = (int(s[i + 1]) != kIntSentinel) ? e[u + 1] : 0.f;
-            } else if constexpr (MASKED) {
-              e[u] = (i < limit) ? e[u] : 0.f;
-              e[u + 1] = (i + 1 < limit) ? e[u + 1] : 0.f;
-            }
-            acc[(w & 1) * 2 + (u >> 1)] = fadd2(acc[(w & 1) * 2 + (u >> 1)], pack_f2(e[u], e[u + 1]));
-          }
-          if constexpr (kPV16) {
-            pk[2 * w] = pack_f16x2(e[0], e[1]);       // p.to(tl.float16), attn_qk_int8_per_block.py:62
-            pk[2 * w + 1] = pack_f16x2(e[2], e[3]);
+        for (int c = 0; c < 16; c += 2) {
+          const int idx = 4 * (c >> 1) + 2 * i;
+          const float y0 = fmaf(__int2float_rn(int(s[idx])), coef[i], nm), y1 = fmaf(__int2float_rn(int(s[idx + 1])), coef[i], nm);
+          float x[2];
+#ifdef SAB_POLY_EXP_PAIRS
+          if (t < SAB_POLY_EXP_PAIRS) {   // column pair t of every 8 columns
+            ex2_poly2(y0, y1, x[0], x[1]);
           } else {
-            pk[w] = pack_e4m3x4(e[0], e[1], e[2], e[3]);
+            x[0] = ex2_approx(y0);
+            x[1] = ex2_approx(y1);
+          }
+#else
+          x[0] = ex2_approx(y0);
+          x[1] = ex2_approx(y1);
+#endif
+#pragma unroll
+          for (int u = 0; u < 2; ++u) {
+            if constexpr (MASKED && kMask) x[u] = (int(s[idx + u]) != kIntSentinel) ? x[u] : 0.f;   // masked-out elements: not a prefix
+            else if constexpr (MASKED) x[u] = (8 * (c >> 1) + 2 * t + u < limit[i]) ? x[u] : 0.f;
+            e[idx + u] = x[u];
+            sum += x[u];
           }
         }
-        {
-          float a0, a1, a2, a3;
-          unpack_f2(fadd2(acc[0], acc[1]), a0, a1);
-          unpack_f2(fadd2(acc[2], acc[3]), a2, a3);
-          d += (a0 + a1) + (a2 + a3);
-        }
-        SAB_TL(4);
-        if constexpr (kPV16) tmem_st32(tS, pk);
-        else tmem_st16(tS, pk);
-        if (!kPV16 && dump && j == 0) {
+        d[i] += sum;
+      }
+    };
+    // additive bias (attn_qk_int8_per_block.py:41,50-51): qk = S*scale + bias in fp32, then the plain online softmax
+    auto tile_bias = [&]() {
+      if constexpr (kMask && kPV16) {
 #pragma unroll
-          for (int w = 0; w < BN / 4; ++w) p.dbg[128 * BN + row * 16 + w] = int(pk[w]);
-        }
-      };
-      // additive bias (attn_qk_int8_per_block.py:41,50-51): qk = S*scale + bias in fp32, then the plain online softmax
-      auto tile_bias = [&]() {
-        if constexpr (kMask && kPV16) {
+        for (int i = 0; i < 2; ++i) {
           float mx = -INFINITY;
 #pragma unroll
-          for (int i = 0; i < BN; ++i) {
+          for (int c = 0; c < 16; ++c) {
+            const int idx = 4 * (c >> 1) + 2 * i + (c & 1);
+            const int key = 8 * (c >> 1) + 2 * t + (c & 1);
             float y = -INFINITY;
-            if (i < limit) {
-              const float bias = float(__ldg(reinterpret_cast<const OutT*>(mrow) + int64_t(i) * p.mask_sn));
-              y = fmaf(__int2float_rn(int(s[i])), coef[kKT ? ((i & 7) >> 1) : 0], bias);
+            if (key < limit[i]) {
+              const float bias = float(__ldg(reinterpret_cast<const OutT*>(mrow[i]) + int64_t(key) * p.mask_sn));
+              y = fmaf(__int2float_rn(int(s[idx])), coef[i], bias);
             }
-            s[i] = __float_as_uint(y);
+            e[idx] = y;
             mx = fmaxf(mx, y);
           }
-          const float m_new = fmaxf(m, mx);     // m starts at the finite mask value: never -inf
-          const float alpha = ex2_approx(m - m_new);
-          d *= alpha;
-          m = m_new;
-          s_alpha[(j & 1) * BM + row] = alpha;
-          mbar_arrive(a_full + (j & 1));
-          uint32_t pk[PCOLS];
-          float sum0 = 0.f, sum1 = 0.f;
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+          mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+          const float m_new = fmaxf(m[i], mx);     // m starts at the finite mask value: never -inf
+          alpha[i] = ex2_approx(m[i] - m_new);
+          d[i] *= alpha[i];
+          m[i] = m_new;
+          float sum = 0.f;
 #pragma unroll
-          for (int i = 0; i < BN; i += 2) {
-            const float e0 = ex2_approx(__uint_as_float(s[i]) - m_new), e1 = ex2_approx(__uint_as_float(s[i + 1]) - m_new);
-            sum0 += e0;
-            sum1 += e1;
-            pk[i / 2] = pack_f16x2(e0, e1);
+          for (int c = 0; c < 16; ++c) {
+            const int idx = 4 * (c >> 1) + 2 * i + (c & 1);
+            e[idx] = ex2_approx(e[idx] - m_new);
+            sum += e[idx];
           }
-          d += sum0 + sum1;
-          tmem_st32(tS, pk);
+          d[i] += sum;
         }
-      };
-      if (kMask && p.mask_kind == 2) tile_bias();
-      else if (kMask || masked_tile) tile(std::true_type{});
-      else tile(std::false_type{});
+      }
+    };
+    if (kMask && p.mask_kind == 2) tile_bias();
+    else if (masked_tile) tile(std::true_type{});
+    else tile(std::false_type{});
 
-      SAB_TL(5);
-      {
-        tc_wait_st();
-        SAB_TL(6);
-        tc_fence_before();
-        mbar_arrive(p_full + (j & 1));
+    // ---- rescale O (registers) when the running max moved; PV(j-1) has completed
+    auto rescale_o = [&]() {
+      if (alpha[0] != 1.0f || alpha[1] != 1.0f) {
+#pragma unroll
+        for (int i = 0; i < NO; i += 4) {
+          o[i] *= alpha[0];
+          o[i + 1] *= alpha[0];
+          o[i + 2] *= alpha[1];
+          o[i + 3] *= alpha[1];
+        }
       }
-      SAB_TL(7);
-    }
+    };
 
-    // ---- epilogue: O / d * v_scale (+ v_mean) -> fp16/bf16, 16-byte stores (…sm89.cuh:572-703)
-    OutT* orow = reinterpret_cast<OutT*>(p.out) + (varlen ? 0 : int64_t(b) * p.o_stride_b) + int64_t(h) * p.o_stride_h +
-                 int64_t(q_off + q_row) * p.o_stride_s;
-    const bool row_ok = q_row < q_len;
-    const float* vs = p.v_scale ? p.v_scale + (int64_t(varlen ? 0 : b) * p.Hkv + hk) * D : nullptr;
-    const float* vm = p.v_mean ? p.v_mean + (int64_t(varlen ? 0 : b) * p.Hkv + hk) * D : nullptr;
-    if (n_kv > 0) {
-      mbar_wait_wd(s_full + ((n_kv + 1) & 1), s_parity(n_kv + 1));   // step(n_kv-1) retired: O is final
-      tc_fence_after();
-      const float inv = (kMask && !(d > 0.f)) ? 0.f : rcp_approx(d);   // a fully masked row yields zeros, not NaN
+    // ---- P -> A fragments, O += P V
+    const uint64_t dV = dV0 + uint64_t(st) * (V_TILE >> 4);
+    if constexpr (kPV16) {
+      uint32_t a[4][4];   // k16 step kk: keys 16kk..16kk+15 = accumulator blocks 2kk, 2kk+1 (same layout: no exchange)
 #pragma unroll
-      for (int ch = 0; ch < D / 32; ++ch) {
-        uint32_t r[32];
-        tmem_ld32(tO + lane_off + ch * 32, r);
-        tc_wait_ld();
-        if (dump) {
+      for (int kk = 0; kk < 4; ++kk) {
+        const int i0 = 8 * kk, i1 = 8 * kk + 4;
+        a[kk][0] = pack_f16x2(e[i0], e[i0 + 1]);   // p.to(tl.float16), attn_qk_int8_per_block.py:62
+        a[kk][1] = pack_f16x2(e[i0 + 2], e[i0 + 3]);
+        a[kk][2] = pack_f16x2(e[i1], e[i1 + 1]);
+        a[kk][3] = pack_f16x2(e[i1 + 2], e[i1 + 3]);
+      }
+      rescale_o();
+      wgmma_fence();
 #pragma unroll
-          for (int i = 0; i < 32; ++i) p.dbg[128 * BN + 128 * 16 + row * D + ch * 32 + i] = int(r[i]);
-        }
-        uint32_t o16[16];
+      for (int kk = 0; kk < 4; ++kk) wgmma_pv_f16(o, a[kk], dV + 2 * kk, 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(o);
+    } else {
+      uint32_t a[2][4];   // k32 chunk c: keys 32c..32c+31 = accumulator blocks 4c..4c+3
 #pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          float a = __uint_as_float(r[i]) * inv, c = __uint_as_float(r[i + 1]) * inv;
-          if (vs) {
-            a *= vs[ch * 32 + i];
-            c *= vs[ch * 32 + i + 1];
-          }
-          if (vm) {
-            a += vm[ch * 32 + i];
-            c += vm[ch * 32 + i + 1];
-          }
-          o16[i / 2] = pack2<OutT>(a, c);
-        }
-        if (row_ok) {
-          uint4* dst = reinterpret_cast<uint4*>(orow + ch * 32);
+      for (int c = 0; c < 2; ++c) {
 #pragma unroll
-          for (int v4 = 0; v4 < 4; ++v4) dst[v4] = make_uint4(o16[4 * v4], o16[4 * v4 + 1], o16[4 * v4 + 2], o16[4 * v4 + 3]);
+        for (int i = 0; i < 2; ++i) {
+          const int b0 = 16 * c + 2 * i;   // register of block 4c, this row
+          const uint32_t x = pack_e4m3x4(e[b0], e[b0 + 1], e[b0 + 4], e[b0 + 5]);         // blocks 4c, 4c+1
+          const uint32_t y = pack_e4m3x4(e[b0 + 8], e[b0 + 9], e[b0 + 12], e[b0 + 13]);   // blocks 4c+2, 4c+3
+          a[c][i] = __byte_perm(__shfl_sync(0xffffffffu, x, src0), __shfl_sync(0xffffffffu, x, src0 + 1), psel);
+          a[c][2 + i] = __byte_perm(__shfl_sync(0xffffffffu, y, src0), __shfl_sync(0xffffffffu, y, src0 + 1), psel);
         }
       }
-      if (dump) {
-        p.dbg[128 * BN + 128 * 16 + 128 * D + row] = __float_as_int(d);
-        p.dbg[128 * BN + 128 * 16 + 128 * D + 128 + row] = __float_as_int(m);
-      }
-    } else if (row_ok) {
-      uint4* dst = reinterpret_cast<uint4*>(orow);
+      float ot[NO];   // this tile's P V, from zero
+      wgmma_fence();
 #pragma unroll
-      for (int v4 = 0; v4 < D / 8; ++v4) dst[v4] = make_uint4(0, 0, 0, 0);
+      for (int c = 0; c < 2; ++c) wgmma_pv_f8(ot, a[c], dV + 2 * c, c > 0);
+      wgmma_commit();
+      rescale_o();    // overlaps the MMA
+      wgmma_wait<0>();
+      fence_regs(ot);
+#pragma unroll
+      for (int i = 0; i < NO; ++i) o[i] += ot[i];
     }
-    if (p.lse != nullptr && row_ok) {
-      // log2 units like the reference kernel (…sm89.cuh:691-703); the offset cancels: log2(sum 2^x)
-      const int64_t li = varlen ? (int64_t(h) * p.Sq + q_off + q_row) : ((int64_t(b) * p.Hq + h) * p.Sq + q_row);
-      p.lse[li] = n_kv > 0 ? lg2_approx(d) + m : -INFINITY;
-    }
+    if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty + st);   // K(j) and V(j) consumed by this warpgroup
   }
 
-  // ---------------- teardown
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) tmem_dealloc<kTmemCols>(tmem_base);
+  // ---- epilogue: O / d * v_scale (+ v_mean) -> fp16/bf16 (…sm89.cuh:572-703)
+  const float* vs = p.v_scale ? p.v_scale + (int64_t(varlen ? 0 : b) * p.Hkv + hk) * D : nullptr;
+  const float* vm = p.v_mean ? p.v_mean + (int64_t(varlen ? 0 : b) * p.Hkv + hk) * D : nullptr;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float dt = d[i];
+    dt += __shfl_xor_sync(0xffffffffu, dt, 1);
+    dt += __shfl_xor_sync(0xffffffffu, dt, 2);
+    const bool row_ok = q_row[i] < q_len;
+    OutT* orow = reinterpret_cast<OutT*>(p.out) + (varlen ? 0 : int64_t(b) * p.o_stride_b) + int64_t(h) * p.o_stride_h +
+                 int64_t(q_off + q_row[i]) * p.o_stride_s;
+    const float inv = (n_kv == 0 || (kMask && !(dt > 0.f))) ? 0.f : rcp_approx(dt);   // a fully masked row yields zeros, not NaN
+    if (row_ok) {
+#pragma unroll
+      for (int nb = 0; nb < D / 8; ++nb) {
+        const int col = 8 * nb + 2 * t;
+        float x0 = o[4 * nb + 2 * i] * inv, x1 = o[4 * nb + 2 * i + 1] * inv;
+        if (vs) {
+          x0 *= vs[col];
+          x1 *= vs[col + 1];
+        }
+        if (vm) {
+          x0 += vm[col];
+          x1 += vm[col + 1];
+        }
+        if (n_kv == 0) x0 = x1 = 0.f;
+        *reinterpret_cast<uint32_t*>(orow + col) = pack2<OutT>(x0, x1);
+      }
+      if (p.lse != nullptr && t == 0) {
+        // log2 units like the reference kernel (…sm89.cuh:691-703); the offset cancels: log2(sum 2^x)
+        const int64_t li = varlen ? (int64_t(h) * p.Sq + q_off + q_row[i]) : ((int64_t(b) * p.Hq + h) * p.Sq + q_row[i]);
+        p.lse[li] = n_kv > 0 ? lg2_approx(dt) + m[i] : -INFINITY;
+      }
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------ host
@@ -549,27 +458,8 @@ static int make_map_u8(CUtensorMap* map, const void* base, uint64_t d0, uint64_t
   return SAB_OK;
 }
 
-// attn_hd64.cu: head_dim 64, four CTAs per SM (S single-buffered); kLazy selects the lazy / exact running max.
-// SAB_HD64_KERNEL=2cta falls back to the generic kernel of this file.
-template <bool kKT, typename OutT, bool kLazy>
-int launch_attn_hd64(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnParams& p, dim3 grid,
-                     cudaStream_t stream);
-static bool use_hd64_kernel() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SAB_HD64_KERNEL");
-    v = (e != nullptr && e[0] == '2') ? 0 : 1;
-  }
-  return v == 1;
-}
-
-// attn_alt.cu: the product kernel of the INT8+FP8 path at head_dim 128 — two softmax warpgroups on alternate key tiles, lazy max.
-template <int D, bool kKT, typename OutT>
-int launch_attn_alt(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnParams& p, dim3 grid,
-                    cudaStream_t stream);
-
-// SAB_ATTN_KERNEL=exact selects the reference's exact running max everywhere (the kernel of this file at head_dim 128, the exact
-// instantiation of attn_hd64.cu): P / m / d are then bit-identical to the reference kernel's.  Default: the lazy-max product kernels.
+// SAB_ATTN_KERNEL=exact selects the reference's exact running max on the INT8+FP8 path: P / m / d are then bit-identical to the
+// reference kernel's.  Default: the lazy max (4 binades).
 static bool exact_max_mode() {
   static int v = -1;
   if (v < 0) {
@@ -578,41 +468,14 @@ static bool exact_max_mode() {
   }
   return v == 1;
 }
+constexpr float kLazyTau = 4.0f;
 
-// attn_q4.cu: one CTA per SM, four softmax warpgroups, separate P buffers.
-template <bool kKT, typename OutT>
-int launch_attn_q4(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnParams& p, dim3 grid,
-                   cudaStream_t stream);
-// Which head_dim-128 kernel: attn_alt.cu unless SAB_ATTN_KERNEL=q4.  A length / wave-quantisation heuristic that gave long key
-// sequences to attn_q4.cu (kernel-only +2-3 % from 256 key tiles on, and waves half as long) was measured on the 2-GPU sequence-
-// parallel bench and LOST 5 % (profiles/r02_bench_n2_q4_dispatch.json: 2490 against 2625 TFLOP/s), so the choice stays explicit.
-static bool prefer_q4(const AttnParams&, dim3) {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("SAB_ATTN_KERNEL");
-    v = (e != nullptr && e[0] == 'q') ? 1 : 0;
-  }
-  return v == 1;
-}
-
-template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false, bool kSeg = false>
-static int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const AttnParams& p,
+template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false>
+static int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, AttnParams p,
                        dim3 grid, cudaStream_t stream) {
-  if constexpr (D == 128 && !kPV16) {   // also the fused-gather form: the producers poll p.seg_flags at run time
-    if (!exact_max_mode() && p.dbg == nullptr && prefer_q4(p, grid)) return launch_attn_q4<kKT, OutT>(tq, tk, tv, p, grid, stream);
-    if (!exact_max_mode() && p.dbg == nullptr) return launch_attn_alt<D, kKT, OutT>(tq, tk, tv, p, grid, stream);
-  }
-  if constexpr (D == 64 && !kPV16) {
-    if (use_hd64_kernel() && p.dbg == nullptr) {
-      if (exact_max_mode()) return launch_attn_hd64<kKT, OutT, false>(tq, tk, tv, p, grid, stream);
-      return launch_attn_hd64<kKT, OutT, true>(tq, tk, tv, p, grid, stream);
-    }
-  }
-  constexpr int NS = kPV16 ? ((D == 128) ? 3 : 6) : ((D == 128) ? 5 : 10);
-  // Q tile + NS x (K + V^T 64-key tile) + alpha hand-off + barriers (97.5 KB at hd128): two CTAs per SM (TMEM: 2 x 256 columns)
-  size_t smem = size_t(BM) * D + size_t(NS) * (BN * D + BN * D * (kPV16 ? 2 : 1)) + 2 * BM * sizeof(float) + 512;
-  if (smem < 80 * 1024) smem = 80 * 1024;
-  auto kern = sage_attn_fwd_kernel<D, kKT, OutT, kPV16, kMask, kSeg>;
+  p.lazy_tau = (kPV16 || exact_max_mode()) ? 0.0f : kLazyTau;
+  constexpr size_t smem = attn_smem_bytes<D, kPV16>();
+  auto kern = sage_attn_fwd_kernel<D, kKT, OutT, kPV16, kMask>;
   static bool configured[64] = {};
   if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
   kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p);
@@ -663,6 +526,7 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
                 "sequence-parallel form needs dense tensors, kv_seg_len %% 128 == 0, Skv %% kv_seg_len == 0, v_s_pad == kv_seg_len");
   if (varlen)
     SAB_REQUIRE(cu_seqlens_k && cu_pad_v && cu_q_scale && cu_k_scale && max_seqlen_q > 0, SAB_ERR_INVALID, "varlen needs cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale and max_seqlen_q");
+  SAB_REQUIRE(debug_dump == nullptr, SAB_ERR_UNSUPPORTED, "debug_dump is not supported by the sm_90a kernel (pass NULL)");
   int st = sab_check_device();
   if (st != SAB_OK) return st;
 
@@ -703,17 +567,8 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
   p.ks_stride_bh = int64_t((Skv + 63) / 64) * p.k_mult;
   p.qs_stride_idx = varlen ? Hq : 1;
   p.ks_stride_idx = varlen ? Hkv : 1;
-  p.ks_vec4 = (k_gran == SAB_GRAN_PER_THREAD && !varlen && aligned16(k_scale)) ? 1 : 0;
   p.cu_q = cu_seqlens_q; p.cu_k = cu_seqlens_k; p.cu_v = cu_pad_v; p.cu_qs = cu_q_scale; p.cu_ks = cu_k_scale;
   p.causal_q_offset = causal_q_offset; p.kv_seg_len = kv_seg_len;
-  p.dbg = debug_dump;
-  if (!varlen && !pv16 && Sq > 0) {   // consumed by attn_alt.cu (D = 128: two 128-byte halves) and attn_hd64.cu
-    // rows past Sq are clipped by the map, so the epilogue can store whole 128-row tiles
-    if ((st = make_map_u8(&p.o_map, out, uint64_t(D) * 2, Sq, Hq, B, uint64_t(o_stride_s) * 2, uint64_t(o_stride_h) * 2,
-                          uint64_t(o_stride_b) * 2, 128, BM, 128)))
-      return st;
-    p.o_tma = 1;
-  }
 
   dim3 grid(p.n_q_tiles, Hq, B);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -735,20 +590,11 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
     return launch_attn<64, false, __half, true, true>(tq, tk, tv, p, grid, s);
   }
   if (tl_seg != nullptr) {
-    SAB_REQUIRE(!pv16 && kv_seg_len > 0 && !is_causal && debug_dump == nullptr, SAB_ERR_UNSUPPORTED,
+    SAB_REQUIRE(!pv16 && kv_seg_len > 0 && !is_causal, SAB_ERR_UNSUPPORTED,
                 "segment flags need the sequence-parallel INT8/FP8 form (kv_seg_len > 0), non-causal");
     SAB_REQUIRE(tl_seg->flags != nullptr && tl_seg->heads_per_flag > 0 && Hkv % tl_seg->heads_per_flag == 0, SAB_ERR_INVALID,
                 "segment flags: null pointer or heads_per_flag (%d) does not divide num_kv_heads (%d)", tl_seg->heads_per_flag, Hkv);
-    p.seg_flags = tl_seg->flags; p.seg_epoch = tl_seg->epoch; p.seg_heads = tl_seg->heads_per_flag;
-#define SAB_LAUNCH_SEG(DD, KT, T) return launch_attn<DD, KT, T, false, false, true>(tq, tk, tv, p, grid, s)
-    if (D == 128) {
-      if (kt) { if (bf) SAB_LAUNCH_SEG(128, true, __nv_bfloat16); else SAB_LAUNCH_SEG(128, true, __half); }
-      else    { if (bf) SAB_LAUNCH_SEG(128, false, __nv_bfloat16); else SAB_LAUNCH_SEG(128, false, __half); }
-    } else {
-      if (kt) { if (bf) SAB_LAUNCH_SEG(64, true, __nv_bfloat16); else SAB_LAUNCH_SEG(64, true, __half); }
-      else    { if (bf) SAB_LAUNCH_SEG(64, false, __nv_bfloat16); else SAB_LAUNCH_SEG(64, false, __half); }
-    }
-#undef SAB_LAUNCH_SEG
+    p.seg_flags = tl_seg->flags; p.seg_epoch = tl_seg->epoch; p.seg_heads = tl_seg->heads_per_flag;   // polled by the producer
   }
 #define SAB_LAUNCH(DD, KT, T)                                                      \
   do {                                                                             \

@@ -1,5 +1,4 @@
-// Shared declarations of the attention kernels (attn_alt.cu: head_dim 128 product kernel; attn_hd64.cu: head_dim 64;
-// attn.cu: exact-max / fp16-PV / masked / sequence-parallel variants and the host dispatch).
+// Shared declarations of the attention kernel (attn.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -8,28 +7,14 @@
 #include "common.cuh"
 #include "ptx.cuh"
 
-#ifdef SAB_TIMELINE
-#define SAB_TL(slot) do { if (tl_on && j >= 16 && j < 48) tl[(j - 16) * 16 + (slot)] = clock64(); } while (0)
-#else
-#define SAB_TL(slot) do {} while (0)
-#endif
-
 namespace sab {
 
 constexpr int BM = 128;  // Q rows per CTA
 constexpr int BN = 64;   // keys per softmax / MMA tile (reference CTA_K)
 constexpr int LK = 128;  // keys per TMA stage (two tiles)
-constexpr uint32_t kTmemCols = 256;
 constexpr float kFp8Offset = 8.807f;      // attn_utils.cuh:30
 constexpr float kMaskValue = -5000000.0f; // attn_utils.cuh:310
 constexpr int kIntSentinel = -(1 << 30);
-#ifdef SAB_NO_TMA_STORE   // A/B switch: direct per-row global stores in the epilogue
-constexpr bool kTmaStoreEpilogue = false;
-#else
-constexpr bool kTmaStoreEpilogue = true;
-#endif
-constexpr int kAlphaCol = 40;  // column of an S buffer (beyond the 16 / 32 P columns) that carries alpha(j) to the correction warps
-
 struct AttnParams {
   const float* q_scale;
   const float* k_scale;
@@ -49,7 +34,6 @@ struct AttnParams {
   int64_t ks_stride_bh;
   int qs_stride_idx;     // dense 1, varlen Hq
   int ks_stride_idx;     // dense 1, varlen Hkv
-  int ks_vec4;           // per-thread K scales, dense, 16-byte aligned: the four scales of a key tile load as one float4
   const int32_t* cu_q;   // varlen (nullable)
   const int32_t* cu_k;
   const int32_t* cu_v;
@@ -57,20 +41,16 @@ struct AttnParams {
   const int32_t* cu_ks;
   int causal_q_offset;   // global index of query row 0 (sequence-parallel causal)
   int kv_seg_len;        // > 0: K/V are rank-major all-gathered segments of this many keys
-  int32_t* dbg;          // nullable debug dump (CTA 0 only)
+  float lazy_tau;        // INT8+FP8 path: the running max moves only by more than this many binades (0: exact max)
   // attention mask of the Triton-path shell (attn_qk_int8_per_block.py:33-52): [B,Hq,Sq,Skv] with arbitrary (also 0) strides
   const void* mask;      // nullable
   int mask_kind;         // 1: bool (uint8, false = masked out), 2: additive bias in the output dtype (fp16 / bf16)
   int64_t mask_sb, mask_sh, mask_sm, mask_sn;   // element strides
-  // sequence-parallel gather fused into the launch (kSeg instantiations): K/V segment `seg` of KV-head group g is complete in
+  // sequence-parallel gather fused into the launch (seg_flags != nullptr): K/V segment `seg` of KV-head group g is complete in
   // this GPU's memory once seg_flags[g * n_segments + seg] == seg_epoch (written in stream order behind the peer copies)
   const uint32_t* seg_flags;   // nullable
   uint32_t seg_epoch;
   int seg_heads;               // KV heads per flag group
-  // dense outputs: byte-typed 4-D map of O (box 128 B x 128 rows, 128-byte swizzle) for the TMA-store epilogue of attn_alt.cu
-  int o_tma;                   // 1: o_map is valid
-  int n_items;                 // attn_q4.cu: length of the work list (Q tiles x heads x batch)
-  CUtensorMap o_map;
 };
 
 __device__ __forceinline__ void mbar_wait_wd(uint64_t* bar, uint32_t parity) {

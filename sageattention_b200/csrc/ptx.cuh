@@ -1,5 +1,5 @@
-// Inline-PTX wrappers for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / ld / st /
-// commit / fences) and the UMMA shared-memory + instruction descriptors.  Hand-written: no CUTLASS.
+// Inline-PTX wrappers for sm_90a (H100): mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA with register
+// accumulators) and its shared-memory matrix descriptor.  Hand-written: no CUTLASS.
 #pragma once
 #include <cstdint>
 #include <cuda.h>
@@ -72,21 +72,11 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, uint32
       ::"r"(smem_u32(bar)), "r"(parity), "r"(hint_ns)
       : "memory");
 }
-// launch_bounds(384, 2) -> 80 registers per thread at launch = a 30720-register pool per CTA, re-split 112 / 80 / 48
-__device__ __forceinline__ void setmaxnreg_inc_112() { asm volatile("setmaxnreg.inc.sync.aligned.u32 112;"); }
-__device__ __forceinline__ void setmaxnreg_dec_48() { asm volatile("setmaxnreg.dec.sync.aligned.u32 48;"); }
-
-// One elected lane of a fully converged warp (the surrounding code stays warp-uniform, so the compiler keeps UMMA
-// descriptors / addresses in uniform registers instead of paying R2UR round trips before every tcgen05 instruction).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.b32 %0, 1, 0, P;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
+// Warpgroup-wide register re-allocation (all four warps of the warpgroup execute it).
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // ------------------------------------------------------------------ TMA
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -118,177 +108,80 @@ __device__ __forceinline__ void tma_store_wait_read() {
   asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05: TMEM management
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_holder) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// tcgen05.commit: arrive (count 1) on an mbarrier once all previously issued tcgen05.mma of this thread retire.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// ------------------------------------------------------------------ tcgen05: TMEM <-> registers
-// 32x32b: thread t of warp w (w%4 selects the 32-lane quadrant) accesses lane 32*(w%4)+t, N consecutive columns.
-#define SAB_R4(a, i) "=r"(a[i]), "=r"(a[i + 1]), "=r"(a[i + 2]), "=r"(a[i + 3])
-#define SAB_W4(a, i) "r"(a[i]), "r"(a[i + 1]), "r"(a[i + 2]), "r"(a[i + 3])
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : SAB_R4(r, 0), SAB_R4(r, 4), SAB_R4(r, 8), SAB_R4(r, 12), SAB_R4(r, 16), SAB_R4(r, 20), SAB_R4(r, 24),
-        SAB_R4(r, 28)
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : SAB_R4(r, 0), SAB_R4(r, 4), SAB_R4(r, 8), SAB_R4(r, 12)
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : SAB_R4(r, 0), SAB_R4(r, 4)
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_chunk(uint32_t taddr, uint32_t (&r)[8]) { tmem_ld8(taddr, r); }
-__device__ __forceinline__ void tmem_ld_chunk(uint32_t taddr, uint32_t (&r)[16]) { tmem_ld16(taddr, r); }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%32], "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31};"
-      ::SAB_W4(r, 0), SAB_W4(r, 4), SAB_W4(r, 8), SAB_W4(r, 12), SAB_W4(r, 16), SAB_W4(r, 20), SAB_W4(r, 24),
-      SAB_W4(r, 28), "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%16], "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15};"
-      ::SAB_W4(r, 0), SAB_W4(r, 4), SAB_W4(r, 8), SAB_W4(r, 12), "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&r)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%8], {%0, %1, %2, %3, %4, %5, %6, %7};" ::SAB_W4(r, 0),
-               SAB_W4(r, 4), "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%4], {%0, %1, %2, %3};" ::"r"(a), "r"(b), "r"(c), "r"(d), "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_st1(uint32_t taddr, uint32_t v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%1], {%0};" ::"r"(v), "r"(taddr) : "memory");
-}
-__device__ __forceinline__ uint32_t tmem_ld1(uint32_t taddr) {
-  uint32_t v;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(v) : "r"(taddr) : "memory");
-  return v;
-}
-#undef SAB_R4
-#undef SAB_W4
-
-// ------------------------------------------------------------------ UMMA descriptors
-// Shared-memory matrix descriptor, K-major operand with hardware swizzle (tile base 1024-B aligned):
-//   [0,14) start address >>4 | [16,30) leading-dim byte offset >>4 (unused for swizzled K-major)
-//   [32,46) stride-dim byte offset >>4 (= 8 rows * swizzle span) | [46,48) version = 1 (sm_100)
-//   [61,64) layout: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B, 6 = SWIZZLE_32B
+// ------------------------------------------------------------------ wgmma
+// Shared-memory matrix descriptor of a K-major operand with hardware swizzle (tile base 1024-B aligned; stepping along K
+// inside the swizzle span adds bytes>>4 to the start address):
+//   [0,14) start address >>4 | [16,30) leading-dim byte offset >>4 (unused for swizzled K-major, 1)
+//   [32,46) stride-dim byte offset >>4 (= 8 rows * swizzle span) | [62,64) layout: 1 = SWIZZLE_128B, 2 = 64B, 3 = 32B
 template <int kSwizzleBytes>
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
+__device__ __forceinline__ uint64_t make_wgmma_desc(uint32_t smem_addr) {
   static_assert(kSwizzleBytes == 128 || kSwizzleBytes == 64 || kSwizzleBytes == 32, "swizzle");
-  constexpr uint64_t layout = kSwizzleBytes == 128 ? 2 : (kSwizzleBytes == 64 ? 4 : 6);
+  constexpr uint64_t layout = kSwizzleBytes == 128 ? 1 : (kSwizzleBytes == 64 ? 2 : 3);
   constexpr uint64_t sbo = (8 * kSwizzleBytes) >> 4;
-  return static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | (sbo << 32) | (1ull << 46) |
-         (layout << 61);
+  return static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4) | (1ull << 16) | (sbo << 32) | (layout << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accesses of accumulator registers across the asynchronous MMA.
+template <int N>
+__device__ __forceinline__ void fence_regs(uint32_t (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
+}
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
 
-// Instruction descriptor (upper 32 bits of the idesc operand):
-//   [4,6) D format (0 f16, 1 f32, 2 s32) | [7,10) A format | [10,13) B format | [15] A major | [16] B major
-//   [17,23) N>>3 | [24,29) M>>4.   kind::i8: format 1 = signed int8.  kind::f8f6f4: format 0 = e4m3.
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t d_fmt, uint32_t a_fmt, uint32_t b_fmt, uint32_t M,
-                                                  uint32_t N) {
-  return (d_fmt << 4) | (a_fmt << 7) | (b_fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// S[64 x 64] (+)= A[smem, 64 x 32 int8] * B[smem, 64 keys x 32 int8]^T, int32 accumulators (32 per thread).
+__device__ __forceinline__ void wgmma_qk_i8(uint32_t (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p;\n\t}"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]), "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]), "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]), "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
 
-// D[tmem] (+)= A[smem] * B[smem], INT8 x INT8 -> INT32, K = 32 per instruction.
-__device__ __forceinline__ void umma_i8_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                           uint32_t accumulate) {
+// O[64 x 64] (+)= P[registers, 64 x 32 e4m3] * V^T[smem, 64 x 32 e4m3]^T, fp32 accumulators.
+__device__ __forceinline__ void wgmma_pv_f8(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
 }
-// D[tmem] (+)= A[tmem] * B[smem], E4M3 x E4M3 -> F32 (or F16), K = 32 per instruction.
-__device__ __forceinline__ void umma_f8_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                           uint32_t accumulate) {
+// O[64 x 64] (+)= P[registers, 64 x 16 f16] * V^T[smem, 64 x 16 f16]^T, fp32 accumulators.
+__device__ __forceinline__ void wgmma_pv_f16(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem], F16 x F16 -> F32, K = 16 per instruction.
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], E4M3 x E4M3.
-__device__ __forceinline__ void umma_f8_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
 }
 
-// ------------------------------------------------------------------ packed fp32x2 arithmetic (sm_100: FFMA2 / FADD2 / FMUL2)
-// Two IEEE round-to-nearest fp32 operations per issued instruction; results are bit-identical to the scalar ops.
-__device__ __forceinline__ uint64_t pack_f2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
+// O[64 x 128] (+)= P[registers, 64 x 32 e4m3] * V^T[smem, 128 x 32 e4m3]^T, fp32 accumulators.
+__device__ __forceinline__ void wgmma_pv_f8(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
 }
-__device__ __forceinline__ void unpack_f2(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t ffma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t fadd2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ uint64_t fmul2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+// O[64 x 128] (+)= P[registers, 64 x 16 f16] * V^T[smem, 128 x 16 f16]^T, fp32 accumulators.
+__device__ __forceinline__ void wgmma_pv_f16(float (&d)[64], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
 }
 
 // ------------------------------------------------------------------ math
@@ -311,23 +204,24 @@ __device__ __forceinline__ float rcp_approx(float x) {
 // default because P stops being bit-identical to the reference kernel's).  y is clamped to >= -126, split into
 // floor(y) + f with the round-down magic add (FADD.RM with 1.5*2^23 leaves floor(y) in the low mantissa bits, exactly),
 // 2^f on [0,1) is a degree-3 minimax polynomial with p(0) = 1 (max relative error 8.6e-5, coefficients fitted in
-// tests/test_poly_exp_numerics.py), and floor(y) is added to the exponent field with one shift-add.  6 packed FMA-pipe
-// instructions per pair + 2 FMNMX + 2 shift-adds, against 2 MUFU.EX2.
+// tests/test_poly_exp_numerics.py), and floor(y) is added to the exponent field with one shift-add.
 __device__ __forceinline__ void ex2_poly2(float y0, float y1, float& e0, float& e1) {
   constexpr float kMagic = 12582912.f;  // 1.5 * 2^23 = 0x4B400000: low 9 bits zero, so (bits << 23) == floor(y) << 23
-  const uint64_t yy = pack_f2(fmaxf(y0, -126.f), fmaxf(y1, -126.f));
-  uint64_t r;
-  asm("add.rm.f32x2 %0, %1, %2;" : "=l"(r) : "l"(yy), "l"(pack_f2(kMagic, kMagic)));
-  const uint64_t fl = fadd2(r, pack_f2(-kMagic, -kMagic));              // floor(y) as a float, exact
-  const uint64_t fr = ffma2(fl, pack_f2(-1.f, -1.f), yy);               // y - floor(y) in [0, 1]
-  uint64_t p = ffma2(fr, pack_f2(0.07706724107265472f, 0.07706724107265472f), pack_f2(0.22764497995376587f, 0.22764497995376587f));
-  p = ffma2(p, fr, pack_f2(0.6951166391372681f, 0.6951166391372681f));
-  p = ffma2(p, fr, pack_f2(1.f, 1.f));
-  float p0, p1, r0, r1;
-  unpack_f2(p, p0, p1);
-  unpack_f2(r, r0, r1);
-  e0 = __int_as_float(__float_as_int(p0) + (__float_as_int(r0) << 23));
-  e1 = __int_as_float(__float_as_int(p1) + (__float_as_int(r1) << 23));
+  const float y[2] = {fmaxf(y0, -126.f), fmaxf(y1, -126.f)};
+  float e[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float r;
+    asm("add.rm.f32 %0, %1, %2;" : "=f"(r) : "f"(y[i]), "f"(kMagic));
+    const float fl = __fadd_rn(r, -kMagic);               // floor(y) as a float, exact
+    const float fr = __fmaf_rn(fl, -1.f, y[i]);           // y - floor(y) in [0, 1]
+    float q = __fmaf_rn(fr, 0.07706724107265472f, 0.22764497995376587f);
+    q = __fmaf_rn(q, fr, 0.6951166391372681f);
+    q = __fmaf_rn(q, fr, 1.f);
+    e[i] = __int_as_float(__float_as_int(q) + (__float_as_int(r) << 23));
+  }
+  e0 = e[0];
+  e1 = e[1];
 }
 // Pack 2 fp32 -> f16x2 (round-nearest-even); low half = a.
 __device__ __forceinline__ uint32_t pack_f16x2(float a, float b) {

@@ -1,6 +1,6 @@
-// Quantisation front-end for sm_100a: K-smoothing mean, INT8 quantisation of Q/K (per-block / per-warp /
+// Quantisation front-end for sm_90a (H100): K-smoothing mean, INT8 quantisation of Q/K (per-block / per-warp /
 // per-thread granularity, CUDA or Triton rounding semantics), per-channel FP8 quantisation of V into the
-// token-contiguous V^T layout the tcgen05 PV MMA consumes.  All kernels are HBM-streaming: 128-bit loads,
+// token-contiguous V^T layout the wgmma PV product consumes.  All kernels are HBM-streaming: 128-bit loads,
 // one read of the input (+ one statistics pre-pass where the algorithm needs a full-sequence reduction),
 // 64/128-bit stores.  Semantics follow csrc/fused/fused.cu and sageattention/triton/quant_per_*.py of the
 // reference (see include/sageattn_b200.h for the per-entry citations).
@@ -40,20 +40,26 @@ __device__ __forceinline__ uint64_t pack2f(float lo, float hi) {
 __device__ __forceinline__ void unpack2f(uint64_t v, float& lo, float& hi) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
 }
+// Pairs of IEEE round-to-nearest fp32 operations on packed operands.  The _rn intrinsics are never contracted into an
+// FMA by the compiler, so each operation rounds on its own exactly as the reference's scalar code does.
 __device__ __forceinline__ uint64_t fmul2q(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2f(a, a0, a1);
+  unpack2f(b, b0, b1);
+  return pack2f(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t fadd2q(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
+  float a0, a1, b0, b1;
+  unpack2f(a, a0, a1);
+  unpack2f(b, b0, b1);
+  return pack2f(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
 }
 __device__ __forceinline__ uint64_t ffma2q(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
+  float a0, a1, b0, b1, c0, c1;
+  unpack2f(a, a0, a1);
+  unpack2f(b, b0, b1);
+  unpack2f(c, c0, c1);
+  return pack2f(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
 }
 __device__ __forceinline__ int8_t cvt_rni_sat_s8(float x) {  // csrc/numeric_conversion.cuh:144-148
   int r;
@@ -342,10 +348,8 @@ __device__ __forceinline__ void quant_int8_tile(const QuantParams& p, const int 
       else centred(wv[w], w, lo, hi);
       uint64_t x2 = pack2f(lo, hi);
       if constexpr (kSms) x2 = fmul2q(x2, sms2);
-      // y must be rounded on its own (the reference rounds x*mult, then converts): ptxas contracts `mul.rn.f32x2` +
-      // `add.rn.f32x2` into one FFMA2 (even with --fmad=false) when y has no other consumer, and the single rounding
-      // flips x.5 ties (63 vs 64).  Both semantics therefore consume y a second time (Triton: y - n; CUDA: the
-      // saturation guard below), which keeps the two instructions apart — checked in SASS (FADD2 count) at build time.
+      // y must be rounded on its own (the reference rounds x*mult, then converts): a multiply-add contracted into one FMA
+      // would flip x.5 ties (63 vs 64).  fmul2q / fadd2q use the non-contractible _rn intrinsics.
       const uint64_t y2 = fmul2q(x2, fac2);
       const uint64_t t2 = fadd2q(y2, magic2);
       if constexpr (kTriton) {
@@ -411,7 +415,7 @@ __global__ void __launch_bounds__(256, 3) quant_int8_kernel(const QuantParams p)
 }
 
 // =====================================================================================================
-// Single-pass K path (SURVEY section 8 f-1): K smoothing mean + INT8 quantisation in ONE launch.  A thread-block cluster of
+// Single-pass K path: K smoothing mean + INT8 quantisation in ONE launch.  A thread-block cluster of
 // kKCluster CTAs owns one (b,h) slice; CTA r takes the 128-row tiles r, r+C, ...  Phase 1: per-channel fp32 sums of its tiles
 // -> shared memory; cluster barrier; every CTA folds the C partial sums in rank order through distributed shared memory
 // (identical result in every CTA), rounds the mean to T like `k.mean` (core.py:773) and rank 0 writes it out.  Phase 2: the
@@ -633,7 +637,7 @@ __global__ void __launch_bounds__(256) v_scale_quant_kernel(const VQuantParams p
 }
 
 // V -> fp16, transposed to [.., D, S_pad] (token-contiguous), zero padded: the B operand of the kind::f16 PV MMA
-// (`v.to(torch.float16)`, sageattention/core.py:297-298, + the K-major layout tcgen05 wants).
+// (`v.to(torch.float16)`, sageattention/core.py:297-298, + the K-major layout the wgmma B operand wants).
 template <typename T, int D>
 __global__ void __launch_bounds__(256) v_transpose_f16_kernel(const VQuantParams p) {
   constexpr int TPR = D / 8;

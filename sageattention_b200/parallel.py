@@ -1,4 +1,4 @@
-"""Sequence-parallel SageAttention over NCCL (SURVEY §8e; BASELINE.json configs[4]).
+"""Sequence-parallel SageAttention over NCCL (BASELINE.json configs[4]).
 
 One process per GPU.  Rank r holds the r-th contiguous slice of the sequence of Q, K and V
 (``[B,H,S/P,D]`` / ``[B,S/P,H,D]``); the output stays sharded like Q.  The reference library has no
@@ -124,7 +124,7 @@ def sageattn_sp(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, tensor_layout
                 gather_chunks: int = 4, **kwargs: Any) -> torch.Tensor:
     """Sequence-parallel `sageattn_qk_int8_pv_fp8_cuda`: local shards in, local output shard out.
 
-    fused_gather=True (non-causal; validated on 2 x B200, bit-identical to the collective path and ~2 % faster at N=2): the K/V exchange
+    fused_gather=True (non-causal; bit-identical to the collective path): the K/V exchange
     is not an NCCL collective before the attention launch but peer copies that run WHILE the one attention launch computes:
     every rank quantises its shard into a symmetric (peer-mapped) buffer, a side stream pulls the peers' shards KV-head chunk
     by chunk with the copy engines (no SMs) and raises one flag per (chunk, segment) in stream order, and the kernel's TMA
@@ -226,8 +226,7 @@ def sageattn_sp(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, tensor_layout
     #      pipelined over KV-head chunks: NCCL gathers chunk c+1 on a side stream while the attention kernel runs on
     #      chunk c (the gather of an 8-bit K/V chunk is ~5x shorter than its attention at S=32K, so all but the first
     #      gather is hidden).  Each chunk's gather output is consumed in place (rank-major segments, kv_seg_len).
-    #      Measured on 2 x B200 (S=32768, H=32): 4 chunks 2.18 PFLOP/s vs 1 chunk 2.31 — the per-launch tail (1024 CTAs =
-    #      3.46 waves of 296) costs more than the 8-bit gather it hides, so the default is overlap_chunks=1.
+    #      Each chunk is its own launch with its own tail wave, so the default is overlap_chunks=1 (one launch).
     o = torch.empty((B, Hq, Sl, D), dtype=dtype, device=dev)
     g = Hq // Hk
     n_chunks = overlap_chunks if (overlap_chunks and B == 1 and Hk % overlap_chunks == 0 and world > 1) else 1
@@ -257,7 +256,7 @@ def sageattn_sp(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, tensor_layout
     return o if lay == 1 else o.transpose(1, 2)
 
 
-# ------------------------------------------------------------------ Ulysses (head-parallel) variant, SURVEY §8e / f-3
+# ------------------------------------------------------------------ Ulysses (head-parallel) variant
 def _seq_to_head_shard(x: torch.Tensor, world: int, group=None) -> torch.Tensor:
     """[B,H,S/P,D] on every rank (sequence-sharded) -> [B,H/P,S,D] (head-sharded): one all_to_all."""
     B, H, Sl, D = x.shape
@@ -307,7 +306,7 @@ def sageattn_ulysses(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, tensor_l
     return o if hnd else o.transpose(1, 2)
 
 
-# ------------------------------------------------------------------ ring attention over return_lse, SURVEY §8 f-3
+# ------------------------------------------------------------------ ring attention over return_lse
 def merge_attention_states(o_a: torch.Tensor, lse_a: torch.Tensor, o_b: torch.Tensor, lse_b: torch.Tensor, hnd: bool = True):
     """Combine two partial attention results over disjoint key sets from their natural-log LSEs (the use the reference
     gives `return_lse`, sageattention/core.py:289-293, 329): softmax weights of the union = exp(lse_x - logaddexp)."""

@@ -1,6 +1,6 @@
 """Quantisation front-end with the reference's Python signatures (sageattention/quant.py:22-293,
 sageattention/triton/quant_per_thread.py:154-203, quant_per_block.py:49-101,
-quant_per_block_varlen.py:60-104) on top of the sm_100a kernels.  Outputs are allocated here and
+quant_per_block_varlen.py:60-104) on top of the sm_90a kernels.  Outputs are allocated here and
 passed to the C ABI (the reference's ownership convention)."""
 from typing import Optional, Tuple
 import torch
@@ -105,8 +105,7 @@ def smooth_quant_k(k: torch.Tensor, qk_quant_gran: str = "per_thread", tensor_la
     (csrc/quant.cu k_smooth_quant_kernel: a thread-block cluster per (b,h) reduces the mean through distributed shared memory and
     quantises right away, so K crosses HBM once).  Returns (km, k_int8, k_scale); k_int8 / k_scale are bit-identical to
     quant_k_int8(k, km) with the returned km (km itself is a different fp32 summation order than k_mean(): same value up to one
-    ulp on rare channels).  OPT-IN: measured on B200 the one launch is slower than k_mean + quant_k_int8 (177 vs 153 us at
-    4x32x8192x128) — the quantisers are latency- not bandwidth-bound, so saving the second HBM read does not pay (DESIGN.md 4.2)."""
+    ulp on rare channels).  OPT-IN: the default path is k_mean + quant_k_int8."""
     from ._capi import SAB_GRAN_PER_WARP, SAB_GRAN_PER_THREAD
     b, h_kv, kv_len, head_dim = _dims(k, tensor_layout)
     lay = _layout(tensor_layout)
@@ -128,7 +127,7 @@ def per_warp_int8(q: torch.Tensor, k: torch.Tensor, km: Optional[torch.Tensor] =
                   WARPQ: int = 32, BLKK: int = 64, tensor_layout: str = "HND"):
     """sageattention/quant.py:105-180: q per WARPQ-row block, k per BLKK block with fused (k - km) in fp32;
     CUDA rounding semantics (cvt.rni, amax floored at 1e-7)."""
-    assert BLKQ == 128 and WARPQ == 32 and BLKK == 64, "sm_100a kernel supports the reference defaults"
+    assert BLKQ == 128 and WARPQ == 32 and BLKK == 64, "sm_90a kernel supports the reference defaults"
     q_int8, q_scale = quant_q_int8(q, "per_warp", tensor_layout)
     k_int8, k_scale = quant_k_int8(k, km, "per_warp", tensor_layout)
     return q_int8, q_scale, k_int8, k_scale
@@ -139,7 +138,7 @@ def per_thread_int8(q: torch.Tensor, k: torch.Tensor, km: Optional[torch.Tensor]
                     tensor_layout: str = "HND"):
     """sageattention/triton/quant_per_thread.py:154-203 (8 q scales per 32-row block, 4 k scales per
     64-key block; `k - km` rounded to the input dtype first; scale = amax/127 + 1e-7)."""
-    assert BLKQ == 128 and WARPQ == 32 and BLKK == 64 and WARPK == 64, "sm_100a kernel supports the reference defaults"
+    assert BLKQ == 128 and WARPQ == 32 and BLKK == 64 and WARPK == 64, "sm_90a kernel supports the reference defaults"
     q_int8, q_scale = quant_q_int8(q, "per_thread", tensor_layout)
     k_int8, k_scale = quant_k_int8(k, km, "per_thread", tensor_layout)
     return q_int8, q_scale, k_int8, k_scale
@@ -173,13 +172,13 @@ def per_channel_fp8(v: torch.Tensor, tensor_layout: str = "HND", scale_max: floa
     """Per-channel e4m3 quantisation of V (sageattention/quant.py:224-293).
     Returns (v_fp8, v_scale, vm).  v_fp8 is ``[B, H_kv, D, ceil(kv_len/128)*128]`` float8_e4m3fn
     (token-contiguous "V transposed", zero padded) for BOTH layouts; unlike the reference it is not
-    16-token permuted (an mma.sync artefact the tcgen05 kernel does not need)."""
+    16-token permuted (an mma.sync artefact the wgmma kernel does not need)."""
     b, h_kv, kv_len, head_dim = _dims(v, tensor_layout)
     padded_len = (kv_len + 127) // 128 * 128
     v_fp8 = torch.empty((b, h_kv, head_dim, padded_len), dtype=torch.float8_e4m3fn, device=v.device)
     v_scale = torch.empty((b, h_kv, head_dim), dtype=torch.float32, device=v.device)
     vm = torch.empty((b, h_kv, head_dim), dtype=torch.float32, device=v.device) if smooth_v else None
-    if fused:   # statistics + quantisation in one cluster launch (measured slower on B200, see DESIGN.md 4.2: opt-in)
+    if fused:   # statistics + quantisation in one cluster launch (opt-in)
         ops.per_channel_fp8_fused(v, v_fp8, v_scale, vm, _layout(tensor_layout), scale_max)
     else:
         ops.per_channel_fp8(v, v_fp8, v_scale, vm, _layout(tensor_layout), scale_max)

@@ -74,7 +74,7 @@ def main():
     # ---- 1. quantisation fixtures (bit-exact targets) ----------------------------------------
     for name, shape, dtype, outlier in [] if only_mask else [
         ("quant_d64_fp16", (1, 2, 200, 64), torch.float16, True),
-        ("quant_d128_bf16", (2, 2, 333, 128), torch.bfloat16, False),
+        ("quant_d128_bf16", (2, 1, 333, 128), torch.bfloat16, False),
     ]:
         q, k, _ = mk(shape, dtype, 1234, outlier)
         km = k.mean(dim=2, keepdim=True)
@@ -145,7 +145,7 @@ def main():
     for name, causal in [("varlen_gqa_d128_nc", False), ("varlen_gqa_d128_c", True)]:
         g = torch.Generator().manual_seed(7)
         lens = [200, 130, 77]
-        T, Hq, Hk, D = sum(lens), 4, 2, 128
+        T, Hq, Hk, D = sum(lens), 2, 1, 128
         q = torch.randn((T, Hq, D), generator=g).half()
         k = (torch.randn((T, Hk, D), generator=g) + 2.0 * torch.randn((1, Hk, D), generator=g)).half()
         v = torch.randn((T, Hk, D), generator=g).half()

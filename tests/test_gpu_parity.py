@@ -1,10 +1,11 @@
-"""GPU parity tests (-m gpu): the sm_100a kernels, called through the public API / C ABI, against
+"""GPU parity tests (-m gpu): the sm_90a kernels, called through the public API / C ABI, against
   (1) the CPU oracle (oracle/sage_oracle.py, pinned to reference-Triton golden fixtures),
   (2) the golden fixtures themselves (tests/golden/*.npz, produced by the real reference Triton kernels),
-  (3) the REAL reference CUDA kernels built for sm_100a (oracle/_ref/*.so), when present.
+  (3) the REAL reference CUDA kernels: their outputs on seeded inputs, stored as a fixed sample of rows in
+      tests/golden/reference_cuda_kernels.npz (tests/golden/make_reference_cuda_golden.py, run on an H100 with oracle/_ref built).
 Tolerances (stated once): quantised tensors and scales bit-exact; attention output max-abs <= 1e-2 against the
 reference kernel (north-star tolerance), <= 5e-3 against the oracle run with the kernel's arithmetic."""
-import importlib.util, os
+import os
 import numpy as np
 import pytest
 import torch
@@ -13,13 +14,14 @@ pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 G = os.path.join(ROOT, "tests", "golden")
 TOL_REF = 1e-2      # north-star tolerance vs the reference kernel
-LAZY_TAU = 4        # csrc/attn_alt.cu SAB_ALT_TAU, csrc/attn_hd64.cu kLazyTau: the product kernels' lazy-max threshold (binades)
+LAZY_TAU = 4        # csrc/attn.cu kLazyTau: the kernel's lazy-max threshold (binades)
+REF_GOLDEN = os.path.join(G, "reference_cuda_kernels.npz")
+REF_ROWS = 144      # rows of each reference output kept in the golden file (16-bit outputs stored as their bits)
 
 
 def _kernel_tau(D):
-    """Which running-max rule the INT8+FP8 kernels use: the product kernels (csrc/attn_alt.cu at head_dim 128, the lazy instantiation
-    of csrc/attn_hd64.cu) keep a LAZY max — it moves only when a P would overflow e4m3; SAB_ATTN_KERNEL=exact keeps the reference's
-    exact max.  The oracle restates both (lazy_tau=...), so the CUDA path is always compared with the oracle run with ITS arithmetic;
+    """Which running-max rule the INT8+FP8 kernel uses: by default a LAZY max (csrc/attn.cu) — it moves only when a P would overflow
+    e4m3; SAB_ATTN_KERNEL=exact keeps the reference's exact max.  The oracle restates both (lazy_tau=...), so the CUDA path is always compared with the oracle run with ITS arithmetic;
     against the reference kernel (exact max) a lazy-max result is a different e4m3 rounding realisation of the same P — compared
     statistically."""
     if os.environ.get("SAB_ATTN_KERNEL", "")[:1] == "e":
@@ -45,16 +47,38 @@ def env():
     import sageattention_b200 as sab
     from sageattention_b200 import ops, _capi
     from oracle import sage_oracle as O
-    assert _capi.lib().sab_check_device() == 0, "not an sm_100 device"
+    assert _capi.lib().sab_check_device() == 0, "not an sm_90 device"
     return sab, ops, O
 
 
-def _ref(name):
-    p = os.path.join(ROOT, "oracle", "_ref", name + ".so")
-    if not os.path.exists(p):
-        return None
-    spec = importlib.util.spec_from_file_location(name, p)
-    m = importlib.util.module_from_spec(spec); spec.loader.exec_module(m); return m
+def _ref_golden():
+    assert os.path.exists(REF_GOLDEN), "tests/golden/reference_cuda_kernels.npz missing"
+    return np.load(REF_GOLDEN)
+
+
+def _row_idx(nrows, seed, n=REF_ROWS):
+    """Fixed, seeded sample of row indices (rows of the tensor viewed as [-1, last dim])."""
+    return np.sort(np.random.RandomState(seed).choice(nrows, min(n, nrows), replace=False))
+
+
+def _rows(t, idx):
+    """Rows `idx` of t viewed as [-1, t.shape[-1]], as a CPU tensor."""
+    return t.reshape(-1, t.shape[-1])[torch.from_numpy(idx).to(t.device)].cpu()
+
+
+def _golden16(z, key, dt):
+    """A stored 16-bit reference output (its bit pattern as int16) as float32."""
+    return torch.from_numpy(z[key].copy()).view(dt).float()
+
+
+def _mk_host(B, H, S, D, dt, Hk=None, seed=0):
+    """Inputs of the comparisons with the reference CUDA kernels: drawn on the CPU, so they are the same on every machine."""
+    g = torch.Generator().manual_seed(seed)
+    Hk = Hk or H
+    q = torch.randn(B, H, S, D, generator=g).to(dt)
+    k = torch.randn(B, Hk, S, D, generator=g) + 4.0 * torch.randn(B, Hk, 1, D, generator=g)
+    v = torch.randn(B, Hk, S, D, generator=g)
+    return q.cuda(), k.to(dt).cuda(), v.to(dt).cuda()
 
 
 def _t(a, dtype):
@@ -74,7 +98,7 @@ def _mk(B, H, S, D, dt, Hk=None, outlier=True, seed=0, Sk=None):
 
 def _check_k_mean(got, k, km_torch):
     """K smoothing mean (sageattention/core.py:773 `k.mean(dim=seq)`): torch reduces in fp32 in ITS launch-dependent order and
-    rounds to the input dtype; the sm_100a kernel reduces in fp32 in a fixed order (csrc/quant.cu channel_stats).  Both are
+    rounds to the input dtype; the sm_90a kernel reduces in fp32 in a fixed order (csrc/quant.cu channel_stats).  Both are
     roundings of the same fp32-accurate sum, so they can only differ where the exact mean sits on a rounding boundary of
     the 16-bit format.  Pin: the kernel's value is a CORRECT rounding of the fp64 mean up to the fp32 summation noise
     (half an ulp + 2^-20 relative), and it is bit-identical to torch.mean on all but a handful of channels.  (Given the
@@ -160,38 +184,30 @@ def test_quant_per_thread_bit_exact_at_full_size(env):
     assert torch.equal(ks, sc.reshape(B, H, -1)) and torch.equal(k8, e8)
 
 
+QREF_CASES = [(2, 3, 333, 128, torch.bfloat16), (1, 2, 1000, 64, torch.float16)]
+
+
 def test_quant_bit_exact_vs_real_reference_kernels(env):
+    """Per-warp Q / per-block K INT8 and per-channel FP8 V against the reference's csrc/fused quantisers (stored rows of their
+    output, the reference's 16-token V permutation undone): bit-exact, scales complete."""
     sab, ops, O = env
-    rf = _ref("ref_fused")
-    if rf is None:
-        pytest.skip("oracle/_ref/ref_fused.so not built")
-    for (B, H, S, D, dt) in [(2, 3, 333, 128, torch.bfloat16), (1, 2, 1000, 64, torch.float16)]:
-        q, k, v = _mk(B, H, S, D, dt)
+    z = _ref_golden()
+    for ci, (B, H, S, D, dt) in enumerate(QREF_CASES):
+        q, k, v = _mk_host(B, H, S, D, dt, seed=ci)
         km = k.mean(dim=2, keepdim=True)
         q8, qs, k8, ks = sab.per_warp_int8(q, k, km)
-        rq8, rk8, rqs, rks = torch.empty_like(q8), torch.empty_like(k8), torch.empty_like(qs), torch.empty_like(ks)
-        rf.quant_per_warp_int8_cuda(q, rq8, rqs, 128, 32, 1)
-        rf.quant_per_block_int8_fuse_sub_mean_cuda(k, km.squeeze(2), rk8, rks, 64, 1)
-        torch.cuda.synchronize()
-        assert torch.equal(q8, rq8) and torch.equal(qs, rqs) and torch.equal(k8, rk8) and torch.equal(ks, rks)
+        ridx = _row_idx(B * H * S, 10 + ci)
+        assert np.array_equal(_rows(q8, ridx).numpy(), z[f"quant{ci}_q8"]) and np.array_equal(qs.cpu().numpy(), z[f"quant{ci}_qs"])
+        assert np.array_equal(_rows(k8, ridx).numpy(), z[f"quant{ci}_k8"]) and np.array_equal(ks.cpu().numpy(), z[f"quant{ci}_ks"])
+        vidx = _row_idx(B * H * D, 20 + ci)
         for smax in (448.0, 2.25):
             v8, vs, _ = sab.per_channel_fp8(v, scale_max=smax, smooth_v=False)
-            pl = (S + 63) // 64 * 64
-            vt = torch.empty((B, H, D, pl), dtype=dt, device="cuda")
-            rf.transpose_pad_permute_cuda(v, vt, 1)
-            r8 = torch.empty(vt.shape, dtype=torch.float8_e4m3fn, device="cuda"); rs = torch.empty_like(vs)
-            rf.scale_fuse_quant_cuda(vt, r8, rs, S, smax, 1)
-            torch.cuda.synchronize()
-            perm = torch.tensor([0, 1, 8, 9, 2, 3, 10, 11, 4, 5, 12, 13, 6, 7, 14, 15], device="cuda")  # quant.py:233
-            ar = torch.arange(pl, device="cuda")
-            src = (ar // 16) * 16 + perm[ar % 16]
-            unperm = torch.empty(pl, dtype=torch.long, device="cuda"); unperm[src] = ar
-            assert torch.equal(r8.view(torch.uint8)[..., unperm][..., :S], v8.view(torch.uint8)[..., :S])
-            assert torch.equal(vs, rs)
+            assert np.array_equal(_rows(v8.view(torch.uint8)[..., :S], vidx).numpy(), z[f"quant{ci}_v8_{smax:g}"])
+            assert np.array_equal(vs.cpu().numpy(), z[f"quant{ci}_vs_{smax:g}"])
 
 
 def test_fused_front_end_matches_the_two_step_calls(env):
-    """SURVEY section 8 f-1 (opt-in, measured slower than the two-step path on B200): `smooth_quant_k` (K mean + INT8 K in one cluster
+    """The single-launch front-end (opt-in): `smooth_quant_k` (K mean + INT8 K in one cluster
     launch) and `per_channel_fp8(fused=True)`.  INT8 / FP8 bytes and scales are bit-identical to the two-step entry points given the
     same mean; the fused mean itself is another fp32 summation order (within one 16-bit ulp of k_mean on rare channels)."""
     sab, ops, O = env
@@ -268,47 +284,47 @@ def test_attention_vs_oracle(env, c):
     assert torch.equal(on.transpose(1, 2), o)
 
 
+ATT_REF_CASES = [(1, 4, 1024, 128, torch.float16, False, "per_warp"), (1, 4, 1024, 64, torch.bfloat16, True, "per_warp"),
+                 (2, 4, 2000, 128, torch.bfloat16, False, "per_thread"), (1, 2, 4096, 128, torch.bfloat16, True, "per_thread"),
+                 (1, 8, 1024, 64, torch.float16, False, "per_thread"), (1, 2, 333, 128, torch.float16, True, "per_thread")]
+
+
 def _check_vs_real_reference_kernel(sab, ops, O):
-    """The CUDA path against the REAL reference sm89 kernels (oracle/_ref, built for sm_100a) on the same quantised operands.
-    Exact-max kernels (head_dim 64, SAB_ATTN_KERNEL=exact): same P / m / d bits as the reference -> <= 4e-3 vs its fp32+fp32 kernel
-    (the residual is the reduced-precision accumulator of the reference's legacy fp8 mma.sync), <= 2e-2 vs its fp32+fp16 kernel (that
-    kernel's own per-tile f16 rounding, attn_utils.cuh:896-974).  Lazy-max kernel (head_dim 128): a different e4m3 rounding realisation
-    of the same P, so the comparison is statistical — mean |diff| <= 2.5e-3, and the error against exact fp32 attention is at the
-    reference kernel's level (mean within 10 %, max within 50 % + 5e-3).  LSE agrees to 5e-4 (log2 units) in every case."""
-    rf, ra = _ref("ref_fused"), _ref("ref_qattn")
-    if rf is None or ra is None:
-        return None
+    """The CUDA path against the REAL reference sm89 kernels (qk_int8_sv_f8_accum_f{16,32}_fuse_v_scale_attn_inst_buf) on the same
+    quantised operands (stored rows of their output and LSE).
+    Exact max (SAB_ATTN_KERNEL=exact): same P / m / d bits as the reference -> <= 4e-3 vs its fp32+fp32 kernel (the residual is the
+    reduced-precision accumulator of the reference's legacy fp8 mma.sync), <= 2e-2 vs its fp32+fp16 kernel (that kernel's own per-tile
+    f16 rounding, attn_utils.cuh:896-974).  Lazy max (default): a different e4m3 rounding realisation of the same P, so the comparison
+    is statistical — mean |diff| <= 2.5e-3, and the error against exact fp32 attention is at the reference kernel's level (mean within
+    10 %, max within 50 % + 5e-3).  LSE agrees to 5e-4 (log2 units) in every case."""
+    z = _ref_golden()
     worst, worst_mean = 0.0, 0.0
-    for (B, H, S, D, dt, causal, gran) in [(1, 4, 1024, 128, torch.float16, False, "per_warp"), (1, 4, 1024, 64, torch.bfloat16, True, "per_warp"),
-                                           (2, 4, 2000, 128, torch.bfloat16, False, "per_thread"), (1, 2, 4096, 128, torch.bfloat16, True, "per_thread"),
-                                           (1, 8, 1024, 64, torch.float16, False, "per_thread"), (1, 2, 333, 128, torch.float16, True, "per_thread")]:
-        q, k, v = _mk(B, H, S, D, dt)
+    for ci, (B, H, S, D, dt, causal, gran) in enumerate(ATT_REF_CASES):
+        q, k, v = _mk_host(B, H, S, D, dt, seed=100 + ci)
         km = k.mean(dim=2, keepdim=True)
         sm = D ** -0.5
         q8, qs, k8, ks = (sab.per_warp_int8 if gran == "per_warp" else sab.per_thread_int8)(q, k, km)
         g = 2 if gran == "per_warp" else 3
         tau = _kernel_tau(D)
-        sd = O.sdpa_fp32(q.cpu(), k.cpu(), v.cpu(), is_causal=causal) if tau is not None else None
-        for smax, fn in [(2.25, ra.qk_int8_sv_f8_accum_f16_fuse_v_scale_attn_inst_buf), (448.0, ra.qk_int8_sv_f8_accum_f32_fuse_v_scale_attn_inst_buf)]:
-            pl = (S + 63) // 64 * 64
-            vt = torch.empty((B, H, D, pl), dtype=dt, device="cuda")
-            rf.transpose_pad_permute_cuda(v, vt, 1)
-            r8 = torch.empty(vt.shape, dtype=torch.float8_e4m3fn, device="cuda"); rs = torch.empty((B, H, D), dtype=torch.float32, device="cuda")
-            rf.scale_fuse_quant_cuda(vt, r8, rs, S, smax, 1)
-            o_ref = torch.empty_like(q)
-            lse_ref = fn(q8, k8, r8, o_ref, qs, ks, rs, 1, int(causal), g, sm, 1)
+        ridx = _row_idx(B * H * S, 100 + ci)
+        sd = _rows(O.sdpa_fp32(q.cpu(), k.cpu(), v.cpu(), is_causal=causal), ridx) if tau is not None else None
+        for smax in (2.25, 448.0):
+            o_ref = _golden16(z, f"attn{ci}_o_{smax:g}", dt)
+            lse_ref = torch.from_numpy(z[f"attn{ci}_lse_{smax:g}"])
             v8, vs, _ = sab.per_channel_fp8(v, scale_max=smax, smooth_v=False)
             o = torch.empty_like(q)
             lse = ops.qk_int8_sv_f8_attn(q8, k8, v8, o, qs, ks, vs, None, 1, int(causal), g, g, sm, 0, 1)
             torch.cuda.synchronize()
-            diff = (o.float() - o_ref.float()).abs()
+            o = _rows(o, ridx).float()
+            lse = _rows(lse.reshape(-1, 1), ridx).reshape(-1)
+            diff = (o - o_ref).abs()
             err = diff.max().item()
             worst, worst_mean = max(worst, err), max(worst_mean, diff.mean().item())
             if tau is None:
                 assert err <= (4e-3 if smax == 448.0 else 2e-2), (B, H, S, D, dt, causal, gran, smax, err)
             else:
                 assert diff.mean().item() <= 2.5e-3, (B, H, S, D, dt, causal, gran, smax, diff.mean().item())
-                e_k, e_r = (o.cpu().float() - sd).abs(), (o_ref.cpu().float() - sd).abs()
+                e_k, e_r = (o - sd).abs(), (o_ref - sd).abs()
                 assert e_k.mean().item() <= 1.10 * e_r.mean().item() + 1e-4, (B, H, S, D, dt, causal, gran, smax)
                 assert e_k.max().item() <= 1.5 * e_r.max().item() + 5e-3, (B, H, S, D, dt, causal, gran, smax)
             assert (lse - lse_ref).abs().max().item() <= 5e-4
@@ -325,26 +341,25 @@ _A16_CASES = [(1, 4, 1024, 128, torch.float16, False, "per_warp", 0.0), (1, 2, 2
               (1, 2, 1024, 128, torch.float16, True, "per_thread", 2.0), (1, 4, 1024, 64, torch.float16, True, "per_warp", 2.0)]
 
 
-def _a16_case(sab, ops, O, rf, ra, case):
-    """One case of the a16 study (two-level f16/f32 PV accumulation, attn_utils.cuh:896-974; v += 2 is the f16-accumulator stress of
-    SURVEY 8d): the real reference "fp32+fp16" kernel, our kernel, and the oracle's f16-emulating / fp32 branches — all on the SAME
-    quantised operands."""
+def _a16_inputs(ci, case):
     B, H, S, D, dt, causal, gran, vshift = case
-    g = torch.Generator(device="cuda").manual_seed(0)
-    q = torch.randn(B, H, S, D, device="cuda", generator=g).to(dt)
-    k = (torch.randn(B, H, S, D, device="cuda", generator=g) + 4.0 * torch.randn(B, H, 1, D, device="cuda", generator=g)).to(dt)
-    v = (torch.randn(B, H, S, D, device="cuda", generator=g) + vshift).to(dt)
+    g = torch.Generator().manual_seed(ci)
+    q = torch.randn(B, H, S, D, generator=g).to(dt)
+    k = (torch.randn(B, H, S, D, generator=g) + 4.0 * torch.randn(B, H, 1, D, generator=g)).to(dt)
+    v = (torch.randn(B, H, S, D, generator=g) + vshift).to(dt)
+    return q.cuda(), k.cuda(), v.cuda()
+
+
+def _a16_case(sab, ops, O, z, ci, case):
+    """One case of the a16 study (two-level f16/f32 PV accumulation, attn_utils.cuh:896-974; v += 2 stresses the f16
+    accumulator): the real reference "fp32+fp16" kernel (stored rows), our kernel, and the oracle's f16-emulating / fp32 branches — all
+    on the SAME quantised operands.  Returns the same rows of each."""
+    B, H, S, D, dt, causal, gran, vshift = case
+    q, k, v = _a16_inputs(ci, case)
     km = k.mean(dim=2, keepdim=True)
     sm = D ** -0.5
     q8, qs, k8, ks = (sab.per_warp_int8 if gran == "per_warp" else sab.per_thread_int8)(q, k, km)
     gi = 2 if gran == "per_warp" else 3
-    pl = (S + 63) // 64 * 64
-    vt = torch.empty((B, H, D, pl), dtype=dt, device="cuda")
-    rf.transpose_pad_permute_cuda(v, vt, 1)
-    r8 = torch.empty(vt.shape, dtype=torch.float8_e4m3fn, device="cuda"); rs = torch.empty((B, H, D), dtype=torch.float32, device="cuda")
-    rf.scale_fuse_quant_cuda(vt, r8, rs, S, 2.25, 1)
-    o_ref = torch.empty_like(q)
-    ra.qk_int8_sv_f8_accum_f16_fuse_v_scale_attn_inst_buf(q8, k8, r8, o_ref, qs, ks, rs, 1, int(causal), gi, sm, 0)
     v8, vs, _ = sab.per_channel_fp8(v, scale_max=2.25, smooth_v=False)
     o = torch.empty_like(q)
     ops.qk_int8_sv_f8_attn(q8, k8, v8, o, qs, ks, vs, None, 1, int(causal), gi, gi, sm, 0, 0)
@@ -354,20 +369,19 @@ def _a16_case(sab, ops, O, rf, ra, case):
     kw = dict(qk_quant_gran=gran, is_causal=causal, sm_scale=sm, out_dtype=torch.float32)
     o_f16 = O.attn_int8_fp8_cuda(*args, pv_accum_dtype="fp32+fp16", **kw)
     o_f32 = O.attn_int8_fp8_cuda(*args, pv_accum_dtype="fp32+fp32", **kw)
-    return o.float().cpu(), o_ref.float().cpu(), o_f16, o_f32, dt
+    ridx = _row_idx(B * H * S, 200 + ci)
+    return _rows(o, ridx).float(), _golden16(z, f"a16_{ci}_o", dt), _rows(o_f16, ridx), _rows(o_f32, ridx), dt
 
 
 def test_a16_oracle_f16_accumulate_branch_vs_real_f16_kernel(env):
     """Pins the oracle's emulate_f16_accum branch (oracle/sage_oracle.py attn_int8_fp8_cuda, pv_accum_dtype="fp32+fp16") to the REAL
     reference kernel `qk_int8_sv_f8_accum_f16_fuse_v_scale_attn_inst_buf`: within 2e-3 plus two units in the last place of the output
-    (measured on B200, profiles/r02_a16_probe.log: 2e-4 .. 1.6e-3, 4.3e-3 = 2 fp16 ulps in the v += 2 causal stress case — the real mma
-    accumulates its 32-key steps with an internal precision the step-wise f16 rounding of the restatement only approximates)."""
+    (the real mma accumulates its 32-key steps with an internal precision the step-wise f16 rounding of the restatement only
+    approximates; the v += 2 causal stress case reaches 2 fp16 ulps)."""
     sab, ops, O = env
-    rf, ra = _ref("ref_fused"), _ref("ref_qattn")
-    if rf is None or ra is None:
-        pytest.skip("oracle/_ref not built")
-    for case in _A16_CASES:
-        _, o_ref, o_f16, _, dt = _a16_case(sab, ops, O, rf, ra, case)
+    z = _ref_golden()
+    for ci, case in enumerate(_A16_CASES):
+        _, o_ref, o_f16, _, dt = _a16_case(sab, ops, O, z, ci, case)
         err = (o_f16 - o_ref).abs()
         assert (err <= 2e-3 + 2.02 * _out_ulp(o_ref, dt)).all(), (case, err.max().item())
 
@@ -376,12 +390,10 @@ def _check_a16_attribution(sab, ops, O):
     """With the EXACT-max kernel (same P bits as the reference): where our output differs from the reference's default "fp32+fp16"
     kernel, the difference IS that kernel's per-tile f16 rounding — our result sits on the exact evaluation of the quantised operands
     (oracle, fp32 accumulation) to 2e-3 + 1 ulp everywhere, and on the rows that differ by more than 5e-3 the reference is the farther one."""
-    rf, ra = _ref("ref_fused"), _ref("ref_qattn")
-    if rf is None or ra is None:
-        return None
+    z = _ref_golden()
     worst = 0.0
-    for case in _A16_CASES:
-        o, o_ref, o_f16, o_f32, dt = _a16_case(sab, ops, O, rf, ra, case)
+    for ci, case in enumerate(_A16_CASES):
+        o, o_ref, o_f16, o_f32, dt = _a16_case(sab, ops, O, z, ci, case)
         e_o, e_r = (o - o_f32).abs(), (o_ref - o_f32).abs()
         assert (e_o <= 2e-3 + 1.01 * _out_ulp(o_f32, dt)).all(), (case, e_o.max().item())
         rows = (o - o_ref).abs().amax(dim=-1) > 5e-3
@@ -394,8 +406,6 @@ def _check_a16_attribution(sab, ops, O):
 def test_attention_vs_real_reference_kernel(env):
     sab, ops, O = env
     r = _check_vs_real_reference_kernel(sab, ops, O)
-    if r is None:
-        pytest.skip("oracle/_ref not built")
     print(f"worst max-abs / mean-abs vs real reference kernels: {r[0]:.3e} / {r[1]:.3e}")
 
 
@@ -417,52 +427,20 @@ def test_exact_max_kernel_matches_reference_kernel_bits():
     print(p.stdout[-300:])
 
 
-def test_q4_kernel_opt_in_matches_the_product_kernel():
-    """SAB_ATTN_KERNEL=q4 selects csrc/attn_q4.cu at head_dim 128 (one CTA per SM, four softmax warpgroups, separate P buffers in
-    TMEM): same lazy-max arithmetic as the product kernel — P, m and the PV accumulation order are identical, only the row sum is
-    combined from four partial sums instead of two — so it has to pass the product kernel's checks against the real reference
-    kernel, and agree with the product kernel itself to an output ulp (the last shape has 256 key tiles per CTA).
-    Subprocess: the kernel choice is read once per process."""
-    import subprocess, sys
-    if not torch.cuda.is_available():
-        pytest.skip("needs a GPU")
-    code = ("import sys; sys.path.insert(0, %r); sys.path.insert(0, %r)\n"
-            "import torch, sageattention_b200 as sab\nfrom sageattention_b200 import ops\nfrom oracle import sage_oracle as O\n"
-            "import test_gpu_parity as T\nr = T._check_vs_real_reference_kernel(sab, ops, O)\nprint('VSREF', r)\n"
-            "outs = []\n"
-            "for (B, H, Hk, S, causal, gran, dt) in [(2, 4, 2, 1000, True, 'per_thread', torch.bfloat16), (1, 40, 40, 2048, False, 'per_warp', torch.float16),\n"
-            "                                        (1, 2, 2, 77, False, 'per_thread', torch.float16), (1, 2, 2, 16384, False, 'per_thread', torch.bfloat16)]:\n"
-            "    g = torch.Generator(device='cuda').manual_seed(S)\n"
-            "    q = torch.randn(B, H, S, 128, device='cuda', generator=g).to(dt); k = torch.randn(B, Hk, S, 128, device='cuda', generator=g).to(dt)\n"
-            "    v = torch.randn(B, Hk, S, 128, device='cuda', generator=g).to(dt)\n"
-            "    o, lse = sab.sageattn_qk_int8_pv_fp8_cuda(q, k, v, is_causal=causal, qk_quant_gran=gran, return_lse=True)\n"
-            "    outs.append((o.float().cpu(), lse.cpu()))\n"
-            "torch.save(outs, sys.argv[1])\nprint('SAVED')\n" % (ROOT, os.path.join(ROOT, "tests")))
-    import tempfile
-    res = {}
-    with tempfile.TemporaryDirectory() as td:
-        for kern in ("q4", "alt"):
-            path = os.path.join(td, kern + ".pt")
-            p = subprocess.run([sys.executable, "-c", code, path], env=dict(os.environ, SAB_ATTN_KERNEL=kern), capture_output=True, text=True, timeout=600)
-            assert p.returncode == 0 and "VSREF" in p.stdout and "SAVED" in p.stdout, p.stdout[-2000:] + p.stderr[-2000:]
-            res[kern] = torch.load(path)
-    for (oq, lq), (oa, la) in zip(res["q4"], res["alt"]):
-        assert (oq - oa).abs().max().item() <= 2 ** -7 * max(1.0, oa.abs().max().item())       # one bf16 ulp of the largest output
-        assert (oq != oa).float().mean().item() < 0.05
-        assert (lq - la).abs().max().item() < 1e-5
+F16PV_CASES = [(1, 4, 4, 1024, 128, torch.float16, False, "per_thread"), (1, 4, 2, 1000, 64, torch.float16, True, "per_warp"),
+               (2, 2, 2, 333, 128, torch.bfloat16, True, "per_thread"), (1, 2, 2, 2048, 64, torch.bfloat16, False, "per_thread")]
 
 
 def test_fp16_pv_cuda_entry_vs_real_reference_kernel_and_oracle(env):
     """sageattn_qk_int8_pv_fp16_cuda (core.py:451-633): per-warp / per-thread INT8 Q,K + FP16 P and V.  Against the REAL
-    reference sm80 kernel (`qk_int8_sv_f16_accum_f32_attn`, csrc/qattn/qk_int_sv_f16_cuda_sm80.cu built for sm_100a) on the same
-    quantised operands, and end to end against the oracle restatement.  Tolerance 2e-3 (fp16 P, fp32 accumulation on both
+    reference sm80 kernel (`qk_int8_sv_f16_accum_f32_attn`, csrc/qattn/qk_int_sv_f16_cuda_sm80.cu; stored rows of its output) on the
+    same quantised operands, and end to end against the oracle restatement.  Tolerance 2e-3 (fp16 P, fp32 accumulation on both
     sides; summation order differs) + one output ulp for bf16."""
     sab, ops, O = env
-    r80 = _ref("ref_qattn80")
+    z = _ref_golden()
     worst = 0.0
-    for (B, H, Hk, S, D, dt, causal, gran) in [(1, 4, 4, 1024, 128, torch.float16, False, "per_thread"), (1, 4, 2, 1000, 64, torch.float16, True, "per_warp"),
-                                               (2, 2, 2, 333, 128, torch.bfloat16, True, "per_thread"), (1, 2, 2, 2048, 64, torch.bfloat16, False, "per_thread")]:
-        q, k, v = _mk(B, H, S, D, dt, Hk=Hk)
+    for ci, (B, H, Hk, S, D, dt, causal, gran) in enumerate(F16PV_CASES):
+        q, k, v = _mk_host(B, H, S, D, dt, Hk=Hk, seed=300 + ci)
         km = k.mean(dim=2, keepdim=True)
         sm = D ** -0.5
         q8, qs, k8, ks = (sab.per_warp_int8 if gran == "per_warp" else sab.per_thread_int8)(q, k, km)
@@ -471,14 +449,11 @@ def test_fp16_pv_cuda_entry_vs_real_reference_kernel_and_oracle(env):
         o = torch.empty_like(q)
         lse = ops.qk_int8_sv_f16_attn(q8, k8, vt, o, qs, ks, 1, int(causal), g, g, sm, 0, 1)
         tol = 2e-3 + (2.0 ** -7 if dt == torch.bfloat16 else 0.0)
-        if r80 is not None:
-            o_ref = torch.empty_like(q)
-            lse_ref = r80.qk_int8_sv_f16_accum_f32_attn(q8, k8, v.to(torch.float16), o_ref, qs, ks, 1, int(causal), g, sm, 1)
-            torch.cuda.synchronize()
-            err = (o.float() - o_ref.float()).abs().max().item()
-            worst = max(worst, err)
-            assert err <= tol, (B, H, S, D, dt, causal, gran, err)
-            assert (lse - lse_ref).abs().max().item() <= 5e-4
+        ridx = _row_idx(B * H * S, 300 + ci)
+        err = (_rows(o, ridx).float() - _golden16(z, f"f16pv{ci}_o", dt)).abs().max().item()
+        worst = max(worst, err)
+        assert err <= tol, (B, H, S, D, dt, causal, gran, err)
+        assert (_rows(lse.reshape(-1, 1), ridx).reshape(-1) - torch.from_numpy(z[f"f16pv{ci}_lse"])).abs().max().item() <= 5e-4
         oe, le = O.attn_int8_fp16_cuda(q8.cpu(), k8.cpu(), v.cpu(), qs.cpu(), ks.cpu(), qk_quant_gran=gran, is_causal=causal,
                                        sm_scale=sm, out_dtype=dt, return_lse=True)
         assert (o.cpu().float() - oe.float()).abs().max().item() <= tol
@@ -489,16 +464,14 @@ def test_fp16_pv_cuda_entry_vs_real_reference_kernel_and_oracle(env):
             assert torch.equal(o2, o)
         oe2 = O.sageattn_qk_int8_pv_fp16_cuda(q.cpu(), k.cpu(), v.cpu(), is_causal=causal, qk_quant_gran=gran)
         assert (o2.cpu().float() - oe2.float()).abs().max().item() <= 2 * tol      # km: torch CPU vs kernel rounding of the mean
-    if r80 is None:
-        pytest.skip("oracle/_ref/ref_qattn80.so not built (oracle comparison passed)")
     print(f"worst max-abs vs real reference sm80 f16 kernel: {worst:.3e}")
 
 
 @pytest.mark.parametrize("name", ["attn_d64_fp16_nc", "attn_d64_fp16_c", "attn_d128_fp16_nc_ragged"])
 def test_triton_path_shell_vs_reference_triton_fixtures(env, name):
-    """sageattn_qk_int8_pv_fp16_triton on sm_100a = bit-exact per-block quantisation + the FP16-PV kernel variant
+    """sageattn_qk_int8_pv_fp16_triton on sm_90a = bit-exact per-block quantisation + the FP16-PV kernel variant
     (kind::f16, Triton-path softmax): output within 4e-3 of the reference Triton kernel (whose tl.dot accumulates each
-    64-key partial product in fp16; tcgen05 accumulates in fp32), LSE within 2e-3."""
+    64-key partial product in fp16; our kernel accumulates in fp32), LSE within 2e-3."""
     sab, ops, O = env
     z = np.load(f"{G}/{name}.npz")
     q, k, v, o_ref = (_t(z[n], torch.float16).cuda() for n in ("q", "k", "v", "o"))
@@ -575,7 +548,7 @@ def test_triton_path_attn_mask_vs_oracle(env):
     assert torch.isfinite(o).all() and o[:, :, 5].abs().max().item() == 0.0
 
 
-# ------------------------------------------------------------------------------------------- API behaviour (SURVEY §9)
+# ------------------------------------------------------------------------------------------- API behaviour
 def test_api_behaviour(env):
     sab, ops, O = env
     q, k, v = _mk(1, 4, 256, 64, torch.float16)
@@ -713,7 +686,7 @@ def test_full_size_config3_varlen_gqa(env):
         assert (o[rows, h].float() - ex).abs().max().item() < 3e-2
 
 
-# ------------------------------------------------------------------------------------------- callers either side of the path (SURVEY §8 f)
+# ------------------------------------------------------------------------------------------- callers either side of the path
 @pytest.mark.gpu
 def test_prequantized_kv_is_bit_identical_to_one_shot_call(env):
     """quantize_kv once + sageattn_prequantized per call == sageattn_qk_int8_pv_fp8_cuda, bit for bit (same kernels)."""

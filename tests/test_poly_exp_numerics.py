@@ -1,7 +1,7 @@
-"""CPU numerics of the opt-in FMA-pipe exponential of the sm_100a attention kernel (csrc/ptx.cuh `ex2_poly2`, builds with
+"""CPU numerics of the opt-in FMA-pipe exponential of the sm_90a attention kernel (csrc/ptx.cuh `ex2_poly2`, builds with
 -DSAB_POLY_EXP_PAIRS=n): a float32 restatement of the instruction sequence, its error against exp2, and what replacing
-n of every 4 column pairs of P by it does to the attention output of the CPU oracle.  This is the evidence DESIGN.md §4.3
-quotes for "far inside the 1e-2 tolerance"; the default build does not use the polynomial."""
+n of every 4 column pairs of P by it does to the attention output of the CPU oracle (far inside the 1e-2 tolerance); the
+default build does not use the polynomial."""
 import numpy as np
 import torch
 
@@ -115,7 +115,7 @@ def test_e4m3_flip_rate_of_P():
 
 
 def test_lazy_rescale_numerics():
-    """-DSAB_LAZY_RESCALE=tau (csrc/attn.cu): P is taken against a stale maximum, i.e. scaled by 2^(m_exact - m_stale) with a
+    """The lazy running max (csrc/attn.cu, lazy_tau): P is taken against a stale maximum, i.e. scaled by 2^(m_exact - m_stale) with a
     non-integer exponent, so its e4m3 rounding is a different realisation of the same quantisation noise: the output is not
     comparable bit for bit with the reference kernel's, but its error against exact attention is the same (mean within 3 %),
     and the LSE (from un-rounded sums) agrees to 1e-5.  The number of tiles in which ANY of a warp's 32 rows moves its maximum —

@@ -222,7 +222,8 @@ def _expand_k_scale(k_scale, gran, Sk, BLKK=64):
 
 def attn_int8_fp8_cuda(q8, k8, v8, q_scale, k_scale, v_scale, *, qk_quant_gran="per_thread",
                        k_quant_gran=None, is_causal=False, sm_scale=1.0, pv_accum_dtype="fp32+fp32",
-                       out_dtype=torch.float16, kv_tile=64, return_lse=False, log2e=LOG2E_CU, exp2_fn=None, lazy_tau=None):
+                       out_dtype=torch.float16, kv_tile=64, return_lse=False, log2e=LOG2E_CU, exp2_fn=None, lazy_tau=None,
+                       v_mean=None, causal_q_offset=0):
     """csrc/qattn/qk_int_sv_f8_cuda_sm89.cuh:44-704 restated on [B,H,S,D] tensors.
 
     q8/k8 int8 [B,Hq|Hkv,S,D]; v8 fp8-e4m3 LOGICAL [B,Hkv,Skv,D]; scales packed as the reference.
@@ -238,7 +239,12 @@ def attn_int8_fp8_cuda(q8, k8, v8, q_scale, k_scale, v_scale, *, qk_quant_gran="
     `exp2_fn` (default torch.exp2) replaces the exponential of P only — used by tests/test_poly_exp_numerics.py to
     quantify the opt-in FMA-pipe polynomial of the sm_90a kernel (csrc/ptx.cuh ex2_poly2) against this restatement.
     `lazy_tau` (default None = the reference rule) restates the lazy running max of the sm_90a kernel: the
-    running max only moves when it grew by more than tau (log2 units) and the exponent offset is 8.807 - tau."""
+    running max only moves when it grew by more than tau (log2 units) and the exponent offset is 8.807 - tau.
+    `v_mean` ([B,Hkv,D] fp32, the smooth_v channel mean) is added after `* v_scale`, as the reference's fuse-v-mean epilogue
+    (…sm89.cuh:572-703) and the sm_90a kernel do.
+    `causal_q_offset` is the global index of q8's first row (the kernel parameter of the same name): the causal mask and the
+    causal early exit use global rows, q_scale stays indexed by local row.  So one 128-row-aligned block of Q
+    (q8[:, :, r0:r0+128] with q_scale sliced to that block) evaluates to exactly those rows of the full evaluation."""
     B, Hq, Sq, D = q8.shape
     _, Hk, Sk, _ = k8.shape
     g = Hq // Hk
@@ -255,10 +261,10 @@ def attn_int8_fp8_cuda(q8, k8, v8, q_scale, k_scale, v_scale, *, qk_quant_gran="
     m = torch.full((B, Hq, Sq), MASK_VALUE, dtype=torch.float32)
     d = torch.ones((B, Hq, Sq), dtype=torch.float32)
     O = torch.zeros((B, Hq, Sq, D), dtype=torch.float32)
-    qi = torch.arange(Sq)[:, None]
+    qi = torch.arange(Sq)[:, None] + causal_q_offset
     for s0 in range(0, Sk, kv_tile):
         s1 = min(s0 + kv_tile, Sk)
-        if is_causal and s0 > Sq - 1:
+        if is_causal and s0 > causal_q_offset + Sq - 1:
             break
         S_i = qf @ kf[:, :, s0:s1].transpose(-1, -2)                               # exact in fp32
         coef = (sm2 * qs_row)[..., None] * ks_key[:, :, None, s0:s1]               # sm_scale*dequant
@@ -286,6 +292,8 @@ def attn_int8_fp8_cuda(q8, k8, v8, q_scale, k_scale, v_scale, *, qk_quant_gran="
             O = O * alpha[..., None] + P8 @ Vt
         m = m_new
     out = (O / d[..., None]) * vsc[:, :, None, :]
+    if v_mean is not None:
+        out = out + v_mean.float().repeat_interleave(g, dim=1)[:, :, None, :]
     out = out.to(out_dtype)
     if return_lse:
         return out, torch.log2(d) + m

@@ -27,6 +27,15 @@ def _ptr(t: Optional[torch.Tensor]):
     return None if t is None else t.data_ptr()
 
 
+def _v_pad(value: torch.Tensor) -> int:
+    """Token extent of the transposed V operand ([..., D, S_pad]).  The C ABI takes no V strides: the kernel's tensor map
+    assumes the packed layout the V quantisers write, so a strided view (e.g. a permuted all-gather buffer) is refused
+    instead of read as the wrong keys."""
+    if not value.is_contiguous():
+        raise ValueError("value (quantised / transposed V) must be contiguous")
+    return value.size(-1)
+
+
 def _bhs_strides(t: torch.Tensor, tensor_layout: int):
     """(stride_b, stride_h, stride_s) in elements; tensor_layout 0 = NHD, 1 = HND (reference encoding)."""
     if tensor_layout == 1:
@@ -225,7 +234,7 @@ def qk_int8_sv_f8_attn(query: torch.Tensor, key: torch.Tensor, value: torch.Tens
         check(lib().sab_qk_int8_sv_f8_attn(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
                                            lse.data_ptr() if return_lse else None, query_scale.data_ptr(), key_scale.data_ptr(),
                                            _ptr(value_scale), _ptr(value_mean), _dt(output), B, Hq, Hkv, Sq, Skv, D,
-                                           *qs, *ks, value.size(-1), *os_, is_causal, q_quant_gran, k_quant_gran,
+                                           *qs, *ks, _v_pad(value), *os_, is_causal, q_quant_gran, k_quant_gran,
                                            float(sm_scale), fold_sm_scale, None, None, None, None, None, 0,
                                            causal_q_offset, kv_seg_len, None, _stream(query)))
     return lse
@@ -256,7 +265,7 @@ def qk_int8_sv_f8_attn_sp(query: torch.Tensor, key: torch.Tensor, value: torch.T
     with torch.cuda.device(query.device):
         check(lib().sab_qk_int8_sv_f8_attn_sp(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(), None,
                                               query_scale.data_ptr(), key_scale.data_ptr(), value_scale.data_ptr(), _dt(output),
-                                              B, Hq, Hkv, Sq, P * kv_seg_len, D, *qs, *ks, value.size(-1), *os_, q_quant_gran,
+                                              B, Hq, Hkv, Sq, P * kv_seg_len, D, *qs, *ks, _v_pad(value), *os_, q_quant_gran,
                                               k_quant_gran, float(sm_scale), kv_seg_len, seg_flags.data_ptr(),
                                               int(seg_epoch) & 0xFFFFFFFF, heads_per_flag, _stream(query)))
 
@@ -281,7 +290,7 @@ def qk_int8_sv_f8_attn_varlen(query: torch.Tensor, key: torch.Tensor, value: tor
                                            query_scale.data_ptr(), key_scale.data_ptr(), value_scale.data_ptr(), None,
                                            _dt(output), nseq, Hq, Hkv, Tq, Tk, D,
                                            0, query.stride(1), query.stride(0), 0, key.stride(1), key.stride(0),
-                                           value.size(-1), 0, output.stride(1), output.stride(0), is_causal,
+                                           _v_pad(value), 0, output.stride(1), output.stride(0), is_causal,
                                            _capi.SAB_GRAN_PER_BLOCK, _capi.SAB_GRAN_PER_BLOCK, float(sm_scale), fold_sm_scale,
                                            cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), cu_pad_v.data_ptr(),
                                            cu_q_scale.data_ptr(), cu_k_scale.data_ptr(), max_seqlen_q, 0, 0, None, _stream(query)))
@@ -337,7 +346,7 @@ def qk_int8_sv_f16_attn(query: torch.Tensor, key: torch.Tensor, value: torch.Ten
     with torch.cuda.device(query.device):
         check(lib().sab_qk_int8_sv_f16_attn(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
                                             lse.data_ptr() if return_lse else None, query_scale.data_ptr(), key_scale.data_ptr(),
-                                            _dt(output), B, Hq, Hkv, Sq, Skv, D, *qs, *ks, value.size(-1), *os_, is_causal,
+                                            _dt(output), B, Hq, Hkv, Sq, Skv, D, *qs, *ks, _v_pad(value), *os_, is_causal,
                                             q_quant_gran, k_quant_gran, float(sm_scale), fold_sm_scale, None, None, None, None,
                                             None, 0, _stream(query)))
     return lse
@@ -371,7 +380,7 @@ def qk_int8_sv_f16_attn_masked(query: torch.Tensor, key: torch.Tensor, value: to
         check(lib().sab_qk_int8_sv_f16_attn_masked(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
                                                    lse.data_ptr() if return_lse else None, query_scale.data_ptr(),
                                                    key_scale.data_ptr(), _dt(output), B, Hq, Hkv, Sq, Skv, D, *qs, *ks,
-                                                   value.size(-1), *os_, q_quant_gran, k_quant_gran, float(sm_scale),
+                                                   _v_pad(value), *os_, q_quant_gran, k_quant_gran, float(sm_scale),
                                                    fold_sm_scale, attn_mask.data_ptr(), kind, *attn_mask.stride(),
                                                    _stream(query)))
     return lse
@@ -398,7 +407,7 @@ def qk_int8_sv_f16_attn_varlen(query: torch.Tensor, key: torch.Tensor, value: to
     with torch.cuda.device(query.device):
         check(lib().sab_qk_int8_sv_f16_attn(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(), None,
                                             query_scale.data_ptr(), key_scale.data_ptr(), _dt(output), nseq, Hq, Hkv, Tq, Tk, D,
-                                            0, query.stride(1), query.stride(0), 0, key.stride(1), key.stride(0), value.size(-1),
+                                            0, query.stride(1), query.stride(0), 0, key.stride(1), key.stride(0), _v_pad(value),
                                             0, output.stride(1), output.stride(0), is_causal, _capi.SAB_GRAN_PER_BLOCK,
                                             _capi.SAB_GRAN_PER_BLOCK, float(sm_scale), fold_sm_scale, cu_seqlens_q.data_ptr(),
                                             cu_seqlens_k.data_ptr(), cu_pad_v.data_ptr(), cu_q_scale.data_ptr(),

@@ -1,0 +1,96 @@
+"""Backward benchmark: forward + backward of sageattn at the headline shape (B=4, H=32, S=8192, D=128, bf16), non-causal and
+causal, on one GPU.  Prints one JSON line with, per mode:
+  * bwd_kernel: the gradient kernels alone (sab_qk_int8_attn_bwd on quantised operands prepared once), ms and TFLOP/s counting
+    10*B*H*S^2*D algorithmic FLOPs (halved for causal; the two-kernel design's recompute of S and dP is not counted);
+  * bwd_call: the whole backward of sageattn (o.backward(dO): Q/K quantiser recompute + gradient kernels);
+  * fwd_bwd: forward + backward of sageattn;
+  * sdpa_flash_bwd: torch SDPA's flash-attention backward on the same inputs, for context;
+and the GPU name and power limit.  CUDA events after warm-up; writes nothing."""
+import argparse
+import json
+import subprocess
+
+import torch
+import torch.nn.functional as F
+
+
+def _events(fn, steps, warmup):
+    for _ in range(warmup):
+        fn()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(steps):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / steps
+
+
+def _gpu():
+    name = torch.cuda.get_device_name(0)
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits", "-i", "0"],
+                           capture_output=True, text=True, timeout=30)
+        pl, clk = (x.strip() for x in r.stdout.strip().split(","))
+        return {"name": name, "power_limit_w": float(pl), "sm_max_mhz": float(clk)}
+    except Exception as e:  # the figures are still stated next to the numbers, as unknown
+        return {"name": name, "power_limit_w": None, "error": str(e)}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--B", type=int, default=4)
+    ap.add_argument("--H", type=int, default=32)
+    ap.add_argument("--S", type=int, default=8192)
+    ap.add_argument("--D", type=int, default=128)
+    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--warmup", type=int, default=3)
+    a = ap.parse_args()
+    assert torch.cuda.is_available(), "bench_backward.py needs a GPU"
+    import sageattention_b200 as sab
+    from sageattention_b200 import ops
+
+    B, H, S, D = a.B, a.H, a.S, a.D
+    dt = torch.bfloat16
+    g = torch.Generator(device="cuda").manual_seed(0)
+    q, k, v, do = (torch.randn(B, H, S, D, device="cuda", dtype=dt, generator=g) for _ in range(4))
+    sm = D ** -0.5
+    out = {"metric": "sageattn backward", "shape": {"B": B, "H": H, "S": S, "D": D, "dtype": "bf16"}, "gpu": _gpu()}
+    for causal in (False, True):
+        flops = 10.0 * B * H * S * S * D * (0.5 if causal else 1.0)
+        # kernels alone, on the operands sageattn's forward uses
+        km = sab.k_mean(k)
+        q8, qs, k8, ks = sab.per_thread_int8(q, k, km)
+        v8, vs, _ = sab.per_channel_fp8(v, scale_max=2.25, smooth_v=False)
+        o = torch.empty_like(q)
+        lse = ops.qk_int8_sv_f8_attn(q8, k8, v8, o, qs, ks, vs, None, 1, int(causal), 3, 3, sm, 0, 1)
+        dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        t_kern = _events(lambda: ops.qk_int8_attn_bwd(q8, k8, qs, ks, q, k, v, o, do, lse, km, dq, dk, dv, 1, int(causal), 3, 3, sm, 0),
+                         a.steps, a.warmup)
+        # the public call
+        qg, kg, vg = (t.clone().requires_grad_(True) for t in (q, k, v))
+
+        def fwd_bwd():
+            qg.grad = kg.grad = vg.grad = None
+            sab.sageattn(qg, kg, vg, is_causal=causal).backward(do)
+
+        t_fb = _events(fwd_bwd, a.steps, a.warmup)
+        ob = sab.sageattn(qg, kg, vg, is_causal=causal)
+        t_bwd = _events(lambda: torch.autograd.grad(ob, (qg, kg, vg), do, retain_graph=True), a.steps, a.warmup)
+        # torch SDPA flash backward, same inputs
+        with torch.nn.attention.sdpa_kernel(torch.nn.attention.SDPBackend.FLASH_ATTENTION):
+            os_ = F.scaled_dot_product_attention(qg, kg, vg, is_causal=causal)
+            t_sdpa = _events(lambda: torch.autograd.grad(os_, (qg, kg, vg), do, retain_graph=True), a.steps, a.warmup)
+        out["causal" if causal else "non_causal"] = {
+            "bwd_kernel": {"ms": round(t_kern, 3), "tflops": round(flops / t_kern / 1e9, 1)},
+            "bwd_call": {"ms": round(t_bwd, 3), "tflops": round(flops / t_bwd / 1e9, 1)},
+            "fwd_bwd": {"ms": round(t_fb, 3)},
+            "sdpa_flash_bwd": {"ms": round(t_sdpa, 3), "tflops": round(flops / t_sdpa / 1e9, 1)},
+        }
+        del ob, os_
+    print(json.dumps(out))
+
+
+if __name__ == "__main__":
+    main()

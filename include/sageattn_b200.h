@@ -256,6 +256,34 @@ int sab_qk_int8_sv_f8_attn_sp(const int8_t* q_int8, const int8_t* k_int8, const 
                               int64_t o_stride_h, int64_t o_stride_s, int q_gran, int k_gran, float sm_scale, int kv_seg_len,
                               const uint32_t* seg_flags, uint32_t seg_epoch, int heads_per_flag, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Backward of the INT8-QK attention (no reference counterpart: the reference is forward-only).  The gradient of attention
+ * evaluated at the forward's quantised logits, a straight-through estimator through the INT8 Q/K, FP8 V and FP8 P roundings:
+ *   S = dequant(q_int8 k_int8^T) * sm_scale (the logits the forward kernel computed: same scales, granularities, fold),
+ *   P = exp2(S*log2e - lse), dV = P^T dO, dP = dO V^T, delta = rowsum(dO o O), dS = P o (dP - delta),
+ *   dQ = dS K * sm_scale, dK = dS^T Q * sm_scale.
+ *   q_int8, k_int8, q_scale, k_scale, q_gran, k_gran, sm_scale, fold_sm_scale : exactly what the forward call received;
+ *   q, k, v : the original 16-bit bhsd tensors (`dtype`); k must be UNsmoothed (the K mean has no gradient term: the rows of dS
+ *             sum to zero), while k_int8 is the smoothed K the forward used, because lse is relative to it;
+ *   o, dout : the forward's output and its gradient (bhsd, `dtype`); lse : [B,Hq,Sq] fp32, the forward's log2 LSE;
+ *   k_mean : optional [B,Hkv,D] (`dtype`), the K smoothing mean the forward subtracted.  dQ is then taken as dS (K - k_mean): the
+ *            same value in exact arithmetic, but the small residue in the row sums of dS (delta comes from the quantised
+ *            forward's O) is not multiplied by a large K mean;
+ *   dq, dk, dv : outputs in `dtype` with the strides of q, k, v.  GQA: dk / dv are summed over the Q heads of each KV head.
+ *   workspace : >= sab_attn_bwd_workspace_bytes(B, Hq, Sq) bytes of device scratch.
+ * Dense only; is_causal needs Sq == Skv (top-left).  Deterministic: no atomics, a fixed summation order.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t sab_attn_bwd_workspace_bytes(int B, int Hq, int Sq);
+int sab_qk_int8_attn_bwd(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale, const void* q,
+                         const void* k, const void* v, const void* o, const void* dout, const float* lse, const void* k_mean,
+                         void* dq, void* dk, void* dv, void* workspace, int dtype, int B, int Hq, int Hkv, int Sq, int Skv, int D,
+                         int64_t q8_stride_b, int64_t q8_stride_h, int64_t q8_stride_s, int64_t k8_stride_b,
+                         int64_t k8_stride_h, int64_t k8_stride_s, int64_t q_stride_b, int64_t q_stride_h, int64_t q_stride_s,
+                         int64_t k_stride_b, int64_t k_stride_h, int64_t k_stride_s, int64_t v_stride_b, int64_t v_stride_h,
+                         int64_t v_stride_s, int64_t o_stride_b, int64_t o_stride_h, int64_t o_stride_s, int64_t do_stride_b,
+                         int64_t do_stride_h, int64_t do_stride_s, int is_causal, int q_gran, int k_gran, float sm_scale,
+                         int fold_sm_scale, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -51,6 +51,92 @@ def _lse_correction(q, km, tensor_layout):
     return torch.matmul(q, kmb.transpose(2, 3)).squeeze(-1).to(torch.float32)
 
 
+# ------------------------------------------------------------------------------------------------ dense calls and their gradient
+def _quant_qk(q, k, kind, tensor_layout, qk_quant_gran, sm_scale, smooth_k, backend):
+    """Q/K front-end of a dense entry point on head-dim-padded q, k: (km, q_int8, q_scale, k_int8, k_scale, q_gran, k_gran,
+    fold_sm_scale).  Deterministic, so the backward re-runs it instead of keeping the 8-bit operands alive."""
+    km = k_mean(k, tensor_layout) if smooth_k else None
+    if kind == "fp16_triton":
+        q_int8, q_scale, k_int8, k_scale = per_block_int8(q, k, km=km, sm_scale=sm_scale, tensor_layout=tensor_layout,
+                                                          semantics=backend)
+        return km, q_int8, q_scale, k_int8, k_scale, SAB_GRAN_PER_BLOCK, SAB_GRAN_PER_BLOCK, 1
+    q_int8, q_scale = quant_q_int8(q, qk_quant_gran, tensor_layout)
+    k_int8, k_scale = quant_k_int8(k, km, qk_quant_gran, tensor_layout)
+    gran = SAB_GRAN_PER_WARP if qk_quant_gran == "per_warp" else SAB_GRAN_PER_THREAD
+    return km, q_int8, q_scale, k_int8, k_scale, gran, gran, 0
+
+
+def _attn_dense(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range, backend,
+                return_lse):
+    """Quantisers + attention kernel of a dense entry point on head-dim-padded q, k, v.  kind: "fp8" (FP8 PV, V range v_range),
+    "fp16_cuda" (FP16 PV, per-warp / per-thread INT8) or "fp16_triton" (FP16 PV, per-block INT8 with sm_scale*log2e folded into
+    q).  Returns (o, the kernel's log2 lse or an empty tensor, km)."""
+    km, q_int8, q_scale, k_int8, k_scale, q_gran, k_gran, fold = _quant_qk(q, k, kind, tensor_layout, qk_quant_gran, sm_scale,
+                                                                          smooth_k, backend)
+    lay = 0 if tensor_layout == "NHD" else 1
+    o = torch.empty(q.size(), dtype=q.dtype, device=q.device)
+    if kind == "fp8":
+        v_fp8, v_scale, vm = per_channel_fp8(v, tensor_layout=tensor_layout, scale_max=v_range, smooth_v=smooth_v)
+        lse = ops.qk_int8_sv_f8_attn(q_int8, k_int8, v_fp8, o, q_scale, k_scale, v_scale, vm, lay, 1 if is_causal else 0,
+                                     q_gran, k_gran, sm_scale, fold, 1 if return_lse else 0)
+    else:
+        v_t = transpose_v_f16(v, tensor_layout=tensor_layout)       # `v.to(torch.float16)`, core.py:297-298, 603
+        lse = ops.qk_int8_sv_f16_attn(q_int8, k_int8, v_t, o, q_scale, k_scale, lay, 1 if is_causal else 0, q_gran, k_gran,
+                                      sm_scale, fold, 1 if return_lse else 0)
+    return o, lse, km
+
+
+class _SageAttnFunction(torch.autograd.Function):
+    """A dense entry point with a gradient: the gradient of attention evaluated at the forward's quantised logits, a
+    straight-through estimator through the INT8 Q/K, FP8 V and FP8 P roundings (include/sageattn_b200.h, sab_qk_int8_attn_bwd).
+    forward: the unchanged forward with the kernel LSE enabled; saves q, k, v, o and the raw LSE.  backward: re-runs the
+    (deterministic) Q/K quantisers instead of saving their 8-bit outputs, then the two gradient kernels.  The LSE and the K mean
+    are returned for the LSE correction and carry no gradient."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range, backend):
+        o, lse, km = _attn_dense(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range,
+                                 backend, True)
+        ctx.save_for_backward(q, k, v, o, lse)
+        ctx.cfg = (kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, backend)
+        km = km if km is not None else q.new_empty(0)
+        ctx.mark_non_differentiable(lse, km)
+        return o, lse, km
+
+    @staticmethod
+    def backward(ctx, do, _dlse, _dkm):
+        kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, backend = ctx.cfg
+        q, k, v, o, lse = ctx.saved_tensors
+        km, q_int8, q_scale, k_int8, k_scale, q_gran, k_gran, fold = _quant_qk(q, k, kind, tensor_layout, qk_quant_gran, sm_scale,
+                                                                             smooth_k, backend)
+        # the kernels read 16-bit rows with 16-byte loads; dq / dk / dv take the strides of q / k / v
+        q, k, v, o, do = (t.contiguous() for t in (q, k, v, o, do))
+        dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        ops.qk_int8_attn_bwd(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv,
+                             0 if tensor_layout == "NHD" else 1, 1 if is_causal else 0, q_gran, k_gran, sm_scale, fold)
+        return dq, dk, dv, None, None, None, None, None, None, None, None, None
+
+
+def _dense_call(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range, backend,
+                return_lse, head_dim_og):
+    """Shared tail of the dense entry points (q, k, v already head-dim padded).  The differentiable form runs only when grad mode
+    is on and q, k or v requires grad; otherwise the forward's launches and bytes are exactly those of the plain call.  The
+    returned lse never carries a gradient."""
+    if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
+        o, lse, km = _SageAttnFunction.apply(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v,
+                                             v_range, backend)
+        q = q.detach()
+    else:
+        o, lse, km = _attn_dense(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range,
+                                 backend, return_lse)
+    o = o[..., :head_dim_og]
+    if return_lse:
+        if smooth_k:
+            return o, lse / _LOG2E + _lse_correction(q, km, tensor_layout) * sm_scale
+        return o, lse / _LOG2E
+    return o
+
+
 def sageattn_qk_int8_pv_fp8_cuda(
     q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, tensor_layout: str = "HND", is_causal: bool = False,
     qk_quant_gran: str = "per_thread", sm_scale: Optional[float] = None, pv_accum_dtype: str = "fp32+fp16",
@@ -64,7 +150,6 @@ def sageattn_qk_int8_pv_fp8_cuda(
     quantisation range: 2.25 for "fp32+fp16", 448 otherwise (core.py:805-807).  smooth_v is honoured
     only for "fp32" (core.py:797-803).  Unknown values raise (the reference silently returns an
     uninitialised tensor)."""
-    dtype = q.dtype
     _check_inputs(q, k, v)
     assert qk_quant_gran in ["per_warp", "per_thread"], "qk_quant_gran must be either 'per_warp' or 'per_thread'."
     if pv_accum_dtype not in ("fp32", "fp32+fp32", "fp32+fp16"):
@@ -81,30 +166,14 @@ def sageattn_qk_int8_pv_fp8_cuda(
     if sm_scale is None:
         sm_scale = head_dim_og ** -0.5
 
-    # front-end: K mean (2 launches), Q / K quantisers, V statistics (2) + FP8 quantiser — 7 launches (reference: 6 + k.mean, core.py:773-809).
-    # The single-launch cluster variants (quant.smooth_quant_k, per_channel_fp8(fused=True)) are opt-in.
-    lse_correction = None
-    km = k_mean(k, tensor_layout) if smooth_k else None
-    if smooth_k and return_lse:
-        lse_correction = _lse_correction(q, km, tensor_layout)
-    q_int8, q_scale = quant_q_int8(q, qk_quant_gran, tensor_layout)
-    k_int8, k_scale = quant_k_int8(k, km, qk_quant_gran, tensor_layout)
-    gran = SAB_GRAN_PER_WARP if qk_quant_gran == "per_warp" else SAB_GRAN_PER_THREAD
-
-    o = torch.empty(q.size(), dtype=dtype, device=q.device)
-
     if pv_accum_dtype in ("fp32+fp32", "fp32+fp16") and smooth_v:
         warnings.warn(f"pv_accum_dtype is '{pv_accum_dtype}', smooth_v will be ignored.")
         smooth_v = False
     quant_v_scale_max = 2.25 if pv_accum_dtype == "fp32+fp16" else 448.0
-    v_fp8, v_scale, vm = per_channel_fp8(v, tensor_layout=tensor_layout, scale_max=quant_v_scale_max, smooth_v=smooth_v)
-
-    lse = ops.qk_int8_sv_f8_attn(q_int8, k_int8, v_fp8, o, q_scale, k_scale, v_scale, vm, _tensor_layout,
-                                 1 if is_causal else 0, gran, gran, sm_scale, 0, 1 if return_lse else 0)
-    o = o[..., :head_dim_og]
-    if return_lse:
-        return o, lse / _LOG2E + lse_correction * sm_scale if smooth_k else lse / _LOG2E
-    return o
+    # front-end: K mean (2 launches), Q / K quantisers, V statistics (2) + FP8 quantiser — 7 launches (reference: 6 + k.mean, core.py:773-809).
+    # The single-launch cluster variants (quant.smooth_quant_k, per_channel_fp8(fused=True)) are opt-in.
+    return _dense_call(q, k, v, "fp8", tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, quant_v_scale_max,
+                       "cuda", return_lse, head_dim_og)
 
 
 def sageattn(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, tensor_layout: str = "HND", is_causal: bool = False,
@@ -153,6 +222,14 @@ def sageattn_qk_int8_pv_fp16_triton(q, k, v, tensor_layout: str = "HND", quantiz
     _tensor_layout = 0 if tensor_layout == "NHD" else 1
     q, k, v, head_dim_og = _pad_head_dim(q, k, v)
     assert q.stride(-1) == 1 and k.stride(-1) == 1 and v.stride(-1) == 1, "Last dim of qkv must be contiguous."
+    if sm_scale is None:
+        sm_scale = 1.0 / (head_dim_og ** 0.5)
+    if quantization_backend not in ("triton", "cuda"):
+        raise ValueError(f"Unsupported quantization backend: {quantization_backend}")
+    if attn_mask is None:
+        return _dense_call(q, k, v, "fp16_triton", tensor_layout, is_causal, "per_block", sm_scale, smooth_k, False, 0.0,
+                           quantization_backend, return_lse, head_dim_og)
+    # attn_mask: forward only
     lse_correction = None
     if smooth_k:
         km = k_mean(k, tensor_layout)
@@ -160,28 +237,20 @@ def sageattn_qk_int8_pv_fp16_triton(q, k, v, tensor_layout: str = "HND", quantiz
             lse_correction = _lse_correction(q, km, tensor_layout)
     else:
         km = None
-    if sm_scale is None:
-        sm_scale = 1.0 / (head_dim_og ** 0.5)
-    if quantization_backend not in ("triton", "cuda"):
-        raise ValueError(f"Unsupported quantization backend: {quantization_backend}")
     q_int8, q_scale, k_int8, k_scale = per_block_int8(q, k, km=km, sm_scale=sm_scale, tensor_layout=tensor_layout,
                                                       semantics=quantization_backend)
     v_t = transpose_v_f16(v, tensor_layout=tensor_layout)       # `v.to(torch.float16)`, core.py:297-298
     o = torch.empty(q.size(), dtype=dtype, device=q.device)
-    if attn_mask is not None:
-        if tensor_layout == "HND":
-            target_shape = (q.shape[0], q.shape[1], q.shape[2], k.shape[2])
-        else:
-            target_shape = (q.shape[0], q.shape[2], q.shape[1], k.shape[1])
-        try:
-            attn_mask = attn_mask.expand(target_shape)     # core.py:314-323; a view: broadcast dims get stride 0
-        except Exception:
-            raise AssertionError(f"attn_mask shape {attn_mask.shape} cannot be broadcast to {target_shape}")
-        lse = ops.qk_int8_sv_f16_attn_masked(q_int8, k_int8, v_t, o, q_scale, k_scale, attn_mask, _tensor_layout,
-                                             SAB_GRAN_PER_BLOCK, SAB_GRAN_PER_BLOCK, sm_scale, 1, 1 if return_lse else 0)
+    if tensor_layout == "HND":
+        target_shape = (q.shape[0], q.shape[1], q.shape[2], k.shape[2])
     else:
-        lse = ops.qk_int8_sv_f16_attn(q_int8, k_int8, v_t, o, q_scale, k_scale, _tensor_layout, 1 if is_causal else 0,
-                                      SAB_GRAN_PER_BLOCK, SAB_GRAN_PER_BLOCK, sm_scale, 1, 1 if return_lse else 0)
+        target_shape = (q.shape[0], q.shape[2], q.shape[1], k.shape[1])
+    try:
+        attn_mask = attn_mask.expand(target_shape)     # core.py:314-323; a view: broadcast dims get stride 0
+    except Exception:
+        raise AssertionError(f"attn_mask shape {attn_mask.shape} cannot be broadcast to {target_shape}")
+    lse = ops.qk_int8_sv_f16_attn_masked(q_int8, k_int8, v_t, o, q_scale, k_scale, attn_mask, _tensor_layout,
+                                         SAB_GRAN_PER_BLOCK, SAB_GRAN_PER_BLOCK, sm_scale, 1, 1 if return_lse else 0)
     o = o[..., :head_dim_og]
     if return_lse:
         return o, lse / _LOG2E + lse_correction * sm_scale if smooth_k else lse / _LOG2E
@@ -199,7 +268,6 @@ def sageattn_qk_int8_pv_fp16_cuda(q, k, v, tensor_layout: str = "HND", is_causal
     core.py:601-617): the kernel always accumulates PV in fp32, i.e. every mode gets the accuracy of "fp32".
     smooth_v exists in the reference only to protect the "fp16" accumulator from overflow (core.py:606-610); with fp32
     accumulation it has nothing to do, so it is accepted and ignored with the reference's warning."""
-    dtype = q.dtype
     _check_inputs(q, k, v)
     assert qk_quant_gran in ["per_warp", "per_thread"], "qk_quant_gran must be either 'per_warp' or 'per_thread'."
     if pv_accum_dtype not in ("fp32", "fp16", "fp16+fp32"):
@@ -214,23 +282,10 @@ def sageattn_qk_int8_pv_fp16_cuda(q, k, v, tensor_layout: str = "HND", is_causal
         assert q.size(seq_dim) == k.size(seq_dim), "qo_len and kv_len must be equal for causal attention."
     if sm_scale is None:
         sm_scale = head_dim_og ** -0.5
-    lse_correction = None
-    km = k_mean(k, tensor_layout) if smooth_k else None
-    if smooth_k and return_lse:
-        lse_correction = _lse_correction(q, km, tensor_layout)
-    q_int8, q_scale = quant_q_int8(q, qk_quant_gran, tensor_layout)
-    k_int8, k_scale = quant_k_int8(k, km, qk_quant_gran, tensor_layout)
-    gran = SAB_GRAN_PER_WARP if qk_quant_gran == "per_warp" else SAB_GRAN_PER_THREAD
     if smooth_v:
         warnings.warn(f"pv_accum_dtype is '{pv_accum_dtype}' (fp32 accumulation on this backend), smooth_v will be ignored.")
-    v_t = transpose_v_f16(v, tensor_layout=tensor_layout)       # `v.to(torch.float16)`, core.py:603
-    o = torch.empty(q.size(), dtype=dtype, device=q.device)
-    lse = ops.qk_int8_sv_f16_attn(q_int8, k_int8, v_t, o, q_scale, k_scale, _tensor_layout, 1 if is_causal else 0,
-                                  gran, gran, sm_scale, 0, 1 if return_lse else 0)
-    o = o[..., :head_dim_og]
-    if return_lse:
-        return o, lse / _LOG2E + lse_correction * sm_scale if smooth_k else lse / _LOG2E
-    return o
+    return _dense_call(q, k, v, "fp16_cuda", tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, False, 0.0, "cuda",
+                       return_lse, head_dim_og)
 
 
 def sageattn_varlen(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu_seqlens_q: torch.Tensor,

@@ -152,11 +152,7 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   for (int i = 0; i < 2; ++i) {
     const int row = row0 + 8 * i;
     q_row[i] = qt * BM + row;  // row index inside the sequence
-    // per-row Q dequant scale (qk_int_sv_f8_cuda_sm89.cuh:98-114)
-    int q_idx = (q_blk0 + qt) * p.q_mult;
-    if (p.q_gran == SAB_GRAN_PER_WARP) q_idx += row >> 5;
-    if (p.q_gran == SAB_GRAN_PER_THREAD) q_idx += (row >> 5) * 8 + (row & 7);
-    qss[i] = qs_base[int64_t(q_idx) * p.qs_stride_idx] * p.sm_scale_log2;
+    qss[i] = q_dequant_log2(p, qs_base, q_blk0 + qt, row);
   }
   const float tau = p.lazy_tau;
   float m[2] = {kMaskValue, kMaskValue};   // running max (log2 units, includes the -8.807 offset on the fp8 path)
@@ -180,7 +176,7 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     {
       // dequant coefficient (…sm89.cuh:116-132, 255-257); tile j == 64-key block j.  Per-thread K scales: the keys of lane t
       // (8i+2t, 8i+2t+1) are all in scale group t.
-      const float ksv = ks_base[int64_t((k_blk0 + j) * (kKT ? 4 : 1) + (kKT ? t : 0)) * p.ks_stride_idx];
+      const float ksv = k_dequant<kKT>(p, ks_base, k_blk0 + j, t);
       coef[0] = ksv * qss[0];
       coef[1] = ksv * qss[1];
     }
@@ -254,14 +250,13 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         alpha[i] = (m_new != m[i]) ? ex2_approx(m[i] - m_new) : 1.0f;
         d[i] *= alpha[i];
         m[i] = m_new;
-        // ---- P = exp2(S*coef - m_new); I2FP is exact (|S| < 2^24) and the FMA is the reference's fmaf(S, sm_scale', -m)
-        //      (attn_utils.cuh:450), so P is bit-identical to the reference kernel's at the same m
+        // ---- P = exp2(S*coef - m_new), bit-identical to the reference kernel's at the same m (logit_log2)
         const float nm = -m_new;
         float sum = 0.f;
 #pragma unroll
         for (int c = 0; c < 16; c += 2) {
           const int idx = 4 * (c >> 1) + 2 * i;
-          const float y0 = fmaf(__int2float_rn(int(s[idx])), coef[i], nm), y1 = fmaf(__int2float_rn(int(s[idx + 1])), coef[i], nm);
+          const float y0 = logit_log2(s[idx], coef[i], nm), y1 = logit_log2(s[idx + 1], coef[i], nm);
           float x[2];
 #ifdef SAB_POLY_EXP_PAIRS
           if (t < SAB_POLY_EXP_PAIRS) {   // column pair t of every 8 columns

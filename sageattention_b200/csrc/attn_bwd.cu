@@ -1,0 +1,490 @@
+// Backward of the INT8-QK attention for sm_90a (H100): the gradient of softmax(S) V evaluated at the forward's quantised logits, a
+// straight-through estimator through the INT8 Q/K, FP8 V and FP8 P roundings:
+//   S  = dequant(q8 k8^T) * sm_scale        (logit_log2, attn_common.cuh: the forward kernel's logits to the bit)
+//   P  = exp2(S*log2e - lse)                 (lse: the forward kernel's own log2 LSE, before the smoothing correction)
+//   dV = P^T dO    dP = dO V^T    delta = rowsum(dO o O)    dS = P o (dP - delta)
+//   dQ = dS K * sm_scale    dK = dS^T Q * sm_scale            (Q, K, V: the original 16-bit tensors)
+// K smoothing needs no term: the rows of dS sum to zero, so the K mean drops out of dQ and dK.  S is still recomputed from the
+// smoothed k8, because the LSE is relative to it, and dQ is taken with the smoothed K (K - mean, rounded to the input dtype): with
+// delta from the quantised forward's O the rows of dS sum to a small residue, which K itself would multiply by its mean.
+//
+// Three launches on the caller's stream, no atomics, so the gradients are bit-reproducible:
+//   bwd_delta_kernel : delta of every Q row (fp32) into the caller's workspace;
+//   bwd_dq_kernel    : one CTA per 128-row Q tile of one (batch, Q head), shaped like the forward: two warpgroups of 64 rows, a loop
+//                      over 64-key tiles; S = Q K^T (INT8), dP = dO V^T, dQ += dS K with dS as the register A operand;
+//   bwd_dkdv_kernel  : one CTA per 128-key tile of one (batch, KV head), two warpgroups of 64 keys, a loop over every Q head of the
+//                      GQA group and every 64-row Q tile, so dK and dV are written once.  S^T = K Q^T (INT8) and dP^T = V dO^T put
+//                      P^T and dS^T in the accumulator layout; rounded to the input dtype they are the register A operand of
+//                      dV += P^T dO and dK += dS^T Q.
+// Products are wgmma with fp32 accumulation: INT8 for S as in the forward, bf16 / f16 for the rest.  Every B operand is K-major in
+// shared memory, in the swizzled layout the forward's TMA loads write; the operands the math needs transposed (dO^T, Q^T, K^T) are
+// transposed by the loaders.  Loads are plain: all threads copy a tile, the CTA synchronises, then computes (no load/compute
+// overlap yet).
+#include <type_traits>
+#include "attn_common.cuh"
+
+namespace sab {
+
+constexpr int kBwdThreads = 256;   // two warpgroups
+
+struct BwdParams {
+  AttnParams a;                    // the forward's scale / size / causal parameters (a.lse, a.out unused)
+  const int8_t* q8;
+  const int8_t* k8;
+  int64_t q8_sb, q8_sh, q8_ss, k8_sb, k8_sh, k8_ss;
+  const uint16_t* q;               // 16-bit tensors (bf16 / f16 bits); dq / dk / dv have the strides of q / k / v
+  const uint16_t* k;
+  const uint16_t* v;
+  const uint16_t* o;
+  const uint16_t* dout;
+  const uint16_t* kmean;           // nullable [B,Hkv,D]: the K smoothing mean, subtracted from the K of dQ += dS K
+  int64_t q_sb, q_sh, q_ss, k_sb, k_sh, k_ss, v_sb, v_sh, v_ss, o_sb, o_sh, o_ss, do_sb, do_sh, do_ss;
+  const float* lse;                // [B,Hq,Sq] log2 units
+  float* delta;                    // [B,Hq,Sq] workspace
+  void* dq;
+  void* dk;
+  void* dv;
+  float sm_scale;
+};
+
+// Byte offset of 16-byte chunk c of row r in a K-major tile of `rows` rows of RB bytes, laid out as a TMA load with swizzle
+// min(RB, 128) writes it: 128-byte column slabs (a longer row continues in the next slab), Swizzle<., 4, 3> inside a slab
+// (address bits [4, 7) ^= bits [7, 10)).  Tile bases are 1024-byte aligned.
+template <int RB>
+__device__ __forceinline__ uint32_t tile_off(int r, int c, int rows) {
+  constexpr int SW = RB < 128 ? RB : 128;
+  constexpr int CPS = SW / 16;
+  const uint32_t o = uint32_t(r) * SW + uint32_t(c % CPS) * 16;
+  return uint32_t(c / CPS) * uint32_t(rows) * SW + (o ^ (((o >> 7) & (CPS - 1)) << 4));
+}
+// wgmma descriptor of rows [r0, r0 + 64) of such a tile, at byte kb along K (one instruction's 32-byte K extent, inside a slab)
+template <int RB>
+__device__ __forceinline__ uint64_t tile_desc(const uint8_t* tile, int rows, int r0, int kb) {
+  constexpr int SW = RB < 128 ? RB : 128;
+  return make_wgmma_desc<SW>(smem_u32(tile + (kb / SW) * rows * SW + r0 * SW)) + uint64_t((kb % SW) >> 4);
+}
+
+// rows [row0, row0 + R) of one (b, h) of a bhsd tensor (E-byte elements, row stride ss elements) into a K-major tile; rows >= limit
+// read as zeros
+template <int R, int D, int E>
+__device__ __forceinline__ void load_tile(uint8_t* tile, const void* base, int64_t ss, int row0, int limit) {
+  constexpr int RB = D * E, CPR = RB / 16;
+  const uint8_t* src = reinterpret_cast<const uint8_t*>(base);
+  for (int idx = threadIdx.x; idx < R * CPR; idx += kBwdThreads) {
+    const int r = idx / CPR, c = idx % CPR;
+    uint4 x = make_uint4(0u, 0u, 0u, 0u);
+    if (row0 + r < limit) x = __ldg(reinterpret_cast<const uint4*>(src + int64_t(row0 + r) * ss * E) + c);
+    *reinterpret_cast<uint4*>(tile + tile_off<RB>(r, c, R)) = x;
+  }
+}
+template <typename T>
+__device__ __forceinline__ uint32_t sub_rn(uint32_t x, float m) {   // 16-bit x - m, rounded to T
+  if constexpr (std::is_same_v<T, __half>) return __half_as_ushort(__float2half_rn(__half2float(__ushort_as_half(uint16_t(x))) - m));
+  else return __bfloat16_as_ushort(__float2bfloat16_rn(__bfloat162float(__ushort_as_bfloat16(uint16_t(x))) - m));
+}
+// the same 64 rows of 16-bit elements transposed: tile row d (128 bytes) holds column d of the 64 rows.  sub (nullable, [D]): a
+// per-column value subtracted in fp32 and rounded to T
+template <int D, typename T>
+__device__ __forceinline__ void load_tile_t(uint8_t* tile, const uint16_t* base, int64_t ss, int row0, int limit,
+                                            const uint16_t* sub = nullptr) {
+  for (int idx = threadIdx.x; idx < D * 8; idx += kBwdThreads) {
+    const int d = idx % D, c = idx / D;   // consecutive threads read consecutive columns of one row
+    float m = 0.f;
+    if (sub != nullptr) {
+      if constexpr (std::is_same_v<T, __half>) m = __half2float(__ushort_as_half(sub[d]));
+      else m = __bfloat162float(__ushort_as_bfloat16(sub[d]));
+    }
+    uint32_t w[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int r = row0 + 8 * c + 2 * j;
+      uint32_t lo = r < limit ? __ldg(base + int64_t(r) * ss + d) : 0u;
+      uint32_t hi = r + 1 < limit ? __ldg(base + int64_t(r + 1) * ss + d) : 0u;
+      if (sub != nullptr) {
+        lo = r < limit ? sub_rn<T>(lo, m) : 0u;
+        hi = r + 1 < limit ? sub_rn<T>(hi, m) : 0u;
+      }
+      w[j] = lo | (hi << 16);
+    }
+    *reinterpret_cast<uint4*>(tile + tile_off<128>(d, c, D)) = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
+template <typename T>
+__device__ __forceinline__ void wgmma_ss(float (&d)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  if constexpr (std::is_same_v<T, __half>) wgmma_ss_f16(d, a_desc, b_desc, accumulate);
+  else wgmma_ss_bf16(d, a_desc, b_desc, accumulate);
+}
+template <typename T, int N>
+__device__ __forceinline__ void wgmma_rs(float (&d)[N], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+  if constexpr (std::is_same_v<T, __half>) wgmma_pv_f16(d, a, b_desc, accumulate);
+  else wgmma_rs_bf16(d, a, b_desc, accumulate);
+}
+// 64 x 64 fp32 accumulator tile -> A fragments of four k16 steps: step kk = accumulator blocks 2kk, 2kk+1 (same layout, no exchange)
+template <typename T>
+__device__ __forceinline__ void acc_to_a(const float (&e)[32], uint32_t (&a)[4][4]) {
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    const int i0 = 8 * kk, i1 = 8 * kk + 4;
+    a[kk][0] = pack2<T>(e[i0], e[i0 + 1]);
+    a[kk][1] = pack2<T>(e[i0 + 2], e[i0 + 3]);
+    a[kk][2] = pack2<T>(e[i1], e[i1 + 1]);
+    a[kk][3] = pack2<T>(e[i1 + 2], e[i1 + 3]);
+  }
+}
+// rows r, r + 8 of a 64 x D fp32 accumulator tile (times `scale`) -> 16-bit row-major memory
+template <typename T, int D>
+__device__ __forceinline__ void store_rows(const float (&acc)[D / 2], T* row0, T* row1, bool ok0, bool ok1, int t, float scale) {
+#pragma unroll
+  for (int nb = 0; nb < D / 8; ++nb) {
+    const int col = 8 * nb + 2 * t;
+    if (ok0) *reinterpret_cast<uint32_t*>(row0 + col) = pack2<T>(acc[4 * nb] * scale, acc[4 * nb + 1] * scale);
+    if (ok1) *reinterpret_cast<uint32_t*>(row1 + col) = pack2<T>(acc[4 * nb + 2] * scale, acc[4 * nb + 3] * scale);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ delta = rowsum(dO o O)
+// one warp per Q row, fixed summation order
+template <typename T>
+__global__ void __launch_bounds__(256) bwd_delta_kernel(const __grid_constant__ BwdParams p, int D) {
+  const int64_t row = int64_t(blockIdx.x) * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= int64_t(p.a.B) * p.a.Hq * p.a.Sq) return;
+  const int s = int(row % p.a.Sq), h = int((row / p.a.Sq) % p.a.Hq), b = int(row / (int64_t(p.a.Sq) * p.a.Hq));
+  const T* o = reinterpret_cast<const T*>(p.o) + b * p.o_sb + h * p.o_sh + s * p.o_ss;
+  const T* g = reinterpret_cast<const T*>(p.dout) + b * p.do_sb + h * p.do_sh + s * p.do_ss;
+  float acc = 0.f;
+  for (int d = 2 * lane; d < D; d += 64) {
+    acc = fmaf(float(o[d]), float(g[d]), acc);
+    acc = fmaf(float(o[d + 1]), float(g[d + 1]), acc);
+  }
+#pragma unroll
+  for (int x = 16; x > 0; x >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, x);
+  if (lane == 0) p.delta[row] = acc;
+}
+
+// ------------------------------------------------------------------------------------------------ dQ
+template <int D>
+constexpr size_t bwd_dq_smem_bytes() {
+  return size_t(128) * D + size_t(128) * D * 2 + size_t(64) * D + size_t(64) * D * 2 + size_t(D) * 64 * 2 + 1024;
+}
+
+template <int D, bool kKT, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_kernel(const __grid_constant__ BwdParams p) {
+  constexpr int QB = 128, KB = 64;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* sQ8 = smem;                       // [128 x D] int8        A of S = Q K^T
+  uint8_t* sdO = sQ8 + QB * D;               // [128 x D] 16-bit      A of dP = dO V^T
+  uint8_t* sK8 = sdO + QB * D * 2;           // [64 x D] int8         B of S
+  uint8_t* sV = sK8 + KB * D;                // [64 x D] 16-bit       B of dP
+  uint8_t* sKt = sV + KB * D * 2;            // [D x 64] 16-bit       B of dQ += dS K
+  const AttnParams& a = p.a;
+
+  int qt = blockIdx.x;
+  if (a.causal) qt = a.n_q_tiles - 1 - qt;   // heaviest tiles first
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int hk = h / (a.Hq / a.Hkv);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2, t = lane & 3;
+  const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // rows row0, row0 + 8 of the Q tile (forward's accumulator layout)
+
+  if ((smem_u32(smem) & 1023u) != 0) __trap();
+  load_tile<QB, D, 1>(sQ8, p.q8 + b * p.q8_sb + h * p.q8_sh, p.q8_ss, qt * QB, a.Sq);
+  load_tile<QB, D, 2>(sdO, p.dout + b * p.do_sb + h * p.do_sh, p.do_ss, qt * QB, a.Sq);
+
+  const float* qs_base = a.q_scale + (int64_t(b) * a.Hq + h) * a.qs_stride_bh;
+  const float* ks_base = a.k_scale + (int64_t(b) * a.Hkv + hk) * a.ks_stride_bh;
+  int q_row[2];
+  float qss[2], nlse[2], dlt[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    q_row[i] = qt * QB + row0 + 8 * i;
+    qss[i] = q_dequant_log2(a, qs_base, qt, row0 + 8 * i);   // scales are padded to whole 128-row blocks
+    const bool ok = q_row[i] < a.Sq;
+    const int64_t li = (int64_t(b) * a.Hq + h) * a.Sq + q_row[i];
+    nlse[i] = ok ? -p.lse[li] : 0.f;
+    dlt[i] = ok ? p.delta[li] : 0.f;
+  }
+  int n_kv = (a.Sk + KB - 1) / KB;
+  if (a.causal) n_kv = min(n_kv, ((qt + 1) * QB + KB - 1) / KB);
+
+  float dq[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) dq[i] = 0.f;
+
+  for (int j = 0; j < n_kv; ++j) {
+    __syncthreads();   // the previous tile's operands are consumed
+    load_tile<KB, D, 1>(sK8, p.k8 + b * p.k8_sb + hk * p.k8_sh, p.k8_ss, j * KB, a.Sk);
+    load_tile<KB, D, 2>(sV, p.v + b * p.v_sb + hk * p.v_sh, p.v_ss, j * KB, a.Sk);
+    // K - mean: the same product in exact arithmetic (the rows of dS sum to zero), but the residue that delta = rowsum(dO o O) of
+    // the quantised forward leaves in those row sums is not multiplied by a large K mean
+    load_tile_t<D, T>(sKt, p.k + b * p.k_sb + hk * p.k_sh, p.k_ss, j * KB, a.Sk,
+                      p.kmean ? p.kmean + (int64_t(b) * a.Hkv + hk) * D : nullptr);
+    fence_proxy_async_smem();   // generic-proxy stores -> visible to wgmma
+    __syncthreads();
+
+    uint32_t s[32];
+    float dp[32];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < D / 32; ++k) wgmma_qk_i8(s, tile_desc<D>(sQ8, QB, wg * 64, 32 * k), tile_desc<D>(sK8, KB, 0, 32 * k), k > 0);
+#pragma unroll
+    for (int k = 0; k < D / 16; ++k) wgmma_ss<T>(dp, tile_desc<2 * D>(sdO, QB, wg * 64, 32 * k), tile_desc<2 * D>(sV, KB, 0, 32 * k), k > 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(s);
+    fence_regs(dp);
+
+    float coef[2];
+    int limit[2];
+    const float ksv = k_dequant<kKT>(a, ks_base, j, t);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      coef[i] = ksv * qss[i];
+      limit[i] = q_row[i] < a.Sq ? a.Sk - j * KB : 0;
+      if (a.causal) limit[i] = min(limit[i], q_row[i] - j * KB + 1);
+    }
+    float ds[32];
+#pragma unroll
+    for (int c = 0; c < 16; ++c) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int idx = 4 * (c >> 1) + 2 * i + (c & 1);
+        const int key = 8 * (c >> 1) + 2 * t + (c & 1);
+        const float pe = key < limit[i] ? ex2_approx(logit_log2(s[idx], coef[i], nlse[i])) : 0.f;
+        ds[idx] = pe * (dp[idx] - dlt[i]);
+      }
+    }
+    uint32_t da[4][4];
+    acc_to_a<T>(ds, da);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_rs<T>(dq, da[kk], tile_desc<128>(sKt, D, 0, 32 * kk), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(dq);
+  }
+
+  T* base = reinterpret_cast<T*>(p.dq) + b * p.q_sb + h * p.q_sh;
+  store_rows<T, D>(dq, base + int64_t(q_row[0]) * p.q_ss, base + int64_t(q_row[1]) * p.q_ss, q_row[0] < a.Sq, q_row[1] < a.Sq, t,
+                   p.sm_scale);
+}
+
+// ------------------------------------------------------------------------------------------------ dK, dV
+template <int D>
+constexpr size_t bwd_dkdv_smem_bytes() {
+  return size_t(128) * D + size_t(128) * D * 2 + size_t(64) * D + size_t(64) * D * 2 + 2 * size_t(D) * 64 * 2 + 3 * 64 * 4 + 1024;
+}
+
+template <int D, bool kKT, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_kernel(const __grid_constant__ BwdParams p) {
+  constexpr int KB = 128, QB = 64;
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* sK8 = smem;                       // [128 x D] int8        A of S^T = K Q^T
+  uint8_t* sV = sK8 + KB * D;                // [128 x D] 16-bit      A of dP^T = V dO^T
+  uint8_t* sQ8 = sV + KB * D * 2;            // [64 x D] int8         B of S^T
+  uint8_t* sdO = sQ8 + QB * D;               // [64 x D] 16-bit       B of dP^T
+  uint8_t* sdOt = sdO + QB * D * 2;          // [D x 64] 16-bit       B of dV += P^T dO
+  uint8_t* sQt = sdOt + D * QB * 2;          // [D x 64] 16-bit       B of dK += dS^T Q
+  float* s_qss = reinterpret_cast<float*>(sQt + D * QB * 2);   // per Q row of the tile: q dequant scale, -lse, delta
+  float* s_nlse = s_qss + QB;
+  float* s_dlt = s_nlse + QB;
+  const AttnParams& a = p.a;
+
+  const int k0 = blockIdx.x * KB, hk = blockIdx.y, b = blockIdx.z;
+  const int G = a.Hq / a.Hkv;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2, t = lane & 3;
+  const int kr = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // keys k0 + kr, k0 + kr + 8 (accumulator rows)
+
+  if ((smem_u32(smem) & 1023u) != 0) __trap();
+  load_tile<KB, D, 1>(sK8, p.k8 + b * p.k8_sb + hk * p.k8_sh, p.k8_ss, k0, a.Sk);
+  load_tile<KB, D, 2>(sV, p.v + b * p.v_sb + hk * p.v_sh, p.v_ss, k0, a.Sk);
+
+  const float* ks_base = a.k_scale + (int64_t(b) * a.Hkv + hk) * a.ks_stride_bh;
+  int key[2];
+  float ksr[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    key[i] = k0 + kr + 8 * i;
+    // per-thread K scales: key % 8 == lane / 4, so its scale group is lane / 8
+    ksr[i] = key[i] < a.Sk ? k_dequant<kKT>(a, ks_base, key[i] / 64, lane >> 3) : 0.f;
+  }
+  float dk[D / 2], dv[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) dk[i] = dv[i] = 0.f;
+
+  const int n_qt = (a.Sq + QB - 1) / QB;
+  const int qt0 = a.causal ? k0 / QB : 0;    // causal (Sq == Skv): rows before the first key see none of this tile
+  for (int hh = 0; hh < G; ++hh) {
+    const int h = hk * G + hh;
+    const float* qs_base = a.q_scale + (int64_t(b) * a.Hq + h) * a.qs_stride_bh;
+    for (int qt = qt0; qt < n_qt; ++qt) {
+      const int q0 = qt * QB;
+      __syncthreads();   // the previous tile's operands are consumed
+      load_tile<QB, D, 1>(sQ8, p.q8 + b * p.q8_sb + h * p.q8_sh, p.q8_ss, q0, a.Sq);
+      load_tile<QB, D, 2>(sdO, p.dout + b * p.do_sb + h * p.do_sh, p.do_ss, q0, a.Sq);
+      load_tile_t<D, T>(sdOt, p.dout + b * p.do_sb + h * p.do_sh, p.do_ss, q0, a.Sq);
+      load_tile_t<D, T>(sQt, p.q + b * p.q_sb + h * p.q_sh, p.q_ss, q0, a.Sq);
+      if (threadIdx.x < QB) {
+        const int r = q0 + threadIdx.x;
+        const bool ok = r < a.Sq;
+        const int64_t li = (int64_t(b) * a.Hq + h) * a.Sq + r;
+        s_qss[threadIdx.x] = ok ? q_dequant_log2(a, qs_base, r / 128, r % 128) : 0.f;
+        s_nlse[threadIdx.x] = ok ? -p.lse[li] : 0.f;
+        s_dlt[threadIdx.x] = ok ? p.delta[li] : 0.f;
+      }
+      fence_proxy_async_smem();
+      __syncthreads();
+
+      uint32_t s[32];
+      float dp[32];
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < D / 32; ++k) wgmma_qk_i8(s, tile_desc<D>(sK8, KB, wg * 64, 32 * k), tile_desc<D>(sQ8, QB, 0, 32 * k), k > 0);
+#pragma unroll
+      for (int k = 0; k < D / 16; ++k) wgmma_ss<T>(dp, tile_desc<2 * D>(sV, KB, wg * 64, 32 * k), tile_desc<2 * D>(sdO, QB, 0, 32 * k), k > 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(s);
+      fence_regs(dp);
+
+      // P^T and dS^T: accumulator row = key, column c = Q row q0 + c
+      float pt[32], dst[32];
+#pragma unroll
+      for (int c = 0; c < 16; ++c) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int idx = 4 * (c >> 1) + 2 * i + (c & 1);
+          const int col = 8 * (c >> 1) + 2 * t + (c & 1);
+          const int q = q0 + col;
+          const bool ok = key[i] < a.Sk && q < a.Sq && (!a.causal || key[i] <= q);
+          const float pe = ok ? ex2_approx(logit_log2(s[idx], ksr[i] * s_qss[col], s_nlse[col])) : 0.f;
+          pt[idx] = pe;
+          dst[idx] = pe * (dp[idx] - s_dlt[col]);
+        }
+      }
+      uint32_t pa[4][4], da[4][4];
+      acc_to_a<T>(pt, pa);
+      acc_to_a<T>(dst, da);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_rs<T>(dv, pa[kk], tile_desc<128>(sdOt, D, 0, 32 * kk), 1);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_rs<T>(dk, da[kk], tile_desc<128>(sQt, D, 0, 32 * kk), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(dv);
+      fence_regs(dk);
+    }
+  }
+
+  T* kb = reinterpret_cast<T*>(p.dk) + b * p.k_sb + hk * p.k_sh;
+  T* vb = reinterpret_cast<T*>(p.dv) + b * p.v_sb + hk * p.v_sh;
+  const bool ok0 = key[0] < a.Sk, ok1 = key[1] < a.Sk;
+  store_rows<T, D>(dk, kb + int64_t(key[0]) * p.k_ss, kb + int64_t(key[1]) * p.k_ss, ok0, ok1, t, p.sm_scale);
+  store_rows<T, D>(dv, vb + int64_t(key[0]) * p.v_ss, vb + int64_t(key[1]) * p.v_ss, ok0, ok1, t, 1.0f);
+}
+
+template <int D, bool kKT, typename T>
+static int launch_bwd(const BwdParams& p, cudaStream_t stream) {
+  const int64_t rows = int64_t(p.a.B) * p.a.Hq * p.a.Sq;
+  bwd_delta_kernel<T><<<unsigned((rows + 7) / 8), 256, 0, stream>>>(p, D);
+  SAB_CUDA_OK(cudaGetLastError());
+  {
+    constexpr size_t smem = bwd_dq_smem_bytes<D>();
+    auto kern = bwd_dq_kernel<D, kKT, T>;
+    static bool configured[64] = {};
+    if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
+    kern<<<dim3(p.a.n_q_tiles, p.a.Hq, p.a.B), kBwdThreads, smem, stream>>>(p);
+    SAB_CUDA_OK(cudaGetLastError());
+  }
+  {
+    constexpr size_t smem = bwd_dkdv_smem_bytes<D>();
+    auto kern = bwd_dkdv_kernel<D, kKT, T>;
+    static bool configured[64] = {};
+    if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
+    kern<<<dim3((p.a.Sk + 127) / 128, p.a.Hkv, p.a.B), kBwdThreads, smem, stream>>>(p);
+    SAB_CUDA_OK(cudaGetLastError());
+  }
+  return SAB_OK;
+}
+
+}  // namespace sab
+
+extern "C" int64_t sab_attn_bwd_workspace_bytes(int B, int Hq, int Sq) {
+  if (B <= 0 || Hq <= 0 || Sq <= 0) return 0;
+  return (int64_t(B) * Hq * Sq * 4 + 255) / 256 * 256;
+}
+
+extern "C" int sab_qk_int8_attn_bwd(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
+                                    const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
+                                    const void* k_mean, void* dq, void* dk, void* dv, void* workspace, int dtype, int B, int Hq, int Hkv, int Sq,
+                                    int Skv, int D, int64_t q8_stride_b, int64_t q8_stride_h, int64_t q8_stride_s,
+                                    int64_t k8_stride_b, int64_t k8_stride_h, int64_t k8_stride_s, int64_t q_stride_b,
+                                    int64_t q_stride_h, int64_t q_stride_s, int64_t k_stride_b, int64_t k_stride_h,
+                                    int64_t k_stride_s, int64_t v_stride_b, int64_t v_stride_h, int64_t v_stride_s,
+                                    int64_t o_stride_b, int64_t o_stride_h, int64_t o_stride_s, int64_t do_stride_b,
+                                    int64_t do_stride_h, int64_t do_stride_s, int is_causal, int q_gran, int k_gran,
+                                    float sm_scale, int fold_sm_scale, void* stream) {
+  using namespace sab;
+  SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
+              SAB_ERR_INVALID, "null tensor pointer");
+  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
+  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "dtype must be fp16 or bf16");
+  SAB_REQUIRE(B > 0 && Hq > 0 && Hkv > 0 && Sq > 0 && Skv > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", B, Hq, Hkv, Sq, Skv);
+  SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
+  SAB_REQUIRE(q_gran >= 1 && q_gran <= 3 && k_gran >= 1 && k_gran <= 3, SAB_ERR_INVALID, "unknown quant granularity q=%d k=%d", q_gran, k_gran);
+  SAB_REQUIRE(!is_causal || Sq == Skv, SAB_ERR_INVALID, "qo_len and kv_len must be equal for causal attention.");
+  const int64_t s16[] = {q_stride_b, q_stride_h, q_stride_s, k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s,
+                         o_stride_b, o_stride_h, o_stride_s, do_stride_b, do_stride_h, do_stride_s};
+  bool ok16 = aligned16(q) && aligned16(k) && aligned16(v) && aligned16(o) && aligned16(dout) && aligned16(dq) && aligned16(dk) && aligned16(dv);
+  for (int64_t s : s16) ok16 = ok16 && s % 8 == 0;
+  SAB_REQUIRE(ok16, SAB_ERR_INVALID, "16-bit tensors must be 16-byte aligned with strides multiple of 8 elements");
+  const int64_t s8[] = {q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s};
+  bool ok8 = aligned16(q_int8) && aligned16(k_int8);
+  for (int64_t s : s8) ok8 = ok8 && s % 16 == 0;
+  SAB_REQUIRE(ok8, SAB_ERR_INVALID, "int8 tensors must be 16-byte aligned with strides multiple of 16");
+  int st = sab_check_device();
+  if (st != SAB_OK) return st;
+
+  BwdParams p{};
+  AttnParams& a = p.a;
+  a.q_scale = q_scale; a.k_scale = k_scale;
+  a.B = B; a.Hq = Hq; a.Hkv = Hkv; a.Sq = Sq; a.Sk = Skv;
+  a.n_q_tiles = (Sq + BM - 1) / BM;
+  a.causal = is_causal ? 1 : 0;
+  a.sm_scale_log2 = fold_sm_scale ? 1.0f : sm_scale * 1.44269504088896340736f;   // as the forward (attn.cu)
+  a.q_gran = q_gran;
+  a.q_mult = q_gran == SAB_GRAN_PER_BLOCK ? 1 : (q_gran == SAB_GRAN_PER_WARP ? 4 : 32);
+  a.k_mult = k_gran == SAB_GRAN_PER_THREAD ? 4 : 1;
+  a.qs_stride_bh = int64_t((Sq + BM - 1) / BM) * a.q_mult;
+  a.ks_stride_bh = int64_t((Skv + 63) / 64) * a.k_mult;
+  a.qs_stride_idx = 1;
+  a.ks_stride_idx = 1;
+  p.q8 = q_int8; p.k8 = k_int8;
+  p.q8_sb = q8_stride_b; p.q8_sh = q8_stride_h; p.q8_ss = q8_stride_s;
+  p.k8_sb = k8_stride_b; p.k8_sh = k8_stride_h; p.k8_ss = k8_stride_s;
+  p.q = static_cast<const uint16_t*>(q); p.k = static_cast<const uint16_t*>(k); p.v = static_cast<const uint16_t*>(v);
+  p.o = static_cast<const uint16_t*>(o); p.dout = static_cast<const uint16_t*>(dout);
+  p.kmean = static_cast<const uint16_t*>(k_mean);
+  p.q_sb = q_stride_b; p.q_sh = q_stride_h; p.q_ss = q_stride_s;
+  p.k_sb = k_stride_b; p.k_sh = k_stride_h; p.k_ss = k_stride_s;
+  p.v_sb = v_stride_b; p.v_sh = v_stride_h; p.v_ss = v_stride_s;
+  p.o_sb = o_stride_b; p.o_sh = o_stride_h; p.o_ss = o_stride_s;
+  p.do_sb = do_stride_b; p.do_sh = do_stride_h; p.do_ss = do_stride_s;
+  p.lse = lse;
+  p.delta = static_cast<float*>(workspace);
+  p.dq = dq; p.dk = dk; p.dv = dv;
+  p.sm_scale = sm_scale;
+
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const bool kt = k_gran == SAB_GRAN_PER_THREAD;
+  const bool bf = dtype == SAB_DTYPE_BF16;
+  if (D == 128) {
+    if (kt) { if (bf) return launch_bwd<128, true, __nv_bfloat16>(p, s); return launch_bwd<128, true, __half>(p, s); }
+    if (bf) return launch_bwd<128, false, __nv_bfloat16>(p, s);
+    return launch_bwd<128, false, __half>(p, s);
+  }
+  if (kt) { if (bf) return launch_bwd<64, true, __nv_bfloat16>(p, s); return launch_bwd<64, true, __half>(p, s); }
+  if (bf) return launch_bwd<64, false, __nv_bfloat16>(p, s);
+  return launch_bwd<64, false, __half>(p, s);
+}

@@ -53,6 +53,27 @@ struct AttnParams {
   int seg_heads;               // KV heads per flag group
 };
 
+// ---- logits of the INT8 path.  The forward (attn.cu) and the backward (attn_bwd.cu) both evaluate them with these helpers: the
+// backward's P must be the forward's P, so the dequantised logit has one definition.
+// Dequant scale of Q row `row` (0..127) of 128-row scale block `blk`, times sm_scale*log2e (1 when folded into q)
+// (…sm89.cuh:98-114).
+__device__ __forceinline__ float q_dequant_log2(const AttnParams& p, const float* qs_base, int blk, int row) {
+  int q_idx = blk * p.q_mult;
+  if (p.q_gran == SAB_GRAN_PER_WARP) q_idx += row >> 5;
+  if (p.q_gran == SAB_GRAN_PER_THREAD) q_idx += (row >> 5) * 8 + (row & 7);
+  return qs_base[int64_t(q_idx) * p.qs_stride_idx] * p.sm_scale_log2;
+}
+// Dequant scale of 64-key block `blk`; per-thread K scales (kKT): of scale group `grp` = keys 8i+2grp, 8i+2grp+1 (…sm89.cuh:116-132).
+template <bool kKT>
+__device__ __forceinline__ float k_dequant(const AttnParams& p, const float* ks_base, int blk, int grp) {
+  return ks_base[int64_t(blk * (kKT ? 4 : 1) + (kKT ? grp : 0)) * p.ks_stride_idx];
+}
+// S * coef - m in log2 units for an int32 logit S, coef = k_dequant * q_dequant_log2.  I2FP is exact (|S| < 2^24) and the FMA is
+// the reference's fmaf(S, sm_scale', -m) (attn_utils.cuh:450).
+__device__ __forceinline__ float logit_log2(uint32_t s, float coef, float neg_m) {
+  return fmaf(__int2float_rn(int(s)), coef, neg_m);
+}
+
 __device__ __forceinline__ void mbar_wait_wd(uint64_t* bar, uint32_t parity) {
 #ifdef SAB_WATCHDOG
   // Debug build: bounded spin.  A wait that never completes reports itself (block 0 only) and is ABANDONED, so the kernel

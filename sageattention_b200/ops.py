@@ -302,6 +302,39 @@ def _(query, key, value, output, query_scale, key_scale, value_scale, cu_seqlens
     return None
 
 
+# ----------------------------------------------------------------------------------------------- backward
+@torch.library.custom_op("sageattention_b200::qk_int8_attn_bwd", mutates_args=("dq", "dk", "dv"), device_types="cuda")
+def qk_int8_attn_bwd(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale: torch.Tensor, k_scale: torch.Tensor, q: torch.Tensor,
+                     k: torch.Tensor, v: torch.Tensor, o: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor,
+                     k_mean: Optional[torch.Tensor], dq: torch.Tensor, dk: torch.Tensor, dv: torch.Tensor, tensor_layout: int,
+                     is_causal: int, q_quant_gran: int, k_quant_gran: int, sm_scale: float, fold_sm_scale: int) -> None:
+    """Gradients of the INT8-QK attention (include/sageattn_b200.h, sab_qk_int8_attn_bwd): q_int8 / k_int8 / scales / granularities /
+    sm_scale / fold_sm_scale as the forward call received them, q / k / v the unquantised (k unsmoothed) 16-bit inputs, o and dout
+    the forward output and its gradient, lse the forward kernel's raw [B,Hq,Sq] log2 LSE, k_mean the K smoothing mean (any shape
+    with B*Hkv*D elements, k's dtype; None without smoothing).  dq / dk / dv must have the strides of q / k / v."""
+    B, Hq, Sq, D = _bhsd(q, tensor_layout)
+    _, Hkv, Skv, _ = _bhsd(k, tensor_layout)
+    for x, y in ((dq, q), (dk, k), (dv, v)):
+        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (B, Hq, Sq), "lse must be [B,Hq,Sq] fp32"
+    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in _bhs_strides(t, tensor_layout)]
+    if k_mean is not None:
+        assert k_mean.numel() == B * Hkv * D and k_mean.dtype == k.dtype, "k_mean must have B*Hkv*D elements of k's dtype"
+        k_mean = k_mean.reshape(B, Hkv, D).contiguous()
+    with torch.cuda.device(q.device):
+        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(B, Hq, Sq), dtype=torch.uint8, device=q.device)
+        check(lib().sab_qk_int8_attn_bwd(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(), k_scale.data_ptr(), q.data_ptr(),
+                                         k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(), lse.data_ptr(), _ptr(k_mean), dq.data_ptr(),
+                                         dk.data_ptr(), dv.data_ptr(), ws.data_ptr(), _dt(q), B, Hq, Hkv, Sq, Skv, D, *strides,
+                                         is_causal, q_quant_gran, k_quant_gran, float(sm_scale), fold_sm_scale, _stream(q)))
+
+
+@qk_int8_attn_bwd.register_fake
+def _(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, tensor_layout, is_causal, q_quant_gran, k_quant_gran,
+      sm_scale, fold_sm_scale):
+    return None
+
+
 # ----------------------------------------------------------------------------------------------- FP16-PV variant
 @torch.library.custom_op("sageattention_b200::v_transpose_f16", mutates_args=("v_f16t",), device_types="cuda")
 def v_transpose_f16(v: torch.Tensor, v_f16t: torch.Tensor, tensor_layout: int) -> None:

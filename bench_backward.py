@@ -5,7 +5,11 @@ causal, on one GPU.  Prints one JSON line with, per mode:
   * bwd_call: the whole backward of sageattn (o.backward(dO): Q/K quantiser recompute + gradient kernels);
   * fwd_bwd: forward + backward of sageattn;
   * sdpa_flash_bwd: torch SDPA's flash-attention backward on the same inputs, for context;
-and the GPU name and power limit.  CUDA events after warm-up; writes nothing."""
+and the GPU name and power limit.  CUDA events after warm-up; writes nothing.
+
+--varlen: the same for sageattn_varlen on a packed GQA batch (lens 4096, 512, 16384, 1024, 8192, 2048; Hq=32, Hkv=8, D=128, bf16),
+non-causal and causal, counting 10*Hq*D*sum(Lq*Lk) FLOPs (only the visible pairs for causal), with the sum of per-sequence torch
+SDPA flash backwards for context."""
 import argparse
 import json
 import subprocess
@@ -38,6 +42,73 @@ def _gpu():
         return {"name": name, "power_limit_w": None, "error": str(e)}
 
 
+VARLEN_LENS = [4096, 512, 16384, 1024, 8192, 2048]
+
+
+def varlen(a):
+    import numpy as np
+    import sageattention_b200 as sab
+    from sageattention_b200 import ops
+    from sageattention_b200.quant import per_block_int8_varlen, transpose_v_f16_varlen
+
+    lens, Hq, Hkv, D = VARLEN_LENS, 32, 8, 128
+    T, L = sum(lens), max(lens)
+    dt = torch.bfloat16
+    g = torch.Generator(device="cuda").manual_seed(0)
+    q, do = (torch.randn(T, Hq, D, device="cuda", dtype=dt, generator=g) for _ in range(2))
+    k, v = (torch.randn(T, Hkv, D, device="cuda", dtype=dt, generator=g) for _ in range(2))
+    cu = torch.tensor([0] + list(np.cumsum(lens)), dtype=torch.int32, device="cuda")
+    sm = D ** -0.5
+    out = {"metric": "sageattn_varlen backward", "shape": {"lens": lens, "Hq": Hq, "Hkv": Hkv, "D": D, "dtype": "bf16"},
+           "gpu": _gpu()}
+    for causal in (False, True):
+        pairs = sum(n * (n + 1) // 2 if causal else n * n for n in lens)
+        flops = 10.0 * Hq * D * pairs
+        # kernels alone, on the operands sageattn_varlen's forward uses
+        km = sab.k_mean(k.unsqueeze(0), "NHD").view(Hkv, D)
+        q8, qs, k8, ks, cqs, cks = per_block_int8_varlen(q, k, cu, cu, L, L, sm_scale=sm, km=km)
+        v_t, cu_pad = transpose_v_f16_varlen(v, cu, L)
+        o = torch.empty_like(q)
+        lse = ops.qk_int8_sv_f16_attn_varlen(q8, k8, v_t, o, qs, ks, cu, cu, cu_pad, cqs, cks, L, int(causal), sm, 1, 1)
+        dq, dk, dv = torch.zeros_like(q), torch.zeros_like(k), torch.zeros_like(v)
+        t_kern = _events(lambda: ops.qk_int8_attn_bwd_varlen(q8, k8, qs, ks, q, k, v, o, do, lse, km, dq, dk, dv, cu, cu, cqs, cks,
+                                                             L, L, int(causal), sm, 1), a.steps, a.warmup)
+        # the public call
+        qg, kg, vg = (t.clone().requires_grad_(True) for t in (q, k, v))
+
+        def fwd_bwd():
+            qg.grad = kg.grad = vg.grad = None
+            sab.sageattn_varlen(qg, kg, vg, cu, cu, L, L, is_causal=causal).backward(do)
+
+        t_fb = _events(fwd_bwd, a.steps, a.warmup)
+        ob = sab.sageattn_varlen(qg, kg, vg, cu, cu, L, L, is_causal=causal)
+        t_bwd = _events(lambda: torch.autograd.grad(ob, (qg, kg, vg), do, retain_graph=True), a.steps, a.warmup)
+        # torch SDPA flash backward of each sequence alone (K / V heads repeated to Hq outside the timed region)
+        seqs = []
+        with torch.nn.attention.sdpa_kernel(torch.nn.attention.SDPBackend.FLASH_ATTENTION):
+            for i in range(len(lens)):
+                s = slice(int(cu[i]), int(cu[i + 1]))
+                qi = q[s].transpose(0, 1).unsqueeze(0).detach().requires_grad_(True)
+                ki, vi = (t[s].transpose(0, 1).repeat_interleave(Hq // Hkv, 0).unsqueeze(0).detach().requires_grad_(True)
+                          for t in (k, v))
+                oi = F.scaled_dot_product_attention(qi, ki, vi, is_causal=causal)
+                seqs.append((oi, (qi, ki, vi), do[s].transpose(0, 1).unsqueeze(0)))
+
+            def sdpa_bwd():
+                for oi, ins, doi in seqs:
+                    torch.autograd.grad(oi, ins, doi, retain_graph=True)
+
+            t_sdpa = _events(sdpa_bwd, a.steps, a.warmup)
+        out["causal" if causal else "non_causal"] = {
+            "bwd_kernel": {"ms": round(t_kern, 3), "tflops": round(flops / t_kern / 1e9, 1)},
+            "bwd_call": {"ms": round(t_bwd, 3), "tflops": round(flops / t_bwd / 1e9, 1)},
+            "fwd_bwd": {"ms": round(t_fb, 3)},
+            "sdpa_flash_bwd_per_sequence": {"ms": round(t_sdpa, 3), "tflops": round(flops / t_sdpa / 1e9, 1)},
+        }
+        del ob, seqs
+    print(json.dumps(out))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--B", type=int, default=4)
@@ -46,8 +117,11 @@ def main():
     ap.add_argument("--D", type=int, default=128)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--varlen", action="store_true", help="sageattn_varlen on a packed GQA batch instead of sageattn")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_backward.py needs a GPU"
+    if a.varlen:
+        return varlen(a)
     import sageattention_b200 as sab
     from sageattention_b200 import ops
 

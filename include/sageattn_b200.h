@@ -271,7 +271,8 @@ int sab_qk_int8_sv_f8_attn_sp(const int8_t* q_int8, const int8_t* k_int8, const 
  *            forward's O) is not multiplied by a large K mean;
  *   dq, dk, dv : outputs in `dtype` with the strides of q, k, v.  GQA: dk / dv are summed over the Q heads of each KV head.
  *   workspace : >= sab_attn_bwd_workspace_bytes(B, Hq, Sq) bytes of device scratch.
- * Dense only; is_causal needs Sq == Skv (top-left).  Deterministic: no atomics, a fixed summation order.
+ * Dense (packed sequences: sab_qk_int8_attn_bwd_varlen below); is_causal needs Sq == Skv (top-left).  Deterministic: no atomics,
+ * a fixed summation order.
  * ---------------------------------------------------------------------------------------------- */
 int64_t sab_attn_bwd_workspace_bytes(int B, int Hq, int Sq);
 int sab_qk_int8_attn_bwd(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale, const void* q,
@@ -283,6 +284,29 @@ int sab_qk_int8_attn_bwd(const int8_t* q_int8, const int8_t* k_int8, const float
                          int64_t v_stride_s, int64_t o_stride_b, int64_t o_stride_h, int64_t o_stride_s, int64_t do_stride_b,
                          int64_t do_stride_h, int64_t do_stride_s, int is_causal, int q_gran, int k_gran, float sm_scale,
                          int fold_sm_scale, void* stream);
+
+/* Varlen form of sab_qk_int8_attn_bwd: the gradient of the packed FP16-PV forward (sab_qk_int8_sv_f16_attn with cu_seqlens, the
+ * kernel behind sageattn_varlen), each sequence on its own.  Same definition as above; the causal mask is top-left inside each
+ * sequence (key j visible to row i iff j <= i), and Lq != Lk is allowed, as in the forward.
+ *   q_int8, k_int8, q, k, v, o, dout, dq, dk, dv : packed [T,H,D] (Tq rows for q / o / dout / dq, Tk for k / v / dk / dv); the
+ *            strides are (stride_t, stride_h) pairs in elements; dq / dk / dv have the strides of q / k / v;
+ *   q_scale, k_scale : per-block [nblocks,Hq] / [nblocks,Hkv], sequence b's blocks starting at cu_q_scale[b] / cu_k_scale[b],
+ *            as sab_quant_per_block_int8_varlen writes them (per_block Q and K, the only varlen granularity);
+ *   lse    : [Hq,Tq] fp32 log2 units, the forward's (row h*Tq + cu_seqlens_q[b] + i);
+ *   k_mean : optional [Hkv,D] (`dtype`), the K mean over all packed tokens the forward subtracted;
+ *   cu_seqlens_q / cu_seqlens_k : [nseq+1] int32 token offsets; max_seqlen_q / max_seqlen_k : the longest sequence of each.
+ *   workspace : >= sab_attn_bwd_workspace_bytes(1, Hq, Tq) bytes of device scratch.
+ * Rows of dq and keys of dk / dv past cu_seqlens_*[nseq] belong to no sequence and are not written; a sequence with keys but no
+ * queries gets zero dk / dv.  Deterministic like the dense form. */
+int sab_qk_int8_attn_bwd_varlen(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale, const void* q,
+                                const void* k, const void* v, const void* o, const void* dout, const float* lse, const void* k_mean,
+                                void* dq, void* dk, void* dv, void* workspace, int dtype, int nseq, int Hq, int Hkv, int Tq, int Tk,
+                                int D, int64_t q8_stride_t, int64_t q8_stride_h, int64_t k8_stride_t, int64_t k8_stride_h,
+                                int64_t q_stride_t, int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h, int64_t v_stride_t,
+                                int64_t v_stride_h, int64_t o_stride_t, int64_t o_stride_h, int64_t do_stride_t, int64_t do_stride_h,
+                                const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k, const int32_t* cu_q_scale,
+                                const int32_t* cu_k_scale, int max_seqlen_q, int max_seqlen_k, int is_causal, float sm_scale,
+                                int fold_sm_scale, void* stream);
 
 #ifdef __cplusplus
 }

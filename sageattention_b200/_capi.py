@@ -44,6 +44,8 @@ EXPORTS = {
                                   [c_void_p, ctypes.c_uint32, c_int, c_void_p]),
     "sab_attn_bwd_workspace_bytes": (c_int64, [c_int] * 3),
     "sab_qk_int8_attn_bwd": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_int64] * 21 + [c_int, c_int, c_int, c_float, c_int, c_void_p]),
+    "sab_qk_int8_attn_bwd_varlen": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_int64] * 14 + [c_void_p] * 4 +
+                                    [c_int, c_int, c_int, c_float, c_int, c_void_p]),
 }
 
 _lib = None

@@ -293,22 +293,68 @@ def sageattn_varlen(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu_seqlen
                     sm_scale: Optional[float] = None, smooth_k: bool = True, **kwargs: Any) -> torch.Tensor:
     """sageattention/core.py:334-448: packed [T,H,D] tensors, per-block INT8 per sequence (Triton rounding,
     bit-exact), K mean over all tokens of the batch (core.py:433), FP16 P and V (fp16 wgmma) like the
-    reference's Triton varlen kernels."""
-    dtype = q.dtype
+    reference's Triton varlen kernels.  Differentiable (no reference counterpart) when grad mode is on and q, k or v requires
+    grad: each sequence gets the dense entry points' straight-through gradient on its own (_SageAttnVarlenFunction)."""
     _check_inputs(q, k, v)
     q, k, v, head_dim_og = _pad_head_dim(q, k, v)
     assert q.stride(-1) == 1 and k.stride(-1) == 1 and v.stride(-1) == 1, "Last dim of qkv must be contiguous."
     assert cu_seqlens_q.is_contiguous() and cu_seqlens_k.is_contiguous(), "cu_seqlens_q and cu_seqlens_k must be contiguous."
+    if sm_scale is None:
+        sm_scale = 1.0 / (head_dim_og ** 0.5)
+    args = (cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, sm_scale, smooth_k)
+    if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
+        o = _SageAttnVarlenFunction.apply(q, k, v, *args)
+    else:
+        o, _ = _attn_varlen(q, k, v, *args, False)
+    return o[..., :head_dim_og]
+
+
+# ------------------------------------------------------------------------------------------------ packed varlen call and its gradient
+def _quant_qk_varlen(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, sm_scale, smooth_k):
+    """Q/K front-end of sageattn_varlen on head-dim-padded packed q, k: (km, q_int8, q_scale, k_int8, k_scale, cu_q_scale,
+    cu_k_scale).  Deterministic, so the backward re-runs it."""
     km = None
     if smooth_k:
         km = k_mean(k.unsqueeze(0), "NHD").view(1, k.size(1), k.size(2))   # mean over all tokens
-    if sm_scale is None:
-        sm_scale = 1.0 / (head_dim_og ** 0.5)
-    q_int8, q_scale, k_int8, k_scale, cu_q_scale, cu_k_scale = per_block_int8_varlen(
-        q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, sm_scale=sm_scale, km=km)
+    return (km,) + per_block_int8_varlen(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, sm_scale=sm_scale, km=km)
+
+
+def _attn_varlen(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, sm_scale, smooth_k, return_lse):
+    """Quantisers + FP16-PV kernel of sageattn_varlen on head-dim-padded packed q, k, v: (o, the kernel's [Hq,Tq] log2 lse or an
+    empty tensor)."""
+    _, q_int8, q_scale, k_int8, k_scale, cu_q_scale, cu_k_scale = _quant_qk_varlen(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q,
+                                                                                  max_seqlen_k, sm_scale, smooth_k)
     v_t, cu_pad = transpose_v_f16_varlen(v, cu_seqlens_k, max_seqlen_k)
-    o = torch.empty(q.shape, dtype=dtype, device=q.device)
-    ops.qk_int8_sv_f16_attn_varlen(q_int8, k_int8, v_t, o, q_scale, k_scale, cu_seqlens_q.to(torch.int32),
-                                   cu_seqlens_k.to(torch.int32), cu_pad, cu_q_scale, cu_k_scale, max_seqlen_q,
-                                   1 if is_causal else 0, sm_scale, 1)
-    return o[..., :head_dim_og]
+    o = torch.empty(q.shape, dtype=q.dtype, device=q.device)
+    lse = ops.qk_int8_sv_f16_attn_varlen(q_int8, k_int8, v_t, o, q_scale, k_scale, cu_seqlens_q.to(torch.int32),
+                                         cu_seqlens_k.to(torch.int32), cu_pad, cu_q_scale, cu_k_scale, max_seqlen_q,
+                                         1 if is_causal else 0, sm_scale, 1, 1 if return_lse else 0)
+    return o, lse
+
+
+class _SageAttnVarlenFunction(torch.autograd.Function):
+    """sageattn_varlen with a gradient: the gradient of _SageAttnFunction applied to each packed sequence on its own
+    (include/sageattn_b200.h, sab_qk_int8_attn_bwd_varlen).  forward: the unchanged varlen forward with the kernel LSE enabled;
+    saves q, k, v, o, the LSE and the cu_seqlens.  backward: re-runs the K mean and the varlen Q/K quantisers, then the two
+    gradient kernels.  Tokens past cu_seqlens[-1] belong to no sequence: their gradient is zero."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, sm_scale, smooth_k):
+        o, lse = _attn_varlen(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, sm_scale, smooth_k, True)
+        ctx.save_for_backward(q, k, v, o, lse, cu_seqlens_q, cu_seqlens_k)
+        ctx.cfg = (max_seqlen_q, max_seqlen_k, is_causal, sm_scale, smooth_k)
+        return o
+
+    @staticmethod
+    def backward(ctx, do):
+        max_seqlen_q, max_seqlen_k, is_causal, sm_scale, smooth_k = ctx.cfg
+        q, k, v, o, lse, cu_seqlens_q, cu_seqlens_k = ctx.saved_tensors
+        km, q_int8, q_scale, k_int8, k_scale, cu_q_scale, cu_k_scale = _quant_qk_varlen(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q,
+                                                                                      max_seqlen_k, sm_scale, smooth_k)
+        # the kernels read 16-bit rows with 16-byte loads; dq / dk / dv take the strides of q / k / v
+        q, k, v, o, do = (t.contiguous() for t in (q, k, v, o, do))
+        dq, dk, dv = torch.zeros_like(q), torch.zeros_like(k), torch.zeros_like(v)
+        ops.qk_int8_attn_bwd_varlen(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv,
+                                    cu_seqlens_q.to(torch.int32), cu_seqlens_k.to(torch.int32), cu_q_scale, cu_k_scale, max_seqlen_q,
+                                    max_seqlen_k, 1 if is_causal else 0, sm_scale, 1)
+        return dq, dk, dv, None, None, None, None, None, None, None

@@ -16,6 +16,10 @@
 //                      GQA group and every 64-row Q tile, so dK and dV are written once.  S^T = K Q^T (INT8) and dP^T = V dO^T put
 //                      P^T and dS^T in the accumulator layout; rounded to the input dtype they are the register A operand of
 //                      dV += P^T dO and dK += dS^T Q.
+// Varlen (p.a.cu_q != nullptr, packed [T,H,D] tensors, per-block scales [nblocks,H]): blockIdx.z is the sequence; the top of each
+// CTA decodes its sequence's token offsets, lengths and first scale blocks once, as the forward does (attn.cu), and the loops below
+// read those.  The causal mask is top-left inside each sequence.  delta runs on the packed rows as B = 1, so it has the LSE's
+// [Hq,Tq] layout.
 // Products are wgmma with fp32 accumulation: INT8 for S as in the forward, bf16 / f16 for the rest.  Every B operand is K-major in
 // shared memory, in the swizzled layout the forward's TMA loads write; the operands the math needs transposed (dO^T, Q^T, K^T) are
 // transposed by the loaders.  Loads are plain: all threads copy a tile, the CTA synchronises, then computes (no load/compute
@@ -28,7 +32,8 @@ namespace sab {
 constexpr int kBwdThreads = 256;   // two warpgroups
 
 struct BwdParams {
-  AttnParams a;                    // the forward's scale / size / causal parameters (a.lse, a.out unused)
+  AttnParams a;                    // the forward's scale / size / causal / varlen parameters (a.lse, a.out unused)
+  int n_k_tiles;                   // 128-key tiles per (batch or sequence, KV head): the dK/dV grid's x
   const int8_t* q8;
   const int8_t* k8;
   int64_t q8_sb, q8_sh, q8_ss, k8_sb, k8_sh, k8_ss;
@@ -37,10 +42,10 @@ struct BwdParams {
   const uint16_t* v;
   const uint16_t* o;
   const uint16_t* dout;
-  const uint16_t* kmean;           // nullable [B,Hkv,D]: the K smoothing mean, subtracted from the K of dQ += dS K
+  const uint16_t* kmean;           // nullable [B,Hkv,D] (varlen [Hkv,D]): the K smoothing mean, subtracted from the K of dQ += dS K
   int64_t q_sb, q_sh, q_ss, k_sb, k_sh, k_ss, v_sb, v_sh, v_ss, o_sb, o_sh, o_ss, do_sb, do_sh, do_ss;
-  const float* lse;                // [B,Hq,Sq] log2 units
-  float* delta;                    // [B,Hq,Sq] workspace
+  const float* lse;                // [B,Hq,Sq] log2 units (varlen [Hq,Tq])
+  float* delta;                    // [B,Hq,Sq] workspace (varlen [Hq,Tq])
   void* dq;
   void* dk;
   void* dv;
@@ -143,6 +148,27 @@ __device__ __forceinline__ void store_rows(const float (&acc)[D / 2], T* row0, T
   }
 }
 
+// ------------------------------------------------------------------------------------------------ work decode
+// The tokens of this CTA's batch entry (attn.cu's work decode).  Dense: batch b, all Sq / Sk rows.  Varlen: sequence b of the
+// packed tensors (stride_b 0), whose scales start at 128-row Q block q_blk0 and 64-key block k_blk0; the scale bases are then h and
+// hk (qs_stride_bh = ks_stride_bh = 1, stride qs_stride_idx = Hq / ks_stride_idx = Hkv), the LSE / delta row h*Tq + q_off + row and
+// the K mean [Hkv,D] (tb = 0).  Each kernel branches on p.a.cu_q once, at the top, into a body compiled for one form: the dense
+// body sees the span as constants (offsets and first blocks 0), so its code is that of a kernel without varlen support.
+struct SeqSpan {
+  int tb;                          // batch index of the scales, LSE, delta and K mean
+  int q_off, q_len, k_off, kv_len;
+  int q_blk0, k_blk0;
+};
+template <bool kVarlen>
+__device__ __forceinline__ SeqSpan seq_span(const AttnParams& a, int b) {
+  if constexpr (!kVarlen) {
+    return SeqSpan{b, 0, a.Sq, 0, a.Sk, 0, 0};
+  } else {
+    const int q_off = a.cu_q[b], k_off = a.cu_k[b];
+    return SeqSpan{0, q_off, a.cu_q[b + 1] - q_off, k_off, a.cu_k[b + 1] - k_off, a.cu_qs[b], a.cu_ks[b]};
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ delta = rowsum(dO o O)
 // one warp per Q row, fixed summation order
 template <typename T>
@@ -169,8 +195,8 @@ constexpr size_t bwd_dq_smem_bytes() {
   return size_t(128) * D + size_t(128) * D * 2 + size_t(64) * D + size_t(64) * D * 2 + size_t(D) * 64 * 2 + 1024;
 }
 
-template <int D, bool kKT, typename T>
-__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_kernel(const __grid_constant__ BwdParams p) {
+template <int D, bool kKT, typename T, bool kVarlen>
+__device__ __forceinline__ void bwd_dq_tile(const BwdParams& p) {
   constexpr int QB = 128, KB = 64;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ8 = smem;                       // [128 x D] int8        A of S = Q K^T
@@ -184,27 +210,29 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_kernel(const __grid_con
   if (a.causal) qt = a.n_q_tiles - 1 - qt;   // heaviest tiles first
   const int h = blockIdx.y, b = blockIdx.z;
   const int hk = h / (a.Hq / a.Hkv);
+  const SeqSpan sq = seq_span<kVarlen>(a, b);
+  if (qt * QB >= sq.q_len) return;           // varlen: a sequence shorter than the longest
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2, t = lane & 3;
   const int row0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // rows row0, row0 + 8 of the Q tile (forward's accumulator layout)
 
   if ((smem_u32(smem) & 1023u) != 0) __trap();
-  load_tile<QB, D, 1>(sQ8, p.q8 + b * p.q8_sb + h * p.q8_sh, p.q8_ss, qt * QB, a.Sq);
-  load_tile<QB, D, 2>(sdO, p.dout + b * p.do_sb + h * p.do_sh, p.do_ss, qt * QB, a.Sq);
+  load_tile<QB, D, 1>(sQ8, p.q8 + b * p.q8_sb + h * p.q8_sh + sq.q_off * p.q8_ss, p.q8_ss, qt * QB, sq.q_len);
+  load_tile<QB, D, 2>(sdO, p.dout + b * p.do_sb + h * p.do_sh + sq.q_off * p.do_ss, p.do_ss, qt * QB, sq.q_len);
 
-  const float* qs_base = a.q_scale + (int64_t(b) * a.Hq + h) * a.qs_stride_bh;
-  const float* ks_base = a.k_scale + (int64_t(b) * a.Hkv + hk) * a.ks_stride_bh;
+  const float* qs_base = a.q_scale + (int64_t(sq.tb) * a.Hq + h) * a.qs_stride_bh;
+  const float* ks_base = a.k_scale + (int64_t(sq.tb) * a.Hkv + hk) * a.ks_stride_bh;
   int q_row[2];
   float qss[2], nlse[2], dlt[2];
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     q_row[i] = qt * QB + row0 + 8 * i;
-    qss[i] = q_dequant_log2(a, qs_base, qt, row0 + 8 * i);   // scales are padded to whole 128-row blocks
-    const bool ok = q_row[i] < a.Sq;
-    const int64_t li = (int64_t(b) * a.Hq + h) * a.Sq + q_row[i];
+    qss[i] = q_dequant_log2(a, qs_base, sq.q_blk0 + qt, row0 + 8 * i);   // scales are padded to whole 128-row blocks
+    const bool ok = q_row[i] < sq.q_len;
+    const int64_t li = (int64_t(sq.tb) * a.Hq + h) * a.Sq + sq.q_off + q_row[i];
     nlse[i] = ok ? -p.lse[li] : 0.f;
     dlt[i] = ok ? p.delta[li] : 0.f;
   }
-  int n_kv = (a.Sk + KB - 1) / KB;
+  int n_kv = (sq.kv_len + KB - 1) / KB;
   if (a.causal) n_kv = min(n_kv, ((qt + 1) * QB + KB - 1) / KB);
 
   float dq[D / 2];
@@ -213,12 +241,12 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_kernel(const __grid_con
 
   for (int j = 0; j < n_kv; ++j) {
     __syncthreads();   // the previous tile's operands are consumed
-    load_tile<KB, D, 1>(sK8, p.k8 + b * p.k8_sb + hk * p.k8_sh, p.k8_ss, j * KB, a.Sk);
-    load_tile<KB, D, 2>(sV, p.v + b * p.v_sb + hk * p.v_sh, p.v_ss, j * KB, a.Sk);
+    load_tile<KB, D, 1>(sK8, p.k8 + b * p.k8_sb + hk * p.k8_sh + sq.k_off * p.k8_ss, p.k8_ss, j * KB, sq.kv_len);
+    load_tile<KB, D, 2>(sV, p.v + b * p.v_sb + hk * p.v_sh + sq.k_off * p.v_ss, p.v_ss, j * KB, sq.kv_len);
     // K - mean: the same product in exact arithmetic (the rows of dS sum to zero), but the residue that delta = rowsum(dO o O) of
     // the quantised forward leaves in those row sums is not multiplied by a large K mean
-    load_tile_t<D, T>(sKt, p.k + b * p.k_sb + hk * p.k_sh, p.k_ss, j * KB, a.Sk,
-                      p.kmean ? p.kmean + (int64_t(b) * a.Hkv + hk) * D : nullptr);
+    load_tile_t<D, T>(sKt, p.k + b * p.k_sb + hk * p.k_sh + sq.k_off * p.k_ss, p.k_ss, j * KB, sq.kv_len,
+                      p.kmean ? p.kmean + (int64_t(sq.tb) * a.Hkv + hk) * D : nullptr);
     fence_proxy_async_smem();   // generic-proxy stores -> visible to wgmma
     __syncthreads();
 
@@ -236,11 +264,11 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_kernel(const __grid_con
 
     float coef[2];
     int limit[2];
-    const float ksv = k_dequant<kKT>(a, ks_base, j, t);
+    const float ksv = k_dequant<kKT>(a, ks_base, sq.k_blk0 + j, t);
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       coef[i] = ksv * qss[i];
-      limit[i] = q_row[i] < a.Sq ? a.Sk - j * KB : 0;
+      limit[i] = q_row[i] < sq.q_len ? sq.kv_len - j * KB : 0;
       if (a.causal) limit[i] = min(limit[i], q_row[i] - j * KB + 1);
     }
     float ds[32];
@@ -264,9 +292,15 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_kernel(const __grid_con
     fence_regs(dq);
   }
 
-  T* base = reinterpret_cast<T*>(p.dq) + b * p.q_sb + h * p.q_sh;
-  store_rows<T, D>(dq, base + int64_t(q_row[0]) * p.q_ss, base + int64_t(q_row[1]) * p.q_ss, q_row[0] < a.Sq, q_row[1] < a.Sq, t,
-                   p.sm_scale);
+  T* base = reinterpret_cast<T*>(p.dq) + b * p.q_sb + h * p.q_sh + sq.q_off * p.q_ss;
+  store_rows<T, D>(dq, base + int64_t(q_row[0]) * p.q_ss, base + int64_t(q_row[1]) * p.q_ss, q_row[0] < sq.q_len,
+                   q_row[1] < sq.q_len, t, p.sm_scale);
+}
+
+template <int D, bool kKT, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_kernel(const __grid_constant__ BwdParams p) {
+  if (p.a.cu_q != nullptr) bwd_dq_tile<D, kKT, T, true>(p);
+  else bwd_dq_tile<D, kKT, T, false>(p);
 }
 
 // ------------------------------------------------------------------------------------------------ dK, dV
@@ -275,8 +309,8 @@ constexpr size_t bwd_dkdv_smem_bytes() {
   return size_t(128) * D + size_t(128) * D * 2 + size_t(64) * D + size_t(64) * D * 2 + 2 * size_t(D) * 64 * 2 + 3 * 64 * 4 + 1024;
 }
 
-template <int D, bool kKT, typename T>
-__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_kernel(const __grid_constant__ BwdParams p) {
+template <int D, bool kKT, typename T, bool kVarlen>
+__device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p) {
   constexpr int KB = 128, QB = 64;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sK8 = smem;                       // [128 x D] int8        A of S^T = K Q^T
@@ -291,44 +325,46 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_kernel(const __grid_c
   const AttnParams& a = p.a;
 
   const int k0 = blockIdx.x * KB, hk = blockIdx.y, b = blockIdx.z;
+  const SeqSpan sq = seq_span<kVarlen>(a, b);
+  if (k0 >= sq.kv_len) return;               // varlen: a sequence shorter than the longest (keys with no queries still store zeros)
   const int G = a.Hq / a.Hkv;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = warp >> 2, t = lane & 3;
   const int kr = wg * 64 + (warp & 3) * 16 + (lane >> 2);   // keys k0 + kr, k0 + kr + 8 (accumulator rows)
 
   if ((smem_u32(smem) & 1023u) != 0) __trap();
-  load_tile<KB, D, 1>(sK8, p.k8 + b * p.k8_sb + hk * p.k8_sh, p.k8_ss, k0, a.Sk);
-  load_tile<KB, D, 2>(sV, p.v + b * p.v_sb + hk * p.v_sh, p.v_ss, k0, a.Sk);
+  load_tile<KB, D, 1>(sK8, p.k8 + b * p.k8_sb + hk * p.k8_sh + sq.k_off * p.k8_ss, p.k8_ss, k0, sq.kv_len);
+  load_tile<KB, D, 2>(sV, p.v + b * p.v_sb + hk * p.v_sh + sq.k_off * p.v_ss, p.v_ss, k0, sq.kv_len);
 
-  const float* ks_base = a.k_scale + (int64_t(b) * a.Hkv + hk) * a.ks_stride_bh;
+  const float* ks_base = a.k_scale + (int64_t(sq.tb) * a.Hkv + hk) * a.ks_stride_bh;
   int key[2];
   float ksr[2];
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     key[i] = k0 + kr + 8 * i;
     // per-thread K scales: key % 8 == lane / 4, so its scale group is lane / 8
-    ksr[i] = key[i] < a.Sk ? k_dequant<kKT>(a, ks_base, key[i] / 64, lane >> 3) : 0.f;
+    ksr[i] = key[i] < sq.kv_len ? k_dequant<kKT>(a, ks_base, sq.k_blk0 + key[i] / 64, lane >> 3) : 0.f;
   }
   float dk[D / 2], dv[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) dk[i] = dv[i] = 0.f;
 
-  const int n_qt = (a.Sq + QB - 1) / QB;
-  const int qt0 = a.causal ? k0 / QB : 0;    // causal (Sq == Skv): rows before the first key see none of this tile
+  const int n_qt = (sq.q_len + QB - 1) / QB;
+  const int qt0 = a.causal ? k0 / QB : 0;    // causal (top-left): rows before the first key see none of this tile
   for (int hh = 0; hh < G; ++hh) {
     const int h = hk * G + hh;
-    const float* qs_base = a.q_scale + (int64_t(b) * a.Hq + h) * a.qs_stride_bh;
+    const float* qs_base = a.q_scale + (int64_t(sq.tb) * a.Hq + h) * a.qs_stride_bh;
     for (int qt = qt0; qt < n_qt; ++qt) {
       const int q0 = qt * QB;
       __syncthreads();   // the previous tile's operands are consumed
-      load_tile<QB, D, 1>(sQ8, p.q8 + b * p.q8_sb + h * p.q8_sh, p.q8_ss, q0, a.Sq);
-      load_tile<QB, D, 2>(sdO, p.dout + b * p.do_sb + h * p.do_sh, p.do_ss, q0, a.Sq);
-      load_tile_t<D, T>(sdOt, p.dout + b * p.do_sb + h * p.do_sh, p.do_ss, q0, a.Sq);
-      load_tile_t<D, T>(sQt, p.q + b * p.q_sb + h * p.q_sh, p.q_ss, q0, a.Sq);
+      load_tile<QB, D, 1>(sQ8, p.q8 + b * p.q8_sb + h * p.q8_sh + sq.q_off * p.q8_ss, p.q8_ss, q0, sq.q_len);
+      load_tile<QB, D, 2>(sdO, p.dout + b * p.do_sb + h * p.do_sh + sq.q_off * p.do_ss, p.do_ss, q0, sq.q_len);
+      load_tile_t<D, T>(sdOt, p.dout + b * p.do_sb + h * p.do_sh + sq.q_off * p.do_ss, p.do_ss, q0, sq.q_len);
+      load_tile_t<D, T>(sQt, p.q + b * p.q_sb + h * p.q_sh + sq.q_off * p.q_ss, p.q_ss, q0, sq.q_len);
       if (threadIdx.x < QB) {
         const int r = q0 + threadIdx.x;
-        const bool ok = r < a.Sq;
-        const int64_t li = (int64_t(b) * a.Hq + h) * a.Sq + r;
-        s_qss[threadIdx.x] = ok ? q_dequant_log2(a, qs_base, r / 128, r % 128) : 0.f;
+        const bool ok = r < sq.q_len;
+        const int64_t li = (int64_t(sq.tb) * a.Hq + h) * a.Sq + sq.q_off + r;
+        s_qss[threadIdx.x] = ok ? q_dequant_log2(a, qs_base, sq.q_blk0 + r / 128, r % 128) : 0.f;
         s_nlse[threadIdx.x] = ok ? -p.lse[li] : 0.f;
         s_dlt[threadIdx.x] = ok ? p.delta[li] : 0.f;
       }
@@ -356,7 +392,7 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_kernel(const __grid_c
           const int idx = 4 * (c >> 1) + 2 * i + (c & 1);
           const int col = 8 * (c >> 1) + 2 * t + (c & 1);
           const int q = q0 + col;
-          const bool ok = key[i] < a.Sk && q < a.Sq && (!a.causal || key[i] <= q);
+          const bool ok = key[i] < sq.kv_len && q < sq.q_len && (!a.causal || key[i] <= q);
           const float pe = ok ? ex2_approx(logit_log2(s[idx], ksr[i] * s_qss[col], s_nlse[col])) : 0.f;
           pt[idx] = pe;
           dst[idx] = pe * (dp[idx] - s_dlt[col]);
@@ -377,18 +413,28 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_kernel(const __grid_c
     }
   }
 
-  T* kb = reinterpret_cast<T*>(p.dk) + b * p.k_sb + hk * p.k_sh;
-  T* vb = reinterpret_cast<T*>(p.dv) + b * p.v_sb + hk * p.v_sh;
-  const bool ok0 = key[0] < a.Sk, ok1 = key[1] < a.Sk;
+  T* kb = reinterpret_cast<T*>(p.dk) + b * p.k_sb + hk * p.k_sh + sq.k_off * p.k_ss;
+  T* vb = reinterpret_cast<T*>(p.dv) + b * p.v_sb + hk * p.v_sh + sq.k_off * p.v_ss;
+  const bool ok0 = key[0] < sq.kv_len, ok1 = key[1] < sq.kv_len;
   store_rows<T, D>(dk, kb + int64_t(key[0]) * p.k_ss, kb + int64_t(key[1]) * p.k_ss, ok0, ok1, t, p.sm_scale);
   store_rows<T, D>(dv, vb + int64_t(key[0]) * p.v_ss, vb + int64_t(key[1]) * p.v_ss, ok0, ok1, t, 1.0f);
 }
 
 template <int D, bool kKT, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_kernel(const __grid_constant__ BwdParams p) {
+  if (p.a.cu_q != nullptr) bwd_dkdv_tile<D, kKT, T, true>(p);
+  else bwd_dkdv_tile<D, kKT, T, false>(p);
+}
+
+template <int D, bool kKT, typename T>
 static int launch_bwd(const BwdParams& p, cudaStream_t stream) {
-  const int64_t rows = int64_t(p.a.B) * p.a.Hq * p.a.Sq;
-  bwd_delta_kernel<T><<<unsigned((rows + 7) / 8), 256, 0, stream>>>(p, D);
-  SAB_CUDA_OK(cudaGetLastError());
+  {
+    BwdParams pd = p;
+    if (p.a.cu_q != nullptr) pd.a.B = 1;   // varlen: every packed row, [Hq,Tq] like the LSE
+    const int64_t rows = int64_t(pd.a.B) * pd.a.Hq * pd.a.Sq;
+    bwd_delta_kernel<T><<<unsigned((rows + 7) / 8), 256, 0, stream>>>(pd, D);
+    SAB_CUDA_OK(cudaGetLastError());
+  }
   {
     constexpr size_t smem = bwd_dq_smem_bytes<D>();
     auto kern = bwd_dq_kernel<D, kKT, T>;
@@ -402,10 +448,75 @@ static int launch_bwd(const BwdParams& p, cudaStream_t stream) {
     auto kern = bwd_dkdv_kernel<D, kKT, T>;
     static bool configured[64] = {};
     if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
-    kern<<<dim3((p.a.Sk + 127) / 128, p.a.Hkv, p.a.B), kBwdThreads, smem, stream>>>(p);
+    kern<<<dim3(p.n_k_tiles, p.a.Hkv, p.a.B), kBwdThreads, smem, stream>>>(p);
     SAB_CUDA_OK(cudaGetLastError());
   }
   return SAB_OK;
+}
+
+// Checks shared by the dense and the varlen entry, after the pointer / size checks: the forward's codes and messages (attn.cu).
+// st: (b, h, s) element strides of q8, k8, q, k, v, o, dout.
+static int check_bwd_layout(const int8_t* q_int8, const int8_t* k_int8, const void* q, const void* k, const void* v,
+                            const void* o, const void* dout, void* dq, void* dk, void* dv, const int64_t (&st)[21]) {
+  bool ok16 = aligned16(q) && aligned16(k) && aligned16(v) && aligned16(o) && aligned16(dout) && aligned16(dq) && aligned16(dk) && aligned16(dv);
+  for (int i = 6; i < 21; ++i) ok16 = ok16 && st[i] % 8 == 0;
+  SAB_REQUIRE(ok16, SAB_ERR_INVALID, "16-bit tensors must be 16-byte aligned with strides multiple of 8 elements");
+  bool ok8 = aligned16(q_int8) && aligned16(k_int8);
+  for (int i = 0; i < 6; ++i) ok8 = ok8 && st[i] % 16 == 0;
+  SAB_REQUIRE(ok8, SAB_ERR_INVALID, "int8 tensors must be 16-byte aligned with strides multiple of 16");
+  return sab_check_device();
+}
+
+// The parameters both entries fill; the varlen entry then adds its sequence tables
+static BwdParams bwd_params(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale, const void* q,
+                            const void* k, const void* v, const void* o, const void* dout, const float* lse, const void* k_mean,
+                            void* dq, void* dk, void* dv, void* workspace, int B, int Hq, int Hkv, int Sq, int Skv,
+                            const int64_t (&st)[21], int is_causal, int q_gran, int k_gran, float sm_scale, int fold_sm_scale) {
+  BwdParams p{};
+  AttnParams& a = p.a;
+  a.q_scale = q_scale; a.k_scale = k_scale;
+  a.B = B; a.Hq = Hq; a.Hkv = Hkv; a.Sq = Sq; a.Sk = Skv;
+  a.n_q_tiles = (Sq + BM - 1) / BM;
+  p.n_k_tiles = (Skv + 127) / 128;
+  a.causal = is_causal ? 1 : 0;
+  a.sm_scale_log2 = fold_sm_scale ? 1.0f : sm_scale * 1.44269504088896340736f;   // as the forward (attn.cu)
+  a.q_gran = q_gran;
+  a.q_mult = q_gran == SAB_GRAN_PER_BLOCK ? 1 : (q_gran == SAB_GRAN_PER_WARP ? 4 : 32);
+  a.k_mult = k_gran == SAB_GRAN_PER_THREAD ? 4 : 1;
+  a.qs_stride_bh = int64_t((Sq + BM - 1) / BM) * a.q_mult;
+  a.ks_stride_bh = int64_t((Skv + 63) / 64) * a.k_mult;
+  a.qs_stride_idx = 1;
+  a.ks_stride_idx = 1;
+  p.q8 = q_int8; p.k8 = k_int8;
+  p.q8_sb = st[0]; p.q8_sh = st[1]; p.q8_ss = st[2];
+  p.k8_sb = st[3]; p.k8_sh = st[4]; p.k8_ss = st[5];
+  p.q = static_cast<const uint16_t*>(q); p.k = static_cast<const uint16_t*>(k); p.v = static_cast<const uint16_t*>(v);
+  p.o = static_cast<const uint16_t*>(o); p.dout = static_cast<const uint16_t*>(dout);
+  p.kmean = static_cast<const uint16_t*>(k_mean);
+  p.q_sb = st[6]; p.q_sh = st[7]; p.q_ss = st[8];
+  p.k_sb = st[9]; p.k_sh = st[10]; p.k_ss = st[11];
+  p.v_sb = st[12]; p.v_sh = st[13]; p.v_ss = st[14];
+  p.o_sb = st[15]; p.o_sh = st[16]; p.o_ss = st[17];
+  p.do_sb = st[18]; p.do_sh = st[19]; p.do_ss = st[20];
+  p.lse = lse;
+  p.delta = static_cast<float*>(workspace);
+  p.dq = dq; p.dk = dk; p.dv = dv;
+  p.sm_scale = sm_scale;
+  return p;
+}
+
+static int dispatch_bwd(const BwdParams& p, int D, int dtype, int k_gran, void* stream) {
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const bool kt = k_gran == SAB_GRAN_PER_THREAD;
+  const bool bf = dtype == SAB_DTYPE_BF16;
+  if (D == 128) {
+    if (kt) { if (bf) return launch_bwd<128, true, __nv_bfloat16>(p, s); return launch_bwd<128, true, __half>(p, s); }
+    if (bf) return launch_bwd<128, false, __nv_bfloat16>(p, s);
+    return launch_bwd<128, false, __half>(p, s);
+  }
+  if (kt) { if (bf) return launch_bwd<64, true, __nv_bfloat16>(p, s); return launch_bwd<64, true, __half>(p, s); }
+  if (bf) return launch_bwd<64, false, __nv_bfloat16>(p, s);
+  return launch_bwd<64, false, __half>(p, s);
 }
 
 }  // namespace sab
@@ -434,57 +545,46 @@ extern "C" int sab_qk_int8_attn_bwd(const int8_t* q_int8, const int8_t* k_int8, 
   SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
   SAB_REQUIRE(q_gran >= 1 && q_gran <= 3 && k_gran >= 1 && k_gran <= 3, SAB_ERR_INVALID, "unknown quant granularity q=%d k=%d", q_gran, k_gran);
   SAB_REQUIRE(!is_causal || Sq == Skv, SAB_ERR_INVALID, "qo_len and kv_len must be equal for causal attention.");
-  const int64_t s16[] = {q_stride_b, q_stride_h, q_stride_s, k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s,
-                         o_stride_b, o_stride_h, o_stride_s, do_stride_b, do_stride_h, do_stride_s};
-  bool ok16 = aligned16(q) && aligned16(k) && aligned16(v) && aligned16(o) && aligned16(dout) && aligned16(dq) && aligned16(dk) && aligned16(dv);
-  for (int64_t s : s16) ok16 = ok16 && s % 8 == 0;
-  SAB_REQUIRE(ok16, SAB_ERR_INVALID, "16-bit tensors must be 16-byte aligned with strides multiple of 8 elements");
-  const int64_t s8[] = {q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s};
-  bool ok8 = aligned16(q_int8) && aligned16(k_int8);
-  for (int64_t s : s8) ok8 = ok8 && s % 16 == 0;
-  SAB_REQUIRE(ok8, SAB_ERR_INVALID, "int8 tensors must be 16-byte aligned with strides multiple of 16");
-  int st = sab_check_device();
-  if (st != SAB_OK) return st;
+  const int64_t st[21] = {q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s, q_stride_b, q_stride_h, q_stride_s,
+                          k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s, o_stride_b, o_stride_h, o_stride_s,
+                          do_stride_b, do_stride_h, do_stride_s};
+  if (int e = check_bwd_layout(q_int8, k_int8, q, k, v, o, dout, dq, dk, dv, st)) return e;
+  const BwdParams p = bwd_params(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, B, Hq, Hkv, Sq,
+                                 Skv, st, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale);
+  return dispatch_bwd(p, D, dtype, k_gran, stream);
+}
 
-  BwdParams p{};
+extern "C" int sab_qk_int8_attn_bwd_varlen(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
+                                           const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                           const float* lse, const void* k_mean, void* dq, void* dk, void* dv, void* workspace,
+                                           int dtype, int nseq, int Hq, int Hkv, int Tq, int Tk, int D, int64_t q8_stride_t,
+                                           int64_t q8_stride_h, int64_t k8_stride_t, int64_t k8_stride_h, int64_t q_stride_t,
+                                           int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h, int64_t v_stride_t,
+                                           int64_t v_stride_h, int64_t o_stride_t, int64_t o_stride_h, int64_t do_stride_t,
+                                           int64_t do_stride_h, const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
+                                           const int32_t* cu_q_scale, const int32_t* cu_k_scale, int max_seqlen_q,
+                                           int max_seqlen_k, int is_causal, float sm_scale, int fold_sm_scale, void* stream) {
+  using namespace sab;
+  SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
+              SAB_ERR_INVALID, "null tensor pointer");
+  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
+  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "dtype must be fp16 or bf16");
+  SAB_REQUIRE(nseq > 0 && Hq > 0 && Hkv > 0 && Tq > 0 && Tk > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", nseq, Hq, Hkv, Tq, Tk);
+  SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
+  SAB_REQUIRE(cu_seqlens_q && cu_seqlens_k && cu_q_scale && cu_k_scale && max_seqlen_q > 0 && max_seqlen_k > 0, SAB_ERR_INVALID,
+              "varlen needs cu_seqlens_q, cu_seqlens_k, cu_q_scale, cu_k_scale, max_seqlen_q and max_seqlen_k");
+  // packed [T,H,D]: no batch stride
+  const int64_t st[21] = {0, q8_stride_h, q8_stride_t, 0, k8_stride_h, k8_stride_t, 0, q_stride_h, q_stride_t, 0, k_stride_h, k_stride_t,
+                          0, v_stride_h, v_stride_t, 0, o_stride_h, o_stride_t, 0, do_stride_h, do_stride_t};
+  if (int e = check_bwd_layout(q_int8, k_int8, q, k, v, o, dout, dq, dk, dv, st)) return e;
+  BwdParams p = bwd_params(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, nseq, Hq, Hkv, Tq, Tk,
+                           st, is_causal, SAB_GRAN_PER_BLOCK, SAB_GRAN_PER_BLOCK, sm_scale, fold_sm_scale);
   AttnParams& a = p.a;
-  a.q_scale = q_scale; a.k_scale = k_scale;
-  a.B = B; a.Hq = Hq; a.Hkv = Hkv; a.Sq = Sq; a.Sk = Skv;
-  a.n_q_tiles = (Sq + BM - 1) / BM;
-  a.causal = is_causal ? 1 : 0;
-  a.sm_scale_log2 = fold_sm_scale ? 1.0f : sm_scale * 1.44269504088896340736f;   // as the forward (attn.cu)
-  a.q_gran = q_gran;
-  a.q_mult = q_gran == SAB_GRAN_PER_BLOCK ? 1 : (q_gran == SAB_GRAN_PER_WARP ? 4 : 32);
-  a.k_mult = k_gran == SAB_GRAN_PER_THREAD ? 4 : 1;
-  a.qs_stride_bh = int64_t((Sq + BM - 1) / BM) * a.q_mult;
-  a.ks_stride_bh = int64_t((Skv + 63) / 64) * a.k_mult;
-  a.qs_stride_idx = 1;
-  a.ks_stride_idx = 1;
-  p.q8 = q_int8; p.k8 = k_int8;
-  p.q8_sb = q8_stride_b; p.q8_sh = q8_stride_h; p.q8_ss = q8_stride_s;
-  p.k8_sb = k8_stride_b; p.k8_sh = k8_stride_h; p.k8_ss = k8_stride_s;
-  p.q = static_cast<const uint16_t*>(q); p.k = static_cast<const uint16_t*>(k); p.v = static_cast<const uint16_t*>(v);
-  p.o = static_cast<const uint16_t*>(o); p.dout = static_cast<const uint16_t*>(dout);
-  p.kmean = static_cast<const uint16_t*>(k_mean);
-  p.q_sb = q_stride_b; p.q_sh = q_stride_h; p.q_ss = q_stride_s;
-  p.k_sb = k_stride_b; p.k_sh = k_stride_h; p.k_ss = k_stride_s;
-  p.v_sb = v_stride_b; p.v_sh = v_stride_h; p.v_ss = v_stride_s;
-  p.o_sb = o_stride_b; p.o_sh = o_stride_h; p.o_ss = o_stride_s;
-  p.do_sb = do_stride_b; p.do_sh = do_stride_h; p.do_ss = do_stride_s;
-  p.lse = lse;
-  p.delta = static_cast<float*>(workspace);
-  p.dq = dq; p.dk = dk; p.dv = dv;
-  p.sm_scale = sm_scale;
-
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const bool kt = k_gran == SAB_GRAN_PER_THREAD;
-  const bool bf = dtype == SAB_DTYPE_BF16;
-  if (D == 128) {
-    if (kt) { if (bf) return launch_bwd<128, true, __nv_bfloat16>(p, s); return launch_bwd<128, true, __half>(p, s); }
-    if (bf) return launch_bwd<128, false, __nv_bfloat16>(p, s);
-    return launch_bwd<128, false, __half>(p, s);
-  }
-  if (kt) { if (bf) return launch_bwd<64, true, __nv_bfloat16>(p, s); return launch_bwd<64, true, __half>(p, s); }
-  if (bf) return launch_bwd<64, false, __nv_bfloat16>(p, s);
-  return launch_bwd<64, false, __half>(p, s);
+  a.n_q_tiles = (max_seqlen_q + BM - 1) / BM;
+  p.n_k_tiles = (max_seqlen_k + 127) / 128;
+  a.qs_stride_bh = a.ks_stride_bh = 1;   // scale bases h / hk (batch index 0), blocks [nblocks,H]: the forward's varlen indexing
+  a.qs_stride_idx = Hq;
+  a.ks_stride_idx = Hkv;
+  a.cu_q = cu_seqlens_q; a.cu_k = cu_seqlens_k; a.cu_qs = cu_q_scale; a.cu_ks = cu_k_scale;
+  return dispatch_bwd(p, D, dtype, SAB_GRAN_PER_BLOCK, stream);
 }

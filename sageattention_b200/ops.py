@@ -335,6 +335,42 @@ def _(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, d
     return None
 
 
+@torch.library.custom_op("sageattention_b200::qk_int8_attn_bwd_varlen", mutates_args=("dq", "dk", "dv"), device_types="cuda")
+def qk_int8_attn_bwd_varlen(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale: torch.Tensor, k_scale: torch.Tensor,
+                            q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, o: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor,
+                            k_mean: Optional[torch.Tensor], dq: torch.Tensor, dk: torch.Tensor, dv: torch.Tensor,
+                            cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor, cu_q_scale: torch.Tensor,
+                            cu_k_scale: torch.Tensor, max_seqlen_q: int, max_seqlen_k: int, is_causal: int, sm_scale: float,
+                            fold_sm_scale: int) -> None:
+    """Gradients of the packed FP16-PV attention (include/sageattn_b200.h, sab_qk_int8_attn_bwd_varlen): packed [T,H,D] tensors,
+    q_int8 / k_int8 / per-block scales / cu_q_scale / cu_k_scale from per_block_int8_varlen, lse the forward's [Hq,Tq] log2 LSE
+    (qk_int8_sv_f16_attn_varlen with return_lse=1), k_mean the K mean over all tokens ([Hkv,D] elements, k's dtype; None without
+    smoothing).  dq / dk / dv must have the strides of q / k / v; rows past cu_seqlens_*[-1] are not written."""
+    Tq, Hq, D = q.shape
+    Tk, Hkv, _ = k.shape
+    for x, y in ((dq, q), (dk, k), (dv, v)):
+        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (Hq, Tq), "lse must be [Hq,Tq] fp32"
+    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in (t.stride(0), t.stride(1))]
+    if k_mean is not None:
+        assert k_mean.numel() == Hkv * D and k_mean.dtype == k.dtype, "k_mean must have Hkv*D elements of k's dtype"
+        k_mean = k_mean.reshape(Hkv, D).contiguous()
+    with torch.cuda.device(q.device):
+        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(1, Hq, Tq), dtype=torch.uint8, device=q.device)
+        check(lib().sab_qk_int8_attn_bwd_varlen(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(), k_scale.data_ptr(),
+                                                q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(), lse.data_ptr(),
+                                                _ptr(k_mean), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), ws.data_ptr(), _dt(q),
+                                                cu_seqlens_q.numel() - 1, Hq, Hkv, Tq, Tk, D, *strides, cu_seqlens_q.data_ptr(),
+                                                cu_seqlens_k.data_ptr(), cu_q_scale.data_ptr(), cu_k_scale.data_ptr(), max_seqlen_q,
+                                                max_seqlen_k, is_causal, float(sm_scale), fold_sm_scale, _stream(q)))
+
+
+@qk_int8_attn_bwd_varlen.register_fake
+def _(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, cu_seqlens_q, cu_seqlens_k, cu_q_scale, cu_k_scale,
+      max_seqlen_q, max_seqlen_k, is_causal, sm_scale, fold_sm_scale):
+    return None
+
+
 # ----------------------------------------------------------------------------------------------- FP16-PV variant
 @torch.library.custom_op("sageattention_b200::v_transpose_f16", mutates_args=("v_f16t",), device_types="cuda")
 def v_transpose_f16(v: torch.Tensor, v_f16t: torch.Tensor, tensor_layout: int) -> None:
@@ -433,21 +469,29 @@ def qk_int8_sv_f16_attn_varlen(query: torch.Tensor, key: torch.Tensor, value: to
                                query_scale: torch.Tensor, key_scale: torch.Tensor, cu_seqlens_q: torch.Tensor,
                                cu_seqlens_k: torch.Tensor, cu_pad_v: torch.Tensor, cu_q_scale: torch.Tensor,
                                cu_k_scale: torch.Tensor, max_seqlen_q: int, is_causal: int, sm_scale: float,
-                               fold_sm_scale: int) -> None:
+                               fold_sm_scale: int, return_lse: int = 0) -> torch.Tensor:
+    """Packed [T,H,D] form of qk_int8_sv_f16_attn: mutates `output`, returns lse ([Hq,Tq] fp32 in log2 units, row
+    h*Tq + cu_seqlens_q[b] + i; rows past cu_seqlens_q[-1] are not written), or an empty tensor when return_lse == 0."""
     Tq, Hq, D = query.shape
     Tk, Hkv, _ = key.shape
     nseq = cu_seqlens_q.numel() - 1
+    lse = torch.empty((Hq, Tq), dtype=torch.float32, device=query.device) if return_lse else \
+        torch.empty((0,), dtype=torch.float32, device=query.device)
     with torch.cuda.device(query.device):
-        check(lib().sab_qk_int8_sv_f16_attn(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(), None,
+        check(lib().sab_qk_int8_sv_f16_attn(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
+                                            lse.data_ptr() if return_lse else None,
                                             query_scale.data_ptr(), key_scale.data_ptr(), _dt(output), nseq, Hq, Hkv, Tq, Tk, D,
                                             0, query.stride(1), query.stride(0), 0, key.stride(1), key.stride(0), _v_pad(value),
                                             0, output.stride(1), output.stride(0), is_causal, _capi.SAB_GRAN_PER_BLOCK,
                                             _capi.SAB_GRAN_PER_BLOCK, float(sm_scale), fold_sm_scale, cu_seqlens_q.data_ptr(),
                                             cu_seqlens_k.data_ptr(), cu_pad_v.data_ptr(), cu_q_scale.data_ptr(),
                                             cu_k_scale.data_ptr(), max_seqlen_q, _stream(query)))
+    return lse
 
 
 @qk_int8_sv_f16_attn_varlen.register_fake
 def _(query, key, value, output, query_scale, key_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale,
-      max_seqlen_q, is_causal, sm_scale, fold_sm_scale):
-    return None
+      max_seqlen_q, is_causal, sm_scale, fold_sm_scale, return_lse=0):
+    if return_lse:
+        return torch.empty((query.size(1), query.size(0)), dtype=torch.float32, device=query.device)
+    return torch.empty((0,), dtype=torch.float32, device=query.device)

@@ -9,7 +9,12 @@ and the GPU name and power limit.  CUDA events after warm-up; writes nothing.
 
 --varlen: the same for sageattn_varlen on a packed GQA batch (lens 4096, 512, 16384, 1024, 8192, 2048; Hq=32, Hkv=8, D=128, bf16),
 non-causal and causal, counting 10*Hq*D*sum(Lq*Lk) FLOPs (only the visible pairs for causal), with the sum of per-sequence torch
-SDPA flash backwards for context."""
+SDPA flash backwards for context.
+
+--masked: the same for sageattn_qk_int8_pv_fp16_triton with attn_mask (B=1, H=32, S=8192, D=128, bf16, non-causal, 10*B*H*S^2*D
+FLOPs whatever the mask hides): (a) a bool mask [1,1,S,S] and (b) a bias [1,H,S,S] that requires grad, so the kernels also write
+the dense dBias.  For context, torch SDPA's memory-efficient backward on the same inputs with the same mask as a float additive
+mask (False -> -inf for (a); bias*ln2, requiring grad, for (b))."""
 import argparse
 import json
 import subprocess
@@ -109,6 +114,58 @@ def varlen(a):
     print(json.dumps(out))
 
 
+def masked(a):
+    import math
+    import sageattention_b200 as sab
+    from sageattention_b200 import ops
+
+    B, H, S, D = 1, 32, 8192, 128
+    dt = torch.bfloat16
+    g = torch.Generator(device="cuda").manual_seed(0)
+    q, k, v, do = (torch.randn(B, H, S, D, device="cuda", dtype=dt, generator=g) for _ in range(4))
+    sm = D ** -0.5
+    flops = 10.0 * B * H * S * S * D
+    out = {"metric": "sageattn_qk_int8_pv_fp16_triton masked backward", "shape": {"B": B, "H": H, "S": S, "D": D, "dtype": "bf16"},
+           "gpu": _gpu()}
+    masks = {
+        "bool_1_1_S_S": torch.rand(1, 1, S, S, device="cuda", generator=g) > 0.2,
+        "bias_1_H_S_S": torch.randn(1, H, S, S, device="cuda", dtype=dt, generator=g).requires_grad_(True),
+    }
+    for name, mask in masks.items():
+        bias = mask.dtype != torch.bool
+        # kernels alone, on the operands the forward uses
+        km = sab.k_mean(k)
+        q8, qs, k8, ks = sab.per_block_int8(q, k, km, sm_scale=sm)
+        me = mask.detach().expand(B, H, S, S)
+        o = torch.empty_like(q)
+        lse = ops.qk_int8_sv_f16_attn_masked(q8, k8, sab.transpose_v_f16(v), o, qs, ks, me, 1, 1, 1, sm, 1, 1)
+        dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        dbias = torch.empty(B, H, S, S, device="cuda", dtype=dt) if bias else None
+        t_kern = _events(lambda: ops.qk_int8_attn_bwd_masked(q8, k8, qs, ks, q, k, v, o, do, lse, km, dq, dk, dv, me, dbias, 1, 1, 1,
+                                                             sm, 1), a.steps, a.warmup)
+        del dbias
+        # the public call
+        qg, kg, vg = (t.clone().requires_grad_(True) for t in (q, k, v))
+        ins = (qg, kg, vg) + ((mask,) if bias else ())
+        ob = sab.sageattn_qk_int8_pv_fp16_triton(qg, kg, vg, attn_mask=mask)
+        t_bwd = _events(lambda: torch.autograd.grad(ob, ins, do, retain_graph=True), a.steps, a.warmup)
+        del ob
+        # torch SDPA memory-efficient backward, same inputs, the mask as a float additive mask
+        fm = (mask.detach().float() * math.log(2.0)).to(dt).requires_grad_(True) if bias else \
+            torch.zeros(mask.shape, device="cuda", dtype=dt).masked_fill(~mask, float("-inf"))
+        with torch.nn.attention.sdpa_kernel(torch.nn.attention.SDPBackend.EFFICIENT_ATTENTION):
+            os_ = F.scaled_dot_product_attention(qg, kg, vg, attn_mask=fm)
+            sins = (qg, kg, vg) + ((fm,) if bias else ())
+            t_sdpa = _events(lambda: torch.autograd.grad(os_, sins, do, retain_graph=True), a.steps, a.warmup)
+        out[name] = {
+            "bwd_kernel": {"ms": round(t_kern, 3), "tflops": round(flops / t_kern / 1e9, 1)},
+            "bwd_call": {"ms": round(t_bwd, 3), "tflops": round(flops / t_bwd / 1e9, 1)},
+            "sdpa_efficient_bwd": {"ms": round(t_sdpa, 3), "tflops": round(flops / t_sdpa / 1e9, 1)},
+        }
+        del os_, fm
+    print(json.dumps(out))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--B", type=int, default=4)
@@ -118,10 +175,13 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--varlen", action="store_true", help="sageattn_varlen on a packed GQA batch instead of sageattn")
+    ap.add_argument("--masked", action="store_true", help="sageattn_qk_int8_pv_fp16_triton with attn_mask instead of sageattn")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_backward.py needs a GPU"
     if a.varlen:
         return varlen(a)
+    if a.masked:
+        return masked(a)
     import sageattention_b200 as sab
     from sageattention_b200 import ops
 

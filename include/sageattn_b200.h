@@ -271,8 +271,8 @@ int sab_qk_int8_sv_f8_attn_sp(const int8_t* q_int8, const int8_t* k_int8, const 
  *            forward's O) is not multiplied by a large K mean;
  *   dq, dk, dv : outputs in `dtype` with the strides of q, k, v.  GQA: dk / dv are summed over the Q heads of each KV head.
  *   workspace : >= sab_attn_bwd_workspace_bytes(B, Hq, Sq) bytes of device scratch.
- * Dense (packed sequences: sab_qk_int8_attn_bwd_varlen below); is_causal needs Sq == Skv (top-left).  Deterministic: no atomics,
- * a fixed summation order.
+ * Dense (packed sequences: sab_qk_int8_attn_bwd_varlen below; with the masked forward's attn_mask: sab_qk_int8_attn_bwd_masked);
+ * is_causal needs Sq == Skv (top-left).  Deterministic: no atomics, a fixed summation order.
  * ---------------------------------------------------------------------------------------------- */
 int64_t sab_attn_bwd_workspace_bytes(int B, int Hq, int Sq);
 int sab_qk_int8_attn_bwd(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale, const void* q,
@@ -307,6 +307,29 @@ int sab_qk_int8_attn_bwd_varlen(const int8_t* q_int8, const int8_t* k_int8, cons
                                 const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k, const int32_t* cu_q_scale,
                                 const int32_t* cu_k_scale, int max_seqlen_q, int max_seqlen_k, int is_causal, float sm_scale,
                                 int fold_sm_scale, void* stream);
+
+/* Masked form of sab_qk_int8_attn_bwd: the gradient of sab_qk_int8_sv_f16_attn_masked (the kernel behind
+ * sageattn_qk_int8_pv_fp16_triton with attn_mask).  Same definition and arguments as sab_qk_int8_attn_bwd without is_causal (the
+ * masked forward is non-causal), with the forward's masked logits:
+ *   SAB_MASK_BOOL : P = 0 where the mask element is 0;
+ *   SAB_MASK_BIAS : P = exp2(x - lse) with x = S*log2e + bias in fp32 (the forward's expression; bias -inf gives P = 0);
+ *   a row with lse = -inf has no visible key (the forward returned zeros): its P and gradients are 0.
+ *   attn_mask, mask_kind, mask_stride_* : exactly what the forward received (element strides of the [B,Hq,Sq,Skv] broadcast view,
+ *            0 allowed); K scales per block / per warp, as the forward requires;
+ *   dbias  : nullable, SAB_MASK_BIAS only: dense row-major [B,Hq,Sq,Skv] in `dtype`, 16-byte aligned, written with
+ *            dBias = ln2 * dS (the bias is added to log2-unit logits, so it acts as bias*ln2 in natural-log units); masked and -inf
+ *            positions get 0.  Summing it over the broadcast dimensions is the caller's (autograd's expand backward).
+ * Deterministic like the dense form: every dBias element is written once, by the CTA that owns its Q row. */
+int sab_qk_int8_attn_bwd_masked(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale, const void* q,
+                                const void* k, const void* v, const void* o, const void* dout, const float* lse, const void* k_mean,
+                                void* dq, void* dk, void* dv, void* workspace, int dtype, int B, int Hq, int Hkv, int Sq, int Skv, int D,
+                                int64_t q8_stride_b, int64_t q8_stride_h, int64_t q8_stride_s, int64_t k8_stride_b,
+                                int64_t k8_stride_h, int64_t k8_stride_s, int64_t q_stride_b, int64_t q_stride_h, int64_t q_stride_s,
+                                int64_t k_stride_b, int64_t k_stride_h, int64_t k_stride_s, int64_t v_stride_b, int64_t v_stride_h,
+                                int64_t v_stride_s, int64_t o_stride_b, int64_t o_stride_h, int64_t o_stride_s, int64_t do_stride_b,
+                                int64_t do_stride_h, int64_t do_stride_s, int q_gran, int k_gran, float sm_scale, int fold_sm_scale,
+                                const void* attn_mask, int mask_kind, int64_t mask_stride_b, int64_t mask_stride_h,
+                                int64_t mask_stride_m, int64_t mask_stride_n, void* dbias, void* stream);
 
 #ifdef __cplusplus
 }

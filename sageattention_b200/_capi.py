@@ -46,6 +46,8 @@ EXPORTS = {
     "sab_qk_int8_attn_bwd": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_int64] * 21 + [c_int, c_int, c_int, c_float, c_int, c_void_p]),
     "sab_qk_int8_attn_bwd_varlen": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_int64] * 14 + [c_void_p] * 4 +
                                     [c_int, c_int, c_int, c_float, c_int, c_void_p]),
+    "sab_qk_int8_attn_bwd_masked": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_int64] * 21 + [c_int, c_int, c_float, c_int] +
+                                    [c_void_p, c_int] + [c_int64] * 4 + [c_void_p, c_void_p]),
 }
 
 _lib = None

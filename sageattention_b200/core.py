@@ -137,6 +137,57 @@ def _dense_call(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale
     return o
 
 
+# ------------------------------------------------------------------------------------------------ masked call and its gradient
+def _expand_mask(attn_mask, q, k, tensor_layout):
+    """attn_mask as the [B,Hq,Sq,Skv] view the masked kernels read (core.py:314-323): broadcast dimensions get stride 0."""
+    if tensor_layout == "HND":
+        target_shape = (q.shape[0], q.shape[1], q.shape[2], k.shape[2])
+    else:
+        target_shape = (q.shape[0], q.shape[2], q.shape[1], k.shape[1])
+    try:
+        return attn_mask.expand(target_shape)
+    except Exception:
+        raise AssertionError(f"attn_mask shape {attn_mask.shape} cannot be broadcast to {target_shape}")
+
+
+class _SageAttnMaskedFunction(torch.autograd.Function):
+    """sageattn_qk_int8_pv_fp16_triton with attn_mask and a gradient: the straight-through gradient of _SageAttnFunction at the
+    forward's masked logits (include/sageattn_b200.h, sab_qk_int8_attn_bwd_masked), and for a float mask dBias = ln2 * dS.
+    forward: the unchanged masked forward with the kernel LSE enabled; saves q, k, v, o, the LSE and the expanded mask view.
+    backward: re-runs the K mean and per_block_int8 with the same quantization_backend, then the two gradient kernels.  The mask
+    arrives as its expanded [B,Hq,Sq,Skv] view, so the kernels write a dense dBias and autograd's expand backward sums it over the
+    broadcast dimensions.  That dBias costs B*Hq*Sq*Skv elements of the bias dtype, allocated during the backward and only when
+    the bias requires grad.  The LSE and the K mean are returned for the LSE correction and carry no gradient."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, attn_mask, tensor_layout, sm_scale, smooth_k, backend):
+        km, q_int8, q_scale, k_int8, k_scale, _, _, _ = _quant_qk(q, k, "fp16_triton", tensor_layout, "per_block", sm_scale, smooth_k,
+                                                                  backend)
+        v_t = transpose_v_f16(v, tensor_layout=tensor_layout)
+        o = torch.empty(q.size(), dtype=q.dtype, device=q.device)
+        lse = ops.qk_int8_sv_f16_attn_masked(q_int8, k_int8, v_t, o, q_scale, k_scale, attn_mask, 0 if tensor_layout == "NHD" else 1,
+                                             SAB_GRAN_PER_BLOCK, SAB_GRAN_PER_BLOCK, sm_scale, 1, 1)
+        ctx.save_for_backward(q, k, v, o, lse, attn_mask)
+        ctx.cfg = (tensor_layout, sm_scale, smooth_k, backend)
+        km = km if km is not None else q.new_empty(0)
+        ctx.mark_non_differentiable(lse, km)
+        return o, lse, km
+
+    @staticmethod
+    def backward(ctx, do, _dlse, _dkm):
+        tensor_layout, sm_scale, smooth_k, backend = ctx.cfg
+        q, k, v, o, lse, attn_mask = ctx.saved_tensors
+        km, q_int8, q_scale, k_int8, k_scale, q_gran, k_gran, fold = _quant_qk(q, k, "fp16_triton", tensor_layout, "per_block",
+                                                                             sm_scale, smooth_k, backend)
+        # the kernels read 16-bit rows with 16-byte loads; dq / dk / dv take the strides of q / k / v
+        q, k, v, o, do = (t.contiguous() for t in (q, k, v, o, do))
+        dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        dbias = torch.empty(attn_mask.shape, dtype=attn_mask.dtype, device=q.device) if ctx.needs_input_grad[3] else None
+        ops.qk_int8_attn_bwd_masked(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv, attn_mask, dbias,
+                                    0 if tensor_layout == "NHD" else 1, q_gran, k_gran, sm_scale, fold)
+        return dq, dk, dv, dbias, None, None, None, None
+
+
 def sageattn_qk_int8_pv_fp8_cuda(
     q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, tensor_layout: str = "HND", is_causal: bool = False,
     qk_quant_gran: str = "per_thread", sm_scale: Optional[float] = None, pv_accum_dtype: str = "fp32+fp16",
@@ -212,7 +263,9 @@ def sageattn_qk_int8_pv_fp16_triton(q, k, v, tensor_layout: str = "HND", quantiz
     V in fp16, softmax without exponent offset — the Triton kernel's numerics, triton/attn_qk_int8_per_block.py).
     attn_mask (bool, or the q dtype as an additive bias; broadcast to [B,Hq,Sq,Skv]; non-causal only) follows
     core.py:248-250, 310-325 and attn_qk_int8_per_block.py:33-52 — including the reference's convention that a float
-    bias is added AFTER the logits were scaled by sm_scale*log2(e), i.e. it acts as bias*ln(2) in natural-log units."""
+    bias is added AFTER the logits were scaled by sm_scale*log2(e), i.e. it acts as bias*ln(2) in natural-log units.
+    Differentiable (no reference counterpart) when grad mode is on and q, k, v or a float attn_mask requires grad, with or without
+    a mask; a float mask then gets dBias = ln(2) * dS, summed over its broadcast dimensions (_SageAttnMaskedFunction)."""
     dtype = q.dtype
     _check_inputs(q, k, v)
     if attn_mask is not None:
@@ -229,7 +282,15 @@ def sageattn_qk_int8_pv_fp16_triton(q, k, v, tensor_layout: str = "HND", quantiz
     if attn_mask is None:
         return _dense_call(q, k, v, "fp16_triton", tensor_layout, is_causal, "per_block", sm_scale, smooth_k, False, 0.0,
                            quantization_backend, return_lse, head_dim_og)
-    # attn_mask: forward only
+    if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad or attn_mask.requires_grad):
+        # the differentiable form (a bool mask cannot require grad); the returned lse carries no gradient
+        o, lse, km = _SageAttnMaskedFunction.apply(q, k, v, _expand_mask(attn_mask, q, k, tensor_layout), tensor_layout, sm_scale,
+                                                   smooth_k, quantization_backend)
+        o = o[..., :head_dim_og]
+        if return_lse:
+            q = q.detach()
+            return o, lse / _LOG2E + _lse_correction(q, km, tensor_layout) * sm_scale if smooth_k else lse / _LOG2E
+        return o
     lse_correction = None
     if smooth_k:
         km = k_mean(k, tensor_layout)
@@ -241,14 +302,7 @@ def sageattn_qk_int8_pv_fp16_triton(q, k, v, tensor_layout: str = "HND", quantiz
                                                       semantics=quantization_backend)
     v_t = transpose_v_f16(v, tensor_layout=tensor_layout)       # `v.to(torch.float16)`, core.py:297-298
     o = torch.empty(q.size(), dtype=dtype, device=q.device)
-    if tensor_layout == "HND":
-        target_shape = (q.shape[0], q.shape[1], q.shape[2], k.shape[2])
-    else:
-        target_shape = (q.shape[0], q.shape[2], q.shape[1], k.shape[1])
-    try:
-        attn_mask = attn_mask.expand(target_shape)     # core.py:314-323; a view: broadcast dims get stride 0
-    except Exception:
-        raise AssertionError(f"attn_mask shape {attn_mask.shape} cannot be broadcast to {target_shape}")
+    attn_mask = _expand_mask(attn_mask, q, k, tensor_layout)
     lse = ops.qk_int8_sv_f16_attn_masked(q_int8, k_int8, v_t, o, q_scale, k_scale, attn_mask, _tensor_layout,
                                          SAB_GRAN_PER_BLOCK, SAB_GRAN_PER_BLOCK, sm_scale, 1, 1 if return_lse else 0)
     o = o[..., :head_dim_og]

@@ -20,6 +20,13 @@
 // CTA decodes its sequence's token offsets, lengths and first scale blocks once, as the forward does (attn.cu), and the loops below
 // read those.  The causal mask is top-left inside each sequence.  delta runs on the packed rows as B = 1, so it has the LSE's
 // [Hq,Tq] layout.
+// Masked (p.a.mask != nullptr, the attn_mask of the dense non-causal FP16-PV forward, per-block / per-warp K scales): separate
+// kernels bwd_dq_masked_kernel / bwd_dkdv_masked_kernel branch once on the mask kind into the same bodies compiled with the mask.
+// P is the forward's masked P: a bool mask (0 = masked out) zeroes elements, a bias enters as exp2(fmaf(S, coef, bias) - lse)
+// (the forward's tile_bias), and a row with lse = -inf (no visible key: the forward returned zeros) has P = 0.  The dQ kernel
+// reads the mask along its rows, as the forward does, and writes dBias = ln2 * dS (the bias is added to log2-unit logits) for
+// the elements of its own rows, so dBias needs no atomics either.  The dK/dV kernel stages each [64 Q rows x 128 keys] mask tile
+// of Q head h in shared memory with the other operands.
 // Products are wgmma with fp32 accumulation: INT8 for S as in the forward, bf16 / f16 for the rest.  Every B operand is K-major in
 // shared memory, in the swizzled layout the forward's TMA loads write; the operands the math needs transposed (dO^T, Q^T, K^T) are
 // transposed by the loaders.  Loads are plain: all threads copy a tile, the CTA synchronises, then computes (no load/compute
@@ -148,6 +155,60 @@ __device__ __forceinline__ void store_rows(const float (&acc)[D / 2], T* row0, T
   }
 }
 
+// ------------------------------------------------------------------------------------------------ attention mask
+// kMask: 0 (unmasked kernels), SAB_MASK_BOOL (uint8 elements, 0 = masked out) or SAB_MASK_BIAS (16-bit elements of T)
+template <int kMask>
+using MaskElem = std::conditional_t<kMask == SAB_MASK_BOOL, uint8_t, uint16_t>;
+constexpr float kLn2 = 0.69314718055994530942f;
+
+// -lse of a row of the masked kernels.  A row whose keys are all masked has lse = -inf (the forward returned zeros): -inf here
+// makes its P exactly 0, where -lse = +inf would give exp2(+inf) on a bool row and -inf + inf = NaN on a bias row.
+__device__ __forceinline__ float masked_nlse(float lse) { return lse == -INFINITY ? -INFINITY : -lse; }
+
+// P of one visible element of a masked kernel: s its int32 logit, coef its dequant coefficient, m its mask element
+template <int kMask, typename T>
+__device__ __forceinline__ float masked_p(uint32_t s, float coef, float nlse, uint32_t m) {
+  if constexpr (kMask == SAB_MASK_BOOL) {
+    return m != 0 ? ex2_approx(logit_log2(s, coef, nlse)) : 0.f;
+  } else {
+    float bias;
+    if constexpr (std::is_same_v<T, __half>) bias = __half2float(__ushort_as_half(uint16_t(m)));
+    else bias = __bfloat162float(__ushort_as_bfloat16(uint16_t(m)));
+    return ex2_approx(fmaf(__int2float_rn(int(s)), coef, bias) + nlse);   // the forward's tile_bias logit, then - lse
+  }
+}
+
+// Row stride (elements) of the dK/dV kernel's staged mask tile: the 4 lanes of a quad read 4 different Q rows of one key, and
+// these strides put them in different banks (272 / 144 bytes, multiples of 16 for the vector stores)
+template <int kMask>
+constexpr int kMaskTileRow = kMask == SAB_MASK_BOOL ? 144 : 136;
+constexpr size_t kMaskTileBytes = size_t(64) * 136 * 2;   // the larger of the two kinds
+
+// Mask elements of rows [q0, q0 + 64) x keys [k0, k0 + 128) of (b, h) into a row-major tile (Q row r at r * kMaskTileRow);
+// elements of rows >= q_len or keys >= kv_len are stored masked (bool 0, bias -inf).  16-byte loads along the keys when the
+// keys are contiguous and the rows 16-byte aligned, element loads with general strides otherwise.
+template <int kMask, typename T>
+__device__ __forceinline__ void load_mask_tile(uint8_t* tile, const AttnParams& a, int b, int h, int q0, int k0, int q_len,
+                                               int kv_len) {
+  using E = MaskElem<kMask>;
+  constexpr int EB = sizeof(E), ROW = kMaskTileRow<kMask>, V = 16 / EB, KB = 128, QB = 64;
+  constexpr E fill = kMask == SAB_MASK_BOOL ? E(0) : E(std::is_same_v<T, __half> ? 0xFC00u : 0xFF80u);   // -inf
+  const E* base = reinterpret_cast<const E*>(a.mask) + int64_t(b) * a.mask_sb + int64_t(h) * a.mask_sh;
+  const bool vec = a.mask_sn == 1 &&
+                   ((reinterpret_cast<uintptr_t>(a.mask) | uint64_t(a.mask_sb * EB) | uint64_t(a.mask_sh * EB) | uint64_t(a.mask_sm * EB)) & 15) == 0;
+  const int step = vec ? V : 1;
+  for (int idx = threadIdx.x * step; idx < QB * KB; idx += kBwdThreads * step) {
+    const int r = idx / KB, c = idx % KB, q = q0 + r, key = k0 + c;
+    const E* src = base + int64_t(q) * a.mask_sm + int64_t(key) * a.mask_sn;
+    E* dst = reinterpret_cast<E*>(tile) + r * ROW + c;
+    if (vec && q < q_len && key + V <= kv_len) {
+      *reinterpret_cast<uint4*>(dst) = __ldg(reinterpret_cast<const uint4*>(src));
+    } else {
+      for (int u = 0; u < step; ++u) dst[u] = (q < q_len && key + u < kv_len) ? __ldg(src + u) : fill;   // sn == 1 when step > 1
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ work decode
 // The tokens of this CTA's batch entry (attn.cu's work decode).  Dense: batch b, all Sq / Sk rows.  Varlen: sequence b of the
 // packed tensors (stride_b 0), whose scales start at 128-row Q block q_blk0 and 64-key block k_blk0; the scale bases are then h and
@@ -195,8 +256,9 @@ constexpr size_t bwd_dq_smem_bytes() {
   return size_t(128) * D + size_t(128) * D * 2 + size_t(64) * D + size_t(64) * D * 2 + size_t(D) * 64 * 2 + 1024;
 }
 
-template <int D, bool kKT, typename T, bool kVarlen>
-__device__ __forceinline__ void bwd_dq_tile(const BwdParams& p) {
+// dbias (masked, nullable): dense [B,Hq,Sq,Skv] in T, written with ln2 * dS
+template <int D, bool kKT, typename T, bool kVarlen, int kMask = 0>
+__device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nullptr) {
   constexpr int QB = 128, KB = 64;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ8 = smem;                       // [128 x D] int8        A of S = Q K^T
@@ -229,8 +291,17 @@ __device__ __forceinline__ void bwd_dq_tile(const BwdParams& p) {
     qss[i] = q_dequant_log2(a, qs_base, sq.q_blk0 + qt, row0 + 8 * i);   // scales are padded to whole 128-row blocks
     const bool ok = q_row[i] < sq.q_len;
     const int64_t li = (int64_t(sq.tb) * a.Hq + h) * a.Sq + sq.q_off + q_row[i];
-    nlse[i] = ok ? -p.lse[li] : 0.f;
+    if constexpr (kMask != 0) nlse[i] = ok ? masked_nlse(p.lse[li]) : -INFINITY;
+    else nlse[i] = ok ? -p.lse[li] : 0.f;
     dlt[i] = ok ? p.delta[li] : 0.f;
+  }
+  // masked: this thread's two rows of the mask (dense, non-varlen); rows >= Sq are never read
+  [[maybe_unused]] const MaskElem<kMask>* mrow[2];
+  if constexpr (kMask != 0) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+      mrow[i] = reinterpret_cast<const MaskElem<kMask>*>(a.mask) + int64_t(b) * a.mask_sb + int64_t(h) * a.mask_sh +
+                int64_t(q_row[i]) * a.mask_sm;
   }
   int n_kv = (sq.kv_len + KB - 1) / KB;
   if (a.causal) n_kv = min(n_kv, ((qt + 1) * QB + KB - 1) / KB);
@@ -240,6 +311,20 @@ __device__ __forceinline__ void bwd_dq_tile(const BwdParams& p) {
   for (int i = 0; i < D / 2; ++i) dq[i] = 0.f;
 
   for (int j = 0; j < n_kv; ++j) {
+    // masked: the mask elements of this thread's S elements of tile j, issued first so that their latency overlaps the tile loads
+    // and the MMAs; rows >= Sq and keys >= Skv are not read
+    [[maybe_unused]] uint32_t mv[32];
+    if constexpr (kMask != 0) {
+#pragma unroll
+      for (int c = 0; c < 16; ++c) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int key = j * KB + 8 * (c >> 1) + 2 * t + (c & 1);
+          mv[4 * (c >> 1) + 2 * i + (c & 1)] =
+              q_row[i] < sq.q_len && key < sq.kv_len ? __ldg(mrow[i] + int64_t(key) * a.mask_sn) : 0u;
+        }
+      }
+    }
     __syncthreads();   // the previous tile's operands are consumed
     load_tile<KB, D, 1>(sK8, p.k8 + b * p.k8_sb + hk * p.k8_sh + sq.k_off * p.k8_ss, p.k8_ss, j * KB, sq.kv_len);
     load_tile<KB, D, 2>(sV, p.v + b * p.v_sb + hk * p.v_sh + sq.k_off * p.v_ss, p.v_ss, j * KB, sq.kv_len);
@@ -278,8 +363,33 @@ __device__ __forceinline__ void bwd_dq_tile(const BwdParams& p) {
       for (int i = 0; i < 2; ++i) {
         const int idx = 4 * (c >> 1) + 2 * i + (c & 1);
         const int key = 8 * (c >> 1) + 2 * t + (c & 1);
-        const float pe = key < limit[i] ? ex2_approx(logit_log2(s[idx], coef[i], nlse[i])) : 0.f;
+        float pe;
+        if constexpr (kMask != 0)
+          pe = key < limit[i] ? masked_p<kMask, T>(s[idx], coef[i], nlse[i], mv[idx]) : 0.f;
+        else
+          pe = key < limit[i] ? ex2_approx(logit_log2(s[idx], coef[i], nlse[i])) : 0.f;
         ds[idx] = pe * (dp[idx] - dlt[i]);
+      }
+    }
+    if constexpr (kMask == SAB_MASK_BIAS) {
+      // dBias = ln2 * dS of this thread's elements (keys 8n + 2t, 8n + 2t + 1 of both rows), rows < Sq and keys < Skv only
+      if (dbias != nullptr) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          if (q_row[i] >= sq.q_len) continue;
+          T* drow = reinterpret_cast<T*>(dbias) + ((int64_t(b) * a.Hq + h) * a.Sq + q_row[i]) * a.Sk;
+#pragma unroll
+          for (int n = 0; n < 8; ++n) {
+            const int key = j * KB + 8 * n + 2 * t, idx = 4 * n + 2 * i;
+            const float g0 = kLn2 * ds[idx], g1 = kLn2 * ds[idx + 1];
+            if (key + 1 < a.Sk && (a.Sk & 1) == 0) {   // an even row length keeps the pair 4-byte aligned
+              *reinterpret_cast<uint32_t*>(drow + key) = pack2<T>(g0, g1);
+            } else {
+              if (key < a.Sk) drow[key] = T(g0);
+              if (key + 1 < a.Sk) drow[key + 1] = T(g1);
+            }
+          }
+        }
       }
     }
     uint32_t da[4][4];
@@ -303,13 +413,20 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_kernel(const __grid_con
   else bwd_dq_tile<D, kKT, T, false>(p);
 }
 
+// the masked form: dense, non-causal, per-block / per-warp K scales (those of the masked forward)
+template <int D, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_masked_kernel(const __grid_constant__ BwdParams p, void* dbias) {
+  if (p.a.mask_kind == SAB_MASK_BOOL) bwd_dq_tile<D, false, T, false, SAB_MASK_BOOL>(p);
+  else bwd_dq_tile<D, false, T, false, SAB_MASK_BIAS>(p, dbias);
+}
+
 // ------------------------------------------------------------------------------------------------ dK, dV
 template <int D>
 constexpr size_t bwd_dkdv_smem_bytes() {
   return size_t(128) * D + size_t(128) * D * 2 + size_t(64) * D + size_t(64) * D * 2 + 2 * size_t(D) * 64 * 2 + 3 * 64 * 4 + 1024;
 }
 
-template <int D, bool kKT, typename T, bool kVarlen>
+template <int D, bool kKT, typename T, bool kVarlen, int kMask = 0>
 __device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p) {
   constexpr int KB = 128, QB = 64;
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -322,6 +439,7 @@ __device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p) {
   float* s_qss = reinterpret_cast<float*>(sQt + D * QB * 2);   // per Q row of the tile: q dequant scale, -lse, delta
   float* s_nlse = s_qss + QB;
   float* s_dlt = s_nlse + QB;
+  [[maybe_unused]] uint8_t* s_mask = reinterpret_cast<uint8_t*>(s_dlt + QB);   // masked: [64 Q rows x 128 keys] (load_mask_tile)
   const AttnParams& a = p.a;
 
   const int k0 = blockIdx.x * KB, hk = blockIdx.y, b = blockIdx.z;
@@ -360,12 +478,14 @@ __device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p) {
       load_tile<QB, D, 2>(sdO, p.dout + b * p.do_sb + h * p.do_sh + sq.q_off * p.do_ss, p.do_ss, q0, sq.q_len);
       load_tile_t<D, T>(sdOt, p.dout + b * p.do_sb + h * p.do_sh + sq.q_off * p.do_ss, p.do_ss, q0, sq.q_len);
       load_tile_t<D, T>(sQt, p.q + b * p.q_sb + h * p.q_sh + sq.q_off * p.q_ss, p.q_ss, q0, sq.q_len);
+      if constexpr (kMask != 0) load_mask_tile<kMask, T>(s_mask, a, b, h, q0, k0, sq.q_len, sq.kv_len);   // Q head h, not hk
       if (threadIdx.x < QB) {
         const int r = q0 + threadIdx.x;
         const bool ok = r < sq.q_len;
         const int64_t li = (int64_t(sq.tb) * a.Hq + h) * a.Sq + sq.q_off + r;
         s_qss[threadIdx.x] = ok ? q_dequant_log2(a, qs_base, sq.q_blk0 + r / 128, r % 128) : 0.f;
-        s_nlse[threadIdx.x] = ok ? -p.lse[li] : 0.f;
+        if constexpr (kMask != 0) s_nlse[threadIdx.x] = ok ? masked_nlse(p.lse[li]) : -INFINITY;
+        else s_nlse[threadIdx.x] = ok ? -p.lse[li] : 0.f;
         s_dlt[threadIdx.x] = ok ? p.delta[li] : 0.f;
       }
       fence_proxy_async_smem();
@@ -393,7 +513,13 @@ __device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p) {
           const int col = 8 * (c >> 1) + 2 * t + (c & 1);
           const int q = q0 + col;
           const bool ok = key[i] < sq.kv_len && q < sq.q_len && (!a.causal || key[i] <= q);
-          const float pe = ok ? ex2_approx(logit_log2(s[idx], ksr[i] * s_qss[col], s_nlse[col])) : 0.f;
+          float pe;
+          if constexpr (kMask != 0)
+            pe = ok ? masked_p<kMask, T>(s[idx], ksr[i] * s_qss[col], s_nlse[col],
+                                         reinterpret_cast<const MaskElem<kMask>*>(s_mask)[col * kMaskTileRow<kMask> + kr + 8 * i])
+                    : 0.f;
+          else
+            pe = ok ? ex2_approx(logit_log2(s[idx], ksr[i] * s_qss[col], s_nlse[col])) : 0.f;
           pt[idx] = pe;
           dst[idx] = pe * (dp[idx] - s_dlt[col]);
         }
@@ -426,8 +552,17 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_kernel(const __grid_c
   else bwd_dkdv_tile<D, kKT, T, false>(p);
 }
 
-template <int D, bool kKT, typename T>
-static int launch_bwd(const BwdParams& p, cudaStream_t stream) {
+template <int D, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_masked_kernel(const __grid_constant__ BwdParams p) {
+  if (p.a.mask_kind == SAB_MASK_BOOL) bwd_dkdv_tile<D, false, T, false, SAB_MASK_BOOL>(p);
+  else bwd_dkdv_tile<D, false, T, false, SAB_MASK_BIAS>(p);
+}
+
+// delta, then the dQ kernel kq (smem_q bytes, arguments p, q_args...) and the dK/dV kernel kkv (smem_kv bytes); cfg_*: their
+// per-device smem opt-in
+template <typename T, typename KQ, typename KKV, typename... QArgs>
+static int launch_bwd_kernels(const BwdParams& p, int D, KQ kq, size_t smem_q, bool (&cfg_q)[64], KKV kkv, size_t smem_kv,
+                              bool (&cfg_kv)[64], cudaStream_t stream, QArgs... q_args) {
   {
     BwdParams pd = p;
     if (p.a.cu_q != nullptr) pd.a.B = 1;   // varlen: every packed row, [Hq,Tq] like the LSE
@@ -435,23 +570,27 @@ static int launch_bwd(const BwdParams& p, cudaStream_t stream) {
     bwd_delta_kernel<T><<<unsigned((rows + 7) / 8), 256, 0, stream>>>(pd, D);
     SAB_CUDA_OK(cudaGetLastError());
   }
-  {
-    constexpr size_t smem = bwd_dq_smem_bytes<D>();
-    auto kern = bwd_dq_kernel<D, kKT, T>;
-    static bool configured[64] = {};
-    if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
-    kern<<<dim3(p.a.n_q_tiles, p.a.Hq, p.a.B), kBwdThreads, smem, stream>>>(p);
-    SAB_CUDA_OK(cudaGetLastError());
-  }
-  {
-    constexpr size_t smem = bwd_dkdv_smem_bytes<D>();
-    auto kern = bwd_dkdv_kernel<D, kKT, T>;
-    static bool configured[64] = {};
-    if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
-    kern<<<dim3(p.n_k_tiles, p.a.Hkv, p.a.B), kBwdThreads, smem, stream>>>(p);
-    SAB_CUDA_OK(cudaGetLastError());
-  }
+  if (int st = ensure_dynamic_smem(kq, smem_q, cfg_q)) return st;
+  kq<<<dim3(p.a.n_q_tiles, p.a.Hq, p.a.B), kBwdThreads, smem_q, stream>>>(p, q_args...);
+  SAB_CUDA_OK(cudaGetLastError());
+  if (int st = ensure_dynamic_smem(kkv, smem_kv, cfg_kv)) return st;
+  kkv<<<dim3(p.n_k_tiles, p.a.Hkv, p.a.B), kBwdThreads, smem_kv, stream>>>(p);
+  SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
+}
+
+template <int D, bool kKT, typename T>
+static int launch_bwd(const BwdParams& p, cudaStream_t stream) {
+  static bool cfg_q[64] = {}, cfg_kv[64] = {};
+  return launch_bwd_kernels<T>(p, D, bwd_dq_kernel<D, kKT, T>, bwd_dq_smem_bytes<D>(), cfg_q, bwd_dkdv_kernel<D, kKT, T>,
+                               bwd_dkdv_smem_bytes<D>(), cfg_kv, stream);
+}
+
+template <int D, typename T>
+static int launch_bwd_masked(const BwdParams& p, void* dbias, cudaStream_t stream) {
+  static bool cfg_q[64] = {}, cfg_kv[64] = {};
+  return launch_bwd_kernels<T>(p, D, bwd_dq_masked_kernel<D, T>, bwd_dq_smem_bytes<D>(), cfg_q, bwd_dkdv_masked_kernel<D, T>,
+                               bwd_dkdv_smem_bytes<D>() + kMaskTileBytes, cfg_kv, stream, dbias);
 }
 
 // Checks shared by the dense and the varlen entry, after the pointer / size checks: the forward's codes and messages (attn.cu).
@@ -587,4 +726,46 @@ extern "C" int sab_qk_int8_attn_bwd_varlen(const int8_t* q_int8, const int8_t* k
   a.ks_stride_idx = Hkv;
   a.cu_q = cu_seqlens_q; a.cu_k = cu_seqlens_k; a.cu_qs = cu_q_scale; a.cu_ks = cu_k_scale;
   return dispatch_bwd(p, D, dtype, SAB_GRAN_PER_BLOCK, stream);
+}
+
+extern "C" int sab_qk_int8_attn_bwd_masked(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
+                                           const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                           const float* lse, const void* k_mean, void* dq, void* dk, void* dv, void* workspace,
+                                           int dtype, int B, int Hq, int Hkv, int Sq, int Skv, int D, int64_t q8_stride_b,
+                                           int64_t q8_stride_h, int64_t q8_stride_s, int64_t k8_stride_b, int64_t k8_stride_h,
+                                           int64_t k8_stride_s, int64_t q_stride_b, int64_t q_stride_h, int64_t q_stride_s,
+                                           int64_t k_stride_b, int64_t k_stride_h, int64_t k_stride_s, int64_t v_stride_b,
+                                           int64_t v_stride_h, int64_t v_stride_s, int64_t o_stride_b, int64_t o_stride_h,
+                                           int64_t o_stride_s, int64_t do_stride_b, int64_t do_stride_h, int64_t do_stride_s,
+                                           int q_gran, int k_gran, float sm_scale, int fold_sm_scale, const void* attn_mask,
+                                           int mask_kind, int64_t mask_stride_b, int64_t mask_stride_h, int64_t mask_stride_m,
+                                           int64_t mask_stride_n, void* dbias, void* stream) {
+  using namespace sab;
+  SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
+              SAB_ERR_INVALID, "null tensor pointer");
+  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
+  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "dtype must be fp16 or bf16");
+  SAB_REQUIRE(B > 0 && Hq > 0 && Hkv > 0 && Sq > 0 && Skv > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", B, Hq, Hkv, Sq, Skv);
+  SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
+  SAB_REQUIRE(q_gran >= 1 && q_gran <= 3 && k_gran >= 1 && k_gran <= 3, SAB_ERR_INVALID, "unknown quant granularity q=%d k=%d", q_gran, k_gran);
+  // the masked forward's checks (attn.cu), then the gradient's own
+  SAB_REQUIRE(k_gran != SAB_GRAN_PER_THREAD, SAB_ERR_UNSUPPORTED,
+              "attn_mask is supported by the dense non-causal fp16-PV path with per-block / per-warp K scales only");
+  SAB_REQUIRE(attn_mask != nullptr && (mask_kind == SAB_MASK_BOOL || mask_kind == SAB_MASK_BIAS), SAB_ERR_INVALID,
+              "attn_mask: null pointer or unknown kind %d", mask_kind);
+  SAB_REQUIRE(dbias == nullptr || mask_kind == SAB_MASK_BIAS, SAB_ERR_INVALID, "dbias needs an additive bias mask (SAB_MASK_BIAS)");
+  SAB_REQUIRE(aligned16(dbias), SAB_ERR_INVALID, "dbias must be 16-byte aligned");
+  const int64_t st[21] = {q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s, q_stride_b, q_stride_h, q_stride_s,
+                          k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s, o_stride_b, o_stride_h, o_stride_s,
+                          do_stride_b, do_stride_h, do_stride_s};
+  if (int e = check_bwd_layout(q_int8, k_int8, q, k, v, o, dout, dq, dk, dv, st)) return e;
+  BwdParams p = bwd_params(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, B, Hq, Hkv, Sq, Skv,
+                           st, 0, q_gran, k_gran, sm_scale, fold_sm_scale);
+  AttnParams& a = p.a;
+  a.mask = attn_mask; a.mask_kind = mask_kind;
+  a.mask_sb = mask_stride_b; a.mask_sh = mask_stride_h; a.mask_sm = mask_stride_m; a.mask_sn = mask_stride_n;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const bool bf = dtype == SAB_DTYPE_BF16;
+  if (D == 128) return bf ? launch_bwd_masked<128, __nv_bfloat16>(p, dbias, s) : launch_bwd_masked<128, __half>(p, dbias, s);
+  return bf ? launch_bwd_masked<64, __nv_bfloat16>(p, dbias, s) : launch_bwd_masked<64, __half>(p, dbias, s);
 }

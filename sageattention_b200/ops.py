@@ -335,6 +335,46 @@ def _(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, d
     return None
 
 
+@torch.library.custom_op("sageattention_b200::qk_int8_attn_bwd_masked", mutates_args=("dq", "dk", "dv", "dbias"), device_types="cuda")
+def qk_int8_attn_bwd_masked(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale: torch.Tensor, k_scale: torch.Tensor, q: torch.Tensor,
+                            k: torch.Tensor, v: torch.Tensor, o: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor,
+                            k_mean: Optional[torch.Tensor], dq: torch.Tensor, dk: torch.Tensor, dv: torch.Tensor,
+                            attn_mask: torch.Tensor, dbias: Optional[torch.Tensor], tensor_layout: int, q_quant_gran: int,
+                            k_quant_gran: int, sm_scale: float, fold_sm_scale: int) -> None:
+    """Gradients of the masked FP16-PV attention (include/sageattn_b200.h, sab_qk_int8_attn_bwd_masked): the arguments of
+    qk_int8_attn_bwd without is_causal, plus the attn_mask view the forward received (qk_int8_sv_f16_attn_masked: [B,Hq,Sq,Skv],
+    strides may be 0) and dbias, None or a contiguous [B,Hq,Sq,Skv] tensor of the mask dtype (a float mask only) written with
+    ln2 * dS."""
+    B, Hq, Sq, D = _bhsd(q, tensor_layout)
+    _, Hkv, Skv, _ = _bhsd(k, tensor_layout)
+    for x, y in ((dq, q), (dk, k), (dv, v)):
+        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (B, Hq, Sq), "lse must be [B,Hq,Sq] fp32"
+    assert attn_mask.dim() == 4 and tuple(attn_mask.shape) == (B, Hq, Sq, Skv), "attn_mask must be expanded to [B,Hq,Sq,Skv]"
+    kind = SAB_MASK_BOOL if attn_mask.dtype == torch.bool else SAB_MASK_BIAS
+    assert kind == SAB_MASK_BOOL or attn_mask.dtype == q.dtype, "attn_mask must be bool or the q dtype"
+    if dbias is not None:
+        assert dbias.dtype == attn_mask.dtype and dbias.is_contiguous() and tuple(dbias.shape) == (B, Hq, Sq, Skv), \
+            "dbias must be a contiguous [B,Hq,Sq,Skv] tensor of the mask dtype"
+    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in _bhs_strides(t, tensor_layout)]
+    if k_mean is not None:
+        assert k_mean.numel() == B * Hkv * D and k_mean.dtype == k.dtype, "k_mean must have B*Hkv*D elements of k's dtype"
+        k_mean = k_mean.reshape(B, Hkv, D).contiguous()
+    with torch.cuda.device(q.device):
+        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(B, Hq, Sq), dtype=torch.uint8, device=q.device)
+        check(lib().sab_qk_int8_attn_bwd_masked(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(), k_scale.data_ptr(),
+                                                q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(), lse.data_ptr(),
+                                                _ptr(k_mean), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), ws.data_ptr(), _dt(q), B, Hq,
+                                                Hkv, Sq, Skv, D, *strides, q_quant_gran, k_quant_gran, float(sm_scale), fold_sm_scale,
+                                                attn_mask.data_ptr(), kind, *attn_mask.stride(), _ptr(dbias), _stream(q)))
+
+
+@qk_int8_attn_bwd_masked.register_fake
+def _(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, attn_mask, dbias, tensor_layout, q_quant_gran,
+      k_quant_gran, sm_scale, fold_sm_scale):
+    return None
+
+
 @torch.library.custom_op("sageattention_b200::qk_int8_attn_bwd_varlen", mutates_args=("dq", "dk", "dv"), device_types="cuda")
 def qk_int8_attn_bwd_varlen(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale: torch.Tensor, k_scale: torch.Tensor,
                             q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, o: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor,

@@ -199,6 +199,24 @@ int sab_qk_int8_sv_f8_attn(const int8_t* q_int8, const int8_t* k_int8, const uin
                            int max_seqlen_q, int causal_q_offset, int kv_seg_len, int32_t* debug_dump,
                            void* stream);
 
+/* Block-sparse form of sab_qk_int8_sv_f8_attn (dense tensors only: no varlen, sequence-parallel or debug arguments).
+ *   block_mask : bool (uint8, 0 = hidden) [Bm,Hm,ceil(Sq/128),ceil(Skv/64)] read through the element strides
+ *                mask_stride_b / _h / _qb / _kb (0 broadcasts a dimension; Bm in {1,B}, Hm in {1,Hq}, indexed by the Q head).
+ *   Key j is visible to query i of head h iff block_mask[b, h, i/128, j/64] (and j <= i when is_causal, which needs Sq == Skv).
+ *   The kernel visits only the visible 128x64 tiles; with an all-visible mask it computes the bytes of sab_qk_int8_sv_f8_attn.
+ *   A row with no visible key returns 0 and lse -inf.
+ *   q_gran per-warp or per-thread (the INT8+FP8 path's), Skv <= 1048576: each CTA keeps its list of visible key blocks in shared
+ *   memory (2 bytes per 64-key block).  The mask is checked before anything touches the device. */
+int sab_qk_int8_sv_f8_attn_blocksparse(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out,
+                                       float* lse, const float* q_scale, const float* k_scale, const float* v_scale,
+                                       const float* v_mean, int out_dtype, int B, int Hq, int Hkv, int Sq, int Skv,
+                                       int D, int64_t q_stride_b, int64_t q_stride_h, int64_t q_stride_s,
+                                       int64_t k_stride_b, int64_t k_stride_h, int64_t k_stride_s, int64_t v_s_pad,
+                                       int64_t o_stride_b, int64_t o_stride_h, int64_t o_stride_s, int is_causal,
+                                       int q_gran, int k_gran, float sm_scale, int fold_sm_scale,
+                                       const uint8_t* block_mask, int64_t mask_stride_b, int64_t mask_stride_h,
+                                       int64_t mask_stride_qb, int64_t mask_stride_kb, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * FP16-PV variant: INT8 QK^T -> fp32 online softmax WITHOUT exponent offset -> FP16 P -> FP16 PV
  * (wgmma f16, fp32 accumulation).  Replaces the Triton attention launchers
@@ -330,6 +348,24 @@ int sab_qk_int8_attn_bwd_masked(const int8_t* q_int8, const int8_t* k_int8, cons
                                 int64_t do_stride_h, int64_t do_stride_s, int q_gran, int k_gran, float sm_scale, int fold_sm_scale,
                                 const void* attn_mask, int mask_kind, int64_t mask_stride_b, int64_t mask_stride_h,
                                 int64_t mask_stride_m, int64_t mask_stride_n, void* dbias, void* stream);
+
+/* Block-sparse form of sab_qk_int8_attn_bwd: the gradient of sab_qk_int8_sv_f8_attn_blocksparse.  Same definition and arguments as
+ * sab_qk_int8_attn_bwd plus exactly the block mask the forward received (same checks, codes and messages); P = 0 on hidden tiles,
+ * and a row with lse = -inf gets zero gradients.  The dQ kernel visits only the visible key blocks of each 128-row Q block; the
+ * dK/dV kernel skips a (Q head, 64-row Q tile) step whose two 64-key blocks are both hidden.  Keys hidden from every row get zero
+ * dk and dv.  Deterministic like the dense form. */
+int sab_qk_int8_attn_bwd_blocksparse(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
+                                     const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
+                                     const void* k_mean, void* dq, void* dk, void* dv, void* workspace, int dtype, int B, int Hq,
+                                     int Hkv, int Sq, int Skv, int D, int64_t q8_stride_b, int64_t q8_stride_h,
+                                     int64_t q8_stride_s, int64_t k8_stride_b, int64_t k8_stride_h, int64_t k8_stride_s,
+                                     int64_t q_stride_b, int64_t q_stride_h, int64_t q_stride_s, int64_t k_stride_b,
+                                     int64_t k_stride_h, int64_t k_stride_s, int64_t v_stride_b, int64_t v_stride_h,
+                                     int64_t v_stride_s, int64_t o_stride_b, int64_t o_stride_h, int64_t o_stride_s,
+                                     int64_t do_stride_b, int64_t do_stride_h, int64_t do_stride_s, int is_causal, int q_gran,
+                                     int k_gran, float sm_scale, int fold_sm_scale, const uint8_t* block_mask,
+                                     int64_t mask_stride_b, int64_t mask_stride_h, int64_t mask_stride_qb, int64_t mask_stride_kb,
+                                     void* stream);
 
 #ifdef __cplusplus
 }

@@ -67,16 +67,21 @@ def _quant_qk(q, k, kind, tensor_layout, qk_quant_gran, sm_scale, smooth_k, back
 
 
 def _attn_dense(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range, backend,
-                return_lse):
+                return_lse, block_mask=None):
     """Quantisers + attention kernel of a dense entry point on head-dim-padded q, k, v.  kind: "fp8" (FP8 PV, V range v_range),
     "fp16_cuda" (FP16 PV, per-warp / per-thread INT8) or "fp16_triton" (FP16 PV, per-block INT8 with sm_scale*log2e folded into
-    q).  Returns (o, the kernel's log2 lse or an empty tensor, km)."""
+    q).  block_mask ("fp8" only): the [B,Hq,ceil(Sq/128),ceil(Skv/64)] bool view of sageattn_blocksparse; the quantisers still
+    see every key.  Returns (o, the kernel's log2 lse or an empty tensor, km)."""
     km, q_int8, q_scale, k_int8, k_scale, q_gran, k_gran, fold = _quant_qk(q, k, kind, tensor_layout, qk_quant_gran, sm_scale,
                                                                           smooth_k, backend)
     lay = 0 if tensor_layout == "NHD" else 1
     o = torch.empty(q.size(), dtype=q.dtype, device=q.device)
     if kind == "fp8":
         v_fp8, v_scale, vm = per_channel_fp8(v, tensor_layout=tensor_layout, scale_max=v_range, smooth_v=smooth_v)
+        if block_mask is not None:
+            return o, ops.qk_int8_sv_f8_attn_blocksparse(q_int8, k_int8, v_fp8, o, q_scale, k_scale, v_scale, vm, block_mask, lay,
+                                                         1 if is_causal else 0, q_gran, k_gran, sm_scale, fold,
+                                                         1 if return_lse else 0), km
         lse = ops.qk_int8_sv_f8_attn(q_int8, k_int8, v_fp8, o, q_scale, k_scale, v_scale, vm, lay, 1 if is_causal else 0,
                                      q_gran, k_gran, sm_scale, fold, 1 if return_lse else 0)
     else:
@@ -91,13 +96,15 @@ class _SageAttnFunction(torch.autograd.Function):
     straight-through estimator through the INT8 Q/K, FP8 V and FP8 P roundings (include/sageattn_b200.h, sab_qk_int8_attn_bwd).
     forward: the unchanged forward with the kernel LSE enabled; saves q, k, v, o and the raw LSE.  backward: re-runs the
     (deterministic) Q/K quantisers instead of saving their 8-bit outputs, then the two gradient kernels.  The LSE and the K mean
-    are returned for the LSE correction and carry no gradient."""
+    are returned for the LSE correction and carry no gradient.  block_mask (sageattn_blocksparse): P = 0 on the hidden tiles, and
+    the block-sparse gradient kernels visit only the visible ones; the mask has no gradient."""
 
     @staticmethod
-    def forward(ctx, q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range, backend):
+    def forward(ctx, q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range, backend,
+                block_mask=None):
         o, lse, km = _attn_dense(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range,
-                                 backend, True)
-        ctx.save_for_backward(q, k, v, o, lse)
+                                 backend, True, block_mask)
+        ctx.save_for_backward(q, k, v, o, lse, block_mask)
         ctx.cfg = (kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, backend)
         km = km if km is not None else q.new_empty(0)
         ctx.mark_non_differentiable(lse, km)
@@ -106,29 +113,34 @@ class _SageAttnFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, do, _dlse, _dkm):
         kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, backend = ctx.cfg
-        q, k, v, o, lse = ctx.saved_tensors
+        q, k, v, o, lse, block_mask = ctx.saved_tensors
         km, q_int8, q_scale, k_int8, k_scale, q_gran, k_gran, fold = _quant_qk(q, k, kind, tensor_layout, qk_quant_gran, sm_scale,
                                                                              smooth_k, backend)
         # the kernels read 16-bit rows with 16-byte loads; dq / dk / dv take the strides of q / k / v
         q, k, v, o, do = (t.contiguous() for t in (q, k, v, o, do))
         dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
-        ops.qk_int8_attn_bwd(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv,
-                             0 if tensor_layout == "NHD" else 1, 1 if is_causal else 0, q_gran, k_gran, sm_scale, fold)
-        return dq, dk, dv, None, None, None, None, None, None, None, None, None
+        if block_mask is not None:
+            ops.qk_int8_attn_bwd_blocksparse(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv, block_mask,
+                                             0 if tensor_layout == "NHD" else 1, 1 if is_causal else 0, q_gran, k_gran, sm_scale,
+                                             fold)
+        else:
+            ops.qk_int8_attn_bwd(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv,
+                                 0 if tensor_layout == "NHD" else 1, 1 if is_causal else 0, q_gran, k_gran, sm_scale, fold)
+        return dq, dk, dv, None, None, None, None, None, None, None, None, None, None
 
 
 def _dense_call(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range, backend,
-                return_lse, head_dim_og):
+                return_lse, head_dim_og, block_mask=None):
     """Shared tail of the dense entry points (q, k, v already head-dim padded).  The differentiable form runs only when grad mode
     is on and q, k or v requires grad; otherwise the forward's launches and bytes are exactly those of the plain call.  The
-    returned lse never carries a gradient."""
+    returned lse never carries a gradient.  block_mask: see _attn_dense."""
     if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
         o, lse, km = _SageAttnFunction.apply(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v,
-                                             v_range, backend)
+                                             v_range, backend, block_mask)
         q = q.detach()
     else:
         o, lse, km = _attn_dense(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range,
-                                 backend, return_lse)
+                                 backend, return_lse, block_mask)
     o = o[..., :head_dim_og]
     if return_lse:
         if smooth_k:
@@ -202,6 +214,13 @@ def sageattn_qk_int8_pv_fp8_cuda(
     only for "fp32" (core.py:797-803).  Unknown values raise (the reference silently returns an
     uninitialised tensor)."""
     _check_inputs(q, k, v)
+    return _qk_int8_pv_fp8(q, k, v, tensor_layout, is_causal, qk_quant_gran, sm_scale, pv_accum_dtype, smooth_k, smooth_v, return_lse)
+
+
+def _qk_int8_pv_fp8(q, k, v, tensor_layout, is_causal, qk_quant_gran, sm_scale, pv_accum_dtype, smooth_k, smooth_v, return_lse,
+                    block_mask=None):
+    """Body of sageattn_qk_int8_pv_fp8_cuda after _check_inputs; block_mask: that of sageattn_blocksparse, checked and expanded by
+    the caller."""
     assert qk_quant_gran in ["per_warp", "per_thread"], "qk_quant_gran must be either 'per_warp' or 'per_thread'."
     if pv_accum_dtype not in ("fp32", "fp32+fp32", "fp32+fp16"):
         raise ValueError(f"Unsupported pv_accum_dtype: {pv_accum_dtype}")
@@ -224,7 +243,41 @@ def sageattn_qk_int8_pv_fp8_cuda(
     # front-end: K mean (2 launches), Q / K quantisers, V statistics (2) + FP8 quantiser — 7 launches (reference: 6 + k.mean, core.py:773-809).
     # The single-launch cluster variants (quant.smooth_quant_k, per_channel_fp8(fused=True)) are opt-in.
     return _dense_call(q, k, v, "fp8", tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, quant_v_scale_max,
-                       "cuda", return_lse, head_dim_og)
+                       "cuda", return_lse, head_dim_og, block_mask)
+
+
+def sageattn_blocksparse(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, block_mask: torch.Tensor, tensor_layout: str = "HND",
+                         is_causal: bool = False, qk_quant_gran: str = "per_thread", sm_scale: Optional[float] = None,
+                         pv_accum_dtype: str = "fp32+fp16", smooth_k: bool = True, smooth_v: bool = False,
+                         return_lse: bool = False) -> torch.Tensor:
+    """Block-sparse sageattn_qk_int8_pv_fp8_cuda (no reference counterpart): the same options, checks, quantisation and numerics,
+    but key j is visible to query i of head h only if block_mask[b, h, i // 128, j // 64] (and j <= i when is_causal), and the
+    kernels visit only the visible 128-query x 64-key tiles.
+
+    block_mask: torch.bool on q's device, shape [Bm, Hm, ceil(Sq/128), ceil(Skv/64)] with Bm in {1, B} and Hm in {1, Hq}
+    (size-1 dimensions broadcast, any strides); indexed by the Q head under GQA; the block indices do not depend on
+    tensor_layout.  The K mean and the V scales are still taken over every key.  A row with no visible key returns 0 (lse -inf).
+    With an all-True mask the output is that of sageattn_qk_int8_pv_fp8_cuda to the bit.  Differentiable when grad mode is on
+    and q, k or v requires grad: the dense straight-through gradient with P = 0 on hidden tiles; the mask has no gradient."""
+    _check_inputs(q, k, v)
+    assert isinstance(block_mask, torch.Tensor) and block_mask.dtype == torch.bool, "block_mask must be a torch.bool tensor."
+    assert block_mask.device == q.device, "All tensors must be on the same device."
+    if tensor_layout not in ("NHD", "HND"):
+        raise ValueError(f"Unknown tensor layout: {tensor_layout}")
+    if tensor_layout == "HND":
+        B, Hq, Sq = q.shape[:3]
+        Skv = k.size(2)
+    else:
+        B, Sq, Hq = q.shape[:3]
+        Skv = k.size(1)
+    nqb, nkb = (Sq + 127) // 128, (Skv + 63) // 64
+    if block_mask.dim() != 4 or tuple(block_mask.shape[2:]) != (nqb, nkb):
+        raise ValueError(f"block_mask shape {tuple(block_mask.shape)} must be [B or 1, Hq or 1, {nqb}, {nkb}] "
+                         f"(ceil(Sq/128), ceil(Skv/64))")
+    if block_mask.size(0) not in (1, B) or block_mask.size(1) not in (1, Hq):
+        raise ValueError(f"block_mask shape {tuple(block_mask.shape)} cannot be broadcast to [{B}, {Hq}, {nqb}, {nkb}]")
+    return _qk_int8_pv_fp8(q, k, v, tensor_layout, is_causal, qk_quant_gran, sm_scale, pv_accum_dtype, smooth_k, smooth_v,
+                           return_lse, block_mask.expand(B, Hq, nqb, nkb))
 
 
 def sageattn(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, tensor_layout: str = "HND", is_causal: bool = False,

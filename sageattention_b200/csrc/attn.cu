@@ -34,13 +34,34 @@ constexpr size_t attn_smem_bytes() {
   return size_t(BM) * D + size_t(kStages) * (BN * D + BN * D * (kPV16 ? 2 : 1)) + (1 + 2 * kStages) * 8 + 1024;
 }
 
+// Shared memory of the block-sparse form behind the INT8+FP8 kernel's barriers: build_kv_list's 64 bytes of counts, then the list
+// of visible 64-key tiles (kv_list_bytes)
+template <int D>
+constexpr uint32_t kKvScratchOff = uint32_t(BM) * D + kStages * (2 * BN * D) + (1 + 2 * kStages) * 8;
+template <int D>
+__device__ __forceinline__ int* kv_scratch(uint8_t* smem) { return reinterpret_cast<int*>(smem + kKvScratchOff<D>); }
+template <int D>
+__device__ __forceinline__ uint16_t* kv_list(uint8_t* smem) { return reinterpret_cast<uint16_t*>(smem + kKvScratchOff<D> + 64); }
+
 // D: head dim (64 / 128).  kKT: per-thread K scales (4 per 64-key block) instead of 1.  OutT: __half / bf16.
 // kPV16: P and V in fp16 with the Triton path's softmax (no exponent offset) — the numerics of the reference's
 // sageattn_qk_int8_pv_fp16_triton / sageattn_varlen kernels (triton/attn_qk_int8_per_block.py:22-128).
-// kMask (kPV16 only): attn_mask of sageattn_qk_int8_pv_fp16_triton — a bool mask marks elements like the out-of-range keys
+// kMask with kPV16: attn_mask of sageattn_qk_int8_pv_fp16_triton — a bool mask marks elements like the out-of-range keys
 // (integer sentinel), an additive bias takes the float path below.
 // Sequence-parallel fused gather (p.seg_flags != nullptr): K/V segments arrive WHILE the kernel runs (peer copies on another
 // stream); the TMA producer polls one flag per (KV-head group, segment) before the first tile of a segment.
+// the two meanings of kMask (namespace-scope, not kernel locals: a local constexpr perturbs the code ptxas emits for the kernel)
+template <bool kPV16, bool kMask>
+constexpr bool kElemMask = kMask && kPV16;    // attn_mask of the FP16-PV path
+template <bool kPV16, bool kMask>
+constexpr bool kSparse = kMask && !kPV16;     // block mask of the INT8+FP8 path
+
+// kMask without kPV16 (INT8+FP8 only): the block-sparse form.  p.mask is then the bool block mask [.,.,ceil(Sq/128),ceil(Skv/64)]
+// with element strides mask_sb / mask_sh / mask_sm (128-row Q blocks) / mask_sn (64-key blocks), and the dynamic shared memory
+// adds kv_list_bytes(ceil(Skv/64)).  The CTA first compacts its row (b, h, qt) of the mask into a shared-memory list of the visible
+// 64-key tiles, ascending and cut at the causal horizon; the loop below then runs over that list, with tile kv_list[j] wherever the
+// dense kernel uses tile j (TMA coordinates, K-scale block, limit, masked_tile).  A row whose list is empty takes the n_kv == 0
+// path; a row that sees none of the listed keys (causal) gets zeros and lse -inf.
 template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
@@ -86,6 +107,10 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   }
   int n_kv = (kv_len + BN - 1) / BN;                 // 64-key tiles
   if (p.causal) n_kv = min(n_kv, (p.causal_q_offset + (qt + 1) * BM + BN - 1) / BN);
+  if constexpr (kSparse<kPV16, kMask>) {
+    const BlockMask bm{static_cast<const uint8_t*>(p.mask), p.mask_sb, p.mask_sh, p.mask_sm, p.mask_sn};
+    n_kv = build_kv_list<kNumThreads>(bm, b, h, qt, n_kv, kv_list<D>(smem), kv_scratch<D>(smem));
+  }
 
   if (threadIdx.x == 0) {
     if ((smem_u32(smem) & 1023u) != 0) __trap();     // swizzled tiles need a 1 KB-aligned base
@@ -111,7 +136,9 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       for (int j = 0; j < n_kv; ++j) {
         const int s = j % kStages;
         const uint32_t ph = (j / kStages) & 1;
-        int kc = k_off + j * BN, vc = v_off + j * BN, kb = tb;
+        int kj = j;   // the 64-key tile loaded in step j
+        if constexpr (kSparse<kPV16, kMask>) kj = kv_list<D>(smem)[j];
+        int kc = k_off + kj * BN, vc = v_off + kj * BN, kb = tb;
         if (p.kv_seg_len > 0) {  // all-gathered layout: segment-major
           const int seg = (j * BN) / p.kv_seg_len;
           kc = vc = j * BN - seg * p.kv_seg_len;
@@ -172,11 +199,13 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   if (n_kv > 0) mbar_wait_wd(q_full, 0);
   for (int j = 0; j < n_kv; ++j) {
     const int st = j % kStages;
+    int kj = j;   // the 64-key tile of step j
+    if constexpr (kSparse<kPV16, kMask>) kj = kv_list<D>(smem)[j];
     float coef[2];
     {
-      // dequant coefficient (…sm89.cuh:116-132, 255-257); tile j == 64-key block j.  Per-thread K scales: the keys of lane t
+      // dequant coefficient (…sm89.cuh:116-132, 255-257); tile kj == 64-key block kj.  Per-thread K scales: the keys of lane t
       // (8i+2t, 8i+2t+1) are all in scale group t.
-      const float ksv = k_dequant<kKT>(p, ks_base, k_blk0 + j, t);
+      const float ksv = k_dequant<kKT>(p, ks_base, k_blk0 + kj, t);
       coef[0] = ksv * qss[0];
       coef[1] = ksv * qss[1];
     }
@@ -184,11 +213,11 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     int limit[2];
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
-      limit[i] = kv_len - j * BN;
-      if (p.causal) limit[i] = min(limit[i], p.causal_q_offset + q_row[i] - j * BN + 1);
-      if (kMask && q_row[i] >= q_len) limit[i] = 0;   // rows past the end: nothing visible, no mask bytes read
+      limit[i] = kv_len - kj * BN;
+      if (p.causal) limit[i] = min(limit[i], p.causal_q_offset + q_row[i] - kj * BN + 1);
+      if (kElemMask<kPV16, kMask> && q_row[i] >= q_len) limit[i] = 0;   // rows past the end: nothing visible, no mask bytes read
     }
-    const bool masked_tile = kMask || (kv_len - j * BN < BN) || (p.causal && (j + 1) * BN > p.causal_q_offset + qt * BM + 1);
+    const bool masked_tile = kElemMask<kPV16, kMask> || (kv_len - kj * BN < BN) || (p.causal && (kj + 1) * BN > p.causal_q_offset + qt * BM + 1);
 
     mbar_wait_wd(kv_full + st, (j / kStages) & 1);
     uint32_t s[32];
@@ -203,7 +232,7 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     fence_regs(s);
 
     [[maybe_unused]] const char* mrow[2] = {nullptr, nullptr};   // this row's 64 mask elements of tile j
-    if constexpr (kMask) {
+    if constexpr (kElemMask<kPV16, kMask>) {
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         const int64_t off = int64_t(b) * p.mask_sb + int64_t(h) * p.mask_sh + int64_t(q_row[i]) * p.mask_sm + int64_t(j) * BN * p.mask_sn;
@@ -271,7 +300,7 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 #endif
 #pragma unroll
           for (int u = 0; u < 2; ++u) {
-            if constexpr (MASKED && kMask) x[u] = (int(s[idx + u]) != kIntSentinel) ? x[u] : 0.f;   // masked-out elements: not a prefix
+            if constexpr (MASKED && kElemMask<kPV16, kMask>) x[u] = (int(s[idx + u]) != kIntSentinel) ? x[u] : 0.f;   // masked-out elements: not a prefix
             else if constexpr (MASKED) x[u] = (8 * (c >> 1) + 2 * t + u < limit[i]) ? x[u] : 0.f;
             e[idx + u] = x[u];
             sum += x[u];
@@ -282,7 +311,7 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     };
     // additive bias (attn_qk_int8_per_block.py:41,50-51): qk = S*scale + bias in fp32, then the plain online softmax
     auto tile_bias = [&]() {
-      if constexpr (kMask && kPV16) {
+      if constexpr (kElemMask<kPV16, kMask>) {
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
           float mx = -INFINITY;
@@ -315,7 +344,7 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         }
       }
     };
-    if (kMask && p.mask_kind == 2) tile_bias();
+    if (kElemMask<kPV16, kMask> && p.mask_kind == 2) tile_bias();
     else if (masked_tile) tile(std::true_type{});
     else tile(std::false_type{});
 
@@ -389,7 +418,8 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     const bool row_ok = q_row[i] < q_len;
     OutT* orow = reinterpret_cast<OutT*>(p.out) + (varlen ? 0 : int64_t(b) * p.o_stride_b) + int64_t(h) * p.o_stride_h +
                  int64_t(q_off + q_row[i]) * p.o_stride_s;
-    const float inv = (n_kv == 0 || (kMask && !(dt > 0.f))) ? 0.f : rcp_approx(dt);   // a fully masked row yields zeros, not NaN
+    // a fully masked row yields zeros, not NaN; block-sparse causal: a row may see none of the listed keys
+    const float inv = (n_kv == 0 || (kMask && !(dt > 0.f))) ? 0.f : rcp_approx(dt);
     if (row_ok) {
 #pragma unroll
       for (int nb = 0; nb < D / 8; ++nb) {
@@ -403,13 +433,13 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
           x0 += vm[col];
           x1 += vm[col + 1];
         }
-        if (n_kv == 0) x0 = x1 = 0.f;
+        if (n_kv == 0 || (kSparse<kPV16, kMask> && !(dt > 0.f))) x0 = x1 = 0.f;
         *reinterpret_cast<uint32_t*>(orow + col) = pack2<OutT>(x0, x1);
       }
       if (p.lse != nullptr && t == 0) {
         // log2 units like the reference kernel (…sm89.cuh:691-703); the offset cancels: log2(sum 2^x)
         const int64_t li = varlen ? (int64_t(h) * p.Sq + q_off + q_row[i]) : ((int64_t(b) * p.Hq + h) * p.Sq + q_row[i]);
-        p.lse[li] = n_kv > 0 ? lg2_approx(dt) + m[i] : -INFINITY;
+        p.lse[li] = n_kv > 0 ? lg2_approx(dt) + m[i] : -INFINITY;   // block-sparse, no visible key: lg2(0) = -inf
       }
     }
   }
@@ -478,8 +508,25 @@ static int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUten
   return SAB_OK;
 }
 
+// the block-sparse form (sage_attn_fwd_kernel<D, kKT, OutT, false, true>): p.mask holds the block mask
+template <int D, bool kKT, typename OutT>
+static int launch_attn_blocksparse(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, AttnParams p,
+                                   dim3 grid, cudaStream_t stream) {
+  p.lazy_tau = exact_max_mode() ? 0.0f : kLazyTau;
+  constexpr size_t smem_max = attn_smem_bytes<D, false>() + kv_list_bytes(kMaxKvBlocks);
+  const size_t smem = attn_smem_bytes<D, false>() + kv_list_bytes((p.Sk + BN - 1) / BN);
+  auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, true>;
+  static bool configured[64] = {};
+  if (int st = ensure_dynamic_smem(kern, smem_max, configured)) return st;
+  kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p);
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
+}
+
 }  // namespace sab
 
+// block mask of the block-sparse entry point, handed to attn_entry by sab_qk_int8_sv_f8_attn_blocksparse (same thread)
+static thread_local const sab::BlockMask* tl_block_mask = nullptr;
 // attention mask of the masked entry point, handed to attn_entry by sab_qk_int8_sv_f16_attn_masked (same thread)
 struct MaskArgs {
   const void* ptr; int kind; int64_t sb, sh, sm, sn;
@@ -591,6 +638,22 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
                 "segment flags: null pointer or heads_per_flag (%d) does not divide num_kv_heads (%d)", tl_seg->heads_per_flag, Hkv);
     p.seg_flags = tl_seg->flags; p.seg_epoch = tl_seg->epoch; p.seg_heads = tl_seg->heads_per_flag;   // polled by the producer
   }
+  if (tl_block_mask != nullptr) {
+    SAB_REQUIRE(!pv16 && !varlen && kv_seg_len == 0 && causal_q_offset == 0, SAB_ERR_UNSUPPORTED,
+                "the block mask is supported by the dense single-GPU INT8/FP8 path only");
+    p.mask = tl_block_mask->ptr;
+    p.mask_sb = tl_block_mask->sb; p.mask_sh = tl_block_mask->sh; p.mask_sm = tl_block_mask->sqb; p.mask_sn = tl_block_mask->skb;
+    if (D == 128) {
+      if (kt) return bf ? launch_attn_blocksparse<128, true, __nv_bfloat16>(tq, tk, tv, p, grid, s)
+                        : launch_attn_blocksparse<128, true, __half>(tq, tk, tv, p, grid, s);
+      return bf ? launch_attn_blocksparse<128, false, __nv_bfloat16>(tq, tk, tv, p, grid, s)
+                : launch_attn_blocksparse<128, false, __half>(tq, tk, tv, p, grid, s);
+    }
+    if (kt) return bf ? launch_attn_blocksparse<64, true, __nv_bfloat16>(tq, tk, tv, p, grid, s)
+                      : launch_attn_blocksparse<64, true, __half>(tq, tk, tv, p, grid, s);
+    return bf ? launch_attn_blocksparse<64, false, __nv_bfloat16>(tq, tk, tv, p, grid, s)
+              : launch_attn_blocksparse<64, false, __half>(tq, tk, tv, p, grid, s);
+  }
 #define SAB_LAUNCH(DD, KT, T)                                                      \
   do {                                                                             \
     if (pv16) return launch_attn<DD, KT, T, true>(tq, tk, tv, p, grid, s);         \
@@ -669,5 +732,26 @@ extern "C" int sab_qk_int8_sv_f16_attn_masked(const int8_t* q_int8, const int8_t
                             k_stride_h, k_stride_s, v_s_pad, o_stride_b, o_stride_h, o_stride_s, 0, q_gran, k_gran, sm_scale,
                             fold_sm_scale, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0, nullptr, stream);
   tl_mask = nullptr;
+  return st;
+}
+
+extern "C" int sab_qk_int8_sv_f8_attn_blocksparse(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out,
+                                                  float* lse, const float* q_scale, const float* k_scale, const float* v_scale,
+                                                  const float* v_mean, int out_dtype, int B, int Hq, int Hkv, int Sq, int Skv,
+                                                  int D, int64_t q_stride_b, int64_t q_stride_h, int64_t q_stride_s,
+                                                  int64_t k_stride_b, int64_t k_stride_h, int64_t k_stride_s, int64_t v_s_pad,
+                                                  int64_t o_stride_b, int64_t o_stride_h, int64_t o_stride_s, int is_causal,
+                                                  int q_gran, int k_gran, float sm_scale, int fold_sm_scale,
+                                                  const uint8_t* block_mask, int64_t mask_stride_b, int64_t mask_stride_h,
+                                                  int64_t mask_stride_qb, int64_t mask_stride_kb, void* stream) {
+  if (int st = sab::check_block_mask(block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb, q_gran, is_causal, Sq, Skv))
+    return st;
+  const sab::BlockMask m{block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb};
+  tl_block_mask = &m;
+  const int st = attn_entry(0, q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, B, Hq, Hkv, Sq, Skv, D,
+                            q_stride_b, q_stride_h, q_stride_s, k_stride_b, k_stride_h, k_stride_s, v_s_pad, o_stride_b, o_stride_h,
+                            o_stride_s, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale, nullptr, nullptr, nullptr, nullptr,
+                            nullptr, 0, 0, 0, nullptr, stream);
+  tl_block_mask = nullptr;
   return st;
 }

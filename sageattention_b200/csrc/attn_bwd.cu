@@ -256,9 +256,10 @@ constexpr size_t bwd_dq_smem_bytes() {
   return size_t(128) * D + size_t(128) * D * 2 + size_t(64) * D + size_t(64) * D * 2 + size_t(D) * 64 * 2 + 1024;
 }
 
-// dbias (masked, nullable): dense [B,Hq,Sq,Skv] in T, written with ln2 * dS
-template <int D, bool kKT, typename T, bool kVarlen, int kMask = 0>
-__device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nullptr) {
+// dbias (masked, nullable): dense [B,Hq,Sq,Skv] in T, written with ln2 * dS.  kSparse: the block-sparse form, which loops over
+// the visible 64-key tiles of its row of *bm (build_kv_list, as the forward does) instead of every tile.
+template <int D, bool kKT, typename T, bool kVarlen, int kMask = 0, bool kSparse = false>
+__device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nullptr, const BlockMask* bm = nullptr) {
   constexpr int QB = 128, KB = 64;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ8 = smem;                       // [128 x D] int8        A of S = Q K^T
@@ -266,6 +267,8 @@ __device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nu
   uint8_t* sK8 = sdO + QB * D * 2;           // [64 x D] int8         B of S
   uint8_t* sV = sK8 + KB * D;                // [64 x D] 16-bit       B of dP
   uint8_t* sKt = sV + KB * D * 2;            // [D x 64] 16-bit       B of dQ += dS K
+  [[maybe_unused]] int* s_scratch = reinterpret_cast<int*>(sKt + D * KB * 2);     // block-sparse: build_kv_list's counts
+  [[maybe_unused]] uint16_t* s_idx = reinterpret_cast<uint16_t*>(s_scratch + 16); // block-sparse: visible 64-key tiles
   const AttnParams& a = p.a;
 
   int qt = blockIdx.x;
@@ -291,7 +294,7 @@ __device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nu
     qss[i] = q_dequant_log2(a, qs_base, sq.q_blk0 + qt, row0 + 8 * i);   // scales are padded to whole 128-row blocks
     const bool ok = q_row[i] < sq.q_len;
     const int64_t li = (int64_t(sq.tb) * a.Hq + h) * a.Sq + sq.q_off + q_row[i];
-    if constexpr (kMask != 0) nlse[i] = ok ? masked_nlse(p.lse[li]) : -INFINITY;
+    if constexpr (kMask != 0 || kSparse) nlse[i] = ok ? masked_nlse(p.lse[li]) : -INFINITY;
     else nlse[i] = ok ? -p.lse[li] : 0.f;
     dlt[i] = ok ? p.delta[li] : 0.f;
   }
@@ -305,12 +308,14 @@ __device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nu
   }
   int n_kv = (sq.kv_len + KB - 1) / KB;
   if (a.causal) n_kv = min(n_kv, ((qt + 1) * QB + KB - 1) / KB);
+  if constexpr (kSparse) n_kv = build_kv_list<kBwdThreads>(*bm, b, h, qt, n_kv, s_idx, s_scratch);
 
   float dq[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) dq[i] = 0.f;
 
-  for (int j = 0; j < n_kv; ++j) {
+  for (int jt = 0; jt < n_kv; ++jt) {
+    const int j = kSparse ? int(s_idx[jt]) : jt;   // the 64-key tile of step jt
     // masked: the mask elements of this thread's S elements of tile j, issued first so that their latency overlaps the tile loads
     // and the MMAs; rows >= Sq and keys >= Skv are not read
     [[maybe_unused]] uint32_t mv[32];
@@ -420,14 +425,24 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_masked_kernel(const __g
   else bwd_dq_tile<D, false, T, false, SAB_MASK_BIAS>(p, dbias);
 }
 
+// the block-sparse form: dense, non-varlen; its dynamic shared memory adds kv_list_bytes(ceil(Skv/64))
+template <int D, bool kKT, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_blocksparse_kernel(const __grid_constant__ BwdParams p,
+                                                                             const __grid_constant__ BlockMask bm) {
+  bwd_dq_tile<D, kKT, T, false, 0, true>(p, nullptr, &bm);
+}
+
 // ------------------------------------------------------------------------------------------------ dK, dV
 template <int D>
 constexpr size_t bwd_dkdv_smem_bytes() {
   return size_t(128) * D + size_t(128) * D * 2 + size_t(64) * D + size_t(64) * D * 2 + 2 * size_t(D) * 64 * 2 + 3 * 64 * 4 + 1024;
 }
 
-template <int D, bool kKT, typename T, bool kVarlen, int kMask = 0>
-__device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p) {
+// kSparse: the block-sparse form.  Warpgroup wg's 64 keys are one block of *bm, and a 64-row Q tile lies in one 128-row block, so
+// each (Q head, Q tile) step has two mask bits: a step with neither set is skipped (no loads, no barriers; the bits are uniform
+// across the CTA), and with one set the other warpgroup takes part in the loads and barriers but adds nothing.
+template <int D, bool kKT, typename T, bool kVarlen, int kMask = 0, bool kSparse = false>
+__device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p, const BlockMask* bm = nullptr) {
   constexpr int KB = 128, QB = 64;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sK8 = smem;                       // [128 x D] int8        A of S^T = K Q^T
@@ -468,11 +483,30 @@ __device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p) {
 
   const int n_qt = (sq.q_len + QB - 1) / QB;
   const int qt0 = a.causal ? k0 / QB : 0;    // causal (top-left): rows before the first key see none of this tile
+  // block-sparse: the raw mask bytes of warpgroup 0's and 1's key blocks for step (hh, qt), loaded one step ahead
+  [[maybe_unused]] const int kb0 = 2 * blockIdx.x, n_kb = (sq.kv_len + 63) / 64;
+  [[maybe_unused]] uint32_t nxt[2] = {0u, 0u};
+  [[maybe_unused]] auto load_bits = [&](int hh, int qt) {
+    const uint8_t* r = bm->ptr + int64_t(b) * bm->sb + int64_t(hk * G + hh) * bm->sh + int64_t(qt / 2) * bm->sqb;
+    nxt[0] = __ldg(r + int64_t(kb0) * bm->skb);
+    nxt[1] = kb0 + 1 < n_kb ? __ldg(r + int64_t(kb0 + 1) * bm->skb) : 0u;
+  };
+  if constexpr (kSparse) {
+    if (qt0 < n_qt) load_bits(0, qt0);
+  }
   for (int hh = 0; hh < G; ++hh) {
     const int h = hk * G + hh;
     const float* qs_base = a.q_scale + (int64_t(sq.tb) * a.Hq + h) * a.qs_stride_bh;
     for (int qt = qt0; qt < n_qt; ++qt) {
       const int q0 = qt * QB;
+      bool visible = true;   // this warpgroup's keys are visible to Q tile qt of head h
+      if constexpr (kSparse) {
+        const bool v0 = nxt[0] != 0u, v1 = nxt[1] != 0u;
+        if (qt + 1 < n_qt) load_bits(hh, qt + 1);
+        else if (hh + 1 < G) load_bits(hh + 1, qt0);
+        if (!v0 && !v1) continue;
+        visible = wg == 0 ? v0 : v1;
+      }
       __syncthreads();   // the previous tile's operands are consumed
       load_tile<QB, D, 1>(sQ8, p.q8 + b * p.q8_sb + h * p.q8_sh + sq.q_off * p.q8_ss, p.q8_ss, q0, sq.q_len);
       load_tile<QB, D, 2>(sdO, p.dout + b * p.do_sb + h * p.do_sh + sq.q_off * p.do_ss, p.do_ss, q0, sq.q_len);
@@ -484,12 +518,13 @@ __device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p) {
         const bool ok = r < sq.q_len;
         const int64_t li = (int64_t(sq.tb) * a.Hq + h) * a.Sq + sq.q_off + r;
         s_qss[threadIdx.x] = ok ? q_dequant_log2(a, qs_base, sq.q_blk0 + r / 128, r % 128) : 0.f;
-        if constexpr (kMask != 0) s_nlse[threadIdx.x] = ok ? masked_nlse(p.lse[li]) : -INFINITY;
+        if constexpr (kMask != 0 || kSparse) s_nlse[threadIdx.x] = ok ? masked_nlse(p.lse[li]) : -INFINITY;
         else s_nlse[threadIdx.x] = ok ? -p.lse[li] : 0.f;
         s_dlt[threadIdx.x] = ok ? p.delta[li] : 0.f;
       }
       fence_proxy_async_smem();
       __syncthreads();
+      if (!visible) continue;   // warpgroup-uniform; the next step starts with a barrier both warpgroups reach
 
       uint32_t s[32];
       float dp[32];
@@ -558,18 +593,28 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_masked_kernel(const _
   else bwd_dkdv_tile<D, false, T, false, SAB_MASK_BIAS>(p);
 }
 
+template <int D, bool kKT, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_blocksparse_kernel(const __grid_constant__ BwdParams p,
+                                                                               const __grid_constant__ BlockMask bm) {
+  bwd_dkdv_tile<D, kKT, T, false, 0, true>(p, &bm);
+}
+
 // delta, then the dQ kernel kq (smem_q bytes, arguments p, q_args...) and the dK/dV kernel kkv (smem_kv bytes); cfg_*: their
 // per-device smem opt-in
+template <typename T>
+static int launch_bwd_delta(const BwdParams& p, int D, cudaStream_t stream) {
+  BwdParams pd = p;
+  if (p.a.cu_q != nullptr) pd.a.B = 1;   // varlen: every packed row, [Hq,Tq] like the LSE
+  const int64_t rows = int64_t(pd.a.B) * pd.a.Hq * pd.a.Sq;
+  bwd_delta_kernel<T><<<unsigned((rows + 7) / 8), 256, 0, stream>>>(pd, D);
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
+}
+
 template <typename T, typename KQ, typename KKV, typename... QArgs>
 static int launch_bwd_kernels(const BwdParams& p, int D, KQ kq, size_t smem_q, bool (&cfg_q)[64], KKV kkv, size_t smem_kv,
                               bool (&cfg_kv)[64], cudaStream_t stream, QArgs... q_args) {
-  {
-    BwdParams pd = p;
-    if (p.a.cu_q != nullptr) pd.a.B = 1;   // varlen: every packed row, [Hq,Tq] like the LSE
-    const int64_t rows = int64_t(pd.a.B) * pd.a.Hq * pd.a.Sq;
-    bwd_delta_kernel<T><<<unsigned((rows + 7) / 8), 256, 0, stream>>>(pd, D);
-    SAB_CUDA_OK(cudaGetLastError());
-  }
+  if (int st = launch_bwd_delta<T>(p, D, stream)) return st;
   if (int st = ensure_dynamic_smem(kq, smem_q, cfg_q)) return st;
   kq<<<dim3(p.a.n_q_tiles, p.a.Hq, p.a.B), kBwdThreads, smem_q, stream>>>(p, q_args...);
   SAB_CUDA_OK(cudaGetLastError());
@@ -591,6 +636,22 @@ static int launch_bwd_masked(const BwdParams& p, void* dbias, cudaStream_t strea
   static bool cfg_q[64] = {}, cfg_kv[64] = {};
   return launch_bwd_kernels<T>(p, D, bwd_dq_masked_kernel<D, T>, bwd_dq_smem_bytes<D>(), cfg_q, bwd_dkdv_masked_kernel<D, T>,
                                bwd_dkdv_smem_bytes<D>() + kMaskTileBytes, cfg_kv, stream, dbias);
+}
+
+template <int D, bool kKT, typename T>
+static int launch_bwd_blocksparse(const BwdParams& p, const BlockMask& bm, cudaStream_t stream) {
+  static bool cfg_q[64] = {}, cfg_kv[64] = {};
+  if (int st = launch_bwd_delta<T>(p, D, stream)) return st;
+  auto kq = bwd_dq_blocksparse_kernel<D, kKT, T>;
+  const size_t smem_q = bwd_dq_smem_bytes<D>() + kv_list_bytes((p.a.Sk + BN - 1) / BN);
+  if (int st = ensure_dynamic_smem(kq, bwd_dq_smem_bytes<D>() + kv_list_bytes(kMaxKvBlocks), cfg_q)) return st;
+  kq<<<dim3(p.a.n_q_tiles, p.a.Hq, p.a.B), kBwdThreads, smem_q, stream>>>(p, bm);
+  SAB_CUDA_OK(cudaGetLastError());
+  auto kkv = bwd_dkdv_blocksparse_kernel<D, kKT, T>;
+  if (int st = ensure_dynamic_smem(kkv, bwd_dkdv_smem_bytes<D>(), cfg_kv)) return st;
+  kkv<<<dim3(p.n_k_tiles, p.a.Hkv, p.a.B), kBwdThreads, bwd_dkdv_smem_bytes<D>(), stream>>>(p, bm);
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
 }
 
 // Checks shared by the dense and the varlen entry, after the pointer / size checks: the forward's codes and messages (attn.cu).
@@ -768,4 +829,44 @@ extern "C" int sab_qk_int8_attn_bwd_masked(const int8_t* q_int8, const int8_t* k
   const bool bf = dtype == SAB_DTYPE_BF16;
   if (D == 128) return bf ? launch_bwd_masked<128, __nv_bfloat16>(p, dbias, s) : launch_bwd_masked<128, __half>(p, dbias, s);
   return bf ? launch_bwd_masked<64, __nv_bfloat16>(p, dbias, s) : launch_bwd_masked<64, __half>(p, dbias, s);
+}
+
+extern "C" int sab_qk_int8_attn_bwd_blocksparse(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale,
+                                                const float* k_scale, const void* q, const void* k, const void* v, const void* o,
+                                                const void* dout, const float* lse, const void* k_mean, void* dq, void* dk, void* dv,
+                                                void* workspace, int dtype, int B, int Hq, int Hkv, int Sq, int Skv, int D,
+                                                int64_t q8_stride_b, int64_t q8_stride_h, int64_t q8_stride_s, int64_t k8_stride_b,
+                                                int64_t k8_stride_h, int64_t k8_stride_s, int64_t q_stride_b, int64_t q_stride_h,
+                                                int64_t q_stride_s, int64_t k_stride_b, int64_t k_stride_h, int64_t k_stride_s,
+                                                int64_t v_stride_b, int64_t v_stride_h, int64_t v_stride_s, int64_t o_stride_b,
+                                                int64_t o_stride_h, int64_t o_stride_s, int64_t do_stride_b, int64_t do_stride_h,
+                                                int64_t do_stride_s, int is_causal, int q_gran, int k_gran, float sm_scale,
+                                                int fold_sm_scale, const uint8_t* block_mask, int64_t mask_stride_b,
+                                                int64_t mask_stride_h, int64_t mask_stride_qb, int64_t mask_stride_kb, void* stream) {
+  using namespace sab;
+  if (int e = check_block_mask(block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb, q_gran, is_causal, Sq, Skv))
+    return e;
+  SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
+              SAB_ERR_INVALID, "null tensor pointer");
+  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
+  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "dtype must be fp16 or bf16");
+  SAB_REQUIRE(B > 0 && Hq > 0 && Hkv > 0 && Sq > 0 && Skv > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", B, Hq, Hkv, Sq, Skv);
+  SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
+  SAB_REQUIRE(k_gran >= 1 && k_gran <= 3, SAB_ERR_INVALID, "unknown quant granularity q=%d k=%d", q_gran, k_gran);
+  const int64_t st[21] = {q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s, q_stride_b, q_stride_h, q_stride_s,
+                          k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s, o_stride_b, o_stride_h, o_stride_s,
+                          do_stride_b, do_stride_h, do_stride_s};
+  if (int e = check_bwd_layout(q_int8, k_int8, q, k, v, o, dout, dq, dk, dv, st)) return e;
+  const BwdParams p = bwd_params(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, B, Hq, Hkv, Sq,
+                                 Skv, st, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale);
+  const BlockMask bm{block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb};
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const bool kt = k_gran == SAB_GRAN_PER_THREAD;
+  const bool bf = dtype == SAB_DTYPE_BF16;
+  if (D == 128) {
+    if (kt) return bf ? launch_bwd_blocksparse<128, true, __nv_bfloat16>(p, bm, s) : launch_bwd_blocksparse<128, true, __half>(p, bm, s);
+    return bf ? launch_bwd_blocksparse<128, false, __nv_bfloat16>(p, bm, s) : launch_bwd_blocksparse<128, false, __half>(p, bm, s);
+  }
+  if (kt) return bf ? launch_bwd_blocksparse<64, true, __nv_bfloat16>(p, bm, s) : launch_bwd_blocksparse<64, true, __half>(p, bm, s);
+  return bf ? launch_bwd_blocksparse<64, false, __nv_bfloat16>(p, bm, s) : launch_bwd_blocksparse<64, false, __half>(p, bm, s);
 }

@@ -91,6 +91,53 @@ __device__ __forceinline__ void mbar_wait_wd(uint64_t* bar, uint32_t parity) {
 #endif
 }
 
+// ---- block-sparse attention (sab_qk_int8_sv_f8_attn_blocksparse / sab_qk_int8_attn_bwd_blocksparse).  A kernel argument, not an
+// AttnParams field, so the parameter offsets of the other kernels do not move.
+struct BlockMask {
+  const uint8_t* ptr;              // bool [Bm,Hm,ceil(Sq/128),ceil(Skv/64)]: key block j visible to 128-row Q block i of head h
+  int64_t sb, sh, sqb, skb;        // element strides, 0 for a broadcast dimension
+};
+// Each visible key block costs one 2-byte entry of shared memory in the kernels that compact a mask row (build_kv_list).
+constexpr int kMaxKvBlocks = 16384;                        // Skv <= 16384 * 64 = 1048576 keys
+constexpr size_t kv_list_bytes(int n_blocks) { return 64 + (size_t(n_blocks) * 2 + 15) / 16 * 16; }   // + per-warp counts
+
+// Ascending indices j < n of the visible 64-key blocks of mask row (b, h, qb) into list, by all NT threads of the CTA (uniform
+// control flow: it synchronises the CTA); returns their count to every thread.  scratch: 64 bytes of shared memory.
+template <int NT>
+__device__ __forceinline__ int build_kv_list(const BlockMask& m, int b, int h, int qb, int n, uint16_t* list, int* scratch) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint8_t* row = m.ptr + int64_t(b) * m.sb + int64_t(h) * m.sh + int64_t(qb) * m.sqb;
+  int total = 0;
+  for (int base = 0; base < n; base += NT) {
+    const int j = base + int(threadIdx.x);
+    const bool vis = j < n && __ldg(row + int64_t(j) * m.skb) != 0;
+    const uint32_t bal = __ballot_sync(0xffffffffu, vis);
+    if (lane == 0) scratch[warp] = __popc(bal);
+    __syncthreads();
+    int pos = total + __popc(bal & ((1u << lane) - 1u));
+    for (int w = 0; w < NT / 32; ++w) {
+      if (w < warp) pos += scratch[w];
+      total += scratch[w];
+    }
+    if (vis) list[pos] = uint16_t(j);
+    __syncthreads();   // the list is complete and scratch may be rewritten
+  }
+  return total;
+}
+
+// Host: the block-sparse entries' checks of the mask arguments, before anything touches the device (forward and backward)
+inline int check_block_mask(const void* block_mask, int64_t sb, int64_t sh, int64_t sqb, int64_t skb, int q_gran, int is_causal,
+                            int Sq, int Skv) {
+  SAB_REQUIRE(block_mask != nullptr, SAB_ERR_INVALID, "block_mask: null pointer");
+  SAB_REQUIRE(sb >= 0 && sh >= 0 && sqb >= 0 && skb >= 0, SAB_ERR_INVALID, "block_mask strides must be >= 0 (0 broadcasts)");
+  SAB_REQUIRE(q_gran == SAB_GRAN_PER_WARP || q_gran == SAB_GRAN_PER_THREAD, SAB_ERR_UNSUPPORTED,
+              "the block-sparse path needs per-warp or per-thread Q scales (q_gran %d)", q_gran);
+  SAB_REQUIRE(!is_causal || Sq == Skv, SAB_ERR_INVALID, "qo_len and kv_len must be equal for causal attention.");
+  SAB_REQUIRE(Skv <= kMaxKvBlocks * BN, SAB_ERR_UNSUPPORTED, "the block-sparse path supports kv_len <= %d (got %d)",
+              kMaxKvBlocks * BN, Skv);
+  return SAB_OK;
+}
+
 // Host: opt a kernel into its dynamic shared-memory size once PER DEVICE (cudaFuncSetAttribute applies to the current
 // device only; a process that drives several GPUs — sageattn_host(device=...), tests — must set it on each).
 template <typename Kern>

@@ -344,6 +344,15 @@ def _(query, key, value, output, query_scale, key_scale, value_scale, cu_seqlens
 
 
 # ----------------------------------------------------------------------------------------------- backward
+def _check_bwd_operands(q_int8, k_int8, q, k, o, dout):
+    """The kernels read o and dout at q's sizes as 16-bit words, and q_int8 / k_int8 at q's / k's sizes as bytes: a smaller
+    tensor would be read out of bounds, another dtype as the wrong words."""
+    for name, t in (("o", o), ("dout", dout)):
+        assert t.shape == q.shape and t.dtype == q.dtype, f"{name} must have q's shape and dtype"
+    for name, t, ref in (("q_int8", q_int8, q), ("k_int8", k_int8, k)):
+        assert t.shape == ref.shape and t.dtype == torch.int8, f"{name} must be int8 with the shape of {name[0]}"
+
+
 @torch.library.custom_op("sageattention_b200::qk_int8_attn_bwd", mutates_args=("dq", "dk", "dv"), device_types="cuda")
 def qk_int8_attn_bwd(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale: torch.Tensor, k_scale: torch.Tensor, q: torch.Tensor,
                      k: torch.Tensor, v: torch.Tensor, o: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor,
@@ -357,6 +366,7 @@ def qk_int8_attn_bwd(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale: torch.
     _, Hkv, Skv, _ = _bhsd(k, tensor_layout)
     for x, y in ((dq, q), (dk, k), (dv, v)):
         assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
+    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
     assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (B, Hq, Sq), "lse must be [B,Hq,Sq] fp32"
     strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in _bhs_strides(t, tensor_layout)]
     if k_mean is not None:
@@ -390,6 +400,7 @@ def qk_int8_attn_bwd_masked(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale:
     _, Hkv, Skv, _ = _bhsd(k, tensor_layout)
     for x, y in ((dq, q), (dk, k), (dv, v)):
         assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
+    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
     assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (B, Hq, Sq), "lse must be [B,Hq,Sq] fp32"
     assert attn_mask.dim() == 4 and tuple(attn_mask.shape) == (B, Hq, Sq, Skv), "attn_mask must be expanded to [B,Hq,Sq,Skv]"
     kind = SAB_MASK_BOOL if attn_mask.dtype == torch.bool else SAB_MASK_BIAS
@@ -428,6 +439,7 @@ def qk_int8_attn_bwd_blocksparse(q_int8: torch.Tensor, k_int8: torch.Tensor, q_s
     _, Hkv, Skv, _ = _bhsd(k, tensor_layout)
     for x, y in ((dq, q), (dk, k), (dv, v)):
         assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
+    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
     assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (B, Hq, Sq), "lse must be [B,Hq,Sq] fp32"
     mask = _block_mask_args(block_mask, B, Hq, Sq, Skv)
     strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in _bhs_strides(t, tensor_layout)]
@@ -464,6 +476,7 @@ def qk_int8_attn_bwd_varlen(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale:
     Tk, Hkv, _ = k.shape
     for x, y in ((dq, q), (dk, k), (dv, v)):
         assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
+    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
     assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (Hq, Tq), "lse must be [Hq,Tq] fp32"
     strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in (t.stride(0), t.stride(1))]
     if k_mean is not None:

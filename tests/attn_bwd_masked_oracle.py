@@ -20,11 +20,12 @@ MASKED = -1.0e4
 
 
 def attn_bwd_masked(q8, k8, q_scale, k_scale, q, k, v, o, do, lse, attn_mask, *, q_gran="per_block", k_gran="per_block",
-                    sm_scale=1.0, fold_sm_scale=False, log2e=O.LOG2E_CU, k_mean=None):
+                    sm_scale=1.0, fold_sm_scale=False, log2e=O.LOG2E_CU, k_mean=None, bound=False):
     """attn_bwd (non-causal) with the forward's masked logits.  attn_mask, broadcastable to [B,Hq,Sq,Sk]: bool (False = masked out:
     P = 0) or an additive bias in log2 units, added to the scaled logits as the forward adds it (-inf: P = 0).  A row with
     lse = -inf has no visible key (the forward returned zeros): its P is 0.  Other arguments as attn_bwd.  Returns
-    (dq, dk, dv, dbias) in fp64, dbias = ln2 * dS as [B,Hq,Sq,Sk]."""
+    (dq, dk, dv, dbias) in fp64, dbias = ln2 * dS as [B,Hq,Sq,Sk]; with bound=True also attn_bwd's elementwise bounds of the four,
+    dBias's being ln2 / sm_scale times that of dS's extra dQ columns (e_dS plus the accumulation term, which only widens it)."""
     B, Hq, Sq, D = q8.shape
     _, Hk, Sk, _ = k8.shape
     if attn_mask.dtype == torch.bool:
@@ -46,7 +47,11 @@ def attn_bwd_masked(q8, k8, q_scale, k_scale, q, k, v, o, do, lse, attn_mask, *,
 
     # no visible key: lse = +inf makes P = exp2(S - lse) exactly 0 (the kernel's -lse = -inf)
     lsex = lse.double().masked_fill(lse == float("-inf"), float("inf"))
-    dq, dk, dv = attn_bwd(q8x, k8x, q_scale, k_scale, zpad(q), kx, zpad(v), zpad(o), zpad(do), lsex, q_gran=q_gran, k_gran=k_gran,
-                          sm_scale=sm_scale, fold_sm_scale=fold_sm_scale, log2e=log2e, k_mean=kmx)
-    dS = dq[..., D:] / sm_scale
-    return dq[..., :D], dk[..., :D], dv[..., :D], math.log(2.0) * dS
+    res = attn_bwd(q8x, k8x, q_scale, k_scale, zpad(q), kx, zpad(v), zpad(o), zpad(do), lsex, q_gran=q_gran, k_gran=k_gran,
+                   sm_scale=sm_scale, fold_sm_scale=fold_sm_scale, log2e=log2e, k_mean=kmx, head_dim=D, bound=bound)
+    dq, dk, dv = res[:3]
+    out = (dq[..., :D], dk[..., :D], dv[..., :D], math.log(2.0) / sm_scale * dq[..., D:])
+    if not bound:
+        return out
+    bq, bk, bv = res[3]
+    return out + ((bq[..., :D], bk[..., :D], bv[..., :D], math.log(2.0) / sm_scale * bq[..., D:]),)

@@ -4,12 +4,16 @@
   3. sageattn gradients against fp64 autograd of exact attention;
   4. bit-reproducibility; 5. SDPA monkey-patch training; 6. torch.compile.
 
-Tolerances (normwise relative error ||g - g_ref|| / ||g_ref||):
-  TOL_ORACLE  5e-3: on the same quantised operands and LSE the kernel differs from the oracle only by the input-dtype rounding of
-              P and dS, fp32 accumulation and ex2.approx.  Measured on an H100 80GB HBM3 (700 W): at most 2.4e-3 for bf16 and 3.0e-4
-              for fp16 over ORACLE_CASES;
-  TOL_EXACT   3e-2: against exact attention the straight-through estimator also carries the INT8 / FP8 quantisation of the forward.
-              Measured on the same GPU: 1.0-1.9 % for dq / dk / dv over the four cases below."""
+Tolerances:
+  oracle      every element within the bound of attn_bwd_oracle (check_elementwise): on the same quantised operands and LSE the
+              kernel differs from the oracle only by the input-dtype rounding of P and dS, fp32 accumulation and ex2.approx, and the
+              bound is derived from exactly that rounding model.  Outputs are NaN-filled, so an unwritten element fails.
+              Measured on an H100 80GB HBM3 (400 W power limit) over ORACLE_CASES: worst ratio of error to bound 0.957; normwise relative
+              errors at most 2.5e-3 for bf16 and 3.0e-4 for fp16, except dq without a K mean (4.3e-3 / 5.6e-4) and dk with one key
+              (Skv = 1: dS is a cancellation residue, dk is near zero and its normwise error 1.5e-2, every element inside the bound);
+  TOL_EXACT   3e-2 (normwise ||g - g_ref|| / ||g_ref||): against exact attention the straight-through estimator also carries the
+              INT8 / FP8 quantisation of the forward.  Measured on an H100 80GB HBM3 (700 W): 1.0-1.9 % for dq / dk / dv over the four
+              cases below."""
 import os
 import re
 
@@ -17,12 +21,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from attn_bwd_oracle import attn_bwd
+from attn_bwd_oracle import attn_bwd, check_elementwise
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 pytestmark = pytest.mark.gpu
 
-TOL_ORACLE = 5e-3
 TOL_EXACT = 3e-2
 GRAN = {"per_block": 1, "per_warp": 2, "per_thread": 3}      # SAB_GRAN_*
 
@@ -33,7 +36,10 @@ def _rel(a, b):
 
 
 # ------------------------------------------------------------------------------------------- 2. kernels vs oracle
-# (D, dtype, layout, causal, Hq, Hkv, gran, Sq, Skv, B): per_block = the folded-scale path of sageattn_qk_int8_pv_fp16_triton
+# (D, dtype, layout, causal, Hq, Hkv, gran, Sq, Skv, B[, data, smooth_k]): per_block = the folded-scale path of
+# sageattn_qk_int8_pv_fp16_triton.  data (default "randn"): "peaked" scales Q by 4 (near one-hot softmax rows), "kchan" offsets
+# four K channels by 30 (a large K mean: the K - mean operand of dQ), "voff" offsets V by 20 (dP and delta cancel in dP - delta).
+# smooth_k False (default True): no K mean, the kernels' kmean == nullptr branch.
 BF, FP = torch.bfloat16, torch.float16
 ORACLE_CASES = [
     (128, BF, "HND", False, 2, 2, "per_thread", 256, 256, 2),
@@ -47,6 +53,51 @@ ORACLE_CASES = [
     (64, BF, "HND", False, 2, 2, "per_thread", 1, 300, 1),           # Sq = 1
     (64, FP, "NHD", False, 2, 2, "per_thread", 17, 100, 2),          # Sq = 17
     (128, BF, "HND", False, 2, 2, "per_thread", 8192, 8192, 1),      # B=1, H=2, S=8192
+    # one key tile and its edges: Skv in {1, 17, 64, 65, 128, 129, 4097} against short and long Sq
+    (64, BF, "HND", False, 2, 2, "per_thread", 17, 1, 1, "randn", True),
+    (128, FP, "NHD", False, 2, 2, "per_warp", 300, 1, 1, "randn", True),
+    (128, BF, "NHD", False, 2, 2, "per_block", 17, 17, 1, "randn", True),
+    (64, FP, "HND", False, 2, 2, "per_thread", 300, 64, 1, "randn", True),
+    (128, FP, "HND", False, 2, 2, "per_thread", 17, 65, 1, "randn", True),
+    (64, BF, "NHD", False, 2, 2, "per_warp", 300, 128, 1, "randn", True),
+    (64, FP, "NHD", False, 2, 2, "per_block", 17, 129, 1, "randn", True),
+    (128, BF, "HND", False, 2, 2, "per_warp", 300, 4097, 1, "randn", True),
+    (64, BF, "HND", False, 1, 1, "per_thread", 17, 4097, 1, "randn", True),
+    # Q tile edges: Sq in {1, 64, 65, 127, 128, 129}
+    (128, FP, "NHD", False, 2, 2, "per_thread", 1, 129, 1, "randn", True),
+    (64, FP, "HND", False, 2, 2, "per_warp", 64, 190, 1, "randn", True),
+    (128, BF, "NHD", False, 2, 2, "per_thread", 65, 64, 1, "randn", True),
+    (64, BF, "NHD", False, 2, 2, "per_block", 127, 300, 1, "randn", True),
+    (128, FP, "HND", False, 2, 2, "per_warp", 128, 65, 1, "randn", True),
+    (64, FP, "NHD", False, 2, 2, "per_thread", 129, 17, 1, "randn", True),
+    # causal S in {1, 63, 64, 65, 128, 129, 255, 257}: the dK/dV loop starts at k0 / 64, the dQ loop ends at the diagonal
+    (64, BF, "HND", True, 2, 2, "per_thread", 1, 1, 1, "randn", True),
+    (128, FP, "NHD", True, 2, 2, "per_warp", 63, 63, 1, "randn", True),
+    (64, FP, "HND", True, 2, 2, "per_block", 64, 64, 1, "randn", True),
+    (128, BF, "NHD", True, 2, 2, "per_thread", 65, 65, 1, "randn", True),
+    (64, BF, "NHD", True, 2, 2, "per_warp", 128, 128, 1, "randn", True),
+    (128, FP, "HND", True, 2, 2, "per_thread", 129, 129, 1, "randn", True),
+    (128, BF, "HND", True, 2, 2, "per_block", 255, 255, 1, "randn", True),
+    (64, FP, "NHD", True, 2, 2, "per_thread", 257, 257, 1, "randn", True),
+    # GQA with B > 1 in NHD
+    (128, BF, "NHD", False, 8, 2, "per_thread", 200, 150, 2, "randn", True),
+    (64, FP, "NHD", True, 6, 2, "per_warp", 190, 190, 3, "randn", True),
+    # no K mean, every instantiation
+    (128, BF, "HND", False, 2, 2, "per_thread", 200, 300, 1, "randn", False),
+    (128, FP, "NHD", True, 2, 2, "per_thread", 200, 200, 1, "randn", False),
+    (128, BF, "NHD", False, 2, 2, "per_warp", 150, 200, 1, "randn", False),
+    (128, FP, "HND", False, 2, 2, "per_block", 150, 150, 1, "randn", False),
+    (64, BF, "NHD", True, 2, 2, "per_thread", 150, 150, 1, "randn", False),
+    (64, FP, "HND", False, 2, 2, "per_thread", 100, 200, 1, "randn", False),
+    (64, BF, "HND", False, 2, 2, "per_warp", 100, 200, 1, "randn", False),
+    (64, FP, "NHD", True, 2, 2, "per_block", 180, 180, 1, "randn", False),
+    # data kinds
+    (128, BF, "HND", True, 2, 2, "per_thread", 256, 256, 1, "peaked", True),
+    (64, FP, "NHD", False, 2, 2, "per_warp", 200, 300, 1, "peaked", True),
+    (128, FP, "HND", False, 2, 2, "per_thread", 200, 260, 1, "kchan", True),
+    (64, BF, "NHD", True, 2, 2, "per_block", 300, 300, 1, "kchan", True),
+    (128, BF, "NHD", False, 4, 2, "per_warp", 200, 200, 1, "voff", True),
+    (64, FP, "HND", True, 2, 2, "per_thread", 256, 256, 1, "voff", True),
 ]
 
 
@@ -60,9 +111,17 @@ def _case_instantiation(c):
     return D, gran == "per_thread", "__nv_bfloat16" if dt == BF else "__half"
 
 
+def _case_options(c):
+    return tuple(c[10:]) or ("randn", True)
+
+
 _INST = _instantiations()
 assert len(_INST) == 8 and _INST == {_case_instantiation(c) for c in ORACLE_CASES}, \
     f"ORACLE_CASES must reach every instantiation of attn_bwd.cu: missing {_INST - {_case_instantiation(c) for c in ORACLE_CASES}}"
+assert {(_case_instantiation(c), c[2]) for c in ORACLE_CASES} == {(i, lay) for i in _INST for lay in ("HND", "NHD")}, \
+    "ORACLE_CASES must reach every instantiation in both layouts"
+assert {_case_instantiation(c) for c in ORACLE_CASES if not _case_options(c)[1]} == _INST, \
+    "ORACLE_CASES must run every instantiation without a K mean"
 
 
 def _shape(B, H, S, D, layout):
@@ -73,19 +132,31 @@ def _hnd(x, layout):
     return (x if layout == "HND" else x.transpose(1, 2)).cpu()
 
 
+def _dev_hnd(x, layout):
+    return x if layout == "HND" else x.transpose(1, 2)
+
+
 @pytest.mark.parametrize("case", ORACLE_CASES, ids=lambda c: "-".join(str(x).replace("torch.", "") for x in c))
 def test_gradient_kernels_match_oracle(case):
     import sageattention_b200 as sab
     from sageattention_b200 import ops
-    D, dt, layout, causal, Hq, Hkv, gran, Sq, Skv, B = case
+    D, dt, layout, causal, Hq, Hkv, gran, Sq, Skv, B = case[:10]
+    data, smooth_k = _case_options(case)
     lay = 1 if layout == "HND" else 0
     g = torch.Generator().manual_seed(Sq + 3 * Skv + D)
-    q = torch.randn(_shape(B, Hq, Sq, D, layout), generator=g).to(dt).cuda()
-    k = (torch.randn(_shape(B, Hkv, Skv, D, layout), generator=g) + 2.0 * torch.randn(D, generator=g)).to(dt).cuda()
-    v = torch.randn(_shape(B, Hkv, Skv, D, layout), generator=g).to(dt).cuda()
-    do = torch.randn(_shape(B, Hq, Sq, D, layout), generator=g).to(dt).cuda()
+    q = torch.randn(_shape(B, Hq, Sq, D, layout), generator=g)
+    k = torch.randn(_shape(B, Hkv, Skv, D, layout), generator=g) + 2.0 * torch.randn(D, generator=g)
+    v = torch.randn(_shape(B, Hkv, Skv, D, layout), generator=g)
+    do = torch.randn(_shape(B, Hq, Sq, D, layout), generator=g)
+    if data == "peaked":
+        q = 4.0 * q
+    elif data == "kchan":
+        k[..., :4] += 30.0
+    elif data == "voff":
+        v = v + 20.0
+    q, k, v, do = (t.to(dt).cuda() for t in (q, k, v, do))
     sm = D ** -0.5
-    km = sab.k_mean(k, layout)
+    km = sab.k_mean(k, layout) if smooth_k else None
     o = torch.empty_like(q)
     if gran == "per_block":
         q8, qs, k8, ks = sab.per_block_int8(q, k, km, sm_scale=sm, tensor_layout=layout)
@@ -98,16 +169,17 @@ def test_gradient_kernels_match_oracle(case):
         lse = ops.qk_int8_sv_f8_attn(q8, k8, v8, o, qs, ks, vs, None, lay, int(causal), GRAN[gran], GRAN[gran], sm, 0, 1)
         qg = kg = GRAN[gran]
         fold = 0
-    dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+    # NaN-filled outputs: every element must be written
+    dq, dk, dv = (torch.full_like(t, float("nan")) for t in (q, k, v))
     ops.qk_int8_attn_bwd(q8, k8, qs, ks, q, k, v, o, do, lse, km, dq, dk, dv, lay, int(causal), qg, kg, sm, fold)
-    torch.cuda.synchronize()
-    ref = attn_bwd(_hnd(q8, layout), _hnd(k8, layout), qs.cpu(), ks.cpu(), _hnd(q, layout), _hnd(k, layout), _hnd(v, layout),
-                     _hnd(o, layout), _hnd(do, layout), lse.cpu(), q_gran=gran, k_gran="per_block" if gran == "per_warp" else gran,
-                     is_causal=causal, sm_scale=sm, fold_sm_scale=bool(fold), k_mean=_hnd(km, layout))
-    for name, got, r in zip(("dq", "dk", "dv"), (dq, dk, dv), ref):
-        assert torch.isfinite(got).all(), name
-        err = _rel(_hnd(got, layout), r)
-        assert err <= TOL_ORACLE, f"{name}: normwise relative error {err:.3e}"
+    # the fp64 reference runs on the GPU
+    *ref, bounds = attn_bwd(_dev_hnd(q8, layout), _dev_hnd(k8, layout), qs, ks, _dev_hnd(q, layout), _dev_hnd(k, layout),
+                            _dev_hnd(v, layout), _dev_hnd(o, layout), _dev_hnd(do, layout), lse, q_gran=gran,
+                            k_gran="per_block" if gran == "per_warp" else gran, is_causal=causal, sm_scale=sm,
+                            fold_sm_scale=bool(fold), k_mean=None if km is None else _dev_hnd(km, layout), bound=True)
+    res = {name: check_elementwise(name, _dev_hnd(got, layout), r, b)
+           for name, got, r, b in zip(("dq", "dk", "dv"), (dq, dk, dv), ref, bounds)}
+    print(f"[oracle] {case}: " + ", ".join(f"{n} ratio {w:.3f} normwise {e:.2e}" for n, (w, e) in res.items()))
 
 
 # ------------------------------------------------------------------------------------------- 1. no behaviour change

@@ -6,10 +6,13 @@ with attn_mask):
   3. public API gradients against fp64 autograd of exact masked attention;
   4. bit-reproducibility; 5. exact zeros on fully masked rows and -inf bias positions; 6. torch.compile.
 
-Tolerances (normwise relative error ||g - g_ref|| / ||g_ref||), as for the dense backward (tests/test_gpu_backward.py):
-  TOL_ORACLE  5e-3: on the same quantised operands and LSE the kernels differ from the oracle only by the input-dtype rounding of P
-              and dS (and of dBias), fp32 accumulation and ex2.approx;
-  TOL_EXACT   3e-2: against exact attention the straight-through estimator also carries the INT8 quantisation of Q and K.
+Tolerances, as for the dense backward (tests/test_gpu_backward.py):
+  oracle      every element, dBias included, within the bound of attn_bwd_oracle (check_elementwise; dBias gets ln2 times dS's),
+              derived from the kernels' rounding model (input-dtype rounding of P and dS and of dBias, fp32 accumulation,
+              ex2.approx).  Measured on an H100 80GB HBM3 (400 W power limit) over ORACLE_CASES: worst ratio of error to bound
+              0.947; normwise relative errors at most 2.4e-3 for bf16 and 3.0e-4 for fp16, dBias 1.7e-3 / 2.1e-4;
+  TOL_EXACT   3e-2 (normwise ||g - g_ref|| / ||g_ref||): against exact attention the straight-through estimator also carries the
+              INT8 quantisation of Q and K.
 The oracle and exact-attention tests print their errors (pytest -s)."""
 import math
 import os
@@ -19,11 +22,11 @@ import pytest
 import torch
 
 from attn_bwd_masked_oracle import attn_bwd_masked
+from attn_bwd_oracle import check_elementwise
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 pytestmark = pytest.mark.gpu
 
-TOL_ORACLE = 5e-3
 TOL_EXACT = 3e-2
 BF, FP = torch.bfloat16, torch.float16
 LN2 = math.log(2.0)
@@ -116,16 +119,12 @@ def test_masked_gradient_kernels_match_oracle(case):
     ops.qk_int8_attn_bwd_masked(q8, k8, qs, ks, q, k, v, o, do, lse, km, dq, dk, dv, mask, dbias, lay, GRAN[gran], GRAN[gran], sm,
                                 fold)
     torch.cuda.synchronize()
-    ref = attn_bwd_masked(_hnd(q8, layout), _hnd(k8, layout), qs.cpu(), ks.cpu(), _hnd(q, layout), _hnd(k, layout), _hnd(v, layout),
-                          _hnd(o, layout), _hnd(do, layout), lse.cpu(), mask.cpu(), q_gran=gran, k_gran="per_block", sm_scale=sm,
-                          fold_sm_scale=bool(fold), k_mean=_hnd(km, layout))
+    *ref, bounds = attn_bwd_masked(_hnd(q8, layout), _hnd(k8, layout), qs.cpu(), ks.cpu(), _hnd(q, layout), _hnd(k, layout),
+                                   _hnd(v, layout), _hnd(o, layout), _hnd(do, layout), lse.cpu(), mask.cpu(), q_gran=gran,
+                                   k_gran="per_block", sm_scale=sm, fold_sm_scale=bool(fold), k_mean=_hnd(km, layout), bound=True)
     got = (_hnd(dq, layout), _hnd(dk, layout), _hnd(dv, layout)) + (() if dbias is None else (dbias.cpu(),))
-    errs = {}
-    for name, x, r in zip(("dq", "dk", "dv", "dbias"), got, ref):
-        assert torch.isfinite(x).all(), name
-        errs[name] = _rel(x, r)
-    print(f"[oracle] {case[:11]} {str(dt)[6:]}: " + ", ".join(f"{n} {e:.2e}" for n, e in errs.items()))
-    assert max(errs.values()) <= TOL_ORACLE, f"normwise relative errors {errs}"
+    res = {name: check_elementwise(name, x, r, b) for name, x, r, b in zip(("dq", "dk", "dv", "dbias"), got, ref, bounds)}
+    print(f"[oracle] {case[:11]} {str(dt)[6:]}: " + ", ".join(f"{n} ratio {w:.3f} normwise {e:.2e}" for n, (w, e) in res.items()))
     if Sq > 1:   # query row 1 is fully masked: lse -inf, zero dq (and dBias) rows
         assert torch.isinf(lse[:, :, 1]).all() and not got[0][:, :, 1].any()
         if dbias is not None:

@@ -6,23 +6,25 @@
   4. sageattn_varlen gradients against fp64 autograd of exact per-sequence attention;
   5. bit-reproducibility and torch.compile; 6. training a packed-sequence block.
 
-Tolerances (normwise relative error ||g - g_ref|| / ||g_ref||), as for the dense backward (tests/test_gpu_backward.py):
-  TOL_ORACLE  5e-3: on the same quantised operands and LSE the kernels differ from the oracle only by the input-dtype rounding of P
-              and dS, fp32 accumulation and ex2.approx.  Measured on an H100 80GB HBM3 (700 W): at most 2.4e-3 for bf16 and 3.0e-4
-              for fp16 over VARLEN_ORACLE_CASES;
-  TOL_EXACT   3e-2: against exact attention the straight-through estimator also carries the INT8 quantisation of Q and K.
-              Measured on the same GPU: 1.1-1.3 % for dq / dk / dv over the four cases below.
+Tolerances, as for the dense backward (tests/test_gpu_backward.py):
+  oracle      every element within the bound of attn_bwd_oracle (check_elementwise), derived from the kernels' rounding model
+              (input-dtype rounding of P and dS, fp32 accumulation, ex2.approx).  Measured on an H100 80GB HBM3 (400 W power limit)
+              over VARLEN_ORACLE_CASES: worst ratio of error to bound 0.997 (fp16 dk, in the case with a one-query sequence,
+              whose keys' dK is one rounded term); normwise relative errors at most 2.4e-3 for bf16 and 3.0e-4 for fp16;
+  TOL_EXACT   3e-2 (normwise ||g - g_ref|| / ||g_ref||): against exact attention the straight-through estimator also carries the
+              INT8 quantisation of Q and K.  Measured on an H100 80GB HBM3 (700 W): 1.1-1.3 % for dq / dk / dv over the four cases
+              below.
 The oracle and exact-attention tests print their errors (pytest -s)."""
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+from attn_bwd_oracle import check_elementwise
 from attn_bwd_varlen_oracle import attn_bwd_varlen
 
 pytestmark = pytest.mark.gpu
 
-TOL_ORACLE = 5e-3
 TOL_EXACT = 3e-2
 BF, FP = torch.bfloat16, torch.float16
 
@@ -77,14 +79,12 @@ def test_varlen_gradient_kernels_match_oracle(case, causal):
     ops.qk_int8_attn_bwd_varlen(q8, k8, qs, ks, q, k, v, o, do, lse, km, dq, dk, dv, cq, ck, cqs, cks, max(lq), max(lk), int(causal),
                                 sm, 1)
     torch.cuda.synchronize()
-    ref = attn_bwd_varlen(q8.cpu(), k8.cpu(), qs.cpu(), ks.cpu(), q.cpu(), k.cpu(), v.cpu(), o.cpu(), do.cpu(), lse.cpu(),
-                          cq.cpu(), ck.cpu(), cqs.cpu(), cks.cpu(), is_causal=causal, sm_scale=sm, k_mean=km.cpu())
-    errs = {}
-    for name, got, r in zip(("dq", "dk", "dv"), (dq, dk, dv), ref):
-        assert torch.isfinite(got).all(), name
-        errs[name] = _rel(got, r)
-    print(f"[oracle] {case[:5]} {str(dt)[6:]} causal={causal}: " + ", ".join(f"{n} {e:.2e}" for n, e in errs.items()))
-    assert max(errs.values()) <= TOL_ORACLE, f"normwise relative errors {errs}"
+    *ref, bounds = attn_bwd_varlen(q8.cpu(), k8.cpu(), qs.cpu(), ks.cpu(), q.cpu(), k.cpu(), v.cpu(), o.cpu(), do.cpu(), lse.cpu(),
+                                   cq.cpu(), ck.cpu(), cqs.cpu(), cks.cpu(), is_causal=causal, sm_scale=sm, k_mean=km.cpu(), bound=True)
+    res = {name: check_elementwise(name, got.cpu(), r, b, dims=("token", "h", "col"))
+           for name, got, r, b in zip(("dq", "dk", "dv"), (dq, dk, dv), ref, bounds)}
+    print(f"[oracle] {case[:5]} {str(dt)[6:]} causal={causal}: " + ", ".join(f"{n} ratio {w:.3f} normwise {e:.2e}"
+                                                                          for n, (w, e) in res.items()))
     for i in range(len(lq)):
         if lq[i] == 0 and lk[i] > 0:
             s = slice(int(ck[i]), int(ck[i + 1]))

@@ -14,6 +14,7 @@ import sageattention_b200 as sab
 from sageattention_b200 import ops
 from attn_blocksparse_oracle import attn_int8_fp8_blocksparse, expand_block_mask
 from attn_bwd_masked_oracle import attn_bwd_masked
+from attn_bwd_oracle import check_elementwise
 from sageattention_b200.core import _quant_qk
 from sageattention_b200.quant import per_channel_fp8
 
@@ -21,7 +22,9 @@ pytestmark = pytest.mark.gpu
 BF, FP = torch.bfloat16, torch.float16
 TOL_EXACT = 6e-2      # max-abs against exact attention (tests/test_gpu_parity.py)
 TOL_GRAD = 3e-2       # normwise against fp64 autograd of exact attention (tests/test_gpu_backward.py)
-TOL_ORACLE = 5e-3     # normwise against the fp64 gradient reference on the kernels' own operands (tests/test_gpu_backward_masked.py)
+# The gradient kernels are checked elementwise against the bound of tests/attn_bwd_oracle.py (check_elementwise) on their own
+# operands.  Measured on an H100 80GB HBM3 (400 W power limit) over BWD_ORACLE_CASES: worst ratio of error to bound 0.854;
+# normwise relative errors at most 2.4e-3 for bf16 and 3.0e-4 for fp16.
 GRAN = {"per_warp": 2, "per_thread": 3}     # SAB_GRAN_*
 
 
@@ -284,15 +287,12 @@ def test_sparse_gradient_kernels_match_oracle(case):
     em = expand_block_mask(bm, Sq, Sk).cpu()
     if causal:
         em = em & torch.ones(Sq, Sk, dtype=torch.bool).tril()
-    ref = attn_bwd_masked(_hnd(q8, layout), _hnd(k8, layout), qs.cpu(), ks.cpu(), _hnd(q, layout), _hnd(k, layout), _hnd(v, layout),
-                          _hnd(o, layout), _hnd(do, layout), lse.cpu(), em, q_gran=gran, k_gran=gran, sm_scale=D ** -0.5,
-                          k_mean=_hnd(km, layout))
-    errs = {}
-    for name, x, r in zip(("dq", "dk", "dv"), (_hnd(dq, layout), _hnd(dk, layout), _hnd(dv, layout)), ref):
-        assert torch.isfinite(x).all(), name
-        errs[name] = ((x.double() - r).norm() / r.norm()).item()
-    print(f"[oracle] {case}: " + ", ".join(f"{n} {e:.2e}" for n, e in errs.items()))
-    assert max(errs.values()) <= TOL_ORACLE, errs
+    *ref, bounds = attn_bwd_masked(_hnd(q8, layout), _hnd(k8, layout), qs.cpu(), ks.cpu(), _hnd(q, layout), _hnd(k, layout),
+                                   _hnd(v, layout), _hnd(o, layout), _hnd(do, layout), lse.cpu(), em, q_gran=gran, k_gran=gran,
+                                   sm_scale=D ** -0.5, k_mean=_hnd(km, layout), bound=True)
+    res = {name: check_elementwise(name, x, r, b)
+           for name, x, r, b in zip(("dq", "dk", "dv"), (_hnd(dq, layout), _hnd(dk, layout), _hnd(dv, layout)), ref, bounds[:3])}
+    print(f"[oracle] {case}: " + ", ".join(f"{n} ratio {w:.3f} normwise {e:.2e}" for n, (w, e) in res.items()))
     hidden_rows = ~em.any(-1)
     assert torch.all(_hnd(dq, layout)[hidden_rows] == 0)
     assert torch.all(_hnd(dk, layout)[:, :, 64:128] == 0) and torch.all(_hnd(dv, layout)[:, :, 64:128] == 0)

@@ -367,6 +367,34 @@ int sab_qk_int8_attn_bwd_blocksparse(const int8_t* q_int8, const int8_t* k_int8,
                                      int64_t mask_stride_b, int64_t mask_stride_h, int64_t mask_stride_qb, int64_t mask_stride_kb,
                                      void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Block-mask prediction from pooled Q/K statistics (no reference counterpart; SpargeAttn's training-free first stage): the
+ * block_mask of sab_qk_int8_sv_f8_attn_blocksparse chosen from per-block means and self-similarities.
+ *
+ * sab_block_stats: x bhsd (`dtype`), D <= 128 and a multiple of 8 (zero padding changes no statistic), 16-byte aligned, strides
+ * multiples of 8 elements; blk 128 (Q) or 64 (K).  For block c of each (b,h), with n = min(blk, S - c*blk) rows, in fp32:
+ *   mean[b,h,c,:] = (1/n) sum_r x_r                                   ([B,H,ceil(S/blk),D] contiguous)
+ *   sim[b,h,c]    = |sum_r x_r/|x_r||^2 / n^2  (a zero row counts 0)   ([B,H,ceil(S/blk)] contiguous)
+ * sim is the mean of the block's n x n cosine-similarity matrix, diagonal included, so 0 <= sim <= 1.
+ *
+ * sab_predict_block_mask: q_mean / q_sim from sab_block_stats(q, blk 128), k_mean / k_sim from sab_block_stats(k, blk 64), the same D;
+ * block_mask: bool bytes [B,Hq,nq,nk] contiguous, nq = ceil(Sq/128), nk = ceil(Skv/64).  Row (b,h,i), hk = h / (Hq/Hkv):
+ *   candidates C_i = { j : k_sim[j] >= sim_threshold }, and 64 j <= 128 i + 127 when is_causal;
+ *   p = softmax over C_i of sm_scale * (q_mean_i . k_mean_j);
+ *   order C_i by p descending, ties by ascending j; j is kept iff the sum of p over the blocks before it in that order is
+ *   < cdf_threshold (the top block is always kept; cdf_threshold >= 1 keeps every candidate);
+ *   forced visible: the whole row if q_sim[i] < sim_threshold, the whole column j if k_sim[j] < sim_threshold, and when is_causal the
+ *   diagonal blocks 128 i <= 64 j + 63 (so no row is empty);
+ *   when is_causal every block with 64 j > 128 i + 127 is hidden, forced ones included.
+ * Checks before touching the device: null pointers, D, Hq % Hkv, Skv <= 1048576, is_causal with Sq != Skv, cdf_threshold <= 0 or
+ * NaN, a NaN sim_threshold, a non-finite sm_scale.  Deterministic (fixed summation orders, no atomics).
+ * ---------------------------------------------------------------------------------------------- */
+int sab_block_stats(const void* x, int dtype, float* mean, float* sim, int B, int H, int S, int D, int64_t stride_b,
+                    int64_t stride_h, int64_t stride_s, int blk, void* stream);
+int sab_predict_block_mask(const float* q_mean, const float* q_sim, const float* k_mean, const float* k_sim, uint8_t* block_mask,
+                           int B, int Hq, int Hkv, int Sq, int Skv, int D, int is_causal, float sm_scale, float cdf_threshold,
+                           float sim_threshold, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

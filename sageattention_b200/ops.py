@@ -498,6 +498,56 @@ def _(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, d
     return None
 
 
+# ----------------------------------------------------------------------------------------------- block-mask prediction
+@torch.library.custom_op("sageattention_b200::block_stats", mutates_args=("mean", "sim"), device_types="cuda")
+def block_stats(x: torch.Tensor, mean: torch.Tensor, sim: torch.Tensor, tensor_layout: int, block_size: int) -> None:
+    """Per-block fp32 mean [B,H,ceil(S/block_size),D] and self-similarity [B,H,ceil(S/block_size)] of x (include/sageattn_b200.h,
+    sab_block_stats); block_size 128 for q, 64 for k.  A view whose rows are not 16-byte aligned is read from a contiguous copy."""
+    B, H, S, D = _bhsd(x, tensor_layout)
+    if x.data_ptr() % 16 or any(s % 8 for s in x.stride()[:-1]):
+        x = x.contiguous()
+    nb = (S + block_size - 1) // block_size
+    assert mean.dtype == torch.float32 and mean.is_contiguous() and tuple(mean.shape) == (B, H, nb, D), \
+        f"mean must be a contiguous fp32 [{B}, {H}, {nb}, {D}] tensor"
+    assert sim.dtype == torch.float32 and sim.is_contiguous() and tuple(sim.shape) == (B, H, nb), \
+        f"sim must be a contiguous fp32 [{B}, {H}, {nb}] tensor"
+    sb, sh, ss = _bhs_strides(x, tensor_layout)
+    with torch.cuda.device(x.device):
+        check(lib().sab_block_stats(x.data_ptr(), _dt(x), mean.data_ptr(), sim.data_ptr(), B, H, S, D, sb, sh, ss, block_size,
+                                    _stream(x)))
+
+
+@block_stats.register_fake
+def _(x, mean, sim, tensor_layout, block_size):
+    return None
+
+
+@torch.library.custom_op("sageattention_b200::predict_block_mask", mutates_args=("block_mask",), device_types="cuda")
+def predict_block_mask(q_mean: torch.Tensor, q_sim: torch.Tensor, k_mean: torch.Tensor, k_sim: torch.Tensor,
+                       block_mask: torch.Tensor, Sq: int, Skv: int, is_causal: int, sm_scale: float, cdf_threshold: float,
+                       sim_threshold: float) -> None:
+    """Writes the bool [B,Hq,ceil(Sq/128),ceil(Skv/64)] block_mask predicted from block_stats of q (block 128) and k (block 64)
+    (include/sageattn_b200.h, sab_predict_block_mask)."""
+    B, Hq, nq, D = q_mean.shape
+    Hkv, nk = k_mean.size(1), k_mean.size(2)
+    assert nq == (Sq + 127) // 128 and nk == (Skv + 63) // 64 and k_mean.size(3) == D and k_mean.size(0) == B, \
+        "q / k statistics do not match Sq / Skv"
+    for t in (q_mean, q_sim, k_mean, k_sim):
+        assert t.dtype == torch.float32 and t.is_contiguous(), "block statistics must be contiguous fp32"
+    assert tuple(q_sim.shape) == (B, Hq, nq) and tuple(k_sim.shape) == (B, Hkv, nk), "sim shapes do not match the means"
+    assert block_mask.dtype == torch.bool and block_mask.is_contiguous() and tuple(block_mask.shape) == (B, Hq, nq, nk), \
+        f"block_mask must be a contiguous bool [{B}, {Hq}, {nq}, {nk}] tensor"
+    with torch.cuda.device(q_mean.device):
+        check(lib().sab_predict_block_mask(q_mean.data_ptr(), q_sim.data_ptr(), k_mean.data_ptr(), k_sim.data_ptr(),
+                                           block_mask.data_ptr(), B, Hq, Hkv, Sq, Skv, D, is_causal, float(sm_scale),
+                                           float(cdf_threshold), float(sim_threshold), _stream(q_mean)))
+
+
+@predict_block_mask.register_fake
+def _(q_mean, q_sim, k_mean, k_sim, block_mask, Sq, Skv, is_causal, sm_scale, cdf_threshold, sim_threshold):
+    return None
+
+
 # ----------------------------------------------------------------------------------------------- FP16-PV variant
 @torch.library.custom_op("sageattention_b200::v_transpose_f16", mutates_args=("v_f16t",), device_types="cuda")
 def v_transpose_f16(v: torch.Tensor, v_f16t: torch.Tensor, tensor_layout: int) -> None:

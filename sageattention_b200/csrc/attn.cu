@@ -6,8 +6,9 @@
 // sageattn_qk_int8_pv_fp16_cuda).  One CTA = one 128-row Q tile of one (batch, head), 384 threads:
 //   warps 0-3 / 4-7 : two consumer warpgroups, 64 Q rows each.  Per 64-key tile: S = Q K^T (wgmma s8, int32 accumulators in
 //                     registers), online softmax in registers, P (e4m3 or f16) handed to the PV wgmma as its register A operand,
-//                     O (fp32, 64 x D) accumulated in registers.  The two warpgroups run independently, so one's softmax overlaps
-//                     the other's tensor-core work.
+//                     O (fp32, 64 x D) accumulated in registers.  The loop is rotated so that each warpgroup issues PV(j-1)
+//                     and QK(j) as one tensor-core phase per tile, and the two warpgroups ping-pong: named barriers hand the
+//                     turn to issue from one to the other, so one's softmax runs while the other's MMAs are on the tensor cores.
 //   warp 8          : TMA producer (Q once; K and V^T 64-key tiles through a kStages-deep mbarrier ring, swizzled smem);
 //                     warps 9-11 only hand their registers over (setmaxnreg: 24 for the producer warpgroup, 240 for consumers).
 // The softmax / MMA tile is 64 keys — the reference's CTA_K — so the running-max sequence, P and d follow
@@ -196,41 +197,34 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   const int src0 = (lane & ~3) | ((t & 1) << 1);
   const uint32_t psel = (t >> 1) ? 0x7632u : 0x5410u;
 
-  if (n_kv > 0) mbar_wait_wd(q_full, 0);
-  for (int j = 0; j < n_kv; ++j) {
-    const int st = j % kStages;
+  // ---- per-tile operands of the softmax, set before the tile's GEMM phase so the K-scale load overlaps it
+  float coef[2];           // dequant coefficient of each row part
+  int limit[2];            // number of visible keys of this tile per row (OOB + causal, attn_utils.cuh:296-351)
+  bool masked_tile = false;
+  auto tile_setup = [&](int j) {
     int kj = j;   // the 64-key tile of step j
     if constexpr (kSparse<kPV16, kMask>) kj = kv_list<D>(smem)[j];
-    float coef[2];
-    {
-      // dequant coefficient (…sm89.cuh:116-132, 255-257); tile kj == 64-key block kj.  Per-thread K scales: the keys of lane t
-      // (8i+2t, 8i+2t+1) are all in scale group t.
-      const float ksv = k_dequant<kKT>(p, ks_base, k_blk0 + kj, t);
-      coef[0] = ksv * qss[0];
-      coef[1] = ksv * qss[1];
-    }
-    // number of visible keys of this tile per row (OOB + causal, attn_utils.cuh:296-351)
-    int limit[2];
+    // dequant coefficient (…sm89.cuh:116-132, 255-257); tile kj == 64-key block kj.  Per-thread K scales: the keys of lane t
+    // (8i+2t, 8i+2t+1) are all in scale group t.
+    const float ksv = k_dequant<kKT>(p, ks_base, k_blk0 + kj, t);
+    coef[0] = ksv * qss[0];
+    coef[1] = ksv * qss[1];
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       limit[i] = kv_len - kj * BN;
       if (p.causal) limit[i] = min(limit[i], p.causal_q_offset + q_row[i] - kj * BN + 1);
       if (kElemMask<kPV16, kMask> && q_row[i] >= q_len) limit[i] = 0;   // rows past the end: nothing visible, no mask bytes read
     }
-    const bool masked_tile = kElemMask<kPV16, kMask> || (kv_len - kj * BN < BN) || (p.causal && (kj + 1) * BN > p.causal_q_offset + qt * BM + 1);
+    masked_tile = kElemMask<kPV16, kMask> || (kv_len - kj * BN < BN) || (p.causal && (kj + 1) * BN > p.causal_q_offset + qt * BM + 1);
+  };
 
-    mbar_wait_wd(kv_full + st, (j / kStages) & 1);
-    uint32_t s[32];
-    wgmma_fence();
-    {
-      const uint64_t dK = dK0 + uint64_t(st) * (K_TILE >> 4);
-#pragma unroll
-      for (int k = 0; k < D / 32; ++k) wgmma_qk_i8(s, dQ + 2 * k, dK + 2 * k, k > 0);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(s);
+  uint32_t s[32];                   // S of the tile in flight (int32)
+  float alpha[2];                   // O rescale factor of the last softmax'd tile
+  uint32_t a[kPV16 ? 4 : 2][4];     // its P as the PV A operand
+  [[maybe_unused]] float ot[NO];    // FP8 path: its P V, from zero
 
+  // ---- S (registers, int32) -> P: running max m, sum d, rescale factor alpha, P as A fragments
+  auto softmax = [&](int j) {
     [[maybe_unused]] const char* mrow[2] = {nullptr, nullptr};   // this row's 64 mask elements of tile j
     if constexpr (kElemMask<kPV16, kMask>) {
 #pragma unroll
@@ -249,7 +243,6 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     }
 
     float e[32];           // P in fp32, same register order as S
-    float alpha[2];
     auto tile = [&](auto masked_tag) {
       constexpr bool MASKED = decltype(masked_tag)::value;
 #pragma unroll
@@ -348,23 +341,9 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     else if (masked_tile) tile(std::true_type{});
     else tile(std::false_type{});
 
-    // ---- rescale O (registers) when the running max moved; PV(j-1) has completed
-    auto rescale_o = [&]() {
-      if (alpha[0] != 1.0f || alpha[1] != 1.0f) {
-#pragma unroll
-        for (int i = 0; i < NO; i += 4) {
-          o[i] *= alpha[0];
-          o[i + 1] *= alpha[0];
-          o[i + 2] *= alpha[1];
-          o[i + 3] *= alpha[1];
-        }
-      }
-    };
-
-    // ---- P -> A fragments, O += P V
-    const uint64_t dV = dV0 + uint64_t(st) * (V_TILE >> 4);
+    // ---- P -> A fragments
     if constexpr (kPV16) {
-      uint32_t a[4][4];   // k16 step kk: keys 16kk..16kk+15 = accumulator blocks 2kk, 2kk+1 (same layout: no exchange)
+      // k16 step kk: keys 16kk..16kk+15 = accumulator blocks 2kk, 2kk+1 (same layout: no exchange)
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk) {
         const int i0 = 8 * kk, i1 = 8 * kk + 4;
@@ -373,15 +352,8 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         a[kk][2] = pack_f16x2(e[i1], e[i1 + 1]);
         a[kk][3] = pack_f16x2(e[i1 + 2], e[i1 + 3]);
       }
-      rescale_o();
-      wgmma_fence();
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) wgmma_pv_f16(o, a[kk], dV + 2 * kk, 1);
-      wgmma_commit();
-      wgmma_wait<0>();
-      fence_regs(o);
     } else {
-      uint32_t a[2][4];   // k32 chunk c: keys 32c..32c+31 = accumulator blocks 4c..4c+3
+      // k32 chunk c: keys 32c..32c+31 = accumulator blocks 4c..4c+3
 #pragma unroll
       for (int c = 0; c < 2; ++c) {
 #pragma unroll
@@ -393,18 +365,96 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
           a[c][2 + i] = __byte_perm(__shfl_sync(0xffffffffu, y, src0), __shfl_sync(0xffffffffu, y, src0 + 1), psel);
         }
       }
-      float ot[NO];   // this tile's P V, from zero
-      wgmma_fence();
+    }
+  };
+
+  // ---- rescale O (registers) by alpha of the tile whose PV comes next.  A separate rounding step, never contracted into an
+  // FMA with the add of that tile's P V: O's per-element sequence is o *= alpha(j); o += PV(j); o *= alpha(j+1); ...
+  auto rescale_o = [&]() {
+    if (alpha[0] != 1.0f || alpha[1] != 1.0f) {
+#pragma unroll
+      for (int i = 0; i < NO; i += 4) {
+        o[i] = __fmul_rn(o[i], alpha[0]);
+        o[i + 1] = __fmul_rn(o[i + 1], alpha[0]);
+        o[i + 2] = __fmul_rn(o[i + 2], alpha[1]);
+        o[i + 3] = __fmul_rn(o[i + 3], alpha[1]);
+      }
+    }
+  };
+  auto issue_qk = [&](int j) {   // S = Q K(j)^T
+    const uint64_t dK = dK0 + uint64_t(j % kStages) * (K_TILE >> 4);
+#pragma unroll
+    for (int k = 0; k < D / 32; ++k) wgmma_qk_i8(s, dQ + 2 * k, dK + 2 * k, k > 0);
+  };
+  auto issue_pv = [&](int j) {   // FP16: O += P V(j) in place (O already rescaled); FP8: ot = P V(j)
+    const uint64_t dV = dV0 + uint64_t(j % kStages) * (V_TILE >> 4);
+    if constexpr (kPV16) {
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_pv_f16(o, a[kk], dV + 2 * kk, 1);
+    } else {
 #pragma unroll
       for (int c = 0; c < 2; ++c) wgmma_pv_f8(ot, a[c], dV + 2 * c, c > 0);
-      wgmma_commit();
-      rescale_o();    // overlaps the MMA
-      wgmma_wait<0>();
+    }
+  };
+  auto finish_pv = [&](int j) {  // after the wait: fold the FP8 tile product into O, release slot j
+    if constexpr (kPV16) {
+      fence_regs(o);
+    } else {
       fence_regs(ot);
 #pragma unroll
       for (int i = 0; i < NO; ++i) o[i] += ot[i];
     }
-    if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty + st);   // K(j) and V(j) consumed by this warpgroup
+    if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty + j % kStages);   // K(j) and V(j) consumed by this warpgroup
+  };
+
+  // ---- main loop, rotated so each warpgroup has ONE tensor-core phase per tile: PV(j-1) and QK(j) issued back to back, then
+  // PV(j-1) folded into O and softmax(j) on the CUDA cores.  The two warpgroups take turns at issuing their phases (named
+  // barrier 1 + wg is this warpgroup's turn, arrived at by the other one right after its commit), so one's softmax runs while
+  // the other's MMAs are on the tensor cores.  Each warpgroup has n_kv + 1 phases; warpgroup 1 hands the first turn to
+  // warpgroup 0 and skips the hand-over after its last phase, so no arrival is left over at exit.  n_kv is uniform per CTA;
+  // with n_kv == 0 no barrier is touched.  Slot j-1 is released one phase later than it was consumed; the ring absorbs it.
+  constexpr uint32_t kTurnThreads = 2 * 128;
+  const uint32_t my_turn = 1 + wg, their_turn = 2 - wg;
+  if (n_kv > 0) {
+    mbar_wait_wd(q_full, 0);
+    if (wg == 1) named_bar_arrive(their_turn, kTurnThreads);
+    tile_setup(0);
+    mbar_wait_wd(kv_full, 0);                  // never hold the turn while waiting on TMA
+    named_bar_sync(my_turn, kTurnThreads);
+    wgmma_fence();
+    issue_qk(0);
+    wgmma_commit();
+    named_bar_arrive(their_turn, kTurnThreads);
+    wgmma_wait<0>();
+    fence_regs(s);
+    softmax(0);
+  }
+  for (int j = 1; j < n_kv; ++j) {
+    tile_setup(j);
+    mbar_wait_wd(kv_full + j % kStages, (j / kStages) & 1);
+    named_bar_sync(my_turn, kTurnThreads);
+    if constexpr (kPV16) rescale_o();          // before the in-place PV
+    wgmma_fence();
+    issue_pv(j - 1);
+    issue_qk(j);
+    wgmma_commit();
+    named_bar_arrive(their_turn, kTurnThreads);
+    if constexpr (!kPV16) rescale_o();         // overlaps the MMAs
+    wgmma_wait<0>();
+    fence_regs(s);
+    finish_pv(j - 1);
+    softmax(j);
+  }
+  if (n_kv > 0) {
+    named_bar_sync(my_turn, kTurnThreads);
+    if constexpr (kPV16) rescale_o();
+    wgmma_fence();
+    issue_pv(n_kv - 1);
+    wgmma_commit();
+    if (wg == 0) named_bar_arrive(their_turn, kTurnThreads);
+    if constexpr (!kPV16) rescale_o();
+    wgmma_wait<0>();
+    finish_pv(n_kv - 1);
   }
 
   // ---- epilogue: O / d * v_scale (+ v_mean) -> fp16/bf16 (…sm89.cuh:572-703)

@@ -72,6 +72,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, uint32
       ::"r"(smem_u32(bar)), "r"(parity), "r"(hint_ns)
       : "memory");
 }
+// Named CTA barrier (id 1..15; id 0 is __syncthreads): bar.sync blocks until n threads (a multiple of 32, the caller's warp
+// included) have arrived at barrier id; bar.arrive counts the calling warp towards that total without waiting.
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t n) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory");
+}
 // Warpgroup-wide register re-allocation (all four warps of the warpgroup execute it).
 template <int N>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }

@@ -217,6 +217,21 @@ int sab_qk_int8_sv_f8_attn_blocksparse(const int8_t* q_int8, const int8_t* k_int
                                        const uint8_t* block_mask, int64_t mask_stride_b, int64_t mask_stride_h,
                                        int64_t mask_stride_qb, int64_t mask_stride_kb, void* stream);
 
+/* Sliding-window form of sab_qk_int8_sv_f8_attn (dense tensors only, as the block-sparse form).
+ *   Key j is visible to query i iff i - window_left <= j <= i + window_right (and j <= i when is_causal, which needs Sq == Skv);
+ *   -1 leaves that side unbounded.  Top-left alignment (query i and key i are the same position); Sq != Skv is allowed when not
+ *   causal.  Each 128-row Q tile visits only the 64-key tiles that meet its rows' windows and masks the elements on the tiles
+ *   an edge crosses.  (-1, -1) computes the bytes of sab_qk_int8_sv_f8_attn, (-1, 0) those of its causal call.
+ *   A row with no visible key returns 0 and lse -inf.  window_left / window_right < -1 and causal with Sq != Skv are refused
+ *   before anything touches the device. */
+int sab_qk_int8_sv_f8_attn_window(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out, float* lse,
+                                  const float* q_scale, const float* k_scale, const float* v_scale, const float* v_mean,
+                                  int out_dtype, int B, int Hq, int Hkv, int Sq, int Skv, int D, int64_t q_stride_b,
+                                  int64_t q_stride_h, int64_t q_stride_s, int64_t k_stride_b, int64_t k_stride_h,
+                                  int64_t k_stride_s, int64_t v_s_pad, int64_t o_stride_b, int64_t o_stride_h,
+                                  int64_t o_stride_s, int is_causal, int q_gran, int k_gran, float sm_scale,
+                                  int fold_sm_scale, int window_left, int window_right, void* stream);
+
 /* ------------------------------------------------------------------------------------------------
  * FP16-PV variant: INT8 QK^T -> fp32 online softmax WITHOUT exponent offset -> FP16 P -> FP16 PV
  * (wgmma f16, fp32 accumulation).  Replaces the Triton attention launchers
@@ -366,6 +381,21 @@ int sab_qk_int8_attn_bwd_blocksparse(const int8_t* q_int8, const int8_t* k_int8,
                                      int k_gran, float sm_scale, int fold_sm_scale, const uint8_t* block_mask,
                                      int64_t mask_stride_b, int64_t mask_stride_h, int64_t mask_stride_qb, int64_t mask_stride_kb,
                                      void* stream);
+
+/* Sliding-window form of sab_qk_int8_attn_bwd: the gradient of sab_qk_int8_sv_f8_attn_window.  Same definition and arguments as
+ * sab_qk_int8_attn_bwd plus exactly the window the forward received (same checks, codes and messages); P = 0 outside the window,
+ * and a row with lse = -inf gets zero gradients.  The dQ kernel walks the forward's tile range of each 128-row Q tile; the dK/dV
+ * kernel of the 128 keys at k0 visits only the 64-row Q tiles that meet rows [k0 - right, k0 + 127 + left].  Keys no row sees
+ * get zero dk and dv.  Deterministic like the dense form. */
+int sab_qk_int8_attn_bwd_window(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale, const void* q,
+                                const void* k, const void* v, const void* o, const void* dout, const float* lse, const void* k_mean,
+                                void* dq, void* dk, void* dv, void* workspace, int dtype, int B, int Hq, int Hkv, int Sq, int Skv, int D,
+                                int64_t q8_stride_b, int64_t q8_stride_h, int64_t q8_stride_s, int64_t k8_stride_b,
+                                int64_t k8_stride_h, int64_t k8_stride_s, int64_t q_stride_b, int64_t q_stride_h, int64_t q_stride_s,
+                                int64_t k_stride_b, int64_t k_stride_h, int64_t k_stride_s, int64_t v_stride_b, int64_t v_stride_h,
+                                int64_t v_stride_s, int64_t o_stride_b, int64_t o_stride_h, int64_t o_stride_s, int64_t do_stride_b,
+                                int64_t do_stride_h, int64_t do_stride_s, int is_causal, int q_gran, int k_gran, float sm_scale,
+                                int fold_sm_scale, int window_left, int window_right, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Block-mask prediction from pooled Q/K statistics (no reference counterpart; SpargeAttn's training-free first stage): the

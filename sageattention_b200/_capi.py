@@ -44,6 +44,8 @@ EXPORTS = {
                                   [c_void_p, ctypes.c_uint32, c_int, c_void_p]),
     "sab_qk_int8_sv_f8_attn_blocksparse": (c_int, [c_void_p] * 9 + [c_int] * 7 + [c_int64] * 10 + [c_int, c_int, c_int, c_float, c_int] +
                                            [c_void_p] + [c_int64] * 4 + [c_void_p]),
+    "sab_qk_int8_sv_f8_attn_window": (c_int, [c_void_p] * 9 + [c_int] * 7 + [c_int64] * 10 + [c_int, c_int, c_int, c_float, c_int] +
+                                      [c_int, c_int, c_void_p]),
     "sab_attn_bwd_workspace_bytes": (c_int64, [c_int] * 3),
     "sab_qk_int8_attn_bwd": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_int64] * 21 + [c_int, c_int, c_int, c_float, c_int, c_void_p]),
     "sab_qk_int8_attn_bwd_varlen": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_int64] * 14 + [c_void_p] * 4 +
@@ -52,6 +54,8 @@ EXPORTS = {
                                     [c_void_p, c_int] + [c_int64] * 4 + [c_void_p, c_void_p]),
     "sab_qk_int8_attn_bwd_blocksparse": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_int64] * 21 + [c_int, c_int, c_int, c_float, c_int] +
                                          [c_void_p] + [c_int64] * 4 + [c_void_p]),
+    "sab_qk_int8_attn_bwd_window": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_int64] * 21 + [c_int, c_int, c_int, c_float, c_int] +
+                                    [c_int, c_int, c_void_p]),
     "sab_block_stats": (c_int, [c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 4 + [c_int64] * 3 + [c_int, c_void_p]),
     "sab_predict_block_mask": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_float] * 3 + [c_void_p]),
 }

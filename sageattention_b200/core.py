@@ -6,6 +6,7 @@ H100 kernels: fused quantisers (csrc/quant.cu) and the wgmma attention kernel (c
 There is no arch dispatch, no Triton, no CPU fallback.
 """
 from typing import Any, Optional
+import numbers
 import warnings
 import torch
 import torch.nn.functional as F
@@ -67,17 +68,22 @@ def _quant_qk(q, k, kind, tensor_layout, qk_quant_gran, sm_scale, smooth_k, back
 
 
 def _attn_dense(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range, backend,
-                return_lse, block_mask=None):
+                return_lse, block_mask=None, window=None):
     """Quantisers + attention kernel of a dense entry point on head-dim-padded q, k, v.  kind: "fp8" (FP8 PV, V range v_range),
     "fp16_cuda" (FP16 PV, per-warp / per-thread INT8) or "fp16_triton" (FP16 PV, per-block INT8 with sm_scale*log2e folded into
-    q).  block_mask ("fp8" only): the [B,Hq,ceil(Sq/128),ceil(Skv/64)] bool view of sageattn_blocksparse; the quantisers still
-    see every key.  Returns (o, the kernel's log2 lse or an empty tensor, km)."""
+    q).  block_mask ("fp8" only): the [B,Hq,ceil(Sq/128),ceil(Skv/64)] bool view of sageattn_blocksparse; window ("fp8" only):
+    the (left, right) of sageattn_window; the quantisers still see every key.  Returns (o, the kernel's log2 lse or an empty
+    tensor, km)."""
     km, q_int8, q_scale, k_int8, k_scale, q_gran, k_gran, fold = _quant_qk(q, k, kind, tensor_layout, qk_quant_gran, sm_scale,
                                                                           smooth_k, backend)
     lay = 0 if tensor_layout == "NHD" else 1
     o = torch.empty(q.size(), dtype=q.dtype, device=q.device)
     if kind == "fp8":
         v_fp8, v_scale, vm = per_channel_fp8(v, tensor_layout=tensor_layout, scale_max=v_range, smooth_v=smooth_v)
+        if window is not None:
+            return o, ops.qk_int8_sv_f8_attn_window(q_int8, k_int8, v_fp8, o, q_scale, k_scale, v_scale, vm, window[0], window[1], lay,
+                                                    1 if is_causal else 0, q_gran, k_gran, sm_scale, fold,
+                                                    1 if return_lse else 0), km
         if block_mask is not None:
             return o, ops.qk_int8_sv_f8_attn_blocksparse(q_int8, k_int8, v_fp8, o, q_scale, k_scale, v_scale, vm, block_mask, lay,
                                                          1 if is_causal else 0, q_gran, k_gran, sm_scale, fold,
@@ -97,15 +103,17 @@ class _SageAttnFunction(torch.autograd.Function):
     forward: the unchanged forward with the kernel LSE enabled; saves q, k, v, o and the raw LSE.  backward: re-runs the
     (deterministic) Q/K quantisers instead of saving their 8-bit outputs, then the two gradient kernels.  The LSE and the K mean
     are returned for the LSE correction and carry no gradient.  block_mask (sageattn_blocksparse): P = 0 on the hidden tiles, and
-    the block-sparse gradient kernels visit only the visible ones; the mask has no gradient."""
+    the block-sparse gradient kernels visit only the visible ones; the mask has no gradient.  window (sageattn_window): P = 0
+    outside the window, and the window gradient kernels visit only the tiles inside it."""
 
     @staticmethod
     def forward(ctx, q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range, backend,
-                block_mask=None):
+                block_mask=None, window=None):
         o, lse, km = _attn_dense(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range,
-                                 backend, True, block_mask)
+                                 backend, True, block_mask, window)
         ctx.save_for_backward(q, k, v, o, lse, block_mask)
         ctx.cfg = (kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, backend)
+        ctx.window = window
         km = km if km is not None else q.new_empty(0)
         ctx.mark_non_differentiable(lse, km)
         return o, lse, km
@@ -119,28 +127,32 @@ class _SageAttnFunction(torch.autograd.Function):
         # the kernels read 16-bit rows with 16-byte loads; dq / dk / dv take the strides of q / k / v
         q, k, v, o, do = (t.contiguous() for t in (q, k, v, o, do))
         dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
-        if block_mask is not None:
+        if ctx.window is not None:
+            ops.qk_int8_attn_bwd_window(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv, ctx.window[0],
+                                        ctx.window[1], 0 if tensor_layout == "NHD" else 1, 1 if is_causal else 0, q_gran, k_gran,
+                                        sm_scale, fold)
+        elif block_mask is not None:
             ops.qk_int8_attn_bwd_blocksparse(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv, block_mask,
                                              0 if tensor_layout == "NHD" else 1, 1 if is_causal else 0, q_gran, k_gran, sm_scale,
                                              fold)
         else:
             ops.qk_int8_attn_bwd(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv,
                                  0 if tensor_layout == "NHD" else 1, 1 if is_causal else 0, q_gran, k_gran, sm_scale, fold)
-        return dq, dk, dv, None, None, None, None, None, None, None, None, None, None
+        return dq, dk, dv, None, None, None, None, None, None, None, None, None, None, None
 
 
 def _dense_call(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range, backend,
-                return_lse, head_dim_og, block_mask=None):
+                return_lse, head_dim_og, block_mask=None, window=None):
     """Shared tail of the dense entry points (q, k, v already head-dim padded).  The differentiable form runs only when grad mode
     is on and q, k or v requires grad; otherwise the forward's launches and bytes are exactly those of the plain call.  The
-    returned lse never carries a gradient.  block_mask: see _attn_dense."""
+    returned lse never carries a gradient.  block_mask, window: see _attn_dense."""
     if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
         o, lse, km = _SageAttnFunction.apply(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v,
-                                             v_range, backend, block_mask)
+                                             v_range, backend, block_mask, window)
         q = q.detach()
     else:
         o, lse, km = _attn_dense(q, k, v, kind, tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range,
-                                 backend, return_lse, block_mask)
+                                 backend, return_lse, block_mask, window)
     o = o[..., :head_dim_og]
     if return_lse:
         if smooth_k:
@@ -218,9 +230,9 @@ def sageattn_qk_int8_pv_fp8_cuda(
 
 
 def _qk_int8_pv_fp8(q, k, v, tensor_layout, is_causal, qk_quant_gran, sm_scale, pv_accum_dtype, smooth_k, smooth_v, return_lse,
-                    block_mask=None):
+                    block_mask=None, window=None):
     """Body of sageattn_qk_int8_pv_fp8_cuda after _check_inputs; block_mask: that of sageattn_blocksparse, checked and expanded by
-    the caller."""
+    the caller; window: the (left, right) of sageattn_window, checked by the caller."""
     assert qk_quant_gran in ["per_warp", "per_thread"], "qk_quant_gran must be either 'per_warp' or 'per_thread'."
     if pv_accum_dtype not in ("fp32", "fp32+fp32", "fp32+fp16"):
         raise ValueError(f"Unsupported pv_accum_dtype: {pv_accum_dtype}")
@@ -243,7 +255,28 @@ def _qk_int8_pv_fp8(q, k, v, tensor_layout, is_causal, qk_quant_gran, sm_scale, 
     # front-end: K mean (2 launches), Q / K quantisers, V statistics (2) + FP8 quantiser — 7 launches (reference: 6 + k.mean, core.py:773-809).
     # The single-launch cluster variants (quant.smooth_quant_k, per_channel_fp8(fused=True)) are opt-in.
     return _dense_call(q, k, v, "fp8", tensor_layout, is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, quant_v_scale_max,
-                       "cuda", return_lse, head_dim_og, block_mask)
+                       "cuda", return_lse, head_dim_og, block_mask, window)
+
+
+def sageattn_window(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, window_size=(-1, -1), tensor_layout: str = "HND",
+                    is_causal: bool = False, qk_quant_gran: str = "per_thread", sm_scale: Optional[float] = None,
+                    pv_accum_dtype: str = "fp32+fp16", smooth_k: bool = True, smooth_v: bool = False,
+                    return_lse: bool = False) -> torch.Tensor:
+    """Sliding-window (local) sageattn_qk_int8_pv_fp8_cuda (no reference counterpart): the same options, checks, quantisation and
+    numerics, but key j is visible to query i only if i - left <= j <= i + right, with (left, right) = window_size (and j <= i
+    when is_causal, which needs Sq == Skv).  -1 leaves a side unbounded; alignment is top-left, as the causal rule (query i and
+    key i are the same position), and Sq != Skv is allowed when not causal.  The kernels visit only the 128-query x 64-key tiles
+    that meet the window and mask the elements on the tiles its edges cross.
+
+    The K mean and the V scales are still taken over every key.  A row with no visible key returns 0 (lse -inf).  window_size
+    (-1, -1) gives the bits of sageattn_qk_int8_pv_fp8_cuda, and (-1, 0) those of its causal call.  Differentiable when grad
+    mode is on and q, k or v requires grad: the dense straight-through gradient with P = 0 outside the window."""
+    if (not isinstance(window_size, (tuple, list)) or len(window_size) != 2 or
+            any(isinstance(w, bool) or not isinstance(w, numbers.Integral) or w < -1 for w in window_size)):
+        raise ValueError(f"window_size must be a pair of ints >= -1 (-1: unbounded), got {window_size!r}")
+    _check_inputs(q, k, v)
+    return _qk_int8_pv_fp8(q, k, v, tensor_layout, is_causal, qk_quant_gran, sm_scale, pv_accum_dtype, smooth_k, smooth_v,
+                           return_lse, window=(int(window_size[0]), int(window_size[1])))
 
 
 def sageattn_blocksparse(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, block_mask: torch.Tensor, tensor_layout: str = "HND",

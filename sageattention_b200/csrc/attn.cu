@@ -63,10 +63,17 @@ constexpr bool kSparse = kMask && !kPV16;     // block mask of the INT8+FP8 path
 // 64-key tiles, ascending and cut at the causal horizon; the loop below then runs over that list, with tile kv_list[j] wherever the
 // dense kernel uses tile j (TMA coordinates, K-scale block, limit, masked_tile).  A row whose list is empty takes the n_kv == 0
 // path; a row that sees none of the listed keys (causal) gets zeros and lse -inf.
-template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false>
+// kWindow (INT8+FP8 only, dense): the sliding-window form; win holds the window (unused by the other forms).  The CTA's rows see
+// the 64-key tiles [j0, j0 + n_kv) (window_tiles), and step j runs tile j0 + j wherever the dense kernel uses tile j.  Each row
+// part has a lower bound lo next to limit (visible keys of the tile: lo <= key < limit), and every tile that crosses either edge
+// of the window for some row of the CTA takes the masked path.  A row part that sees nothing of a tile keeps m and d (its
+// maximum is the mask value, so the lazy max does not move) and adds P = 0, also before its first visible tile; a row that sees
+// no key at all gets zeros and lse -inf.
+template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false, bool kWindow = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnParams p) {
+                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnParams p,
+                     const __grid_constant__ Window win) {
   constexpr uint32_t K_TILE = BN * D;
   constexpr uint32_t V_TILE = D * BN * (kPV16 ? 2 : 1);
   constexpr int SWQK = D;                        // swizzle span of the Q/K tiles (= row bytes)
@@ -112,6 +119,12 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     const BlockMask bm{static_cast<const uint8_t*>(p.mask), p.mask_sb, p.mask_sh, p.mask_sm, p.mask_sn};
     n_kv = build_kv_list<kNumThreads>(bm, b, h, qt, n_kv, kv_list<D>(smem), kv_scratch<D>(smem));
   }
+  [[maybe_unused]] int j0 = 0;   // window form: the first 64-key tile of the CTA's range
+  if constexpr (kWindow) {
+    int j1;
+    window_tiles(win, p.causal != 0, qt * BM, min(qt * BM + BM, q_len) - 1, kv_len, j0, j1);
+    n_kv = j1 - j0;
+  }
 
   if (threadIdx.x == 0) {
     if ((smem_u32(smem) & 1023u) != 0) __trap();     // swizzled tiles need a 1 KB-aligned base
@@ -139,6 +152,7 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         const uint32_t ph = (j / kStages) & 1;
         int kj = j;   // the 64-key tile loaded in step j
         if constexpr (kSparse<kPV16, kMask>) kj = kv_list<D>(smem)[j];
+        if constexpr (kWindow) kj = j0 + j;
         int kc = k_off + kj * BN, vc = v_off + kj * BN, kb = tb;
         if (p.kv_seg_len > 0) {  // all-gathered layout: segment-major
           const int seg = (j * BN) / p.kv_seg_len;
@@ -200,10 +214,12 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   // ---- per-tile operands of the softmax, set before the tile's GEMM phase so the K-scale load overlaps it
   float coef[2];           // dequant coefficient of each row part
   int limit[2];            // number of visible keys of this tile per row (OOB + causal, attn_utils.cuh:296-351)
+  [[maybe_unused]] int lo[2];   // window form: first visible key of this tile per row (keys lo <= key < limit are visible)
   bool masked_tile = false;
   auto tile_setup = [&](int j) {
     int kj = j;   // the 64-key tile of step j
     if constexpr (kSparse<kPV16, kMask>) kj = kv_list<D>(smem)[j];
+    if constexpr (kWindow) kj = j0 + j;
     // dequant coefficient (…sm89.cuh:116-132, 255-257); tile kj == 64-key block kj.  Per-thread K scales: the keys of lane t
     // (8i+2t, 8i+2t+1) are all in scale group t.
     const float ksv = k_dequant<kKT>(p, ks_base, k_blk0 + kj, t);
@@ -214,8 +230,17 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       limit[i] = kv_len - kj * BN;
       if (p.causal) limit[i] = min(limit[i], p.causal_q_offset + q_row[i] - kj * BN + 1);
       if (kElemMask<kPV16, kMask> && q_row[i] >= q_len) limit[i] = 0;   // rows past the end: nothing visible, no mask bytes read
+      if constexpr (kWindow) {
+        if (win.right >= 0) limit[i] = min(limit[i], q_row[i] + win.right + 1 - kj * BN);
+        lo[i] = win.left >= 0 ? q_row[i] - win.left - kj * BN : 0;
+      }
     }
     masked_tile = kElemMask<kPV16, kMask> || (kv_len - kj * BN < BN) || (p.causal && (kj + 1) * BN > p.causal_q_offset + qt * BM + 1);
+    if constexpr (kWindow) {
+      // the top row's window ends inside the tile, or the bottom row's starts after its first key
+      masked_tile = masked_tile || (win.right >= 0 && (kj + 1) * BN - 1 > qt * BM + win.right) ||
+                    (win.left >= 0 && kj * BN < qt * BM + BM - 1 - win.left);
+    }
   };
 
   uint32_t s[32];                   // S of the tile in flight (int32)
@@ -252,7 +277,10 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 #pragma unroll
         for (int c = 0; c < 16; ++c) {
           const int idx = 4 * (c >> 1) + 2 * i + (c & 1);
-          if constexpr (MASKED) {
+          if constexpr (MASKED && kWindow) {
+            const int key = 8 * (c >> 1) + 2 * t + (c & 1);
+            if (key >= limit[i] || key < lo[i]) s[idx] = uint32_t(kIntSentinel);
+          } else if constexpr (MASKED) {
             if (8 * (c >> 1) + 2 * t + (c & 1) >= limit[i]) s[idx] = uint32_t(kIntSentinel);
           }
           v = max(v, int(s[idx]));
@@ -294,6 +322,7 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 #pragma unroll
           for (int u = 0; u < 2; ++u) {
             if constexpr (MASKED && kElemMask<kPV16, kMask>) x[u] = (int(s[idx + u]) != kIntSentinel) ? x[u] : 0.f;   // masked-out elements: not a prefix
+            else if constexpr (MASKED && kWindow) x[u] = (8 * (c >> 1) + 2 * t + u < limit[i] && 8 * (c >> 1) + 2 * t + u >= lo[i]) ? x[u] : 0.f;
             else if constexpr (MASKED) x[u] = (8 * (c >> 1) + 2 * t + u < limit[i]) ? x[u] : 0.f;
             e[idx + u] = x[u];
             sum += x[u];
@@ -468,8 +497,8 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     const bool row_ok = q_row[i] < q_len;
     OutT* orow = reinterpret_cast<OutT*>(p.out) + (varlen ? 0 : int64_t(b) * p.o_stride_b) + int64_t(h) * p.o_stride_h +
                  int64_t(q_off + q_row[i]) * p.o_stride_s;
-    // a fully masked row yields zeros, not NaN; block-sparse causal: a row may see none of the listed keys
-    const float inv = (n_kv == 0 || (kMask && !(dt > 0.f))) ? 0.f : rcp_approx(dt);
+    // a fully masked row yields zeros, not NaN; block-sparse causal or a window: a row may see none of the CTA's keys
+    const float inv = (n_kv == 0 || ((kMask || kWindow) && !(dt > 0.f))) ? 0.f : rcp_approx(dt);
     if (row_ok) {
 #pragma unroll
       for (int nb = 0; nb < D / 8; ++nb) {
@@ -483,13 +512,13 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
           x0 += vm[col];
           x1 += vm[col + 1];
         }
-        if (n_kv == 0 || (kSparse<kPV16, kMask> && !(dt > 0.f))) x0 = x1 = 0.f;
+        if (n_kv == 0 || ((kSparse<kPV16, kMask> || kWindow) && !(dt > 0.f))) x0 = x1 = 0.f;
         *reinterpret_cast<uint32_t*>(orow + col) = pack2<OutT>(x0, x1);
       }
       if (p.lse != nullptr && t == 0) {
         // log2 units like the reference kernel (…sm89.cuh:691-703); the offset cancels: log2(sum 2^x)
         const int64_t li = varlen ? (int64_t(h) * p.Sq + q_off + q_row[i]) : ((int64_t(b) * p.Hq + h) * p.Sq + q_row[i]);
-        p.lse[li] = n_kv > 0 ? lg2_approx(dt) + m[i] : -INFINITY;   // block-sparse, no visible key: lg2(0) = -inf
+        p.lse[li] = n_kv > 0 ? lg2_approx(dt) + m[i] : -INFINITY;   // block-sparse / window, no visible key: lg2(0) = -inf
       }
     }
   }
@@ -553,7 +582,21 @@ static int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUten
   auto kern = sage_attn_fwd_kernel<D, kKT, OutT, kPV16, kMask>;
   static bool configured[64] = {};
   if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
-  kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p);
+  kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p, Window{-1, -1});
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
+}
+
+// the sliding-window form (sage_attn_fwd_kernel<D, kKT, OutT, false, false, true>)
+template <int D, bool kKT, typename OutT>
+static int launch_attn_window(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, AttnParams p, Window w,
+                              dim3 grid, cudaStream_t stream) {
+  p.lazy_tau = exact_max_mode() ? 0.0f : kLazyTau;
+  constexpr size_t smem = attn_smem_bytes<D, false>();
+  auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, false, true>;
+  static bool configured[64] = {};
+  if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
+  kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p, w);
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
 }
@@ -568,7 +611,7 @@ static int launch_attn_blocksparse(const CUtensorMap& tq, const CUtensorMap& tk,
   auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, true>;
   static bool configured[64] = {};
   if (int st = ensure_dynamic_smem(kern, smem_max, configured)) return st;
-  kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p);
+  kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p, Window{-1, -1});
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
 }
@@ -577,6 +620,8 @@ static int launch_attn_blocksparse(const CUtensorMap& tq, const CUtensorMap& tk,
 
 // block mask of the block-sparse entry point, handed to attn_entry by sab_qk_int8_sv_f8_attn_blocksparse (same thread)
 static thread_local const sab::BlockMask* tl_block_mask = nullptr;
+// window of the sliding-window entry point, handed to attn_entry by sab_qk_int8_sv_f8_attn_window (same thread)
+static thread_local const sab::Window* tl_window = nullptr;
 // attention mask of the masked entry point, handed to attn_entry by sab_qk_int8_sv_f16_attn_masked (same thread)
 struct MaskArgs {
   const void* ptr; int kind; int64_t sb, sh, sm, sn;
@@ -704,6 +749,21 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
     return bf ? launch_attn_blocksparse<64, false, __nv_bfloat16>(tq, tk, tv, p, grid, s)
               : launch_attn_blocksparse<64, false, __half>(tq, tk, tv, p, grid, s);
   }
+  if (tl_window != nullptr) {
+    SAB_REQUIRE(!pv16 && !varlen && kv_seg_len == 0 && causal_q_offset == 0, SAB_ERR_UNSUPPORTED,
+                "the window is supported by the dense single-GPU INT8/FP8 path only");
+    const Window w = *tl_window;
+    if (D == 128) {
+      if (kt) return bf ? launch_attn_window<128, true, __nv_bfloat16>(tq, tk, tv, p, w, grid, s)
+                        : launch_attn_window<128, true, __half>(tq, tk, tv, p, w, grid, s);
+      return bf ? launch_attn_window<128, false, __nv_bfloat16>(tq, tk, tv, p, w, grid, s)
+                : launch_attn_window<128, false, __half>(tq, tk, tv, p, w, grid, s);
+    }
+    if (kt) return bf ? launch_attn_window<64, true, __nv_bfloat16>(tq, tk, tv, p, w, grid, s)
+                      : launch_attn_window<64, true, __half>(tq, tk, tv, p, w, grid, s);
+    return bf ? launch_attn_window<64, false, __nv_bfloat16>(tq, tk, tv, p, w, grid, s)
+              : launch_attn_window<64, false, __half>(tq, tk, tv, p, w, grid, s);
+  }
 #define SAB_LAUNCH(DD, KT, T)                                                      \
   do {                                                                             \
     if (pv16) return launch_attn<DD, KT, T, true>(tq, tk, tv, p, grid, s);         \
@@ -803,5 +863,23 @@ extern "C" int sab_qk_int8_sv_f8_attn_blocksparse(const int8_t* q_int8, const in
                             o_stride_s, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale, nullptr, nullptr, nullptr, nullptr,
                             nullptr, 0, 0, 0, nullptr, stream);
   tl_block_mask = nullptr;
+  return st;
+}
+
+extern "C" int sab_qk_int8_sv_f8_attn_window(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out, float* lse,
+                                             const float* q_scale, const float* k_scale, const float* v_scale, const float* v_mean,
+                                             int out_dtype, int B, int Hq, int Hkv, int Sq, int Skv, int D, int64_t q_stride_b,
+                                             int64_t q_stride_h, int64_t q_stride_s, int64_t k_stride_b, int64_t k_stride_h,
+                                             int64_t k_stride_s, int64_t v_s_pad, int64_t o_stride_b, int64_t o_stride_h,
+                                             int64_t o_stride_s, int is_causal, int q_gran, int k_gran, float sm_scale,
+                                             int fold_sm_scale, int window_left, int window_right, void* stream) {
+  if (int st = sab::check_window(window_left, window_right, is_causal, Sq, Skv)) return st;
+  const sab::Window w{window_left, window_right};
+  tl_window = &w;
+  const int st = attn_entry(0, q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, B, Hq, Hkv, Sq, Skv, D,
+                            q_stride_b, q_stride_h, q_stride_s, k_stride_b, k_stride_h, k_stride_s, v_s_pad, o_stride_b, o_stride_h,
+                            o_stride_s, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale, nullptr, nullptr, nullptr, nullptr,
+                            nullptr, 0, 0, 0, nullptr, stream);
+  tl_window = nullptr;
   return st;
 }

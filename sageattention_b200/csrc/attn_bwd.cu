@@ -257,9 +257,11 @@ constexpr size_t bwd_dq_smem_bytes() {
 }
 
 // dbias (masked, nullable): dense [B,Hq,Sq,Skv] in T, written with ln2 * dS.  kSparse: the block-sparse form, which loops over
-// the visible 64-key tiles of its row of *bm (build_kv_list, as the forward does) instead of every tile.
-template <int D, bool kKT, typename T, bool kVarlen, int kMask = 0, bool kSparse = false>
-__device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nullptr, const BlockMask* bm = nullptr) {
+// the visible 64-key tiles of its row of *bm (build_kv_list, as the forward does) instead of every tile.  kWindow: the
+// sliding-window form, which walks the forward's tile range of the window *win with the forward's per-row bounds lo <= key < limit.
+template <int D, bool kKT, typename T, bool kVarlen, int kMask = 0, bool kSparse = false, bool kWindow = false>
+__device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nullptr, const BlockMask* bm = nullptr,
+                                            const Window* win = nullptr) {
   constexpr int QB = 128, KB = 64;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ8 = smem;                       // [128 x D] int8        A of S = Q K^T
@@ -294,7 +296,7 @@ __device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nu
     qss[i] = q_dequant_log2(a, qs_base, sq.q_blk0 + qt, row0 + 8 * i);   // scales are padded to whole 128-row blocks
     const bool ok = q_row[i] < sq.q_len;
     const int64_t li = (int64_t(sq.tb) * a.Hq + h) * a.Sq + sq.q_off + q_row[i];
-    if constexpr (kMask != 0 || kSparse) nlse[i] = ok ? masked_nlse(p.lse[li]) : -INFINITY;
+    if constexpr (kMask != 0 || kSparse || kWindow) nlse[i] = ok ? masked_nlse(p.lse[li]) : -INFINITY;
     else nlse[i] = ok ? -p.lse[li] : 0.f;
     dlt[i] = ok ? p.delta[li] : 0.f;
   }
@@ -309,13 +311,20 @@ __device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nu
   int n_kv = (sq.kv_len + KB - 1) / KB;
   if (a.causal) n_kv = min(n_kv, ((qt + 1) * QB + KB - 1) / KB);
   if constexpr (kSparse) n_kv = build_kv_list<kBwdThreads>(*bm, b, h, qt, n_kv, s_idx, s_scratch);
+  [[maybe_unused]] int j0 = 0;   // window form: the first 64-key tile of the CTA's range
+  if constexpr (kWindow) {
+    int j1;
+    window_tiles(*win, a.causal != 0, qt * QB, min(qt * QB + QB, sq.q_len) - 1, sq.kv_len, j0, j1);
+    n_kv = j1 - j0;
+  }
 
   float dq[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) dq[i] = 0.f;
 
   for (int jt = 0; jt < n_kv; ++jt) {
-    const int j = kSparse ? int(s_idx[jt]) : jt;   // the 64-key tile of step jt
+    int j = kSparse ? int(s_idx[jt]) : jt;   // the 64-key tile of step jt
+    if constexpr (kWindow) j = j0 + jt;
     // masked: the mask elements of this thread's S elements of tile j, issued first so that their latency overlaps the tile loads
     // and the MMAs; rows >= Sq and keys >= Skv are not read
     [[maybe_unused]] uint32_t mv[32];
@@ -354,12 +363,17 @@ __device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nu
 
     float coef[2];
     int limit[2];
+    [[maybe_unused]] int lo[2];   // window form: first visible key of the tile per row
     const float ksv = k_dequant<kKT>(a, ks_base, sq.k_blk0 + j, t);
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       coef[i] = ksv * qss[i];
       limit[i] = q_row[i] < sq.q_len ? sq.kv_len - j * KB : 0;
       if (a.causal) limit[i] = min(limit[i], q_row[i] - j * KB + 1);
+      if constexpr (kWindow) {
+        if (win->right >= 0) limit[i] = min(limit[i], q_row[i] + win->right + 1 - j * KB);
+        lo[i] = win->left >= 0 ? q_row[i] - win->left - j * KB : 0;
+      }
     }
     float ds[32];
 #pragma unroll
@@ -371,6 +385,8 @@ __device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nu
         float pe;
         if constexpr (kMask != 0)
           pe = key < limit[i] ? masked_p<kMask, T>(s[idx], coef[i], nlse[i], mv[idx]) : 0.f;
+        else if constexpr (kWindow)
+          pe = key < limit[i] && key >= lo[i] ? ex2_approx(logit_log2(s[idx], coef[i], nlse[i])) : 0.f;
         else
           pe = key < limit[i] ? ex2_approx(logit_log2(s[idx], coef[i], nlse[i])) : 0.f;
         ds[idx] = pe * (dp[idx] - dlt[i]);
@@ -432,6 +448,13 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_blocksparse_kernel(cons
   bwd_dq_tile<D, kKT, T, false, 0, true>(p, nullptr, &bm);
 }
 
+// the sliding-window form: dense, non-varlen
+template <int D, bool kKT, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_window_kernel(const __grid_constant__ BwdParams p,
+                                                                        const __grid_constant__ Window win) {
+  bwd_dq_tile<D, kKT, T, false, 0, false, true>(p, nullptr, nullptr, &win);
+}
+
 // ------------------------------------------------------------------------------------------------ dK, dV
 template <int D>
 constexpr size_t bwd_dkdv_smem_bytes() {
@@ -441,8 +464,10 @@ constexpr size_t bwd_dkdv_smem_bytes() {
 // kSparse: the block-sparse form.  Warpgroup wg's 64 keys are one block of *bm, and a 64-row Q tile lies in one 128-row block, so
 // each (Q head, Q tile) step has two mask bits: a step with neither set is skipped (no loads, no barriers; the bits are uniform
 // across the CTA), and with one set the other warpgroup takes part in the loads and barriers but adds nothing.
-template <int D, bool kKT, typename T, bool kVarlen, int kMask = 0, bool kSparse = false>
-__device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p, const BlockMask* bm = nullptr) {
+// kWindow: the sliding-window form.  The loop runs only over the 64-row Q tiles that meet rows [k0 - right, k0 + 127 + left] (the
+// rows that see a key of the tile under *win), clipped to the causal start, and every element outside the window gets P = 0.
+template <int D, bool kKT, typename T, bool kVarlen, int kMask = 0, bool kSparse = false, bool kWindow = false>
+__device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p, const BlockMask* bm = nullptr, const Window* win = nullptr) {
   constexpr int KB = 128, QB = 64;
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sK8 = smem;                       // [128 x D] int8        A of S^T = K Q^T
@@ -481,8 +506,12 @@ __device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p, const BlockMas
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) dk[i] = dv[i] = 0.f;
 
-  const int n_qt = (sq.q_len + QB - 1) / QB;
-  const int qt0 = a.causal ? k0 / QB : 0;    // causal (top-left): rows before the first key see none of this tile
+  int n_qt = (sq.q_len + QB - 1) / QB;
+  int qt0 = a.causal ? k0 / QB : 0;          // causal (top-left): rows before the first key see none of this tile
+  if constexpr (kWindow) {
+    if (win->right >= 0) qt0 = max(qt0, max(0, k0 - win->right) / QB);
+    if (win->left >= 0) n_qt = min(n_qt, (k0 + KB - 1 + win->left) / QB + 1);
+  }
   // block-sparse: the raw mask bytes of warpgroup 0's and 1's key blocks for step (hh, qt), loaded one step ahead
   [[maybe_unused]] const int kb0 = 2 * blockIdx.x, n_kb = (sq.kv_len + 63) / 64;
   [[maybe_unused]] uint32_t nxt[2] = {0u, 0u};
@@ -518,7 +547,7 @@ __device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p, const BlockMas
         const bool ok = r < sq.q_len;
         const int64_t li = (int64_t(sq.tb) * a.Hq + h) * a.Sq + sq.q_off + r;
         s_qss[threadIdx.x] = ok ? q_dequant_log2(a, qs_base, sq.q_blk0 + r / 128, r % 128) : 0.f;
-        if constexpr (kMask != 0 || kSparse) s_nlse[threadIdx.x] = ok ? masked_nlse(p.lse[li]) : -INFINITY;
+        if constexpr (kMask != 0 || kSparse || kWindow) s_nlse[threadIdx.x] = ok ? masked_nlse(p.lse[li]) : -INFINITY;
         else s_nlse[threadIdx.x] = ok ? -p.lse[li] : 0.f;
         s_dlt[threadIdx.x] = ok ? p.delta[li] : 0.f;
       }
@@ -547,7 +576,8 @@ __device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p, const BlockMas
           const int idx = 4 * (c >> 1) + 2 * i + (c & 1);
           const int col = 8 * (c >> 1) + 2 * t + (c & 1);
           const int q = q0 + col;
-          const bool ok = key[i] < sq.kv_len && q < sq.q_len && (!a.causal || key[i] <= q);
+          bool ok = key[i] < sq.kv_len && q < sq.q_len && (!a.causal || key[i] <= q);
+          if constexpr (kWindow) ok = ok && (win->left < 0 || q - key[i] <= win->left) && (win->right < 0 || key[i] - q <= win->right);
           float pe;
           if constexpr (kMask != 0)
             pe = ok ? masked_p<kMask, T>(s[idx], ksr[i] * s_qss[col], s_nlse[col],
@@ -597,6 +627,12 @@ template <int D, bool kKT, typename T>
 __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_blocksparse_kernel(const __grid_constant__ BwdParams p,
                                                                                const __grid_constant__ BlockMask bm) {
   bwd_dkdv_tile<D, kKT, T, false, 0, true>(p, &bm);
+}
+
+template <int D, bool kKT, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_window_kernel(const __grid_constant__ BwdParams p,
+                                                                          const __grid_constant__ Window win) {
+  bwd_dkdv_tile<D, kKT, T, false, 0, false, true>(p, nullptr, &win);
 }
 
 // delta, then the dQ kernel kq (smem_q bytes, arguments p, q_args...) and the dK/dV kernel kkv (smem_kv bytes); cfg_*: their
@@ -650,6 +686,21 @@ static int launch_bwd_blocksparse(const BwdParams& p, const BlockMask& bm, cudaS
   auto kkv = bwd_dkdv_blocksparse_kernel<D, kKT, T>;
   if (int st = ensure_dynamic_smem(kkv, bwd_dkdv_smem_bytes<D>(), cfg_kv)) return st;
   kkv<<<dim3(p.n_k_tiles, p.a.Hkv, p.a.B), kBwdThreads, bwd_dkdv_smem_bytes<D>(), stream>>>(p, bm);
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
+}
+
+template <int D, bool kKT, typename T>
+static int launch_bwd_window(const BwdParams& p, const Window& w, cudaStream_t stream) {
+  static bool cfg_q[64] = {}, cfg_kv[64] = {};
+  if (int st = launch_bwd_delta<T>(p, D, stream)) return st;
+  auto kq = bwd_dq_window_kernel<D, kKT, T>;
+  if (int st = ensure_dynamic_smem(kq, bwd_dq_smem_bytes<D>(), cfg_q)) return st;
+  kq<<<dim3(p.a.n_q_tiles, p.a.Hq, p.a.B), kBwdThreads, bwd_dq_smem_bytes<D>(), stream>>>(p, w);
+  SAB_CUDA_OK(cudaGetLastError());
+  auto kkv = bwd_dkdv_window_kernel<D, kKT, T>;
+  if (int st = ensure_dynamic_smem(kkv, bwd_dkdv_smem_bytes<D>(), cfg_kv)) return st;
+  kkv<<<dim3(p.n_k_tiles, p.a.Hkv, p.a.B), kBwdThreads, bwd_dkdv_smem_bytes<D>(), stream>>>(p, w);
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
 }
@@ -869,4 +920,42 @@ extern "C" int sab_qk_int8_attn_bwd_blocksparse(const int8_t* q_int8, const int8
   }
   if (kt) return bf ? launch_bwd_blocksparse<64, true, __nv_bfloat16>(p, bm, s) : launch_bwd_blocksparse<64, true, __half>(p, bm, s);
   return bf ? launch_bwd_blocksparse<64, false, __nv_bfloat16>(p, bm, s) : launch_bwd_blocksparse<64, false, __half>(p, bm, s);
+}
+
+extern "C" int sab_qk_int8_attn_bwd_window(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
+                                           const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                           const float* lse, const void* k_mean, void* dq, void* dk, void* dv, void* workspace,
+                                           int dtype, int B, int Hq, int Hkv, int Sq, int Skv, int D, int64_t q8_stride_b,
+                                           int64_t q8_stride_h, int64_t q8_stride_s, int64_t k8_stride_b, int64_t k8_stride_h,
+                                           int64_t k8_stride_s, int64_t q_stride_b, int64_t q_stride_h, int64_t q_stride_s,
+                                           int64_t k_stride_b, int64_t k_stride_h, int64_t k_stride_s, int64_t v_stride_b,
+                                           int64_t v_stride_h, int64_t v_stride_s, int64_t o_stride_b, int64_t o_stride_h,
+                                           int64_t o_stride_s, int64_t do_stride_b, int64_t do_stride_h, int64_t do_stride_s,
+                                           int is_causal, int q_gran, int k_gran, float sm_scale, int fold_sm_scale,
+                                           int window_left, int window_right, void* stream) {
+  using namespace sab;
+  if (int e = check_window(window_left, window_right, is_causal, Sq, Skv)) return e;
+  SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
+              SAB_ERR_INVALID, "null tensor pointer");
+  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
+  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "dtype must be fp16 or bf16");
+  SAB_REQUIRE(B > 0 && Hq > 0 && Hkv > 0 && Sq > 0 && Skv > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", B, Hq, Hkv, Sq, Skv);
+  SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
+  SAB_REQUIRE(q_gran >= 1 && q_gran <= 3 && k_gran >= 1 && k_gran <= 3, SAB_ERR_INVALID, "unknown quant granularity q=%d k=%d", q_gran, k_gran);
+  const int64_t st[21] = {q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s, q_stride_b, q_stride_h, q_stride_s,
+                          k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s, o_stride_b, o_stride_h, o_stride_s,
+                          do_stride_b, do_stride_h, do_stride_s};
+  if (int e = check_bwd_layout(q_int8, k_int8, q, k, v, o, dout, dq, dk, dv, st)) return e;
+  const BwdParams p = bwd_params(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, B, Hq, Hkv, Sq,
+                                 Skv, st, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale);
+  const Window w{window_left, window_right};
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const bool kt = k_gran == SAB_GRAN_PER_THREAD;
+  const bool bf = dtype == SAB_DTYPE_BF16;
+  if (D == 128) {
+    if (kt) return bf ? launch_bwd_window<128, true, __nv_bfloat16>(p, w, s) : launch_bwd_window<128, true, __half>(p, w, s);
+    return bf ? launch_bwd_window<128, false, __nv_bfloat16>(p, w, s) : launch_bwd_window<128, false, __half>(p, w, s);
+  }
+  if (kt) return bf ? launch_bwd_window<64, true, __nv_bfloat16>(p, w, s) : launch_bwd_window<64, true, __half>(p, w, s);
+  return bf ? launch_bwd_window<64, false, __nv_bfloat16>(p, w, s) : launch_bwd_window<64, false, __half>(p, w, s);
 }

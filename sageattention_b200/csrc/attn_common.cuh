@@ -138,6 +138,35 @@ inline int check_block_mask(const void* block_mask, int64_t sb, int64_t sh, int6
   return SAB_OK;
 }
 
+// ---- sliding-window attention (sab_qk_int8_sv_f8_attn_window / sab_qk_int8_attn_bwd_window).  A kernel argument, not an
+// AttnParams field, so the parameter offsets of the other kernels do not move.
+struct Window {
+  int left, right;                 // key j visible to query i iff i - left <= j <= i + right (top-left); -1: that side unbounded
+};
+
+// The 64-key tiles [j_lo, j_hi) that hold a key visible to some row of [r_lo, r_hi] (r_hi inclusive): the window, the causal
+// horizon and kv_len.  Empty (j_lo == j_hi) when no row of the range sees any key.
+__device__ __forceinline__ void window_tiles(const Window& w, bool causal, int r_lo, int r_hi, int kv_len, int& j_lo, int& j_hi) {
+  const int k_lo = w.left < 0 ? 0 : max(0, r_lo - w.left);
+  int k_hi = kv_len - 1;
+  if (w.right >= 0) k_hi = min(k_hi, r_hi + w.right);
+  if (causal) k_hi = min(k_hi, r_hi);
+  j_lo = k_lo / BN;
+  j_hi = k_hi >= k_lo ? k_hi / BN + 1 : j_lo;
+}
+
+// Host: the window entries' checks, before anything touches the device (forward and backward).  A side that reaches past every
+// row (left >= Sq) or every key (right >= Skv) is set to -1: the same visibility, and the kernels' index arithmetic then stays
+// below Sq + Skv.
+inline int check_window(int& left, int& right, int is_causal, int Sq, int Skv) {
+  SAB_REQUIRE(left >= -1 && right >= -1, SAB_ERR_INVALID, "window_size sides must be >= -1 (-1: unbounded), got (%d, %d)", left,
+              right);
+  SAB_REQUIRE(!is_causal || Sq == Skv, SAB_ERR_INVALID, "qo_len and kv_len must be equal for causal attention.");
+  if (left >= Sq) left = -1;
+  if (right >= Skv) right = -1;
+  return SAB_OK;
+}
+
 // Host: opt a kernel into its dynamic shared-memory size once PER DEVICE (cudaFuncSetAttribute applies to the current
 // device only; a process that drives several GPUs — sageattn_host(device=...), tests — must set it on each).
 template <typename Kern>

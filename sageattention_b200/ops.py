@@ -290,6 +290,38 @@ def _(query, key, value, output, query_scale, key_scale, value_scale, value_mean
     return torch.empty((0,), dtype=torch.float32, device=query.device)
 
 
+@torch.library.custom_op("sageattention_b200::qk_int8_sv_f8_attn_window", mutates_args=("output",), device_types="cuda")
+def qk_int8_sv_f8_attn_window(query: torch.Tensor, key: torch.Tensor, value: torch.Tensor, output: torch.Tensor,
+                              query_scale: torch.Tensor, key_scale: torch.Tensor, value_scale: Optional[torch.Tensor],
+                              value_mean: Optional[torch.Tensor], window_left: int, window_right: int, tensor_layout: int,
+                              is_causal: int, q_quant_gran: int, k_quant_gran: int, sm_scale: float, fold_sm_scale: int,
+                              return_lse: int) -> torch.Tensor:
+    """qk_int8_sv_f8_attn restricted to a sliding window (include/sageattn_b200.h, sab_qk_int8_sv_f8_attn_window): key j is
+    visible to query i iff i - window_left <= j <= i + window_right (-1: that side unbounded), and j <= i when causal.  Returns
+    lse as qk_int8_sv_f8_attn does; a row with no visible key gets 0 and lse -inf."""
+    B, Hq, Sq, D = _bhsd(query, tensor_layout)
+    _, Hkv, Skv, _ = _bhsd(key, tensor_layout)
+    qs, ks, os_ = _bhs_strides(query, tensor_layout), _bhs_strides(key, tensor_layout), _bhs_strides(output, tensor_layout)
+    lse = torch.empty((B, Hq, Sq), dtype=torch.float32, device=query.device) if return_lse else \
+        torch.empty((0,), dtype=torch.float32, device=query.device)
+    with torch.cuda.device(query.device):
+        check(lib().sab_qk_int8_sv_f8_attn_window(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
+                                                  lse.data_ptr() if return_lse else None, query_scale.data_ptr(), key_scale.data_ptr(),
+                                                  _ptr(value_scale), _ptr(value_mean), _dt(output), B, Hq, Hkv, Sq, Skv, D, *qs, *ks,
+                                                  _v_pad(value), *os_, is_causal, q_quant_gran, k_quant_gran, float(sm_scale),
+                                                  fold_sm_scale, window_left, window_right, _stream(query)))
+    return lse
+
+
+@qk_int8_sv_f8_attn_window.register_fake
+def _(query, key, value, output, query_scale, key_scale, value_scale, value_mean, window_left, window_right, tensor_layout,
+      is_causal, q_quant_gran, k_quant_gran, sm_scale, fold_sm_scale, return_lse):
+    B, Hq, Sq, D = _bhsd(query, tensor_layout)
+    if return_lse:
+        return torch.empty((B, Hq, Sq), dtype=torch.float32, device=query.device)
+    return torch.empty((0,), dtype=torch.float32, device=query.device)
+
+
 @torch.library.custom_op("sageattention_b200::qk_int8_sv_f8_attn_sp", mutates_args=("output",), device_types="cuda")
 def qk_int8_sv_f8_attn_sp(query: torch.Tensor, key: torch.Tensor, value: torch.Tensor, output: torch.Tensor,
                           query_scale: torch.Tensor, key_scale: torch.Tensor, value_scale: torch.Tensor, q_quant_gran: int,
@@ -458,6 +490,39 @@ def qk_int8_attn_bwd_blocksparse(q_int8: torch.Tensor, k_int8: torch.Tensor, q_s
 @qk_int8_attn_bwd_blocksparse.register_fake
 def _(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, block_mask, tensor_layout, is_causal,
       q_quant_gran, k_quant_gran, sm_scale, fold_sm_scale):
+    return None
+
+
+@torch.library.custom_op("sageattention_b200::qk_int8_attn_bwd_window", mutates_args=("dq", "dk", "dv"), device_types="cuda")
+def qk_int8_attn_bwd_window(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale: torch.Tensor, k_scale: torch.Tensor,
+                            q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, o: torch.Tensor, dout: torch.Tensor,
+                            lse: torch.Tensor, k_mean: Optional[torch.Tensor], dq: torch.Tensor, dk: torch.Tensor,
+                            dv: torch.Tensor, window_left: int, window_right: int, tensor_layout: int, is_causal: int,
+                            q_quant_gran: int, k_quant_gran: int, sm_scale: float, fold_sm_scale: int) -> None:
+    """Gradients of the sliding-window attention (include/sageattn_b200.h, sab_qk_int8_attn_bwd_window): the arguments of
+    qk_int8_attn_bwd plus the window the forward received (qk_int8_sv_f8_attn_window)."""
+    B, Hq, Sq, D = _bhsd(q, tensor_layout)
+    _, Hkv, Skv, _ = _bhsd(k, tensor_layout)
+    for x, y in ((dq, q), (dk, k), (dv, v)):
+        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
+    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (B, Hq, Sq), "lse must be [B,Hq,Sq] fp32"
+    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in _bhs_strides(t, tensor_layout)]
+    if k_mean is not None:
+        assert k_mean.numel() == B * Hkv * D and k_mean.dtype == k.dtype, "k_mean must have B*Hkv*D elements of k's dtype"
+        k_mean = k_mean.reshape(B, Hkv, D).contiguous()
+    with torch.cuda.device(q.device):
+        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(B, Hq, Sq), dtype=torch.uint8, device=q.device)
+        check(lib().sab_qk_int8_attn_bwd_window(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(), k_scale.data_ptr(),
+                                                q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(),
+                                                lse.data_ptr(), _ptr(k_mean), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
+                                                ws.data_ptr(), _dt(q), B, Hq, Hkv, Sq, Skv, D, *strides, is_causal, q_quant_gran,
+                                                k_quant_gran, float(sm_scale), fold_sm_scale, window_left, window_right, _stream(q)))
+
+
+@qk_int8_attn_bwd_window.register_fake
+def _(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, window_left, window_right, tensor_layout,
+      is_causal, q_quant_gran, k_quant_gran, sm_scale, fold_sm_scale):
     return None
 
 

@@ -340,7 +340,9 @@ __device__ __forceinline__ void quant_int8_tile(const QuantParams& p, const int 
     const uint64_t fac2 = pack2f(fac, fac);
     const uint32_t* wv = reinterpret_cast<const uint32_t*>(&raw[ps]);
     uint32_t tb[8];     // bit patterns of y + 1.5*2^23: low byte = int8
-    float dmax = 0.f;
+    // A denormal scale (bf16 block with amax < 127 * 2^-128) has RN(1/scale) = inf: y and y - n are inf / NaN, which fmaxf
+    // drops, so the residual starts above the threshold and the row takes the exact sequence (IEEE x / scale is finite).
+    float dmax = (kTriton && !(fac <= 3.402823466e+38f)) ? 1.f : 0.f;
 #pragma unroll
     for (int w = 0; w < 4; ++w) {
       float lo, hi;

@@ -425,6 +425,63 @@ int sab_predict_block_mask(const float* q_mean, const float* q_sim, const float*
                            int B, int Hq, int Hkv, int Sq, int Skv, int D, int is_causal, float sm_scale, float cdf_threshold,
                            float sim_threshold, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Packed variable-length INT8+FP8 attention with per-sequence statistics (no reference counterpart): the building blocks of
+ * sageattn_varlen_qk_int8_pv_fp8_cuda.  Inputs are packed [T,H,D] (token stride stride_t, head stride stride_h); cu_seqlens
+ * [nseq+1] int32 device, sequence b = tokens [cu_seqlens[b], cu_seqlens[b+1]) (empty sequences allowed); max_seqlen >= every
+ * length (it sizes the grids; a larger value only adds idle CTAs).  Every statistic is taken per sequence, so sequence b gets
+ * the bits of the dense entry points on that sequence alone; tokens past cu_seqlens[nseq] belong to no sequence and are not
+ * read or written.  Unlike the varlen forms above (one K mean and one V scale over all packed tokens).
+ *
+ * sab_k_mean_varlen: mean [nseq,H,D] (`dtype`), bit for bit sab_k_mean of each sequence (same 1024-token chunks, aligned to the
+ *   sequence's first token, same fold); an empty sequence gets 0.  workspace >= sab_k_mean_varlen_workspace_bytes(...).
+ * sab_quant_int8_varlen: the Q (is_key == 0) or K (is_key != 0) half of per_thread_int8 (granularity SAB_GRAN_PER_THREAD,
+ *   sab_quant_per_thread_int8's semantics) or per_warp_int8 (SAB_GRAN_PER_WARP, sab_quant_per_block_int8 with blk 32 / 64 and
+ *   SAB_SEM_CUDA) on each sequence.  Blocks restart at every sequence: cu_scale [nseq+1] int32 device is the exclusive cumsum of
+ *   ceil(L_b/128) (Q) or ceil(L_b/64) (K), and sequence b's scales are rows [cu_scale[b]*mult, (cu_scale[b]+nblk_b)*mult) of
+ *   scale [rows,H] fp32, mult = 4 (per-warp Q), 32 (per-thread Q), 1 (per-warp K), 4 (per-thread K), in the column order of
+ *   the dense call.  mean: optional [nseq,H,D] (`dtype`) K smoothing mean of each sequence (K only).
+ * sab_per_channel_fp8_varlen: v_scale (and v_mean when not NULL, smooth_v) [nseq,H,D] fp32 of each sequence as
+ *   sab_per_channel_fp8 computes them (v_mean's denominator is L_b rounded up to 16); an empty sequence gets 0.  v_fp8
+ *   [H,D,t_pad] e4m3, sequence b at token columns [cu_pad[b], cu_pad[b] + ceil(L_b/128)*128), zero padded (cu_pad: exclusive
+ *   cumsum of ceil(L_b/128)*128, int32 device).  workspace >= sab_per_channel_fp8_varlen_workspace_bytes(...).
+ * sab_qk_int8_sv_f8_attn_varlen: the forward of sab_qk_int8_sv_f8_attn's varlen form with per-warp / per-thread scales from
+ *   sab_quant_int8_varlen (q_gran, k_gran) and the per-sequence v_scale / v_mean [nseq,Hkv,D] of sab_per_channel_fp8_varlen
+ *   (sm_scale never folded).  out [Tq,Hq,D]; lse (optional) [Hq,Tq] fp32 log2 units.  Causal is top-left inside each sequence
+ *   (Lq != Lk allowed).  A sequence with no keys gets zero rows and lse -inf; rows past cu_seqlens_q[nseq] are not written.
+ *   Needs Tk > 0.
+ * sab_qk_int8_attn_bwd_varlen_seq: the gradient of sab_qk_int8_sv_f8_attn_varlen; sab_qk_int8_attn_bwd_varlen's arguments plus
+ *   q_gran / k_gran, with k_mean the per-sequence [nseq,Hkv,D] mean of sab_k_mean_varlen (NULL without smoothing) and lse the
+ *   forward's [Hq,Tq] log2 LSE.  For every sequence, dq / dk / dv are the bits of sab_qk_int8_attn_bwd on that sequence alone;
+ *   rows and keys past cu_seqlens_*[nseq] are not written, and keys of a sequence with no queries get zeros.
+ * ---------------------------------------------------------------------------------------------- */
+int64_t sab_k_mean_varlen_workspace_bytes(int nseq, int H, int max_seqlen, int D);
+int sab_k_mean_varlen(const void* k, int dtype, void* mean, const int32_t* cu_seqlens, int nseq, int max_seqlen, int H, int D,
+                      int64_t stride_t, int64_t stride_h, void* workspace, void* stream);
+int sab_quant_int8_varlen(const void* x, int dtype, const void* mean, int8_t* out, float* scale, const int32_t* cu_seqlens,
+                          const int32_t* cu_scale, int nseq, int max_seqlen, int H, int D, int64_t x_stride_t, int64_t x_stride_h,
+                          int64_t o_stride_t, int64_t o_stride_h, int granularity, int is_key, void* stream);
+int64_t sab_per_channel_fp8_varlen_workspace_bytes(int nseq, int H, int max_seqlen, int D);
+int sab_per_channel_fp8_varlen(const void* v, int dtype, uint8_t* v_fp8, float* v_scale, float* v_mean, const int32_t* cu_seqlens,
+                               const int32_t* cu_pad, int nseq, int max_seqlen, int H, int D, int64_t stride_t, int64_t stride_h,
+                               int64_t t_pad, float scale_max, void* workspace, void* stream);
+int sab_qk_int8_sv_f8_attn_varlen(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out, float* lse,
+                                  const float* q_scale, const float* k_scale, const float* v_scale, const float* v_mean, int out_dtype,
+                                  int nseq, int Hq, int Hkv, int Tq, int Tk, int D, int64_t q_stride_t, int64_t q_stride_h,
+                                  int64_t k_stride_t, int64_t k_stride_h, int64_t v_t_pad, int64_t o_stride_t, int64_t o_stride_h,
+                                  int is_causal, int q_gran, int k_gran, float sm_scale, const int32_t* cu_seqlens_q,
+                                  const int32_t* cu_seqlens_k, const int32_t* cu_pad_v, const int32_t* cu_q_scale,
+                                  const int32_t* cu_k_scale, int max_seqlen_q, void* stream);
+int sab_qk_int8_attn_bwd_varlen_seq(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale, const void* q,
+                                    const void* k, const void* v, const void* o, const void* dout, const float* lse, const void* k_mean,
+                                    void* dq, void* dk, void* dv, void* workspace, int dtype, int nseq, int Hq, int Hkv, int Tq, int Tk,
+                                    int D, int64_t q8_stride_t, int64_t q8_stride_h, int64_t k8_stride_t, int64_t k8_stride_h,
+                                    int64_t q_stride_t, int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h, int64_t v_stride_t,
+                                    int64_t v_stride_h, int64_t o_stride_t, int64_t o_stride_h, int64_t do_stride_t, int64_t do_stride_h,
+                                    const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k, const int32_t* cu_q_scale,
+                                    const int32_t* cu_k_scale, int max_seqlen_q, int max_seqlen_k, int is_causal, int q_gran,
+                                    int k_gran, float sm_scale, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

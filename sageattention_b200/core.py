@@ -14,7 +14,8 @@ import torch.nn.functional as F
 from . import ops
 from ._capi import SAB_GRAN_PER_BLOCK, SAB_GRAN_PER_WARP, SAB_GRAN_PER_THREAD
 from .quant import (k_mean, per_block_int8, per_warp_int8, per_thread_int8, per_channel_fp8, quant_q_int8, quant_k_int8, smooth_quant_k,
-                    per_block_int8_varlen, per_channel_fp8_varlen, transpose_v_f16, transpose_v_f16_varlen)
+                    per_block_int8_varlen, per_channel_fp8_varlen, transpose_v_f16, transpose_v_f16_varlen, k_mean_varlen,
+                    quant_q_int8_varlen, quant_k_int8_varlen, per_channel_fp8_varlen_seq)
 
 _LOG2E = 1.44269504
 
@@ -498,3 +499,150 @@ class _SageAttnVarlenFunction(torch.autograd.Function):
                                     cu_seqlens_q.to(torch.int32), cu_seqlens_k.to(torch.int32), cu_q_scale, cu_k_scale, max_seqlen_q,
                                     max_seqlen_k, 1 if is_causal else 0, sm_scale, 1)
         return dq, dk, dv, None, None, None, None, None, None, None
+
+
+# ------------------------------------------------------------------------------------------------ packed INT8+FP8 call and its gradient
+def _quant_qk_varlen_f8(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, qk_quant_gran, smooth_k):
+    """Q/K front-end of sageattn_varlen_qk_int8_pv_fp8_cuda on head-dim-padded packed q, k, every statistic per sequence: (km
+    [nseq,Hkv,D] or None, q_int8, q_scale, cu_q_scale, k_int8, k_scale, cu_k_scale).  Deterministic, so the backward re-runs it."""
+    km = k_mean_varlen(k, cu_seqlens_k, max_seqlen_k) if smooth_k else None
+    q_int8, q_scale, cu_q_scale = quant_q_int8_varlen(q, cu_seqlens_q, max_seqlen_q, qk_quant_gran)
+    k_int8, k_scale, cu_k_scale = quant_k_int8_varlen(k, km, cu_seqlens_k, max_seqlen_k, qk_quant_gran)
+    return km, q_int8, q_scale, cu_q_scale, k_int8, k_scale, cu_k_scale
+
+
+def _attn_varlen_f8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale, smooth_k,
+                    smooth_v, v_range, return_lse):
+    """Quantisers + INT8+FP8 kernel of sageattn_varlen_qk_int8_pv_fp8_cuda on head-dim-padded packed q, k, v (cu_seqlens int32):
+    (o, the kernel's [Hq,Tq] log2 lse or an empty tensor, km)."""
+    km, q_int8, q_scale, cu_q_scale, k_int8, k_scale, cu_k_scale = _quant_qk_varlen_f8(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q,
+                                                                                     max_seqlen_k, qk_quant_gran, smooth_k)
+    v_fp8, v_scale, vm, cu_pad = per_channel_fp8_varlen_seq(v, cu_seqlens_k, max_seqlen_k, v_range, smooth_v)
+    o = torch.empty(q.shape, dtype=q.dtype, device=q.device)
+    gran = SAB_GRAN_PER_WARP if qk_quant_gran == "per_warp" else SAB_GRAN_PER_THREAD
+    lse = ops.qk_int8_sv_f8_attn_varlen_seq(q_int8, k_int8, v_fp8, o, q_scale, k_scale, v_scale, vm, cu_seqlens_q, cu_seqlens_k, cu_pad,
+                                            cu_q_scale, cu_k_scale, max_seqlen_q, 1 if is_causal else 0, gran, gran, sm_scale,
+                                            1 if return_lse else 0)
+    return o, lse, km
+
+
+def _lse_correction_varlen(q, km, cu_seqlens_q):
+    """[Hq,Tq] fp32: q . km[b] for each token of sequence b, in the input dtype, the correction _lse_correction adds for the dense
+    call on that sequence.  The mean is gathered per token on the device (no host sync), [Tq,Hkv,D] (at most the size of q), and
+    each token's Hq/Hkv query heads take their dot products with it in one batched product: memory and work grow with Tq, not with
+    Tq * nseq.  cuBLAS picks its kernel by shape, so the fp32 sum of an element may be taken in another order than in the dense
+    call's product before its rounding to the input dtype: the two can then differ by one unit in the last place, or by more where
+    the sum cancels (measured on an H100: 0 of 1.03M elements differ at configs[3]; 47 (bf16) and 662 (fp16) of 0.8M with a
+    thousand sequences of 0..200 tokens)."""
+    Tq, Hq, D = q.shape
+    Hkv = km.size(1)
+    seq = torch.searchsorted(cu_seqlens_q[1:], torch.arange(Tq, device=q.device, dtype=cu_seqlens_q.dtype), right=True)
+    seq = seq.clamp_(max=km.size(0) - 1)                                                         # rows past cu_seqlens_q[-1]
+    kmt = km.index_select(0, seq)                                                                # [Tq,Hkv,D]
+    corr = torch.matmul(q.reshape(Tq, Hkv, Hq // Hkv, D), kmt.unsqueeze(-1))                         # [Tq,Hkv,Hq/Hkv,1]
+    return corr.view(Tq, Hq).t().to(torch.float32)
+
+
+class _SageAttnVarlenFp8Function(torch.autograd.Function):
+    """sageattn_varlen_qk_int8_pv_fp8_cuda with a gradient: the straight-through gradient of _SageAttnFunction applied to each packed
+    sequence on its own (include/sageattn_b200.h, sab_qk_int8_attn_bwd_varlen_seq).  forward: the unchanged forward with the kernel
+    LSE enabled; saves q, k, v, o, the LSE and the cu_seqlens.  backward: re-runs the per-sequence K mean and Q/K quantisers, then
+    the gradient kernels.  Tokens past cu_seqlens[-1] belong to no sequence: their gradient is zero.  The LSE and the K means are
+    returned for the LSE correction and carry no gradient."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale, smooth_k,
+                smooth_v, v_range):
+        o, lse, km = _attn_varlen_f8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale,
+                                     smooth_k, smooth_v, v_range, True)
+        ctx.save_for_backward(q, k, v, o, lse, cu_seqlens_q, cu_seqlens_k)
+        ctx.cfg = (max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale, smooth_k)
+        km = km if km is not None else q.new_empty(0)
+        ctx.mark_non_differentiable(lse, km)
+        return o, lse, km
+
+    @staticmethod
+    def backward(ctx, do, _dlse, _dkm):
+        max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale, smooth_k = ctx.cfg
+        q, k, v, o, lse, cu_seqlens_q, cu_seqlens_k = ctx.saved_tensors
+        km, q_int8, q_scale, cu_q_scale, k_int8, k_scale, cu_k_scale = _quant_qk_varlen_f8(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q,
+                                                                                         max_seqlen_k, qk_quant_gran, smooth_k)
+        # the kernels read 16-bit rows with 16-byte loads; dq / dk / dv take the strides of q / k / v
+        q, k, v, o, do = (t.contiguous() for t in (q, k, v, o, do))
+        dq, dk, dv = torch.zeros_like(q), torch.zeros_like(k), torch.zeros_like(v)
+        gran = SAB_GRAN_PER_WARP if qk_quant_gran == "per_warp" else SAB_GRAN_PER_THREAD
+        ops.qk_int8_attn_bwd_varlen_seq(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv, cu_seqlens_q, cu_seqlens_k,
+                                        cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, 1 if is_causal else 0, gran, gran, sm_scale)
+        return dq, dk, dv, None, None, None, None, None, None, None, None, None, None
+
+
+def _check_cu_seqlens(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k):
+    if q.dim() != 3 or k.dim() != 3:
+        raise ValueError(f"q, k and v must be packed [T, H, D] tensors (got q {tuple(q.shape)}, k {tuple(k.shape)})")
+    for name, cu in (("cu_seqlens_q", cu_seqlens_q), ("cu_seqlens_k", cu_seqlens_k)):
+        if not isinstance(cu, torch.Tensor) or cu.dim() != 1 or cu.dtype not in (torch.int32, torch.int64) or cu.numel() < 2:
+            raise ValueError(f"{name} must be a 1-D int32 or int64 tensor of nseq + 1 >= 2 offsets")
+        if cu.device != q.device:
+            raise ValueError(f"{name} must be on q's device")
+    if cu_seqlens_q.numel() != cu_seqlens_k.numel():
+        raise ValueError(f"cu_seqlens_q and cu_seqlens_k must have the same length ({cu_seqlens_q.numel()} != {cu_seqlens_k.numel()})")
+    for name, m in (("max_seqlen_q", max_seqlen_q), ("max_seqlen_k", max_seqlen_k)):
+        if isinstance(m, bool) or not isinstance(m, numbers.Integral) or m < 1:
+            raise ValueError(f"{name} must be an int >= 1, got {m!r}")
+    if q.size(0) == 0 or k.size(0) == 0:
+        raise ValueError("the packed batch must hold at least one query and one key")
+
+
+def sageattn_varlen_qk_int8_pv_fp8_cuda(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu_seqlens_q: torch.Tensor,
+                                        cu_seqlens_k: torch.Tensor, max_seqlen_q: int, max_seqlen_k: int, is_causal: bool = False,
+                                        qk_quant_gran: str = "per_thread", sm_scale: Optional[float] = None,
+                                        pv_accum_dtype: str = "fp32+fp16", smooth_k: bool = True, smooth_v: bool = False,
+                                        return_lse: bool = False):
+    """Packed variable-length sageattn_qk_int8_pv_fp8_cuda (no reference counterpart): q [Tq,Hq,D], k / v [Tk,Hkv,D] (GQA:
+    Hq % Hkv == 0), sequence b = q[cu_seqlens_q[b]:cu_seqlens_q[b+1]] against k / v[cu_seqlens_k[b]:cu_seqlens_k[b+1]]
+    (cu_seqlens int32 or int64, same length; max_seqlen_* >= every length).  Options, checks and warnings are those of
+    sageattn_qk_int8_pv_fp8_cuda.
+
+    Contract: each sequence's output rows (and lse rows) are the bits of sageattn_qk_int8_pv_fp8_cuda(q_b[None], k_b[None],
+    v_b[None], tensor_layout="NHD", ...) with the same options; packing changes no sequence's result.  So every statistic is
+    per sequence: the K smoothing mean, the Q / K INT8 blocks (which restart at every sequence) and the V FP8 scales and mean.
+    This differs from sageattn_varlen, which takes one K mean over all packed tokens, as the reference's varlen call does.
+
+    is_causal: top-left inside each sequence, Lq != Lk allowed.  Empty sequences are allowed: a sequence without keys returns
+    zero rows and lse -inf.  Rows past cu_seqlens_q[-1] are not written.  return_lse: also returns the [Hq,Tq] fp32 LSE in
+    natural-log units (flash-attn's varlen convention), with each sequence's own K-mean correction (the kernel's LSE is the dense
+    call's to the bit; the correction q . km is a per-token product whose fp32 sum can be taken in another order than the dense
+    call's before its rounding to the input dtype, see _lse_correction_varlen: so lse, unlike the output, is not bit-identical
+    to the dense call's on every element).  Differentiable when grad
+    mode is on and q, k or v requires grad: for every sequence, dq / dk / dv are the bits of the dense backward of the
+    one-sequence call; tokens past cu_seqlens_*[-1] and keys of a sequence without queries get zero gradients."""
+    _check_inputs(q, k, v)
+    assert qk_quant_gran in ["per_warp", "per_thread"], "qk_quant_gran must be either 'per_warp' or 'per_thread'."
+    if pv_accum_dtype not in ("fp32", "fp32+fp32", "fp32+fp16"):
+        raise ValueError(f"Unsupported pv_accum_dtype: {pv_accum_dtype}")
+    _check_cu_seqlens(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k)
+    if k.shape != v.shape:
+        raise ValueError(f"k and v must have the same shape (got {tuple(k.shape)} and {tuple(v.shape)})")
+    if q.size(1) % k.size(1) != 0:
+        raise ValueError(f"num_qo_heads ({q.size(1)}) must be divisible by num_kv_heads ({k.size(1)})")
+    q, k, v, head_dim_og = _pad_head_dim(q, k, v)
+    assert q.stride(-1) == 1 and k.stride(-1) == 1 and v.stride(-1) == 1, "Last dim of qkv must be contiguous."
+    if sm_scale is None:
+        sm_scale = head_dim_og ** -0.5
+    if pv_accum_dtype in ("fp32+fp32", "fp32+fp16") and smooth_v:
+        warnings.warn(f"pv_accum_dtype is '{pv_accum_dtype}', smooth_v will be ignored.")
+        smooth_v = False
+    v_range = 2.25 if pv_accum_dtype == "fp32+fp16" else 448.0
+    cu_q, cu_k = cu_seqlens_q.to(torch.int32).contiguous(), cu_seqlens_k.to(torch.int32).contiguous()
+    args = (cu_q, cu_k, int(max_seqlen_q), int(max_seqlen_k), is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range)
+    if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
+        o, lse, km = _SageAttnVarlenFp8Function.apply(q, k, v, *args)
+        q = q.detach()
+    else:
+        o, lse, km = _attn_varlen_f8(q, k, v, *args, return_lse)
+    o = o[..., :head_dim_og]
+    if return_lse:
+        if smooth_k:
+            return o, lse / _LOG2E + _lse_correction_varlen(q, km, cu_q) * sm_scale
+        return o, lse / _LOG2E
+    return o

@@ -69,7 +69,9 @@ constexpr bool kSparse = kMask && !kPV16;     // block mask of the INT8+FP8 path
 // of the window for some row of the CTA takes the masked path.  A row part that sees nothing of a tile keeps m and d (its
 // maximum is the mask value, so the lazy max does not move) and adds P = 0, also before its first visible tile; a row that sees
 // no key at all gets zeros and lse -inf.
-template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false, bool kWindow = false>
+// kSeqV (INT8+FP8 only, varlen): per-sequence V statistics, v_scale / v_mean [nseq,Hkv,D] indexed by the sequence, where the other
+// varlen forms read one [Hkv,D] table for the whole packed batch.
+template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false, bool kWindow = false, bool kSeqV = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnParams p,
@@ -487,8 +489,8 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   }
 
   // ---- epilogue: O / d * v_scale (+ v_mean) -> fp16/bf16 (…sm89.cuh:572-703)
-  const float* vs = p.v_scale ? p.v_scale + (int64_t(varlen ? 0 : b) * p.Hkv + hk) * D : nullptr;
-  const float* vm = p.v_mean ? p.v_mean + (int64_t(varlen ? 0 : b) * p.Hkv + hk) * D : nullptr;
+  const float* vs = p.v_scale ? p.v_scale + (int64_t(varlen && !kSeqV ? 0 : b) * p.Hkv + hk) * D : nullptr;
+  const float* vm = p.v_mean ? p.v_mean + (int64_t(varlen && !kSeqV ? 0 : b) * p.Hkv + hk) * D : nullptr;
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     float dt = d[i];
@@ -601,6 +603,20 @@ static int launch_attn_window(const CUtensorMap& tq, const CUtensorMap& tk, cons
   return SAB_OK;
 }
 
+// the varlen form with per-sequence V statistics (sage_attn_fwd_kernel<D, kKT, OutT, false, false, false, true>)
+template <int D, bool kKT, typename OutT>
+static int launch_attn_seqv(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, AttnParams p, dim3 grid,
+                            cudaStream_t stream) {
+  p.lazy_tau = exact_max_mode() ? 0.0f : kLazyTau;
+  constexpr size_t smem = attn_smem_bytes<D, false>();
+  auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, false, false, true>;
+  static bool configured[64] = {};
+  if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
+  kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p, Window{-1, -1});
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
+}
+
 // the block-sparse form (sage_attn_fwd_kernel<D, kKT, OutT, false, true>): p.mask holds the block mask
 template <int D, bool kKT, typename OutT>
 static int launch_attn_blocksparse(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, AttnParams p,
@@ -622,6 +638,8 @@ static int launch_attn_blocksparse(const CUtensorMap& tq, const CUtensorMap& tk,
 static thread_local const sab::BlockMask* tl_block_mask = nullptr;
 // window of the sliding-window entry point, handed to attn_entry by sab_qk_int8_sv_f8_attn_window (same thread)
 static thread_local const sab::Window* tl_window = nullptr;
+// set by sab_qk_int8_sv_f8_attn_varlen (same thread): v_scale / v_mean are per sequence
+static thread_local bool tl_seq_v = false;
 // attention mask of the masked entry point, handed to attn_entry by sab_qk_int8_sv_f16_attn_masked (same thread)
 struct MaskArgs {
   const void* ptr; int kind; int64_t sb, sh, sm, sn;
@@ -764,6 +782,20 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
     return bf ? launch_attn_window<64, false, __nv_bfloat16>(tq, tk, tv, p, w, grid, s)
               : launch_attn_window<64, false, __half>(tq, tk, tv, p, w, grid, s);
   }
+  if (tl_seq_v) {
+    SAB_REQUIRE(!pv16 && varlen && kv_seg_len == 0 && causal_q_offset == 0, SAB_ERR_UNSUPPORTED,
+                "per-sequence V statistics need the packed single-GPU INT8/FP8 path");
+    if (D == 128) {
+      if (kt) return bf ? launch_attn_seqv<128, true, __nv_bfloat16>(tq, tk, tv, p, grid, s)
+                        : launch_attn_seqv<128, true, __half>(tq, tk, tv, p, grid, s);
+      return bf ? launch_attn_seqv<128, false, __nv_bfloat16>(tq, tk, tv, p, grid, s)
+                : launch_attn_seqv<128, false, __half>(tq, tk, tv, p, grid, s);
+    }
+    if (kt) return bf ? launch_attn_seqv<64, true, __nv_bfloat16>(tq, tk, tv, p, grid, s)
+                      : launch_attn_seqv<64, true, __half>(tq, tk, tv, p, grid, s);
+    return bf ? launch_attn_seqv<64, false, __nv_bfloat16>(tq, tk, tv, p, grid, s)
+              : launch_attn_seqv<64, false, __half>(tq, tk, tv, p, grid, s);
+  }
 #define SAB_LAUNCH(DD, KT, T)                                                      \
   do {                                                                             \
     if (pv16) return launch_attn<DD, KT, T, true>(tq, tk, tv, p, grid, s);         \
@@ -881,5 +913,28 @@ extern "C" int sab_qk_int8_sv_f8_attn_window(const int8_t* q_int8, const int8_t*
                             o_stride_s, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale, nullptr, nullptr, nullptr, nullptr,
                             nullptr, 0, 0, 0, nullptr, stream);
   tl_window = nullptr;
+  return st;
+}
+
+extern "C" int sab_qk_int8_sv_f8_attn_varlen(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out, float* lse,
+                                             const float* q_scale, const float* k_scale, const float* v_scale, const float* v_mean,
+                                             int out_dtype, int nseq, int Hq, int Hkv, int Tq, int Tk, int D, int64_t q_stride_t,
+                                             int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h, int64_t v_t_pad,
+                                             int64_t o_stride_t, int64_t o_stride_h, int is_causal, int q_gran, int k_gran,
+                                             float sm_scale, const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
+                                             const int32_t* cu_pad_v, const int32_t* cu_q_scale, const int32_t* cu_k_scale,
+                                             int max_seqlen_q, void* stream) {
+  SAB_REQUIRE(q_gran == SAB_GRAN_PER_WARP || q_gran == SAB_GRAN_PER_THREAD, SAB_ERR_INVALID,
+              "q_gran must be SAB_GRAN_PER_WARP or SAB_GRAN_PER_THREAD (got %d)", q_gran);
+  SAB_REQUIRE(k_gran == SAB_GRAN_PER_WARP || k_gran == SAB_GRAN_PER_THREAD, SAB_ERR_INVALID,
+              "k_gran must be SAB_GRAN_PER_WARP or SAB_GRAN_PER_THREAD (got %d)", k_gran);
+  SAB_REQUIRE(v_scale != nullptr && cu_seqlens_q != nullptr && nseq > 0 && Tk > 0, SAB_ERR_INVALID,
+              "the packed INT8/FP8 form needs v_scale, cu_seqlens_q, nseq > 0 and Tk > 0");
+  tl_seq_v = true;
+  const int st = attn_entry(0, q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq, Hkv, Tq, Tk, D,
+                            0, q_stride_h, q_stride_t, 0, k_stride_h, k_stride_t, v_t_pad, 0, o_stride_h, o_stride_t, is_causal, q_gran,
+                            k_gran, sm_scale, 0, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale, max_seqlen_q, 0, 0,
+                            nullptr, stream);
+  tl_seq_v = false;
   return st;
 }

@@ -259,7 +259,8 @@ constexpr size_t bwd_dq_smem_bytes() {
 // dbias (masked, nullable): dense [B,Hq,Sq,Skv] in T, written with ln2 * dS.  kSparse: the block-sparse form, which loops over
 // the visible 64-key tiles of its row of *bm (build_kv_list, as the forward does) instead of every tile.  kWindow: the
 // sliding-window form, which walks the forward's tile range of the window *win with the forward's per-row bounds lo <= key < limit.
-template <int D, bool kKT, typename T, bool kVarlen, int kMask = 0, bool kSparse = false, bool kWindow = false>
+// kSeqMean (varlen): the K mean is [nseq,Hkv,D], one per sequence, instead of one [Hkv,D] mean for the packed batch.
+template <int D, bool kKT, typename T, bool kVarlen, int kMask = 0, bool kSparse = false, bool kWindow = false, bool kSeqMean = false>
 __device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nullptr, const BlockMask* bm = nullptr,
                                             const Window* win = nullptr) {
   constexpr int QB = 128, KB = 64;
@@ -345,7 +346,7 @@ __device__ __forceinline__ void bwd_dq_tile(const BwdParams& p, void* dbias = nu
     // K - mean: the same product in exact arithmetic (the rows of dS sum to zero), but the residue that delta = rowsum(dO o O) of
     // the quantised forward leaves in those row sums is not multiplied by a large K mean
     load_tile_t<D, T>(sKt, p.k + b * p.k_sb + hk * p.k_sh + sq.k_off * p.k_ss, p.k_ss, j * KB, sq.kv_len,
-                      p.kmean ? p.kmean + (int64_t(sq.tb) * a.Hkv + hk) * D : nullptr);
+                      p.kmean ? p.kmean + (int64_t(kSeqMean ? b : sq.tb) * a.Hkv + hk) * D : nullptr);
     fence_proxy_async_smem();   // generic-proxy stores -> visible to wgmma
     __syncthreads();
 
@@ -432,6 +433,12 @@ template <int D, bool kKT, typename T>
 __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_kernel(const __grid_constant__ BwdParams p) {
   if (p.a.cu_q != nullptr) bwd_dq_tile<D, kKT, T, true>(p);
   else bwd_dq_tile<D, kKT, T, false>(p);
+}
+
+// the varlen form with a per-sequence K mean (sab_qk_int8_attn_bwd_varlen_seq)
+template <int D, bool kKT, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_varlen_seq_kernel(const __grid_constant__ BwdParams p) {
+  bwd_dq_tile<D, kKT, T, true, 0, false, false, true>(p);
 }
 
 // the masked form: dense, non-causal, per-block / per-warp K scales (those of the masked forward)
@@ -664,6 +671,14 @@ template <int D, bool kKT, typename T>
 static int launch_bwd(const BwdParams& p, cudaStream_t stream) {
   static bool cfg_q[64] = {}, cfg_kv[64] = {};
   return launch_bwd_kernels<T>(p, D, bwd_dq_kernel<D, kKT, T>, bwd_dq_smem_bytes<D>(), cfg_q, bwd_dkdv_kernel<D, kKT, T>,
+                               bwd_dkdv_smem_bytes<D>(), cfg_kv, stream);
+}
+
+// varlen with a per-sequence K mean: its own dQ kernel; the dK/dV kernel does not read the mean
+template <int D, bool kKT, typename T>
+static int launch_bwd_varlen_seq(const BwdParams& p, cudaStream_t stream) {
+  static bool cfg_q[64] = {}, cfg_kv[64] = {};
+  return launch_bwd_kernels<T>(p, D, bwd_dq_varlen_seq_kernel<D, kKT, T>, bwd_dq_smem_bytes<D>(), cfg_q, bwd_dkdv_kernel<D, kKT, T>,
                                bwd_dkdv_smem_bytes<D>(), cfg_kv, stream);
 }
 
@@ -958,4 +973,49 @@ extern "C" int sab_qk_int8_attn_bwd_window(const int8_t* q_int8, const int8_t* k
   }
   if (kt) return bf ? launch_bwd_window<64, true, __nv_bfloat16>(p, w, s) : launch_bwd_window<64, true, __half>(p, w, s);
   return bf ? launch_bwd_window<64, false, __nv_bfloat16>(p, w, s) : launch_bwd_window<64, false, __half>(p, w, s);
+}
+
+extern "C" int sab_qk_int8_attn_bwd_varlen_seq(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
+                                               const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                               const float* lse, const void* k_mean, void* dq, void* dk, void* dv, void* workspace,
+                                               int dtype, int nseq, int Hq, int Hkv, int Tq, int Tk, int D, int64_t q8_stride_t,
+                                               int64_t q8_stride_h, int64_t k8_stride_t, int64_t k8_stride_h, int64_t q_stride_t,
+                                               int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h, int64_t v_stride_t,
+                                               int64_t v_stride_h, int64_t o_stride_t, int64_t o_stride_h, int64_t do_stride_t,
+                                               int64_t do_stride_h, const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
+                                               const int32_t* cu_q_scale, const int32_t* cu_k_scale, int max_seqlen_q,
+                                               int max_seqlen_k, int is_causal, int q_gran, int k_gran, float sm_scale, void* stream) {
+  using namespace sab;
+  SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
+              SAB_ERR_INVALID, "null tensor pointer");
+  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
+  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "dtype must be fp16 or bf16");
+  SAB_REQUIRE(nseq > 0 && Hq > 0 && Hkv > 0 && Tq > 0 && Tk > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", nseq, Hq, Hkv, Tq, Tk);
+  SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
+  SAB_REQUIRE((q_gran == SAB_GRAN_PER_WARP || q_gran == SAB_GRAN_PER_THREAD) && (k_gran == SAB_GRAN_PER_WARP || k_gran == SAB_GRAN_PER_THREAD),
+              SAB_ERR_INVALID, "q_gran / k_gran must be SAB_GRAN_PER_WARP or SAB_GRAN_PER_THREAD (got %d, %d)", q_gran, k_gran);
+  SAB_REQUIRE(cu_seqlens_q && cu_seqlens_k && cu_q_scale && cu_k_scale && max_seqlen_q > 0 && max_seqlen_k > 0, SAB_ERR_INVALID,
+              "varlen needs cu_seqlens_q, cu_seqlens_k, cu_q_scale, cu_k_scale, max_seqlen_q and max_seqlen_k");
+  // packed [T,H,D]: no batch stride
+  const int64_t st[21] = {0, q8_stride_h, q8_stride_t, 0, k8_stride_h, k8_stride_t, 0, q_stride_h, q_stride_t, 0, k_stride_h, k_stride_t,
+                          0, v_stride_h, v_stride_t, 0, o_stride_h, o_stride_t, 0, do_stride_h, do_stride_t};
+  if (int e = check_bwd_layout(q_int8, k_int8, q, k, v, o, dout, dq, dk, dv, st)) return e;
+  BwdParams p = bwd_params(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, nseq, Hq, Hkv, Tq, Tk,
+                           st, is_causal, q_gran, k_gran, sm_scale, 0);
+  AttnParams& a = p.a;
+  a.n_q_tiles = (max_seqlen_q + BM - 1) / BM;
+  p.n_k_tiles = (max_seqlen_k + 127) / 128;
+  a.qs_stride_bh = a.ks_stride_bh = 1;   // as sab_qk_int8_attn_bwd_varlen: scale bases h / hk, rows [blocks * mult, H]
+  a.qs_stride_idx = Hq;
+  a.ks_stride_idx = Hkv;
+  a.cu_q = cu_seqlens_q; a.cu_k = cu_seqlens_k; a.cu_qs = cu_q_scale; a.cu_ks = cu_k_scale;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const bool kt = k_gran == SAB_GRAN_PER_THREAD;
+  const bool bf = dtype == SAB_DTYPE_BF16;
+  if (D == 128) {
+    if (kt) return bf ? launch_bwd_varlen_seq<128, true, __nv_bfloat16>(p, s) : launch_bwd_varlen_seq<128, true, __half>(p, s);
+    return bf ? launch_bwd_varlen_seq<128, false, __nv_bfloat16>(p, s) : launch_bwd_varlen_seq<128, false, __half>(p, s);
+  }
+  if (kt) return bf ? launch_bwd_varlen_seq<64, true, __nv_bfloat16>(p, s) : launch_bwd_varlen_seq<64, true, __half>(p, s);
+  return bf ? launch_bwd_varlen_seq<64, false, __nv_bfloat16>(p, s) : launch_bwd_varlen_seq<64, false, __half>(p, s);
 }

@@ -83,14 +83,23 @@ __device__ __forceinline__ uint32_t pack_e4m3x4_q(float a, float b, float c, flo
 // =====================================================================================================
 constexpr int kStatChunk = 1024;
 
-template <typename T, int D>
+// kSeq: packed [T,H,D] input, blockIdx.z = sequence b = tokens [cu[b], cu[b+1]); its chunks start at the sequence's first token, so
+// the partials of a sequence are those of the dense call on that sequence alone.
+template <typename T, int D, bool kSeq = false>
 __global__ void __launch_bounds__(256) channel_stats_stage1(const T* __restrict__ x, float* __restrict__ part, int S,
-                                                             int64_t sb, int64_t sh, int64_t ss, int nchunk) {
+                                                             int64_t sb, int64_t sh, int64_t ss, int nchunk,
+                                                             const int32_t* __restrict__ cu = nullptr) {
   constexpr int TPR = D / 8;        // threads per token row
   constexpr int RPP = 256 / TPR;    // rows per pass
   const int chunk = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int tr = threadIdx.x / TPR, tc = threadIdx.x % TPR;
   const T* base = x + b * sb + h * sh + tc * 8;
+  if constexpr (kSeq) {
+    const int t0 = cu[b];
+    S = cu[b + 1] - t0;
+    if (chunk * kStatChunk >= S) return;
+    base += int64_t(t0) * ss;
+  }
   float sum[8], mx[8], mn[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) { sum[i] = 0.f; mx[i] = -INFINITY; mn[i] = INFINITY; }
@@ -115,14 +124,32 @@ __global__ void __launch_bounds__(256) channel_stats_stage1(const T* __restrict_
 }
 
 // mode 0: K mean -> T [B,H,D].  mode 1: V scale (+ mean) -> fp32.  mode 2: raw sum / max / min -> fp32.
-template <typename T>
+// kSeq (modes 0 and 1): grid (H, nseq), sequence b = blockIdx.y of length cu[b+1] - cu[b] folds its own chunks; an empty sequence
+// gets mean 0, scale 0 and reciprocal 0.
+template <typename T, bool kSeq = false>
 __global__ void channel_stats_stage2(const float* __restrict__ part, int nchunk, int D, int S, int mode, T* mean_out,
-                                     float* scale_out, float* vmean_out, float scale_max, float* recp_out) {
-  const int bh = blockIdx.x, d = threadIdx.x;
+                                     float* scale_out, float* vmean_out, float scale_max, float* recp_out,
+                                     const int32_t* __restrict__ cu = nullptr) {
+  const int bh = kSeq ? blockIdx.y * gridDim.x + blockIdx.x : blockIdx.x, d = threadIdx.x;
   if (d >= D) return;
   const float* p = part + int64_t(bh) * nchunk * 3 * D;
+  int nc = nchunk;
+  if constexpr (kSeq) {
+    S = cu[blockIdx.y + 1] - cu[blockIdx.y];
+    nc = (S + kStatChunk - 1) / kStatChunk;
+    if (S == 0) {
+      if (mode == 0) {
+        mean_out[int64_t(bh) * D + d] = from_f<T>(0.f);
+      } else {
+        scale_out[int64_t(bh) * D + d] = 0.f;
+        recp_out[int64_t(bh) * D + d] = 0.f;
+        if (vmean_out) vmean_out[int64_t(bh) * D + d] = 0.f;
+      }
+      return;
+    }
+  }
   float a = 0.f, m1 = -INFINITY, m2 = INFINITY;
-  for (int c = 0; c < nchunk; ++c) { a += p[c * 3 * D + d]; m1 = fmaxf(m1, p[c * 3 * D + D + d]); m2 = fminf(m2, p[c * 3 * D + 2 * D + d]); }
+  for (int c = 0; c < nc; ++c) { a += p[c * 3 * D + d]; m1 = fmaxf(m1, p[c * 3 * D + D + d]); m2 = fminf(m2, p[c * 3 * D + 2 * D + d]); }
   if (mode == 2) {
     scale_out[int64_t(bh) * D + d] = a;
     vmean_out[int64_t(bh) * D + d] = m1;
@@ -189,6 +216,18 @@ __device__ __forceinline__ uint32_t round_pair<__half>(float lo, float hi) {
 }
 
 constexpr int kQfTriton = 1, kQfMean = 2, kQfSmScale = 4;   // FLAGS bits of quant_int8_kernel
+// FLAGS bit of the per-sequence varlen form (sab_quant_int8_varlen): the mean is [nseq,H,D], and the scales of sequence b are the
+// rows [cu_scale[b] * mult, (cu_scale[b] + nblk) * mult) of a [rows,H] table, cu_scale counting 128-row Q / 64-key K blocks.  Every
+// group of those blocks is written, as the dense call writes every column of its ceil(S/128)*4 / *32 or ceil(S/64) / *4 scales.
+constexpr int kQfSeq = 8;
+
+// Scale-table geometry of the per-sequence form: rows per scale block (128 Q rows, or 64 keys) and scales per block
+template <int MODE>
+__device__ __forceinline__ int seq_scale_unit(int blk) { return (MODE == kGroupThreadK || (MODE == kGroupBlock && blk == 64)) ? 64 : 128; }
+template <int MODE>
+__device__ __forceinline__ int seq_scale_mult(int blk) {
+  return MODE == kGroupThreadQ ? 32 : (MODE == kGroupThreadK ? 4 : seq_scale_unit<MODE>(blk) / blk);
+}
 
 // FLAGS (compile time): rounding semantics, fused mean subtraction, fused sm_scale multiply — no per-element
 // runtime conditionals.  The tile stays in registers as raw 16-bit words (NP x 16 B per thread).
@@ -219,6 +258,7 @@ __device__ __forceinline__ void quant_int8_tile(const QuantParams& p, const int 
     x_off = int64_t(t0) * p.xss + int64_t(h) * p.xsh;
     o_off = int64_t(t0) * p.oss + int64_t(h) * p.osh;
     scale_row0 = p.cu_scale[b];
+    if constexpr ((FLAGS & kQfSeq) != 0) scale_row0 *= seq_scale_mult<MODE>(p.blk);
   } else {
     x_off = int64_t(b) * p.xsb + int64_t(h) * p.xsh;
     o_off = int64_t(b) * p.osb + int64_t(h) * p.osh;
@@ -312,7 +352,10 @@ __device__ __forceinline__ void quant_int8_tile(const QuantParams& p, const int 
     s_scale[g] = mult;
     s_inv[g] = mult > 0.f ? __fdiv_rn(1.0f, mult) : 0.f;   // all-zero block (scale 0): reference 0/0 -> NaN -> int8 0
     const int gcol = tile * ngroups + g;
-    if (varlen) {
+    if constexpr ((FLAGS & kQfSeq) != 0) {
+      const int unit = seq_scale_unit<MODE>(p.blk);
+      if (gcol < (S + unit - 1) / unit * seq_scale_mult<MODE>(p.blk)) p.scale[int64_t(scale_row0 + gcol) * p.H + h] = scale;
+    } else if (varlen) {
       const int nblk = (S + p.blk - 1) / p.blk;
       if (gcol < nblk) p.scale[int64_t(scale_row0 + gcol) * p.H + h] = scale;
     } else if (gcol < p.scale_cols) {
@@ -412,7 +455,8 @@ template <typename T, int D, int MODE, int FLAGS>
 __global__ void __launch_bounds__(256, 3) quant_int8_kernel(const QuantParams p) {
   const int h = blockIdx.y, b = blockIdx.z;
   const T* mean_bh = nullptr;
-  if constexpr ((FLAGS & kQfMean) != 0) mean_bh = reinterpret_cast<const T*>(p.mean) + (int64_t(p.cu != nullptr ? 0 : b) * p.H + h) * D;
+  if constexpr ((FLAGS & kQfMean) != 0)
+    mean_bh = reinterpret_cast<const T*>(p.mean) + (int64_t((FLAGS & kQfSeq) == 0 && p.cu != nullptr ? 0 : b) * p.H + h) * D;
   quant_int8_tile<T, D, MODE, FLAGS>(p, blockIdx.x, h, b, mean_bh);
 }
 
@@ -559,10 +603,11 @@ __device__ __forceinline__ void v_quant_transpose_tile(const VQuantParams& p, co
   }
 }
 
-template <typename T, int D>
+// kSeq: varlen with per-sequence statistics, recp / vmean [nseq,H,D]
+template <typename T, int D, bool kSeq = false>
 __global__ void __launch_bounds__(256) v_quant_transpose_kernel(const VQuantParams p) {
   const int h = blockIdx.y, b = blockIdx.z;
-  const int64_t bh = int64_t(p.cu != nullptr ? 0 : b) * p.H + h;
+  const int64_t bh = int64_t(!kSeq && p.cu != nullptr ? 0 : b) * p.H + h;
   v_quant_transpose_tile<T, D>(p, blockIdx.x, h, b, p.recp + bh * D, p.vmean ? p.vmean + bh * D : nullptr);
 }
 
@@ -723,6 +768,23 @@ static int launch_quant_t(const QuantParams& p, int mode, dim3 grid, cudaStream_
     default: return launch_quant_f<T, D, 7>(p, mode, grid, st);
   }
 }
+// the per-sequence varlen form: per-thread Q / K (Triton semantics) and per-warp Q / K (CUDA semantics); a mean on K only
+template <typename T, int D>
+static int launch_quant_seq_t(const QuantParams& p, int mode, dim3 grid, cudaStream_t st) {
+  const bool mean = p.mean != nullptr;
+  if (mode == kGroupThreadQ) quant_int8_kernel<T, D, kGroupThreadQ, kQfTriton | kQfSeq><<<grid, 256, 0, st>>>(p);
+  else if (mode == kGroupThreadK && mean) quant_int8_kernel<T, D, kGroupThreadK, kQfTriton | kQfMean | kQfSeq><<<grid, 256, 0, st>>>(p);
+  else if (mode == kGroupThreadK) quant_int8_kernel<T, D, kGroupThreadK, kQfTriton | kQfSeq><<<grid, 256, 0, st>>>(p);
+  else if (mean) quant_int8_kernel<T, D, kGroupBlock, kQfMean | kQfSeq><<<grid, 256, 0, st>>>(p);
+  else quant_int8_kernel<T, D, kGroupBlock, kQfSeq><<<grid, 256, 0, st>>>(p);
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
+}
+static int launch_quant_seq(const QuantParams& p, int dtype, int D, int mode, dim3 grid, cudaStream_t st) {
+  if (dtype == SAB_DTYPE_FP16) return D == 128 ? launch_quant_seq_t<__half, 128>(p, mode, grid, st) : launch_quant_seq_t<__half, 64>(p, mode, grid, st);
+  return D == 128 ? launch_quant_seq_t<__nv_bfloat16, 128>(p, mode, grid, st) : launch_quant_seq_t<__nv_bfloat16, 64>(p, mode, grid, st);
+}
+
 static int launch_quant(const QuantParams& p, int dtype, int D, int mode, dim3 grid, cudaStream_t st) {
   if (dtype == SAB_DTYPE_FP16) return D == 128 ? launch_quant_t<__half, 128>(p, mode, grid, st) : launch_quant_t<__half, 64>(p, mode, grid, st);
   return D == 128 ? launch_quant_t<__nv_bfloat16, 128>(p, mode, grid, st) : launch_quant_t<__nv_bfloat16, 64>(p, mode, grid, st);
@@ -979,4 +1041,107 @@ extern "C" int sab_per_channel_fp8_fused(const void* v, int dtype, uint8_t* v_fp
   }
   if (D == 128) return launch_cluster(v_scale_quant_kernel<__nv_bfloat16, 128>, grid, s, p, v_scale, v_mean);
   return launch_cluster(v_scale_quant_kernel<__nv_bfloat16, 64>, grid, s, p, v_scale, v_mean);
+}
+
+// ---------------------------------------------------------------------------------------------- per-sequence varlen front-end
+// Packed [T,H,D] inputs, every statistic and scale block taken per sequence: sequence b gives the bits of the dense call on
+// tokens [cu_seqlens[b], cu_seqlens[b+1]) alone.
+extern "C" int64_t sab_k_mean_varlen_workspace_bytes(int nseq, int H, int max_seqlen, int D) {
+  return sab_k_mean_workspace_bytes(nseq, H, max_seqlen, D);
+}
+extern "C" int64_t sab_per_channel_fp8_varlen_workspace_bytes(int nseq, int H, int max_seqlen, int D) {
+  return sab_per_channel_fp8_workspace_bytes(nseq, H, max_seqlen, D);
+}
+
+template <typename T, int D>
+static void launch_stats_seq(const void* x, float* part, const int32_t* cu, int nseq, int H, int nchunk, int64_t sh, int64_t ss,
+                             cudaStream_t st) {
+  channel_stats_stage1<T, D, true><<<dim3(nchunk, H, nseq), 256, 0, st>>>(reinterpret_cast<const T*>(x), part, 0, 0, sh, ss, nchunk, cu);
+}
+static int run_stats_seq(const void* x, int dtype, float* part, const int32_t* cu, int nseq, int H, int nchunk, int D, int64_t sh,
+                         int64_t ss, cudaStream_t st) {
+  if (dtype == SAB_DTYPE_FP16) {
+    if (D == 128) launch_stats_seq<__half, 128>(x, part, cu, nseq, H, nchunk, sh, ss, st);
+    else launch_stats_seq<__half, 64>(x, part, cu, nseq, H, nchunk, sh, ss, st);
+  } else {
+    if (D == 128) launch_stats_seq<__nv_bfloat16, 128>(x, part, cu, nseq, H, nchunk, sh, ss, st);
+    else launch_stats_seq<__nv_bfloat16, 64>(x, part, cu, nseq, H, nchunk, sh, ss, st);
+  }
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
+}
+
+extern "C" int sab_k_mean_varlen(const void* k, int dtype, void* mean, const int32_t* cu_seqlens, int nseq, int max_seqlen, int H,
+                                 int D, int64_t stride_t, int64_t stride_h, void* workspace, void* stream) {
+  int st = check_common(k, dtype, D, 0, stride_h, stride_t);
+  if (st) return st;
+  SAB_REQUIRE(mean && workspace && cu_seqlens && nseq > 0 && max_seqlen > 0 && H > 0, SAB_ERR_INVALID, "bad arguments to sab_k_mean_varlen");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const int nchunk = (max_seqlen + kStatChunk - 1) / kStatChunk;
+  float* part = reinterpret_cast<float*>(workspace);
+  if ((st = run_stats_seq(k, dtype, part, cu_seqlens, nseq, H, nchunk, D, stride_h, stride_t, s))) return st;
+  if (dtype == SAB_DTYPE_FP16)
+    channel_stats_stage2<__half, true><<<dim3(H, nseq), 128, 0, s>>>(part, nchunk, D, 0, 0, reinterpret_cast<__half*>(mean), nullptr,
+                                                                     nullptr, 0.f, nullptr, cu_seqlens);
+  else
+    channel_stats_stage2<__nv_bfloat16, true><<<dim3(H, nseq), 128, 0, s>>>(part, nchunk, D, 0, 0, reinterpret_cast<__nv_bfloat16*>(mean),
+                                                                            nullptr, nullptr, 0.f, nullptr, cu_seqlens);
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
+}
+
+extern "C" int sab_quant_int8_varlen(const void* x, int dtype, const void* mean, int8_t* out, float* scale, const int32_t* cu_seqlens,
+                                     const int32_t* cu_scale, int nseq, int max_seqlen, int H, int D, int64_t x_stride_t,
+                                     int64_t x_stride_h, int64_t o_stride_t, int64_t o_stride_h, int granularity, int is_key,
+                                     void* stream) {
+  int st = check_common(x, dtype, D, 0, x_stride_h, x_stride_t);
+  if (st) return st;
+  SAB_REQUIRE(out && scale && cu_seqlens && cu_scale && nseq > 0 && max_seqlen > 0 && H > 0, SAB_ERR_INVALID,
+              "bad arguments to sab_quant_int8_varlen");
+  SAB_REQUIRE(granularity == SAB_GRAN_PER_WARP || granularity == SAB_GRAN_PER_THREAD, SAB_ERR_INVALID,
+              "granularity must be SAB_GRAN_PER_WARP or SAB_GRAN_PER_THREAD (got %d)", granularity);
+  SAB_REQUIRE(mean == nullptr || is_key, SAB_ERR_INVALID, "the mean is subtracted from K only (is_key == 0)");
+  SAB_REQUIRE((reinterpret_cast<uintptr_t>(out) & 7) == 0 && o_stride_t % 8 == 0 && o_stride_h % 8 == 0, SAB_ERR_INVALID,
+              "int8 output must be 8-byte aligned");
+  const bool pt = granularity == SAB_GRAN_PER_THREAD;
+  QuantParams p{};
+  p.x = x; p.mean = mean; p.out = out; p.scale = scale; p.H = H; p.S = 0; p.scale_cols = 0;
+  p.xsh = x_stride_h; p.xss = x_stride_t; p.osh = o_stride_h; p.oss = o_stride_t;
+  // per-thread: quant_per_thread.py semantics (sab_quant_per_thread_int8); per-warp: csrc/fused/fused.cu (blk 32 Q, 64 K)
+  p.blk = is_key ? 64 : 32;
+  p.semantics = pt ? SAB_SEM_TRITON : SAB_SEM_CUDA;
+  p.eps_after = pt ? 1 : 0;
+  p.has_sm_scale = 0; p.sm_scale = 1.f;
+  p.cu = cu_seqlens; p.cu_scale = cu_scale;
+  const int mode = pt ? (is_key ? kGroupThreadK : kGroupThreadQ) : kGroupBlock;
+  return launch_quant_seq(p, dtype, D, mode, dim3((max_seqlen + 127) / 128, H, nseq), reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int sab_per_channel_fp8_varlen(const void* v, int dtype, uint8_t* v_fp8, float* v_scale, float* v_mean,
+                                          const int32_t* cu_seqlens, const int32_t* cu_pad, int nseq, int max_seqlen, int H, int D,
+                                          int64_t stride_t, int64_t stride_h, int64_t t_pad, float scale_max, void* workspace,
+                                          void* stream) {
+  int st = check_common(v, dtype, D, 0, stride_h, stride_t);
+  if (st) return st;
+  SAB_REQUIRE(v_fp8 && v_scale && workspace && cu_seqlens && cu_pad && nseq > 0 && max_seqlen > 0 && H > 0, SAB_ERR_INVALID,
+              "bad arguments to sab_per_channel_fp8_varlen");
+  SAB_REQUIRE(t_pad % 128 == 0 && aligned16(v_fp8), SAB_ERR_INVALID, "t_pad must be a multiple of 128 and v_fp8 16-byte aligned");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const int nchunk = (max_seqlen + kStatChunk - 1) / kStatChunk;
+  float* part = reinterpret_cast<float*>(workspace);
+  float* recp = part + int64_t(nseq) * H * nchunk * 3 * D;
+  if ((st = run_stats_seq(v, dtype, part, cu_seqlens, nseq, H, nchunk, D, stride_h, stride_t, s))) return st;
+  channel_stats_stage2<__half, true><<<dim3(H, nseq), 128, 0, s>>>(part, nchunk, D, 0, 1, nullptr, v_scale, v_mean, scale_max, recp,
+                                                                   cu_seqlens);
+  SAB_CUDA_OK(cudaGetLastError());
+  VQuantParams p{};
+  p.v = v; p.out = v_fp8; p.recp = recp; p.vmean = v_mean; p.H = H; p.S = 0;
+  p.sb = 0; p.sh = stride_h; p.ss = stride_t; p.s_pad = t_pad; p.scale_max = scale_max; p.cu = cu_seqlens; p.cu_pad = cu_pad;
+  const dim3 grid((max_seqlen + 127) / 128, H, nseq);
+#define SAB_VQ(T, DD) v_quant_transpose_kernel<T, DD, true><<<grid, 256, 0, s>>>(p)
+  if (dtype == SAB_DTYPE_FP16) { if (D == 128) SAB_VQ(__half, 128); else SAB_VQ(__half, 64); }
+  else { if (D == 128) SAB_VQ(__nv_bfloat16, 128); else SAB_VQ(__nv_bfloat16, 64); }
+#undef SAB_VQ
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
 }

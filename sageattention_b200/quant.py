@@ -221,3 +221,69 @@ def transpose_v_f16_varlen(v: torch.Tensor, cu_seqlens_k: torch.Tensor, max_seql
     v_t = torch.empty((h_kv, head_dim, t_pad), dtype=torch.float16, device=v.device)
     ops.v_transpose_f16_varlen(v, v_t, cu32, cu_pad, max_seqlen_k)
     return v_t, cu_pad
+
+
+# ------------------------------------------------------------------------------------------------ packed, per-sequence statistics
+def varlen_block_table(cu_seqlens: torch.Tensor, blk: int) -> torch.Tensor:
+    """[nseq+1] int32: exclusive cumsum of ceil(L_b / blk) over the sequence lengths of cu_seqlens, on its device (no sync)."""
+    cu32 = cu_seqlens.to(torch.int32)
+    lens = cu32[1:] - cu32[:-1]
+    return torch.nn.functional.pad(torch.cumsum((lens + blk - 1) // blk, dim=0), (1, 0), value=0).to(torch.int32)
+
+
+def varlen_scale_rows(T: int, nseq: int, blk: int, mult: int) -> int:
+    """Rows of a per-sequence scale table without a device->host sync: sum_b ceil(L_b/blk) <= T // blk + nseq blocks."""
+    return (T // blk + nseq) * mult
+
+
+def k_mean_varlen(k: torch.Tensor, cu_seqlens_k: torch.Tensor, max_seqlen_k: int) -> torch.Tensor:
+    """Per-sequence `k.mean(dim=seq)` of packed k [T,H,D]: [nseq,H,D] in k.dtype, each sequence bit for bit k_mean() of that
+    sequence alone (0 for an empty one)."""
+    nseq = cu_seqlens_k.numel() - 1
+    mean = torch.empty((nseq, k.size(1), k.size(2)), dtype=k.dtype, device=k.device)
+    ops.k_mean_varlen(k, mean, cu_seqlens_k.to(torch.int32), max_seqlen_k)
+    return mean
+
+
+def quant_q_int8_varlen(q: torch.Tensor, cu_seqlens_q: torch.Tensor, max_seqlen_q: int, qk_quant_gran: str = "per_thread"):
+    """quant_q_int8 per packed sequence: (q_int8 [T,H,D], q_scale [rows,H], cu_q_scale [nseq+1] in 128-row blocks).  Sequence
+    b's scales are rows [cu_q_scale[b] * mult, ...) with mult 4 (per_warp) or 32 (per_thread), in quant_q_int8's order."""
+    from ._capi import SAB_GRAN_PER_WARP, SAB_GRAN_PER_THREAD
+    nseq = cu_seqlens_q.numel() - 1
+    mult = 4 if qk_quant_gran == "per_warp" else 32
+    cu_q_scale = varlen_block_table(cu_seqlens_q, 128)
+    q_int8 = torch.empty(q.shape, dtype=torch.int8, device=q.device)
+    q_scale = torch.empty((varlen_scale_rows(q.size(0), nseq, 128, mult), q.size(1)), dtype=torch.float32, device=q.device)
+    ops.quant_int8_varlen(q, None, q_int8, q_scale, cu_seqlens_q.to(torch.int32), cu_q_scale, max_seqlen_q,
+                          SAB_GRAN_PER_WARP if qk_quant_gran == "per_warp" else SAB_GRAN_PER_THREAD, False)
+    return q_int8, q_scale, cu_q_scale
+
+
+def quant_k_int8_varlen(k: torch.Tensor, km: Optional[torch.Tensor], cu_seqlens_k: torch.Tensor, max_seqlen_k: int,
+                        qk_quant_gran: str = "per_thread"):
+    """quant_k_int8 per packed sequence with the fused `k - km[b]` (km [nseq,H,D] or None): (k_int8, k_scale [rows,H],
+    cu_k_scale [nseq+1] in 64-key blocks).  Sequence b's scales are rows [cu_k_scale[b] * mult, ...), mult 1 (per_warp) or 4."""
+    from ._capi import SAB_GRAN_PER_WARP, SAB_GRAN_PER_THREAD
+    nseq = cu_seqlens_k.numel() - 1
+    mult = 1 if qk_quant_gran == "per_warp" else 4
+    cu_k_scale = varlen_block_table(cu_seqlens_k, 64)
+    k_int8 = torch.empty(k.shape, dtype=torch.int8, device=k.device)
+    k_scale = torch.empty((varlen_scale_rows(k.size(0), nseq, 64, mult), k.size(1)), dtype=torch.float32, device=k.device)
+    ops.quant_int8_varlen(k, None if km is None else km.contiguous(), k_int8, k_scale, cu_seqlens_k.to(torch.int32), cu_k_scale,
+                          max_seqlen_k, SAB_GRAN_PER_WARP if qk_quant_gran == "per_warp" else SAB_GRAN_PER_THREAD, True)
+    return k_int8, k_scale, cu_k_scale
+
+
+def per_channel_fp8_varlen_seq(v: torch.Tensor, cu_seqlens_k: torch.Tensor, max_seqlen_k: int, scale_max: float = 448.0,
+                               smooth_v: bool = False):
+    """per_channel_fp8 per packed sequence: (v_fp8 [H,D,T_pad], v_scale [nseq,H,D], vm [nseq,H,D] or None, cu_pad).  Sequence b
+    occupies token columns [cu_pad[b], cu_pad[b] + ceil(L_b/128)*128), zero padded, as in per_channel_fp8_varlen."""
+    T, h_kv, head_dim = v.shape
+    nseq = cu_seqlens_k.numel() - 1
+    cu_pad = varlen_block_table(cu_seqlens_k, 128) * 128
+    t_pad = (T + 127 * nseq + 127) // 128 * 128          # upper bound, no host sync
+    v_fp8 = torch.empty((h_kv, head_dim, t_pad), dtype=torch.float8_e4m3fn, device=v.device)
+    v_scale = torch.empty((nseq, h_kv, head_dim), dtype=torch.float32, device=v.device)
+    vm = torch.empty((nseq, h_kv, head_dim), dtype=torch.float32, device=v.device) if smooth_v else None
+    ops.per_channel_fp8_varlen_seq(v, v_fp8, v_scale, vm, cu_seqlens_k.to(torch.int32), cu_pad, max_seqlen_k, scale_max)
+    return v_fp8, v_scale, vm, cu_pad

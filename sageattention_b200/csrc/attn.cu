@@ -9,6 +9,9 @@
 //                     O (fp32, 64 x D) accumulated in registers.  The loop is rotated so that each warpgroup issues PV(j-1)
 //                     and QK(j) as one tensor-core phase per tile, and the two warpgroups ping-pong: named barriers hand the
 //                     turn to issue from one to the other, so one's softmax runs while the other's MMAs are on the tensor cores.
+//                     The loop is bound by each warpgroup's serial path (phase, then softmax), not by the tensor cores, so at
+//                     D = 128 softmax(j) starts when QK(j) is done and runs under PV(j-1): a step at hd=128, S=8192 went from
+//                     1693 to 1555 cycles (H100 SXM, 700 W; -DSAB_PHASE_CLOCKS, tools/phase_clocks.py).
 //   warp 8          : TMA producer (Q once; K and V^T 64-key tiles through a kStages-deep mbarrier ring, swizzled smem);
 //                     warps 9-11 only hand their registers over (setmaxnreg: 24 for the producer warpgroup, 240 for consumers).
 // The softmax / MMA tile is 64 keys — the reference's CTA_K — so the running-max sequence, P and d follow
@@ -43,6 +46,41 @@ template <int D>
 __device__ __forceinline__ int* kv_scratch(uint8_t* smem) { return reinterpret_cast<int*>(smem + kKvScratchOff<D>); }
 template <int D>
 __device__ __forceinline__ uint16_t* kv_list(uint8_t* smem) { return reinterpret_cast<uint16_t*>(smem + kKvScratchOff<D> + 64); }
+
+// Per-phase cycle counts of the consumer loop, for measurement builds only (-DSAB_PHASE_CLOCKS; tools/phase_clocks.py reads
+// them).  Each consumer warpgroup sums clock64() spans over its main-loop steps j >= 1 (PV(j-1) + QK(j)): from taking its turn
+// to the end of the wait for S(j) (the tensor-core phase, including any wait behind the other warpgroup's phase; at D = 128 it
+// ends when QK(j) is done), and from there to the end of the fold + softmax; the whole loop is timed as well.  The sums over all warpgroups of a launch are added to
+// g_phase_clk: {phase cycles, fold + softmax cycles, loop cycles, steps, warpgroups}.  The product build compiles none of it.
+#ifdef SAB_PHASE_CLOCKS
+__device__ unsigned long long g_phase_clk[5];
+struct PhaseClocks {
+  long long mma = 0, soft = 0, loop0 = 0, t = 0;
+  int n = 0;
+  __device__ __forceinline__ void loop_start() { loop0 = clock64(); }
+  __device__ __forceinline__ void turn() { t = clock64(); }
+  __device__ __forceinline__ void mma_done() { const long long c = clock64(); mma += c - t; t = c; ++n; }
+  __device__ __forceinline__ void soft_done() { soft += clock64() - t; }
+  __device__ __forceinline__ void flush() {
+    const long long loop = clock64() - loop0;
+    if ((threadIdx.x & 127) == 0 && n > 0) {
+      atomicAdd(&g_phase_clk[0], (unsigned long long)mma);
+      atomicAdd(&g_phase_clk[1], (unsigned long long)soft);
+      atomicAdd(&g_phase_clk[2], (unsigned long long)loop);
+      atomicAdd(&g_phase_clk[3], (unsigned long long)n);
+      atomicAdd(&g_phase_clk[4], 1ull);
+    }
+  }
+};
+#else
+struct PhaseClocks {
+  __device__ __forceinline__ void loop_start() {}
+  __device__ __forceinline__ void turn() {}
+  __device__ __forceinline__ void mma_done() {}
+  __device__ __forceinline__ void soft_done() {}
+  __device__ __forceinline__ void flush() {}
+};
+#endif
 
 // D: head dim (64 / 128).  kKT: per-thread K scales (4 per 64-key block) instead of 1.  OutT: __half / bf16.
 // kPV16: P and V in fp16 with the Triton path's softmax (no exponent offset) — the numerics of the reference's
@@ -247,10 +285,11 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 
   uint32_t s[32];                   // S of the tile in flight (int32)
   float alpha[2];                   // O rescale factor of the last softmax'd tile
-  uint32_t a[kPV16 ? 4 : 2][4];     // its P as the PV A operand
+  uint32_t a[kPV16 ? 4 : 2][4];     // P of the tile whose PV comes next, as the PV A operand
   [[maybe_unused]] float ot[NO];    // FP8 path: its P V, from zero
 
   // ---- S (registers, int32) -> P: running max m, sum d, rescale factor alpha, P as A fragments
+  float e[32];                      // P of the last softmax in fp32, same register order as S
   auto softmax = [&](int j) {
     [[maybe_unused]] const char* mrow[2] = {nullptr, nullptr};   // this row's 64 mask elements of tile j
     if constexpr (kElemMask<kPV16, kMask>) {
@@ -269,7 +308,6 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       }
     }
 
-    float e[32];           // P in fp32, same register order as S
     auto tile = [&](auto masked_tag) {
       constexpr bool MASKED = decltype(masked_tag)::value;
 #pragma unroll
@@ -372,7 +410,10 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     else if (masked_tile) tile(std::true_type{});
     else tile(std::false_type{});
 
-    // ---- P -> A fragments
+  };
+
+  // ---- P -> A fragments of the PV operand.  Only once the PV that read a has completed.
+  auto pack_p = [&]() {
     if constexpr (kPV16) {
       // k16 step kk: keys 16kk..16kk+15 = accumulator blocks 2kk, 2kk+1 (same layout: no exchange)
 #pragma unroll
@@ -438,14 +479,22 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty + j % kStages);   // K(j) and V(j) consumed by this warpgroup
   };
 
-  // ---- main loop, rotated so each warpgroup has ONE tensor-core phase per tile: PV(j-1) and QK(j) issued back to back, then
-  // PV(j-1) folded into O and softmax(j) on the CUDA cores.  The two warpgroups take turns at issuing their phases (named
-  // barrier 1 + wg is this warpgroup's turn, arrived at by the other one right after its commit), so one's softmax runs while
-  // the other's MMAs are on the tensor cores.  Each warpgroup has n_kv + 1 phases; warpgroup 1 hands the first turn to
-  // warpgroup 0 and skips the hand-over after its last phase, so no arrival is left over at exit.  n_kv is uniform per CTA;
-  // with n_kv == 0 no barrier is touched.  Slot j-1 is released one phase later than it was consumed; the ring absorbs it.
+  // ---- main loop, rotated so each warpgroup has ONE tensor-core phase per tile: QK(j) and PV(j-1) issued back to back, then
+  // softmax(j) and the fold of PV(j-1) into O on the CUDA cores.  At D = 128 the two products are separate commit groups, QK(j)
+  // first, and softmax(j) starts as soon as QK(j) has completed, under PV(j-1) (an m64n128k32 pair, half the phase); O is folded
+  // after it.  At D = 64 PV(j-1) is an m64n64k32 pair with little to hide, and one commit group measured faster (hd=64 rows of
+  // bench.py 1.3 % slower with the split, H100 SXM, 700 W).  Either way O's per-element sequence is o *= alpha(j-1), then
+  // o += PV(j-1) (softmax(j) does not touch O) and P(j) overwrites the PV operand a only after PV(j-1) has completed (pack_p),
+  // so the output is the same to the bit.  The two warpgroups take turns at issuing their phases (named barrier 1 + wg is this
+  // warpgroup's turn, arrived at by the other one right after its commit), so one's softmax runs while the other's MMAs are on
+  // the tensor cores.  Each warpgroup has n_kv + 1 phases; warpgroup 1 hands the first turn to warpgroup 0 and skips the
+  // hand-over after its last phase, so no arrival is left over at exit.  n_kv is uniform per CTA; with n_kv == 0 no barrier is
+  // touched.  Slot j-1 is released one phase later than it was consumed; the ring absorbs it.
+  constexpr bool kSoftmaxUnderPV = D == 128;
   constexpr uint32_t kTurnThreads = 2 * 128;
   const uint32_t my_turn = 1 + wg, their_turn = 2 - wg;
+  PhaseClocks clk;
+  clk.loop_start();
   if (n_kv > 0) {
     mbar_wait_wd(q_full, 0);
     if (wg == 1) named_bar_arrive(their_turn, kTurnThreads);
@@ -459,22 +508,43 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     wgmma_wait<0>();
     fence_regs(s);
     softmax(0);
+    pack_p();
   }
   for (int j = 1; j < n_kv; ++j) {
     tile_setup(j);
     mbar_wait_wd(kv_full + j % kStages, (j / kStages) & 1);
     named_bar_sync(my_turn, kTurnThreads);
+    clk.turn();
     if constexpr (kPV16) rescale_o();          // before the in-place PV
     wgmma_fence();
-    issue_pv(j - 1);
-    issue_qk(j);
-    wgmma_commit();
+    if constexpr (kSoftmaxUnderPV) {
+      issue_qk(j);
+      wgmma_commit();
+      issue_pv(j - 1);
+      wgmma_commit();
+    } else {
+      issue_pv(j - 1);
+      issue_qk(j);
+      wgmma_commit();
+    }
     named_bar_arrive(their_turn, kTurnThreads);
     if constexpr (!kPV16) rescale_o();         // overlaps the MMAs
-    wgmma_wait<0>();
-    fence_regs(s);
-    finish_pv(j - 1);
-    softmax(j);
+    if constexpr (kSoftmaxUnderPV) {
+      wgmma_wait<1>();                         // S(j) is ready; PV(j-1) may still run
+      fence_regs(s);
+      clk.mma_done();
+      softmax(j);
+      wgmma_wait<0>();
+      finish_pv(j - 1);
+    } else {
+      wgmma_wait<0>();
+      fence_regs(s);
+      clk.mma_done();
+      finish_pv(j - 1);
+      softmax(j);
+    }
+    pack_p();
+    clk.soft_done();
   }
   if (n_kv > 0) {
     named_bar_sync(my_turn, kTurnThreads);
@@ -487,6 +557,7 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     wgmma_wait<0>();
     finish_pv(n_kv - 1);
   }
+  clk.flush();
 
   // ---- epilogue: O / d * v_scale (+ v_mean) -> fp16/bf16 (…sm89.cuh:572-703)
   const float* vs = p.v_scale ? p.v_scale + (int64_t(varlen && !kSeqV ? 0 : b) * p.Hkv + hk) * D : nullptr;
@@ -938,3 +1009,14 @@ extern "C" int sab_qk_int8_sv_f8_attn_varlen(const int8_t* q_int8, const int8_t*
   tl_seq_v = false;
   return st;
 }
+
+#ifdef SAB_PHASE_CLOCKS
+// measurement builds: copy out the phase-cycle sums of sab::g_phase_clk (see PhaseClocks) and reset them
+extern "C" int sab_phase_clocks_read(unsigned long long* out5) {
+  SAB_CUDA_OK(cudaDeviceSynchronize());
+  SAB_CUDA_OK(cudaMemcpyFromSymbol(out5, sab::g_phase_clk, sizeof(unsigned long long) * 5));
+  const unsigned long long zero[5] = {};
+  SAB_CUDA_OK(cudaMemcpyToSymbol(sab::g_phase_clk, zero, sizeof(zero)));
+  return SAB_OK;
+}
+#endif

@@ -8,7 +8,14 @@ the window crosses, which take the masked path) against the dense kernel's, and 
 for the gradient kernels (10*D per pair) against the dense backward's, and splits each backward call into its delta, dQ and dK/dV
 kernels (torch.profiler).  Prints one JSON line with the GPU name and power limit.  CUDA events; writes nothing.
 
-    python bench_window.py [--steps 5] [--warmup 2] [--reps 3] [--backward]
+--varlen: sageattn_varlen_window's kernels on the packed lengths of bench_varlen_fp8.py (2048, 16384, 4096, 512, 1024, 8192;
+Hq=32, Hkv=8, D=128, bf16) with the same three windows (Hq=32 for all three), against the packed kernel without a window
+(sageattn_varlen_qk_int8_pv_fp8_cuda's) and the dense window kernels run once per sequence (summed), all three timed alternately
+in the same run.  Visible pairs and tiles are summed over the sequences; 4*Hq*D*(visible pairs)/t for every kernel, the packed
+dense kernel included (it computes more pairs than the window keeps).  --varlen --backward does the same for the gradient kernels
+(10*Hq*D per pair).
+
+    python bench_window.py [--steps 5] [--warmup 2] [--reps 3] [--backward] [--varlen]
 """
 import argparse
 import json
@@ -46,13 +53,98 @@ def _visible(S, causal, left, right):
     return pairs, tiles, masked, dense
 
 
+VARLEN_LENS = [2048, 16384, 4096, 512, 1024, 8192]   # bench_varlen_fp8.py's packed lengths, in its order
+VARLEN_WINDOWS = [(True, (1024, 0)), (True, (4096, 0)), (False, (2048, 2048))]
+
+
+def _visible_varlen(lens, causal, left, right):
+    """_visible summed over packed sequences (Lq == Lk): (pairs, tiles, masked, dense tiles) of one head."""
+    return tuple(sum(x) for x in zip(*(_visible(L, causal, left, right) for L in lens)))
+
+
+def _alternate_all(fns, a):
+    """Median ms of each function of fns, timed in turn in every round (as _alternate does for two)."""
+    ts = {n: [] for n in fns}
+    for _ in range(a.reps):
+        for n, f in fns.items():
+            ts[n].append(_events(f, a.steps, a.warmup))
+    return {n: statistics.median(t) for n, t in ts.items()}
+
+
+def main_varlen(a):
+    import sageattention_b200 as sab
+    from sageattention_b200 import ops, quant as Q
+    from sageattention_b200.core import _quant_qk, _quant_qk_varlen_f8
+    from sageattention_b200._capi import SAB_GRAN_PER_THREAD as PT
+
+    lens, Hq, Hkv, D = VARLEN_LENS, 32, 8, 128
+    out = {"metric": "sageattn_varlen_window " + ("backward" if a.backward else "forward") + " kernels vs packed dense and per-sequence",
+           "gpu": _gpu(), "dtype": "bf16", "seqlens": lens, "Hq": Hq, "Hkv": Hkv, "D": D, "cases": []}
+    cu = torch.tensor([0] + torch.tensor(lens).cumsum(0).tolist(), dtype=torch.int32, device="cuda")
+    T, L = int(cu[-1]), max(lens)
+    spans = [(int(cu[i]), int(cu[i + 1])) for i in range(len(lens))]
+    g = torch.Generator(device="cuda").manual_seed(0)
+    q, do = (torch.randn(T, Hq, D, device="cuda", dtype=torch.bfloat16, generator=g) for _ in range(2))
+    k, v = (torch.randn(T, Hkv, D, device="cuda", dtype=torch.bfloat16, generator=g) for _ in range(2))
+    sm = D ** -0.5
+    km, q8, qs, cqs, k8, ks, cks = _quant_qk_varlen_f8(q, k, cu, cu, L, L, "per_thread", True)
+    v8, vs, vm, cpad = Q.per_channel_fp8_varlen_seq(v, cu, L, 2.25)
+    ow, od = torch.empty_like(q), torch.empty_like(q)
+    dense = []   # each sequence's dense operands (NHD, batch 1)
+    for s, e in spans:
+        qb, kb, vb = q[s:e][None], k[s:e][None], v[s:e][None]
+        kmb, q8d, qsd, k8d, ksd, _, _, _ = _quant_qk(qb, kb, "fp8", "NHD", "per_thread", sm, True, "cuda")
+        v8d, vsd, _ = Q.per_channel_fp8(vb, "NHD", 2.25, False)
+        dense.append((qb, kb, vb, do[s:e][None], kmb, q8d, qsd, k8d, ksd, v8d, vsd, torch.empty_like(qb)))
+    for causal, (left, right) in VARLEN_WINDOWS:
+        c = int(causal)
+        win = lambda ret=0: ops.qk_int8_sv_f8_attn_varlen_window(q8, k8, v8, ow, qs, ks, vs, None, cu, cu, cpad, cqs, cks, L, left, right,
+                                                                c, PT, PT, sm, ret)
+        packed = lambda ret=0: ops.qk_int8_sv_f8_attn_varlen_seq(q8, k8, v8, od, qs, ks, vs, None, cu, cu, cpad, cqs, cks, L, c, PT, PT,
+                                                                sm, ret)
+        per_seq = lambda ret=0: [ops.qk_int8_sv_f8_attn_window(d[5], d[7], d[9], d[11], d[6], d[8], d[10], None, left, right, 0, c, PT,
+                                                               PT, sm, 0, ret) for d in dense]
+        pairs, tiles, masked, dense_tiles = _visible_varlen(lens, causal, left, right)
+        dense_pairs = sum(Ls * (Ls + 1) // 2 if causal else Ls * Ls for Ls in lens)
+        case = {"causal": causal, "window": [left, right], "visible_pairs_per_head": pairs,
+                "visible_fraction_of_dense": round(pairs / dense_pairs, 4), "tiles_visited_per_head": tiles,
+                "masked_tiles_per_head": masked, "tiles_fraction_of_dense": round(tiles / dense_tiles, 4)}
+        per = 10.0 if a.backward else 4.0
+        if not a.backward:
+            t = _alternate_all({"packed_window": win, "packed_dense": packed, "per_sequence_window": per_seq}, a)
+            tc = _events(lambda: sab.sageattn_varlen_window(q, k, v, cu, cu, L, L, (left, right), is_causal=causal), a.steps, a.warmup)
+            case["packed_window_call_ms"] = round(tc, 3)
+        else:
+            lw, ld, ls = win(1), packed(1), per_seq(1)
+            gq, gk, gv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+            bw = lambda: ops.qk_int8_attn_bwd_varlen_window(q8, k8, qs, ks, q, k, v, ow, do, lw, km, gq, gk, gv, cu, cu, cqs, cks, L, L,
+                                                            left, right, c, PT, PT, sm)
+            bd = lambda: ops.qk_int8_attn_bwd_varlen_seq(q8, k8, qs, ks, q, k, v, od, do, ld, km, gq, gk, gv, cu, cu, cqs, cks, L, L, c,
+                                                         PT, PT, sm)
+            grads = [tuple(torch.empty_like(x) for x in d[:3]) for d in dense]
+            bs = lambda: [ops.qk_int8_attn_bwd_window(d[5], d[7], d[6], d[8], d[0], d[1], d[2], d[11], d[3], l, d[4], *gr, left, right, 0,
+                                                      c, PT, PT, sm, 0) for d, l, gr in zip(dense, ls, grads)]
+            t = _alternate_all({"packed_window": bw, "packed_dense": bd, "per_sequence_window": bs}, a)
+            case["per_kernel_ms"] = {"packed_window": _split(bw, a), "packed_dense": _split(bd, a)}
+        for n, tn in t.items():
+            case[f"{n}_ms"] = round(tn, 3)
+            case[f"{n}_tflops_visible"] = round(per * Hq * D * pairs / tn / 1e9, 1)
+        case["packed_window_over_per_sequence"] = round(t["packed_window"] / t["per_sequence_window"], 4)
+        case["packed_window_over_packed_dense"] = round(t["packed_window"] / t["packed_dense"], 4)
+        out["cases"].append(case)
+    print(json.dumps(out))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--backward", action="store_true")
+    ap.add_argument("--varlen", action="store_true")
     a = ap.parse_args()
+    if a.varlen:
+        return main_varlen(a)
     import sageattention_b200 as sab
     from sageattention_b200 import ops
     from sageattention_b200.core import _quant_qk

@@ -482,6 +482,35 @@ int sab_qk_int8_attn_bwd_varlen_seq(const int8_t* q_int8, const int8_t* k_int8, 
                                     const int32_t* cu_k_scale, int max_seqlen_q, int max_seqlen_k, int is_causal, int q_gran,
                                     int k_gran, float sm_scale, void* stream);
 
+/* Sliding-window forms of the packed per-sequence INT8+FP8 attention (no reference counterpart): sab_qk_int8_sv_f8_attn_varlen and
+ * sab_qk_int8_attn_bwd_varlen_seq with the window of sab_qk_int8_sv_f8_attn_window, applied inside each sequence.  Key j of
+ * sequence b is visible to its query i iff i - window_left <= j <= i + window_right (-1: that side unbounded; top-left inside the
+ * sequence), j < Lk_b, and j <= i when is_causal (Lq != Lk allowed); no window reaches into a neighbouring sequence.  Each
+ * sequence's window is clamped at its own lengths (a side >= Lq_b or >= Lk_b becomes -1, as sab_qk_int8_sv_f8_attn_window clamps
+ * it for the dense call), so sequence b gets the bits of the dense window entry on that sequence alone, forward and gradient.
+ * Causal with (left, right) is non-causal with (left, 0).  (-1, -1) computes the bits of the entries without a window, (-1, 0)
+ * non-causal those of their causal call.  A row with no visible key returns 0 and lse -inf and gets zero gradients; keys no row
+ * sees get zero dk and dv.  window_left / window_right < -1 and missing sequence tables are refused before anything touches the
+ * device; a side is first clamped at max_seqlen_q (left) and at Tk (forward) or max_seqlen_k (gradient, right). */
+int sab_qk_int8_sv_f8_attn_varlen_window(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out, float* lse,
+                                         const float* q_scale, const float* k_scale, const float* v_scale, const float* v_mean,
+                                         int out_dtype, int nseq, int Hq, int Hkv, int Tq, int Tk, int D, int64_t q_stride_t,
+                                         int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h, int64_t v_t_pad,
+                                         int64_t o_stride_t, int64_t o_stride_h, int is_causal, int q_gran, int k_gran, float sm_scale,
+                                         const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k, const int32_t* cu_pad_v,
+                                         const int32_t* cu_q_scale, const int32_t* cu_k_scale, int max_seqlen_q, int window_left,
+                                         int window_right, void* stream);
+int sab_qk_int8_attn_bwd_varlen_window(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
+                                       const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
+                                       const void* k_mean, void* dq, void* dk, void* dv, void* workspace, int dtype, int nseq, int Hq,
+                                       int Hkv, int Tq, int Tk, int D, int64_t q8_stride_t, int64_t q8_stride_h, int64_t k8_stride_t,
+                                       int64_t k8_stride_h, int64_t q_stride_t, int64_t q_stride_h, int64_t k_stride_t,
+                                       int64_t k_stride_h, int64_t v_stride_t, int64_t v_stride_h, int64_t o_stride_t,
+                                       int64_t o_stride_h, int64_t do_stride_t, int64_t do_stride_h, const int32_t* cu_seqlens_q,
+                                       const int32_t* cu_seqlens_k, const int32_t* cu_q_scale, const int32_t* cu_k_scale,
+                                       int max_seqlen_q, int max_seqlen_k, int is_causal, int q_gran, int k_gran, float sm_scale,
+                                       int window_left, int window_right, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

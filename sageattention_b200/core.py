@@ -272,12 +272,18 @@ def sageattn_window(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, window_si
     The K mean and the V scales are still taken over every key.  A row with no visible key returns 0 (lse -inf).  window_size
     (-1, -1) gives the bits of sageattn_qk_int8_pv_fp8_cuda, and (-1, 0) those of its causal call.  Differentiable when grad
     mode is on and q, k or v requires grad: the dense straight-through gradient with P = 0 outside the window."""
+    window = _check_window_size(window_size)
+    _check_inputs(q, k, v)
+    return _qk_int8_pv_fp8(q, k, v, tensor_layout, is_causal, qk_quant_gran, sm_scale, pv_accum_dtype, smooth_k, smooth_v,
+                           return_lse, window=window)
+
+
+def _check_window_size(window_size):
+    """window_size as a pair of Python ints >= -1, or ValueError."""
     if (not isinstance(window_size, (tuple, list)) or len(window_size) != 2 or
             any(isinstance(w, bool) or not isinstance(w, numbers.Integral) or w < -1 for w in window_size)):
         raise ValueError(f"window_size must be a pair of ints >= -1 (-1: unbounded), got {window_size!r}")
-    _check_inputs(q, k, v)
-    return _qk_int8_pv_fp8(q, k, v, tensor_layout, is_causal, qk_quant_gran, sm_scale, pv_accum_dtype, smooth_k, smooth_v,
-                           return_lse, window=(int(window_size[0]), int(window_size[1])))
+    return int(window_size[0]), int(window_size[1])
 
 
 def sageattn_blocksparse(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, block_mask: torch.Tensor, tensor_layout: str = "HND",
@@ -512,14 +518,19 @@ def _quant_qk_varlen_f8(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seql
 
 
 def _attn_varlen_f8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale, smooth_k,
-                    smooth_v, v_range, return_lse):
+                    smooth_v, v_range, return_lse, window=None):
     """Quantisers + INT8+FP8 kernel of sageattn_varlen_qk_int8_pv_fp8_cuda on head-dim-padded packed q, k, v (cu_seqlens int32):
-    (o, the kernel's [Hq,Tq] log2 lse or an empty tensor, km)."""
+    (o, the kernel's [Hq,Tq] log2 lse or an empty tensor, km).  window: the (left, right) of sageattn_varlen_window, checked and
+    clamped by the caller; the quantisers still see every key of each sequence."""
     km, q_int8, q_scale, cu_q_scale, k_int8, k_scale, cu_k_scale = _quant_qk_varlen_f8(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q,
                                                                                      max_seqlen_k, qk_quant_gran, smooth_k)
     v_fp8, v_scale, vm, cu_pad = per_channel_fp8_varlen_seq(v, cu_seqlens_k, max_seqlen_k, v_range, smooth_v)
     o = torch.empty(q.shape, dtype=q.dtype, device=q.device)
     gran = SAB_GRAN_PER_WARP if qk_quant_gran == "per_warp" else SAB_GRAN_PER_THREAD
+    if window is not None:
+        return o, ops.qk_int8_sv_f8_attn_varlen_window(q_int8, k_int8, v_fp8, o, q_scale, k_scale, v_scale, vm, cu_seqlens_q, cu_seqlens_k,
+                                                       cu_pad, cu_q_scale, cu_k_scale, max_seqlen_q, window[0], window[1],
+                                                       1 if is_causal else 0, gran, gran, sm_scale, 1 if return_lse else 0), km
     lse = ops.qk_int8_sv_f8_attn_varlen_seq(q_int8, k_int8, v_fp8, o, q_scale, k_scale, v_scale, vm, cu_seqlens_q, cu_seqlens_k, cu_pad,
                                             cu_q_scale, cu_k_scale, max_seqlen_q, 1 if is_causal else 0, gran, gran, sm_scale,
                                             1 if return_lse else 0)
@@ -548,15 +559,17 @@ class _SageAttnVarlenFp8Function(torch.autograd.Function):
     sequence on its own (include/sageattn_b200.h, sab_qk_int8_attn_bwd_varlen_seq).  forward: the unchanged forward with the kernel
     LSE enabled; saves q, k, v, o, the LSE and the cu_seqlens.  backward: re-runs the per-sequence K mean and Q/K quantisers, then
     the gradient kernels.  Tokens past cu_seqlens[-1] belong to no sequence: their gradient is zero.  The LSE and the K means are
-    returned for the LSE correction and carry no gradient."""
+    returned for the LSE correction and carry no gradient.  window (sageattn_varlen_window): P = 0 outside each sequence's window,
+    and the window gradient kernels visit only the tiles inside it."""
 
     @staticmethod
     def forward(ctx, q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale, smooth_k,
-                smooth_v, v_range):
+                smooth_v, v_range, window=None):
         o, lse, km = _attn_varlen_f8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale,
-                                     smooth_k, smooth_v, v_range, True)
+                                     smooth_k, smooth_v, v_range, True, window)
         ctx.save_for_backward(q, k, v, o, lse, cu_seqlens_q, cu_seqlens_k)
         ctx.cfg = (max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale, smooth_k)
+        ctx.window = window
         km = km if km is not None else q.new_empty(0)
         ctx.mark_non_differentiable(lse, km)
         return o, lse, km
@@ -571,9 +584,15 @@ class _SageAttnVarlenFp8Function(torch.autograd.Function):
         q, k, v, o, do = (t.contiguous() for t in (q, k, v, o, do))
         dq, dk, dv = torch.zeros_like(q), torch.zeros_like(k), torch.zeros_like(v)
         gran = SAB_GRAN_PER_WARP if qk_quant_gran == "per_warp" else SAB_GRAN_PER_THREAD
-        ops.qk_int8_attn_bwd_varlen_seq(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv, cu_seqlens_q, cu_seqlens_k,
-                                        cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, 1 if is_causal else 0, gran, gran, sm_scale)
-        return dq, dk, dv, None, None, None, None, None, None, None, None, None, None
+        if ctx.window is not None:
+            ops.qk_int8_attn_bwd_varlen_window(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv, cu_seqlens_q,
+                                               cu_seqlens_k, cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, ctx.window[0],
+                                               ctx.window[1], 1 if is_causal else 0, gran, gran, sm_scale)
+        else:
+            ops.qk_int8_attn_bwd_varlen_seq(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv, cu_seqlens_q,
+                                            cu_seqlens_k, cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, 1 if is_causal else 0, gran,
+                                            gran, sm_scale)
+        return dq, dk, dv, None, None, None, None, None, None, None, None, None, None, None
 
 
 def _check_cu_seqlens(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k):
@@ -617,6 +636,50 @@ def sageattn_varlen_qk_int8_pv_fp8_cuda(q: torch.Tensor, k: torch.Tensor, v: tor
     mode is on and q, k or v requires grad: for every sequence, dq / dk / dv are the bits of the dense backward of the
     one-sequence call; tokens past cu_seqlens_*[-1] and keys of a sequence without queries get zero gradients."""
     _check_inputs(q, k, v)
+    return _varlen_qk_int8_pv_fp8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale,
+                                  pv_accum_dtype, smooth_k, smooth_v, return_lse)
+
+
+def _varlen_window_arg(window, max_seqlen_q, max_seqlen_k):
+    """The (left, right) the packed window kernels receive: a side that reaches past the longest sequence (left >= max_seqlen_q,
+    right >= max_seqlen_k) sees as much as -1 in every sequence and becomes -1, so a Python int of any size reaches the C ABI
+    as an int32 (ctypes would truncate it silently).  The kernels clamp again at each sequence's own lengths."""
+    left, right = window
+    return (-1 if left >= max_seqlen_q else left), (-1 if right >= max_seqlen_k else right)
+
+
+def sageattn_varlen_window(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor,
+                           max_seqlen_q: int, max_seqlen_k: int, window_size=(-1, -1), is_causal: bool = False,
+                           qk_quant_gran: str = "per_thread", sm_scale: Optional[float] = None, pv_accum_dtype: str = "fp32+fp16",
+                           smooth_k: bool = True, smooth_v: bool = False, return_lse: bool = False):
+    """Sliding-window (local) attention on packed sequences (no reference counterpart): sageattn_varlen_qk_int8_pv_fp8_cuda with the
+    window_size of sageattn_window applied inside each sequence.  The options, checks, warnings, V ranges and packed layout are
+    those of sageattn_varlen_qk_int8_pv_fp8_cuda; window_size is a pair (left, right) of ints >= -1 (ValueError otherwise, before
+    any launch): key j of a sequence is visible to its query i iff i - left <= j <= i + right (-1 leaves a side unbounded), top-left
+    inside the sequence, and j <= i when is_causal.  A window never reaches into a neighbouring sequence.
+
+    Contract: "sageattn_window, per sequence".  Sequence b's output rows are the bits of sageattn_window(q_b[None], k_b[None],
+    v_b[None], window_size, tensor_layout="NHD", is_causal=..., <same options>); every statistic (K mean, INT8 blocks, V scales and
+    mean) is taken per sequence, and each sequence sees the window clamped at its own lengths, as the dense call would.  Causal is
+    allowed with Lq != Lk (top-left), which sageattn_window refuses; causal with (left, right) is non-causal with (left, 0), so such
+    a sequence gets the bits of sageattn_window(..., (left, 0), is_causal=False) on it.  window_size (-1, -1) gives the bits of
+    sageattn_varlen_qk_int8_pv_fp8_cuda, and (-1, 0) non-causal those of its causal call.
+
+    An empty sequence or a row with no visible key gives zero rows and lse -inf; rows past cu_seqlens_q[-1] are not written.
+    return_lse gives [Hq,Tq] in natural-log units with sageattn_varlen_qk_int8_pv_fp8_cuda's caveat: the kernel's LSE is the dense
+    call's to the bit, the per-token K-mean correction within one unit of it.  Differentiable when grad mode is on and q, k or v
+    requires grad: for every sequence, dq / dk / dv are the bits of the dense window backward of the one-sequence call; tokens past
+    the end, keys of a sequence without queries and keys no query's window reaches get zero gradients."""
+    window = _check_window_size(window_size)
+    _check_inputs(q, k, v)
+    return _varlen_qk_int8_pv_fp8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale,
+                                  pv_accum_dtype, smooth_k, smooth_v, return_lse, window)
+
+
+def _varlen_qk_int8_pv_fp8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale,
+                           pv_accum_dtype, smooth_k, smooth_v, return_lse, window=None):
+    """Body of sageattn_varlen_qk_int8_pv_fp8_cuda after _check_inputs; window: the (left, right) of sageattn_varlen_window, checked
+    by the caller (_check_window_size) and clamped here (_varlen_window_arg)."""
     assert qk_quant_gran in ["per_warp", "per_thread"], "qk_quant_gran must be either 'per_warp' or 'per_thread'."
     if pv_accum_dtype not in ("fp32", "fp32+fp32", "fp32+fp16"):
         raise ValueError(f"Unsupported pv_accum_dtype: {pv_accum_dtype}")
@@ -633,13 +696,15 @@ def sageattn_varlen_qk_int8_pv_fp8_cuda(q: torch.Tensor, k: torch.Tensor, v: tor
         warnings.warn(f"pv_accum_dtype is '{pv_accum_dtype}', smooth_v will be ignored.")
         smooth_v = False
     v_range = 2.25 if pv_accum_dtype == "fp32+fp16" else 448.0
+    if window is not None:
+        window = _varlen_window_arg(window, int(max_seqlen_q), int(max_seqlen_k))
     cu_q, cu_k = cu_seqlens_q.to(torch.int32).contiguous(), cu_seqlens_k.to(torch.int32).contiguous()
     args = (cu_q, cu_k, int(max_seqlen_q), int(max_seqlen_k), is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range)
     if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
-        o, lse, km = _SageAttnVarlenFp8Function.apply(q, k, v, *args)
+        o, lse, km = _SageAttnVarlenFp8Function.apply(q, k, v, *args, window)
         q = q.detach()
     else:
-        o, lse, km = _attn_varlen_f8(q, k, v, *args, return_lse)
+        o, lse, km = _attn_varlen_f8(q, k, v, *args, return_lse, window)
     o = o[..., :head_dim_og]
     if return_lse:
         if smooth_k:

@@ -109,11 +109,13 @@ constexpr bool kSparse = kMask && !kPV16;     // block mask of the INT8+FP8 path
 // no key at all gets zeros and lse -inf.
 // kSeqV (INT8+FP8 only, varlen): per-sequence V statistics, v_scale / v_mean [nseq,Hkv,D] indexed by the sequence, where the other
 // varlen forms read one [Hkv,D] table for the whole packed batch.
+// kWindow with kSeqV: the packed window form.  Each sequence sees the window clamped at its own lengths (seq_window), so its rows
+// take the dense window kernel's path on that sequence alone, tile for tile.
 template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false, bool kWindow = false, bool kSeqV = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnParams p,
-                     const __grid_constant__ Window win) {
+                     const __grid_constant__ Window win_arg) {
   constexpr uint32_t K_TILE = BN * D;
   constexpr uint32_t V_TILE = D * BN * (kPV16 ? 2 : 1);
   constexpr int SWQK = D;                        // swizzle span of the Q/K tiles (= row bytes)
@@ -153,6 +155,10 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     tb = 0;
     if (qt * BM >= q_len) return;  // attn_qk_int8_block_varlen.py:84-85
   }
+  // the packed window form reads its sequence's clamped copy; every other form reads the kernel argument itself
+  [[maybe_unused]] Window seq_win;
+  if constexpr (kWindow && kSeqV) seq_win = seq_window(win_arg, q_len, kv_len);
+  const Window& win = (kWindow && kSeqV) ? seq_win : win_arg;
   int n_kv = (kv_len + BN - 1) / BN;                 // 64-key tiles
   if (p.causal) n_kv = min(n_kv, (p.causal_q_offset + (qt + 1) * BM + BN - 1) / BN);
   if constexpr (kSparse<kPV16, kMask>) {
@@ -660,13 +666,14 @@ static int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUten
   return SAB_OK;
 }
 
-// the sliding-window form (sage_attn_fwd_kernel<D, kKT, OutT, false, false, true>)
-template <int D, bool kKT, typename OutT>
+// the sliding-window form (sage_attn_fwd_kernel<D, kKT, OutT, false, false, true, kSeqV>); kSeqV: the packed form with
+// per-sequence V statistics
+template <int D, bool kKT, typename OutT, bool kSeqV = false>
 static int launch_attn_window(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, AttnParams p, Window w,
                               dim3 grid, cudaStream_t stream) {
   p.lazy_tau = exact_max_mode() ? 0.0f : kLazyTau;
   constexpr size_t smem = attn_smem_bytes<D, false>();
-  auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, false, true>;
+  auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, false, true, kSeqV>;
   static bool configured[64] = {};
   if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
   kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p, w);
@@ -839,9 +846,21 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
               : launch_attn_blocksparse<64, false, __half>(tq, tk, tv, p, grid, s);
   }
   if (tl_window != nullptr) {
-    SAB_REQUIRE(!pv16 && !varlen && kv_seg_len == 0 && causal_q_offset == 0, SAB_ERR_UNSUPPORTED,
-                "the window is supported by the dense single-GPU INT8/FP8 path only");
+    SAB_REQUIRE(!pv16 && (!varlen || tl_seq_v) && kv_seg_len == 0 && causal_q_offset == 0, SAB_ERR_UNSUPPORTED,
+                "the window is supported by the dense and the packed (per-sequence) single-GPU INT8/FP8 paths only");
     const Window w = *tl_window;
+    if (tl_seq_v) {
+      if (D == 128) {
+        if (kt) return bf ? launch_attn_window<128, true, __nv_bfloat16, true>(tq, tk, tv, p, w, grid, s)
+                          : launch_attn_window<128, true, __half, true>(tq, tk, tv, p, w, grid, s);
+        return bf ? launch_attn_window<128, false, __nv_bfloat16, true>(tq, tk, tv, p, w, grid, s)
+                  : launch_attn_window<128, false, __half, true>(tq, tk, tv, p, w, grid, s);
+      }
+      if (kt) return bf ? launch_attn_window<64, true, __nv_bfloat16, true>(tq, tk, tv, p, w, grid, s)
+                        : launch_attn_window<64, true, __half, true>(tq, tk, tv, p, w, grid, s);
+      return bf ? launch_attn_window<64, false, __nv_bfloat16, true>(tq, tk, tv, p, w, grid, s)
+                : launch_attn_window<64, false, __half, true>(tq, tk, tv, p, w, grid, s);
+    }
     if (D == 128) {
       if (kt) return bf ? launch_attn_window<128, true, __nv_bfloat16>(tq, tk, tv, p, w, grid, s)
                         : launch_attn_window<128, true, __half>(tq, tk, tv, p, w, grid, s);
@@ -1007,6 +1026,29 @@ extern "C" int sab_qk_int8_sv_f8_attn_varlen(const int8_t* q_int8, const int8_t*
                             k_gran, sm_scale, 0, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale, max_seqlen_q, 0, 0,
                             nullptr, stream);
   tl_seq_v = false;
+  return st;
+}
+
+extern "C" int sab_qk_int8_sv_f8_attn_varlen_window(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out,
+                                                    float* lse, const float* q_scale, const float* k_scale, const float* v_scale,
+                                                    const float* v_mean, int out_dtype, int nseq, int Hq, int Hkv, int Tq, int Tk, int D,
+                                                    int64_t q_stride_t, int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h,
+                                                    int64_t v_t_pad, int64_t o_stride_t, int64_t o_stride_h, int is_causal, int q_gran,
+                                                    int k_gran, float sm_scale, const int32_t* cu_seqlens_q,
+                                                    const int32_t* cu_seqlens_k, const int32_t* cu_pad_v, const int32_t* cu_q_scale,
+                                                    const int32_t* cu_k_scale, int max_seqlen_q, int window_left, int window_right,
+                                                    void* stream) {
+  // no sequence is longer than the packed batch: the right side is clamped at Tk
+  if (int st = sab::check_window_varlen(window_left, window_right, max_seqlen_q, Tk)) return st;
+  SAB_REQUIRE(cu_seqlens_q && cu_seqlens_k && cu_pad_v && cu_q_scale && cu_k_scale && nseq > 0, SAB_ERR_INVALID,
+              "the packed window needs cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale and nseq > 0");
+  const sab::Window w{window_left, window_right};
+  tl_window = &w;
+  const int st = sab_qk_int8_sv_f8_attn_varlen(q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq,
+                                               Hkv, Tq, Tk, D, q_stride_t, q_stride_h, k_stride_t, k_stride_h, v_t_pad, o_stride_t,
+                                               o_stride_h, is_causal, q_gran, k_gran, sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v,
+                                               cu_q_scale, cu_k_scale, max_seqlen_q, stream);
+  tl_window = nullptr;
   return st;
 }
 

@@ -462,6 +462,16 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_window_kernel(const __g
   bwd_dq_tile<D, kKT, T, false, 0, false, true>(p, nullptr, nullptr, &win);
 }
 
+// the packed sliding-window form with a per-sequence K mean: sequence blockIdx.z sees the window clamped at its own lengths, as
+// the forward does (seq_window)
+template <int D, bool kKT, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_varlen_window_kernel(const __grid_constant__ BwdParams p,
+                                                                               const __grid_constant__ Window win) {
+  const int b = blockIdx.z;
+  const Window w = seq_window(win, p.a.cu_q[b + 1] - p.a.cu_q[b], p.a.cu_k[b + 1] - p.a.cu_k[b]);
+  bwd_dq_tile<D, kKT, T, true, 0, false, true, true>(p, nullptr, nullptr, &w);
+}
+
 // ------------------------------------------------------------------------------------------------ dK, dV
 template <int D>
 constexpr size_t bwd_dkdv_smem_bytes() {
@@ -642,6 +652,14 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_window_kernel(const _
   bwd_dkdv_tile<D, kKT, T, false, 0, false, true>(p, nullptr, &win);
 }
 
+template <int D, bool kKT, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_varlen_window_kernel(const __grid_constant__ BwdParams p,
+                                                                                 const __grid_constant__ Window win) {
+  const int b = blockIdx.z;
+  const Window w = seq_window(win, p.a.cu_q[b + 1] - p.a.cu_q[b], p.a.cu_k[b + 1] - p.a.cu_k[b]);
+  bwd_dkdv_tile<D, kKT, T, true, 0, false, true>(p, nullptr, &w);
+}
+
 // delta, then the dQ kernel kq (smem_q bytes, arguments p, q_args...) and the dK/dV kernel kkv (smem_kv bytes); cfg_*: their
 // per-device smem opt-in
 template <typename T>
@@ -705,15 +723,16 @@ static int launch_bwd_blocksparse(const BwdParams& p, const BlockMask& bm, cudaS
   return SAB_OK;
 }
 
-template <int D, bool kKT, typename T>
+// kVarlen: the packed form (grids sized from the longest sequence by the caller, as for sab_qk_int8_attn_bwd_varlen_seq)
+template <int D, bool kKT, typename T, bool kVarlen = false>
 static int launch_bwd_window(const BwdParams& p, const Window& w, cudaStream_t stream) {
   static bool cfg_q[64] = {}, cfg_kv[64] = {};
   if (int st = launch_bwd_delta<T>(p, D, stream)) return st;
-  auto kq = bwd_dq_window_kernel<D, kKT, T>;
+  auto kq = kVarlen ? bwd_dq_varlen_window_kernel<D, kKT, T> : bwd_dq_window_kernel<D, kKT, T>;
   if (int st = ensure_dynamic_smem(kq, bwd_dq_smem_bytes<D>(), cfg_q)) return st;
   kq<<<dim3(p.a.n_q_tiles, p.a.Hq, p.a.B), kBwdThreads, bwd_dq_smem_bytes<D>(), stream>>>(p, w);
   SAB_CUDA_OK(cudaGetLastError());
-  auto kkv = bwd_dkdv_window_kernel<D, kKT, T>;
+  auto kkv = kVarlen ? bwd_dkdv_varlen_window_kernel<D, kKT, T> : bwd_dkdv_window_kernel<D, kKT, T>;
   if (int st = ensure_dynamic_smem(kkv, bwd_dkdv_smem_bytes<D>(), cfg_kv)) return st;
   kkv<<<dim3(p.n_k_tiles, p.a.Hkv, p.a.B), kBwdThreads, bwd_dkdv_smem_bytes<D>(), stream>>>(p, w);
   SAB_CUDA_OK(cudaGetLastError());
@@ -975,16 +994,16 @@ extern "C" int sab_qk_int8_attn_bwd_window(const int8_t* q_int8, const int8_t* k
   return bf ? launch_bwd_window<64, false, __nv_bfloat16>(p, w, s) : launch_bwd_window<64, false, __half>(p, w, s);
 }
 
-extern "C" int sab_qk_int8_attn_bwd_varlen_seq(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
-                                               const void* q, const void* k, const void* v, const void* o, const void* dout,
-                                               const float* lse, const void* k_mean, void* dq, void* dk, void* dv, void* workspace,
-                                               int dtype, int nseq, int Hq, int Hkv, int Tq, int Tk, int D, int64_t q8_stride_t,
-                                               int64_t q8_stride_h, int64_t k8_stride_t, int64_t k8_stride_h, int64_t q_stride_t,
-                                               int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h, int64_t v_stride_t,
-                                               int64_t v_stride_h, int64_t o_stride_t, int64_t o_stride_h, int64_t do_stride_t,
-                                               int64_t do_stride_h, const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
-                                               const int32_t* cu_q_scale, const int32_t* cu_k_scale, int max_seqlen_q,
-                                               int max_seqlen_k, int is_causal, int q_gran, int k_gran, float sm_scale, void* stream) {
+// sab_qk_int8_attn_bwd_varlen_seq and, with a window w (already checked), sab_qk_int8_attn_bwd_varlen_window
+static int bwd_varlen_seq(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale, const void* q,
+                          const void* k, const void* v, const void* o, const void* dout, const float* lse, const void* k_mean, void* dq,
+                          void* dk, void* dv, void* workspace, int dtype, int nseq, int Hq, int Hkv, int Tq, int Tk, int D,
+                          int64_t q8_stride_t, int64_t q8_stride_h, int64_t k8_stride_t, int64_t k8_stride_h, int64_t q_stride_t,
+                          int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h, int64_t v_stride_t, int64_t v_stride_h,
+                          int64_t o_stride_t, int64_t o_stride_h, int64_t do_stride_t, int64_t do_stride_h,
+                          const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k, const int32_t* cu_q_scale,
+                          const int32_t* cu_k_scale, int max_seqlen_q, int max_seqlen_k, int is_causal, int q_gran, int k_gran,
+                          float sm_scale, const sab::Window* w, void* stream) {
   using namespace sab;
   SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
               SAB_ERR_INVALID, "null tensor pointer");
@@ -1012,10 +1031,53 @@ extern "C" int sab_qk_int8_attn_bwd_varlen_seq(const int8_t* q_int8, const int8_
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const bool kt = k_gran == SAB_GRAN_PER_THREAD;
   const bool bf = dtype == SAB_DTYPE_BF16;
+  if (w != nullptr) {
+    if (D == 128) {
+      if (kt) return bf ? launch_bwd_window<128, true, __nv_bfloat16, true>(p, *w, s) : launch_bwd_window<128, true, __half, true>(p, *w, s);
+      return bf ? launch_bwd_window<128, false, __nv_bfloat16, true>(p, *w, s) : launch_bwd_window<128, false, __half, true>(p, *w, s);
+    }
+    if (kt) return bf ? launch_bwd_window<64, true, __nv_bfloat16, true>(p, *w, s) : launch_bwd_window<64, true, __half, true>(p, *w, s);
+    return bf ? launch_bwd_window<64, false, __nv_bfloat16, true>(p, *w, s) : launch_bwd_window<64, false, __half, true>(p, *w, s);
+  }
   if (D == 128) {
     if (kt) return bf ? launch_bwd_varlen_seq<128, true, __nv_bfloat16>(p, s) : launch_bwd_varlen_seq<128, true, __half>(p, s);
     return bf ? launch_bwd_varlen_seq<128, false, __nv_bfloat16>(p, s) : launch_bwd_varlen_seq<128, false, __half>(p, s);
   }
   if (kt) return bf ? launch_bwd_varlen_seq<64, true, __nv_bfloat16>(p, s) : launch_bwd_varlen_seq<64, true, __half>(p, s);
   return bf ? launch_bwd_varlen_seq<64, false, __nv_bfloat16>(p, s) : launch_bwd_varlen_seq<64, false, __half>(p, s);
+}
+
+extern "C" int sab_qk_int8_attn_bwd_varlen_seq(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
+                                               const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                               const float* lse, const void* k_mean, void* dq, void* dk, void* dv, void* workspace,
+                                               int dtype, int nseq, int Hq, int Hkv, int Tq, int Tk, int D, int64_t q8_stride_t,
+                                               int64_t q8_stride_h, int64_t k8_stride_t, int64_t k8_stride_h, int64_t q_stride_t,
+                                               int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h, int64_t v_stride_t,
+                                               int64_t v_stride_h, int64_t o_stride_t, int64_t o_stride_h, int64_t do_stride_t,
+                                               int64_t do_stride_h, const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
+                                               const int32_t* cu_q_scale, const int32_t* cu_k_scale, int max_seqlen_q,
+                                               int max_seqlen_k, int is_causal, int q_gran, int k_gran, float sm_scale, void* stream) {
+  return bwd_varlen_seq(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, dtype, nseq, Hq, Hkv, Tq,
+                        Tk, D, q8_stride_t, q8_stride_h, k8_stride_t, k8_stride_h, q_stride_t, q_stride_h, k_stride_t, k_stride_h,
+                        v_stride_t, v_stride_h, o_stride_t, o_stride_h, do_stride_t, do_stride_h, cu_seqlens_q, cu_seqlens_k,
+                        cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, is_causal, q_gran, k_gran, sm_scale, nullptr, stream);
+}
+
+extern "C" int sab_qk_int8_attn_bwd_varlen_window(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale,
+                                                  const float* k_scale, const void* q, const void* k, const void* v, const void* o,
+                                                  const void* dout, const float* lse, const void* k_mean, void* dq, void* dk, void* dv,
+                                                  void* workspace, int dtype, int nseq, int Hq, int Hkv, int Tq, int Tk, int D,
+                                                  int64_t q8_stride_t, int64_t q8_stride_h, int64_t k8_stride_t, int64_t k8_stride_h,
+                                                  int64_t q_stride_t, int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h,
+                                                  int64_t v_stride_t, int64_t v_stride_h, int64_t o_stride_t, int64_t o_stride_h,
+                                                  int64_t do_stride_t, int64_t do_stride_h, const int32_t* cu_seqlens_q,
+                                                  const int32_t* cu_seqlens_k, const int32_t* cu_q_scale, const int32_t* cu_k_scale,
+                                                  int max_seqlen_q, int max_seqlen_k, int is_causal, int q_gran, int k_gran,
+                                                  float sm_scale, int window_left, int window_right, void* stream) {
+  if (int e = sab::check_window_varlen(window_left, window_right, max_seqlen_q, max_seqlen_k)) return e;
+  const sab::Window w{window_left, window_right};
+  return bwd_varlen_seq(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, dtype, nseq, Hq, Hkv, Tq,
+                        Tk, D, q8_stride_t, q8_stride_h, k8_stride_t, k8_stride_h, q_stride_t, q_stride_h, k_stride_t, k_stride_h,
+                        v_stride_t, v_stride_h, o_stride_t, o_stride_h, do_stride_t, do_stride_h, cu_seqlens_q, cu_seqlens_k,
+                        cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, is_causal, q_gran, k_gran, sm_scale, &w, stream);
 }

@@ -167,6 +167,26 @@ inline int check_window(int& left, int& right, int is_causal, int Sq, int Skv) {
   return SAB_OK;
 }
 
+// Host: the packed window entries' checks (sab_qk_int8_sv_f8_attn_varlen_window / sab_qk_int8_attn_bwd_varlen_window).  Causal is
+// top-left inside each sequence and needs no Lq == Lk.  A side is clamped at the longest sequence (max_q rows, max_k keys) so
+// that the kernels' index arithmetic stays in int32; each kernel then clamps it again at its own sequence's lengths
+// (seq_window), which is what the dense entry does for that sequence alone.
+inline int check_window_varlen(int& left, int& right, int max_q, int max_k) {
+  SAB_REQUIRE(left >= -1 && right >= -1, SAB_ERR_INVALID, "window_size sides must be >= -1 (-1: unbounded), got (%d, %d)", left,
+              right);
+  SAB_REQUIRE(max_q > 0 && max_k > 0, SAB_ERR_INVALID, "the packed window needs a query bound and a key bound > 0 (got %d, %d)",
+              max_q, max_k);
+  if (left >= max_q) left = -1;
+  if (right >= max_k) right = -1;
+  return SAB_OK;
+}
+
+// Device: the window a packed sequence of q_len rows and kv_len keys sees, clamped as check_window clamps it for the dense call
+// on that sequence.  The clamp keeps the visibility and decides which tiles take the masked path (tile_setup in attn.cu).
+__device__ __forceinline__ Window seq_window(const Window& w, int q_len, int kv_len) {
+  return Window{w.left >= q_len ? -1 : w.left, w.right >= kv_len ? -1 : w.right};
+}
+
 // Host: opt a kernel into its dynamic shared-memory size once PER DEVICE (cudaFuncSetAttribute applies to the current
 // device only; a process that drives several GPUs — sageattn_host(device=...), tests — must set it on each).
 template <typename Kern>

@@ -683,6 +683,75 @@ def _(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, d
     return None
 
 
+@torch.library.custom_op("sageattention_b200::qk_int8_sv_f8_attn_varlen_window", mutates_args=("output",), device_types="cuda")
+def qk_int8_sv_f8_attn_varlen_window(query: torch.Tensor, key: torch.Tensor, value: torch.Tensor, output: torch.Tensor,
+                                     query_scale: torch.Tensor, key_scale: torch.Tensor, value_scale: torch.Tensor,
+                                     value_mean: Optional[torch.Tensor], cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor,
+                                     cu_pad_v: torch.Tensor, cu_q_scale: torch.Tensor, cu_k_scale: torch.Tensor, max_seqlen_q: int,
+                                     window_left: int, window_right: int, is_causal: int, q_quant_gran: int, k_quant_gran: int,
+                                     sm_scale: float, return_lse: int) -> torch.Tensor:
+    """qk_int8_sv_f8_attn_varlen_seq restricted to a sliding window inside each sequence (include/sageattn_b200.h,
+    sab_qk_int8_sv_f8_attn_varlen_window); window_left / window_right must fit in a C int (the entry point clamps them first).
+    Returns the [Hq,Tq] log2 LSE when return_lse, else an empty tensor; a row with no visible key gets 0 and lse -inf."""
+    Tq, Hq, D = query.shape
+    Tk, Hkv, _ = key.shape
+    lse = torch.empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32, device=query.device)
+    with torch.cuda.device(query.device):
+        check(lib().sab_qk_int8_sv_f8_attn_varlen_window(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
+                                                         lse.data_ptr() if return_lse else None, query_scale.data_ptr(),
+                                                         key_scale.data_ptr(), value_scale.data_ptr(), _ptr(value_mean), _dt(output),
+                                                         cu_seqlens_q.numel() - 1, Hq, Hkv, Tq, Tk, D, query.stride(0), query.stride(1),
+                                                         key.stride(0), key.stride(1), _v_pad(value), output.stride(0), output.stride(1),
+                                                         is_causal, q_quant_gran, k_quant_gran, float(sm_scale), cu_seqlens_q.data_ptr(),
+                                                         cu_seqlens_k.data_ptr(), cu_pad_v.data_ptr(), cu_q_scale.data_ptr(),
+                                                         cu_k_scale.data_ptr(), max_seqlen_q, window_left, window_right, _stream(query)))
+    return lse
+
+
+@qk_int8_sv_f8_attn_varlen_window.register_fake
+def _(query, key, value, output, query_scale, key_scale, value_scale, value_mean, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale,
+      cu_k_scale, max_seqlen_q, window_left, window_right, is_causal, q_quant_gran, k_quant_gran, sm_scale, return_lse):
+    Tq, Hq, _ = query.shape
+    return query.new_empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32)
+
+
+@torch.library.custom_op("sageattention_b200::qk_int8_attn_bwd_varlen_window", mutates_args=("dq", "dk", "dv"), device_types="cuda")
+def qk_int8_attn_bwd_varlen_window(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale: torch.Tensor, k_scale: torch.Tensor,
+                                   q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, o: torch.Tensor, dout: torch.Tensor,
+                                   lse: torch.Tensor, k_mean: Optional[torch.Tensor], dq: torch.Tensor, dk: torch.Tensor,
+                                   dv: torch.Tensor, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor, cu_q_scale: torch.Tensor,
+                                   cu_k_scale: torch.Tensor, max_seqlen_q: int, max_seqlen_k: int, window_left: int,
+                                   window_right: int, is_causal: int, q_quant_gran: int, k_quant_gran: int, sm_scale: float) -> None:
+    """Gradients of qk_int8_sv_f8_attn_varlen_window (include/sageattn_b200.h, sab_qk_int8_attn_bwd_varlen_window): the arguments
+    of qk_int8_attn_bwd_varlen_seq plus the window the forward received."""
+    Tq, Hq, D = q.shape
+    Tk, Hkv, _ = k.shape
+    nseq = cu_seqlens_q.numel() - 1
+    for x, y in ((dq, q), (dk, k), (dv, v)):
+        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
+    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (Hq, Tq), "lse must be [Hq,Tq] fp32"
+    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in (t.stride(0), t.stride(1))]
+    if k_mean is not None:
+        assert k_mean.numel() == nseq * Hkv * D and k_mean.dtype == k.dtype, "k_mean must have nseq*Hkv*D elements of k's dtype"
+        k_mean = k_mean.reshape(nseq, Hkv, D).contiguous()
+    with torch.cuda.device(q.device):
+        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(1, Hq, Tq), dtype=torch.uint8, device=q.device)
+        check(lib().sab_qk_int8_attn_bwd_varlen_window(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(), k_scale.data_ptr(),
+                                                       q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(),
+                                                       lse.data_ptr(), _ptr(k_mean), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
+                                                       ws.data_ptr(), _dt(q), nseq, Hq, Hkv, Tq, Tk, D, *strides, cu_seqlens_q.data_ptr(),
+                                                       cu_seqlens_k.data_ptr(), cu_q_scale.data_ptr(), cu_k_scale.data_ptr(),
+                                                       max_seqlen_q, max_seqlen_k, is_causal, q_quant_gran, k_quant_gran,
+                                                       float(sm_scale), window_left, window_right, _stream(q)))
+
+
+@qk_int8_attn_bwd_varlen_window.register_fake
+def _(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, cu_seqlens_q, cu_seqlens_k, cu_q_scale, cu_k_scale,
+      max_seqlen_q, max_seqlen_k, window_left, window_right, is_causal, q_quant_gran, k_quant_gran, sm_scale):
+    return None
+
+
 # ----------------------------------------------------------------------------------------------- block-mask prediction
 @torch.library.custom_op("sageattention_b200::block_stats", mutates_args=("mean", "sim"), device_types="cuda")
 def block_stats(x: torch.Tensor, mean: torch.Tensor, sim: torch.Tensor, tensor_layout: int, block_size: int) -> None:

@@ -511,6 +511,60 @@ int sab_qk_int8_attn_bwd_varlen_window(const int8_t* q_int8, const int8_t* k_int
                                        int max_seqlen_q, int max_seqlen_k, int is_causal, int q_gran, int k_gran, float sm_scale,
                                        int window_left, int window_right, void* stream);
 
+/* Block-sparse forms of the packed per-sequence INT8+FP8 attention (no reference counterpart): sab_qk_int8_sv_f8_attn_varlen and
+ * sab_qk_int8_attn_bwd_varlen_seq with the block mask of sab_qk_int8_sv_f8_attn_blocksparse, applied inside each sequence.
+ *   block_mask : bool (uint8, 0 = hidden) [nseq or 1, Hq or 1, ceil(max_seqlen_q/128), ceil(max_seqlen_k/64)] read through the
+ *                element strides mask_stride_b / _h / _qb / _kb (0 broadcasts a dimension; indexed by the Q head).  Sequence b's
+ *                blocks start at its own first token, as its INT8 blocks do; entries past its own ceil(Lq_b/128) x ceil(Lk_b/64)
+ *                blocks are never read.
+ *   Key j of sequence b is visible to its query i iff block_mask[b, h, i/128, j/64], j < Lk_b, and j <= i when is_causal (top-left
+ *   inside the sequence, Lq != Lk allowed).  Sequence b gets the bits of the dense block-sparse entry on that sequence alone with
+ *   mask slice [b, :, :ceil(Lq_b/128), :ceil(Lk_b/64)], forward and gradient; with an all-visible mask, the bits of the entries
+ *   without a mask.  A row with no visible key returns 0 and lse -inf and gets zero gradients; keys no row sees get zero dk and dv.
+ *   max_seqlen_k <= 1048576 (each CTA keeps its list of visible key blocks in shared memory, 2 bytes per 64-key block of the longest
+ *   sequence).  Refused before anything touches the device: a null mask, negative strides, per-block Q scales, max_seqlen_k >
+ *   1048576, missing sequence tables. */
+int sab_qk_int8_sv_f8_attn_varlen_blocksparse(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out, float* lse,
+                                              const float* q_scale, const float* k_scale, const float* v_scale, const float* v_mean,
+                                              int out_dtype, int nseq, int Hq, int Hkv, int Tq, int Tk, int D, int64_t q_stride_t,
+                                              int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h, int64_t v_t_pad,
+                                              int64_t o_stride_t, int64_t o_stride_h, int is_causal, int q_gran, int k_gran,
+                                              float sm_scale, const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
+                                              const int32_t* cu_pad_v, const int32_t* cu_q_scale, const int32_t* cu_k_scale,
+                                              int max_seqlen_q, int max_seqlen_k, const uint8_t* block_mask, int64_t mask_stride_b,
+                                              int64_t mask_stride_h, int64_t mask_stride_qb, int64_t mask_stride_kb, void* stream);
+int sab_qk_int8_attn_bwd_varlen_blocksparse(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
+                                            const void* q, const void* k, const void* v, const void* o, const void* dout,
+                                            const float* lse, const void* k_mean, void* dq, void* dk, void* dv, void* workspace,
+                                            int dtype, int nseq, int Hq, int Hkv, int Tq, int Tk, int D, int64_t q8_stride_t,
+                                            int64_t q8_stride_h, int64_t k8_stride_t, int64_t k8_stride_h, int64_t q_stride_t,
+                                            int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h, int64_t v_stride_t,
+                                            int64_t v_stride_h, int64_t o_stride_t, int64_t o_stride_h, int64_t do_stride_t,
+                                            int64_t do_stride_h, const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
+                                            const int32_t* cu_q_scale, const int32_t* cu_k_scale, int max_seqlen_q, int max_seqlen_k,
+                                            int is_causal, int q_gran, int k_gran, float sm_scale, const uint8_t* block_mask,
+                                            int64_t mask_stride_b, int64_t mask_stride_h, int64_t mask_stride_qb,
+                                            int64_t mask_stride_kb, void* stream);
+
+/* Packed forms of the block-mask prediction (no reference counterpart): sab_block_stats and sab_predict_block_mask of every packed
+ * sequence on its own.  Inputs and sequence tables as the packed entries above (cu_seqlens int32 device, max_seqlen >= every length).
+ * sab_block_stats_varlen: x packed [T,H,D]; blocks of blk rows restart at each sequence's first token.  mean [nseq,H,nblk,D] and
+ *   sim [nseq,H,nblk] contiguous fp32 with nblk = ceil(max_seqlen/blk); block c of sequence b gets the bits of sab_block_stats on
+ *   that sequence alone, and blocks past the end of a sequence get 0.  Checks of sab_block_stats.
+ * sab_predict_block_mask_varlen: statistics from sab_block_stats_varlen (q: blk 128, k: blk 64); block_mask bool bytes
+ *   [nseq,Hq,ceil(max_seqlen_q/128),ceil(max_seqlen_k/64)] contiguous.  Slice [b, :, :ceil(Lq_b/128), :ceil(Lk_b/64)] is the bits
+ *   of sab_predict_block_mask on sequence b alone (each sequence sorts on its own power-of-two length, so its prefix masses are
+ *   summed in the dense call's order); every other byte is 0, and so is every byte of a sequence without queries or keys.  Causal
+ *   is top-left inside each sequence with the same rules, Lq != Lk allowed.  The lengths are read on the device.  Checks of
+ *   sab_predict_block_mask (with max_seqlen_k for kv_len), except that causal needs no Lq == Lk; missing sequence tables are
+ *   refused too. */
+int sab_block_stats_varlen(const void* x, int dtype, float* mean, float* sim, const int32_t* cu_seqlens, int nseq, int max_seqlen,
+                           int H, int D, int64_t stride_t, int64_t stride_h, int blk, void* stream);
+int sab_predict_block_mask_varlen(const float* q_mean, const float* q_sim, const float* k_mean, const float* k_sim,
+                                  uint8_t* block_mask, const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k, int nseq, int Hq,
+                                  int Hkv, int max_seqlen_q, int max_seqlen_k, int D, int is_causal, float sm_scale,
+                                  float cdf_threshold, float sim_threshold, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -70,8 +70,14 @@ EXPORTS = {
                                              [c_void_p] * 5 + [c_int, c_int, c_int, c_void_p]),
     "sab_qk_int8_attn_bwd_varlen_window": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_int64] * 14 + [c_void_p] * 4 +
                                            [c_int] * 5 + [c_float, c_int, c_int, c_void_p]),
+    "sab_qk_int8_sv_f8_attn_varlen_blocksparse": (c_int, [c_void_p] * 9 + [c_int] * 7 + [c_int64] * 7 + [c_int, c_int, c_int, c_float] +
+                                                  [c_void_p] * 5 + [c_int, c_int, c_void_p] + [c_int64] * 4 + [c_void_p]),
+    "sab_qk_int8_attn_bwd_varlen_blocksparse": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_int64] * 14 + [c_void_p] * 4 +
+                                                [c_int] * 5 + [c_float, c_void_p] + [c_int64] * 4 + [c_void_p]),
     "sab_block_stats": (c_int, [c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 4 + [c_int64] * 3 + [c_int, c_void_p]),
     "sab_predict_block_mask": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_float] * 3 + [c_void_p]),
+    "sab_block_stats_varlen": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 4 + [c_int64] * 2 + [c_int, c_void_p]),
+    "sab_predict_block_mask_varlen": (c_int, [c_void_p] * 7 + [c_int] * 7 + [c_float] * 3 + [c_void_p]),
 }
 
 _lib = None

@@ -18,6 +18,7 @@ from .quant import (k_mean, per_block_int8, per_warp_int8, per_thread_int8, per_
                     quant_q_int8_varlen, quant_k_int8_varlen, per_channel_fp8_varlen_seq)
 
 _LOG2E = 1.44269504
+_MAX_BLOCKSPARSE_KV = 1 << 20   # 64 * 16384 key blocks: the longest key range a block-sparse CTA compacts in shared memory
 
 
 def _check_inputs(q, k, v):
@@ -518,10 +519,11 @@ def _quant_qk_varlen_f8(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seql
 
 
 def _attn_varlen_f8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale, smooth_k,
-                    smooth_v, v_range, return_lse, window=None):
+                    smooth_v, v_range, return_lse, block_mask=None, window=None):
     """Quantisers + INT8+FP8 kernel of sageattn_varlen_qk_int8_pv_fp8_cuda on head-dim-padded packed q, k, v (cu_seqlens int32):
     (o, the kernel's [Hq,Tq] log2 lse or an empty tensor, km).  window: the (left, right) of sageattn_varlen_window, checked and
-    clamped by the caller; the quantisers still see every key of each sequence."""
+    clamped by the caller; block_mask: the [nseq,Hq,.,.] bool view of sageattn_varlen_blocksparse, checked and expanded by the
+    caller.  The quantisers still see every key of each sequence."""
     km, q_int8, q_scale, cu_q_scale, k_int8, k_scale, cu_k_scale = _quant_qk_varlen_f8(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q,
                                                                                      max_seqlen_k, qk_quant_gran, smooth_k)
     v_fp8, v_scale, vm, cu_pad = per_channel_fp8_varlen_seq(v, cu_seqlens_k, max_seqlen_k, v_range, smooth_v)
@@ -531,6 +533,11 @@ def _attn_varlen_f8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqle
         return o, ops.qk_int8_sv_f8_attn_varlen_window(q_int8, k_int8, v_fp8, o, q_scale, k_scale, v_scale, vm, cu_seqlens_q, cu_seqlens_k,
                                                        cu_pad, cu_q_scale, cu_k_scale, max_seqlen_q, window[0], window[1],
                                                        1 if is_causal else 0, gran, gran, sm_scale, 1 if return_lse else 0), km
+    if block_mask is not None:
+        return o, ops.qk_int8_sv_f8_attn_varlen_blocksparse(q_int8, k_int8, v_fp8, o, q_scale, k_scale, v_scale, vm, cu_seqlens_q,
+                                                            cu_seqlens_k, cu_pad, cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k,
+                                                            block_mask, 1 if is_causal else 0, gran, gran, sm_scale,
+                                                            1 if return_lse else 0), km
     lse = ops.qk_int8_sv_f8_attn_varlen_seq(q_int8, k_int8, v_fp8, o, q_scale, k_scale, v_scale, vm, cu_seqlens_q, cu_seqlens_k, cu_pad,
                                             cu_q_scale, cu_k_scale, max_seqlen_q, 1 if is_causal else 0, gran, gran, sm_scale,
                                             1 if return_lse else 0)
@@ -560,14 +567,15 @@ class _SageAttnVarlenFp8Function(torch.autograd.Function):
     LSE enabled; saves q, k, v, o, the LSE and the cu_seqlens.  backward: re-runs the per-sequence K mean and Q/K quantisers, then
     the gradient kernels.  Tokens past cu_seqlens[-1] belong to no sequence: their gradient is zero.  The LSE and the K means are
     returned for the LSE correction and carry no gradient.  window (sageattn_varlen_window): P = 0 outside each sequence's window,
-    and the window gradient kernels visit only the tiles inside it."""
+    and the window gradient kernels visit only the tiles inside it.  block_mask (sageattn_varlen_blocksparse): P = 0 on each
+    sequence's hidden tiles, and the block-sparse gradient kernels visit only the visible ones; the mask has no gradient."""
 
     @staticmethod
     def forward(ctx, q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale, smooth_k,
-                smooth_v, v_range, window=None):
+                smooth_v, v_range, block_mask=None, window=None):
         o, lse, km = _attn_varlen_f8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale,
-                                     smooth_k, smooth_v, v_range, True, window)
-        ctx.save_for_backward(q, k, v, o, lse, cu_seqlens_q, cu_seqlens_k)
+                                     smooth_k, smooth_v, v_range, True, block_mask, window)
+        ctx.save_for_backward(q, k, v, o, lse, cu_seqlens_q, cu_seqlens_k, block_mask)
         ctx.cfg = (max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale, smooth_k)
         ctx.window = window
         km = km if km is not None else q.new_empty(0)
@@ -577,7 +585,7 @@ class _SageAttnVarlenFp8Function(torch.autograd.Function):
     @staticmethod
     def backward(ctx, do, _dlse, _dkm):
         max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale, smooth_k = ctx.cfg
-        q, k, v, o, lse, cu_seqlens_q, cu_seqlens_k = ctx.saved_tensors
+        q, k, v, o, lse, cu_seqlens_q, cu_seqlens_k, block_mask = ctx.saved_tensors
         km, q_int8, q_scale, cu_q_scale, k_int8, k_scale, cu_k_scale = _quant_qk_varlen_f8(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q,
                                                                                          max_seqlen_k, qk_quant_gran, smooth_k)
         # the kernels read 16-bit rows with 16-byte loads; dq / dk / dv take the strides of q / k / v
@@ -588,11 +596,15 @@ class _SageAttnVarlenFp8Function(torch.autograd.Function):
             ops.qk_int8_attn_bwd_varlen_window(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv, cu_seqlens_q,
                                                cu_seqlens_k, cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, ctx.window[0],
                                                ctx.window[1], 1 if is_causal else 0, gran, gran, sm_scale)
+        elif block_mask is not None:
+            ops.qk_int8_attn_bwd_varlen_blocksparse(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv, cu_seqlens_q,
+                                                    cu_seqlens_k, cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, block_mask,
+                                                    1 if is_causal else 0, gran, gran, sm_scale)
         else:
             ops.qk_int8_attn_bwd_varlen_seq(q_int8, k_int8, q_scale, k_scale, q, k, v, o, do, lse, km, dq, dk, dv, cu_seqlens_q,
                                             cu_seqlens_k, cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, 1 if is_causal else 0, gran,
                                             gran, sm_scale)
-        return dq, dk, dv, None, None, None, None, None, None, None, None, None, None, None
+        return dq, dk, dv, None, None, None, None, None, None, None, None, None, None, None, None
 
 
 def _check_cu_seqlens(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k):
@@ -676,10 +688,61 @@ def sageattn_varlen_window(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu
                                   pv_accum_dtype, smooth_k, smooth_v, return_lse, window)
 
 
+def _varlen_block_mask(block_mask, q, cu_seqlens_q, max_seqlen_q, max_seqlen_k):
+    """block_mask of sageattn_varlen_blocksparse checked against the packed batch and expanded to [nseq,Hq,nqb,nkb], or
+    ValueError (the wording of sageattn_blocksparse).  max_seqlen_k is limited to MAX_KV_LEN: each CTA compacts one mask row of
+    ceil(max_seqlen_k/64) blocks in shared memory."""
+    nseq, Hq = cu_seqlens_q.numel() - 1, q.size(1)
+    nqb, nkb = (max_seqlen_q + 127) // 128, (max_seqlen_k + 63) // 64
+    if block_mask.dim() != 4 or tuple(block_mask.shape[2:]) != (nqb, nkb):
+        raise ValueError(f"block_mask shape {tuple(block_mask.shape)} must be [nseq or 1, Hq or 1, {nqb}, {nkb}] "
+                         f"(ceil(max_seqlen_q/128), ceil(max_seqlen_k/64))")
+    if block_mask.size(0) not in (1, nseq) or block_mask.size(1) not in (1, Hq):
+        raise ValueError(f"block_mask shape {tuple(block_mask.shape)} cannot be broadcast to [{nseq}, {Hq}, {nqb}, {nkb}]")
+    if max_seqlen_k > _MAX_BLOCKSPARSE_KV:
+        raise ValueError(f"the block-sparse path supports max_seqlen_k <= {_MAX_BLOCKSPARSE_KV} (got {max_seqlen_k})")
+    return block_mask.expand(nseq, Hq, nqb, nkb)
+
+
+def sageattn_varlen_blocksparse(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu_seqlens_q: torch.Tensor,
+                                cu_seqlens_k: torch.Tensor, max_seqlen_q: int, max_seqlen_k: int, block_mask: torch.Tensor,
+                                is_causal: bool = False, qk_quant_gran: str = "per_thread", sm_scale: Optional[float] = None,
+                                pv_accum_dtype: str = "fp32+fp16", smooth_k: bool = True, smooth_v: bool = False,
+                                return_lse: bool = False):
+    """Block-sparse attention on packed sequences (no reference counterpart): sageattn_varlen_qk_int8_pv_fp8_cuda with the block
+    mask of sageattn_blocksparse applied inside each sequence.  The options, checks, warnings, V ranges and packed layout are
+    those of sageattn_varlen_qk_int8_pv_fp8_cuda (GQA, int32 / int64 cu_seqlens, empty sequences, max_seqlen_* >= every length).
+
+    block_mask: torch.bool on q's device, shape [nseq or 1, Hq or 1, ceil(max_seqlen_q/128), ceil(max_seqlen_k/64)] (size-1
+    dimensions broadcast, any strides), indexed by the Q head under GQA.  Key j of sequence b is visible to its query i iff
+    block_mask[b, h, i // 128, j // 64], with the blocks of each sequence starting at its own first token (as its INT8 blocks do),
+    and j <= i when is_causal.  Entries past sequence b's own ceil(Lq_b/128) x ceil(Lk_b/64) blocks are ignored.  A wrong shape
+    raises ValueError before any launch; max_seqlen_k <= 1048576.  The mask costs nseq * Hq * ceil(max_seqlen_q/128) *
+    ceil(max_seqlen_k/64) bytes when not broadcast (about 6 MB for six sequences of up to 16384 tokens and 32 heads).
+
+    Contract: "sageattn_blocksparse, per sequence".  Sequence b's output rows are the bits of sageattn_blocksparse(q_b[None],
+    k_b[None], v_b[None], block_mask[b, :, :nq_b, :nk_b][None], tensor_layout="NHD", <same options>) for every sequence the dense
+    call accepts (non-causal, or causal with Lq == Lk); every statistic is per sequence.  is_causal is top-left inside each
+    sequence, Lq != Lk allowed (no dense counterpart): key j is visible to query i iff the mask allows tile (i // 128, j // 64)
+    and j <= i.  With an all-True mask the result (o, lse, dq, dk, dv) is that of sageattn_varlen_qk_int8_pv_fp8_cuda to the bit.
+
+    A row with no visible key gives 0 and lse -inf; rows past cu_seqlens_q[-1] are not written.  return_lse gives [Hq,Tq] in
+    natural-log units with sageattn_varlen_qk_int8_pv_fp8_cuda's caveat: the kernel's LSE is exact, the per-token K-mean correction
+    within one unit.  Differentiable when grad mode is on and q, k or v requires grad: for every sequence, dq / dk / dv are the bits
+    of the dense block-sparse backward of the one-sequence call; tokens past the end, keys of a sequence without queries and keys
+    hidden from every row get zero gradients.  The mask has no gradient."""
+    _check_inputs(q, k, v)
+    assert isinstance(block_mask, torch.Tensor) and block_mask.dtype == torch.bool, "block_mask must be a torch.bool tensor."
+    assert block_mask.device == q.device, "All tensors must be on the same device."
+    return _varlen_qk_int8_pv_fp8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale,
+                                  pv_accum_dtype, smooth_k, smooth_v, return_lse, block_mask=block_mask)
+
+
 def _varlen_qk_int8_pv_fp8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, qk_quant_gran, sm_scale,
-                           pv_accum_dtype, smooth_k, smooth_v, return_lse, window=None):
+                           pv_accum_dtype, smooth_k, smooth_v, return_lse, window=None, block_mask=None):
     """Body of sageattn_varlen_qk_int8_pv_fp8_cuda after _check_inputs; window: the (left, right) of sageattn_varlen_window, checked
-    by the caller (_check_window_size) and clamped here (_varlen_window_arg)."""
+    by the caller (_check_window_size) and clamped here (_varlen_window_arg); block_mask: the mask of sageattn_varlen_blocksparse,
+    checked and expanded here (_varlen_block_mask) once the sequence tables are."""
     assert qk_quant_gran in ["per_warp", "per_thread"], "qk_quant_gran must be either 'per_warp' or 'per_thread'."
     if pv_accum_dtype not in ("fp32", "fp32+fp32", "fp32+fp16"):
         raise ValueError(f"Unsupported pv_accum_dtype: {pv_accum_dtype}")
@@ -688,6 +751,8 @@ def _varlen_qk_int8_pv_fp8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, ma
         raise ValueError(f"k and v must have the same shape (got {tuple(k.shape)} and {tuple(v.shape)})")
     if q.size(1) % k.size(1) != 0:
         raise ValueError(f"num_qo_heads ({q.size(1)}) must be divisible by num_kv_heads ({k.size(1)})")
+    if block_mask is not None:
+        block_mask = _varlen_block_mask(block_mask, q, cu_seqlens_q, int(max_seqlen_q), int(max_seqlen_k))
     q, k, v, head_dim_og = _pad_head_dim(q, k, v)
     assert q.stride(-1) == 1 and k.stride(-1) == 1 and v.stride(-1) == 1, "Last dim of qkv must be contiguous."
     if sm_scale is None:
@@ -701,10 +766,10 @@ def _varlen_qk_int8_pv_fp8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, ma
     cu_q, cu_k = cu_seqlens_q.to(torch.int32).contiguous(), cu_seqlens_k.to(torch.int32).contiguous()
     args = (cu_q, cu_k, int(max_seqlen_q), int(max_seqlen_k), is_causal, qk_quant_gran, sm_scale, smooth_k, smooth_v, v_range)
     if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
-        o, lse, km = _SageAttnVarlenFp8Function.apply(q, k, v, *args, window)
+        o, lse, km = _SageAttnVarlenFp8Function.apply(q, k, v, *args, block_mask, window)
         q = q.detach()
     else:
-        o, lse, km = _attn_varlen_f8(q, k, v, *args, return_lse, window)
+        o, lse, km = _attn_varlen_f8(q, k, v, *args, return_lse, block_mask, window)
     o = o[..., :head_dim_og]
     if return_lse:
         if smooth_k:

@@ -111,6 +111,9 @@ constexpr bool kSparse = kMask && !kPV16;     // block mask of the INT8+FP8 path
 // varlen forms read one [Hkv,D] table for the whole packed batch.
 // kWindow with kSeqV: the packed window form.  Each sequence sees the window clamped at its own lengths (seq_window), so its rows
 // take the dense window kernel's path on that sequence alone, tile for tile.
+// kMask (block-sparse) with kSeqV: the packed block-sparse form.  b is the sequence and qt its own Q tile, so the CTA compacts mask
+// row (b, h, qt) of a [nseq,Hq,ceil(max_seqlen_q/128),ceil(max_seqlen_k/64)] mask, cut at its sequence's n_kv and causal horizon:
+// the dense block-sparse kernel's path on that sequence alone.
 template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false, bool kWindow = false, bool kSeqV = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
@@ -695,14 +698,15 @@ static int launch_attn_seqv(const CUtensorMap& tq, const CUtensorMap& tk, const 
   return SAB_OK;
 }
 
-// the block-sparse form (sage_attn_fwd_kernel<D, kKT, OutT, false, true>): p.mask holds the block mask
-template <int D, bool kKT, typename OutT>
-static int launch_attn_blocksparse(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, AttnParams p,
+// the block-sparse form (sage_attn_fwd_kernel<D, kKT, OutT, false, true, false, kSeqV>): p.mask holds the block mask; kSeqV: the
+// packed form with per-sequence V statistics.  max_k: the longest key range a CTA compacts (Skv dense, max_seqlen_k packed).
+template <int D, bool kKT, typename OutT, bool kSeqV = false>
+static int launch_attn_blocksparse(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, AttnParams p, int max_k,
                                    dim3 grid, cudaStream_t stream) {
   p.lazy_tau = exact_max_mode() ? 0.0f : kLazyTau;
   constexpr size_t smem_max = attn_smem_bytes<D, false>() + kv_list_bytes(kMaxKvBlocks);
-  const size_t smem = attn_smem_bytes<D, false>() + kv_list_bytes((p.Sk + BN - 1) / BN);
-  auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, true>;
+  const size_t smem = attn_smem_bytes<D, false>() + kv_list_bytes((max_k + BN - 1) / BN);
+  auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, true, false, kSeqV>;
   static bool configured[64] = {};
   if (int st = ensure_dynamic_smem(kern, smem_max, configured)) return st;
   kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p, Window{-1, -1});
@@ -714,6 +718,9 @@ static int launch_attn_blocksparse(const CUtensorMap& tq, const CUtensorMap& tk,
 
 // block mask of the block-sparse entry point, handed to attn_entry by sab_qk_int8_sv_f8_attn_blocksparse (same thread)
 static thread_local const sab::BlockMask* tl_block_mask = nullptr;
+// with tl_block_mask, set by sab_qk_int8_sv_f8_attn_varlen_blocksparse (same thread): max_seqlen_k, which sizes each CTA's list of
+// visible key blocks (the packed Skv is the total key count)
+static thread_local int tl_block_mask_max_k = 0;
 // window of the sliding-window entry point, handed to attn_entry by sab_qk_int8_sv_f8_attn_window (same thread)
 static thread_local const sab::Window* tl_window = nullptr;
 // set by sab_qk_int8_sv_f8_attn_varlen (same thread): v_scale / v_mean are per sequence
@@ -830,20 +837,33 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
     p.seg_flags = tl_seg->flags; p.seg_epoch = tl_seg->epoch; p.seg_heads = tl_seg->heads_per_flag;   // polled by the producer
   }
   if (tl_block_mask != nullptr) {
-    SAB_REQUIRE(!pv16 && !varlen && kv_seg_len == 0 && causal_q_offset == 0, SAB_ERR_UNSUPPORTED,
-                "the block mask is supported by the dense single-GPU INT8/FP8 path only");
+    SAB_REQUIRE(!pv16 && (!varlen || tl_seq_v) && kv_seg_len == 0 && causal_q_offset == 0, SAB_ERR_UNSUPPORTED,
+                "the block mask is supported by the dense and the packed (per-sequence) single-GPU INT8/FP8 paths only");
     p.mask = tl_block_mask->ptr;
     p.mask_sb = tl_block_mask->sb; p.mask_sh = tl_block_mask->sh; p.mask_sm = tl_block_mask->sqb; p.mask_sn = tl_block_mask->skb;
-    if (D == 128) {
-      if (kt) return bf ? launch_attn_blocksparse<128, true, __nv_bfloat16>(tq, tk, tv, p, grid, s)
-                        : launch_attn_blocksparse<128, true, __half>(tq, tk, tv, p, grid, s);
-      return bf ? launch_attn_blocksparse<128, false, __nv_bfloat16>(tq, tk, tv, p, grid, s)
-                : launch_attn_blocksparse<128, false, __half>(tq, tk, tv, p, grid, s);
+    if (tl_seq_v) {
+      const int mk = tl_block_mask_max_k;
+      if (D == 128) {
+        if (kt) return bf ? launch_attn_blocksparse<128, true, __nv_bfloat16, true>(tq, tk, tv, p, mk, grid, s)
+                          : launch_attn_blocksparse<128, true, __half, true>(tq, tk, tv, p, mk, grid, s);
+        return bf ? launch_attn_blocksparse<128, false, __nv_bfloat16, true>(tq, tk, tv, p, mk, grid, s)
+                  : launch_attn_blocksparse<128, false, __half, true>(tq, tk, tv, p, mk, grid, s);
+      }
+      if (kt) return bf ? launch_attn_blocksparse<64, true, __nv_bfloat16, true>(tq, tk, tv, p, mk, grid, s)
+                        : launch_attn_blocksparse<64, true, __half, true>(tq, tk, tv, p, mk, grid, s);
+      return bf ? launch_attn_blocksparse<64, false, __nv_bfloat16, true>(tq, tk, tv, p, mk, grid, s)
+                : launch_attn_blocksparse<64, false, __half, true>(tq, tk, tv, p, mk, grid, s);
     }
-    if (kt) return bf ? launch_attn_blocksparse<64, true, __nv_bfloat16>(tq, tk, tv, p, grid, s)
-                      : launch_attn_blocksparse<64, true, __half>(tq, tk, tv, p, grid, s);
-    return bf ? launch_attn_blocksparse<64, false, __nv_bfloat16>(tq, tk, tv, p, grid, s)
-              : launch_attn_blocksparse<64, false, __half>(tq, tk, tv, p, grid, s);
+    if (D == 128) {
+      if (kt) return bf ? launch_attn_blocksparse<128, true, __nv_bfloat16>(tq, tk, tv, p, Skv, grid, s)
+                        : launch_attn_blocksparse<128, true, __half>(tq, tk, tv, p, Skv, grid, s);
+      return bf ? launch_attn_blocksparse<128, false, __nv_bfloat16>(tq, tk, tv, p, Skv, grid, s)
+                : launch_attn_blocksparse<128, false, __half>(tq, tk, tv, p, Skv, grid, s);
+    }
+    if (kt) return bf ? launch_attn_blocksparse<64, true, __nv_bfloat16>(tq, tk, tv, p, Skv, grid, s)
+                      : launch_attn_blocksparse<64, true, __half>(tq, tk, tv, p, Skv, grid, s);
+    return bf ? launch_attn_blocksparse<64, false, __nv_bfloat16>(tq, tk, tv, p, Skv, grid, s)
+              : launch_attn_blocksparse<64, false, __half>(tq, tk, tv, p, Skv, grid, s);
   }
   if (tl_window != nullptr) {
     SAB_REQUIRE(!pv16 && (!varlen || tl_seq_v) && kv_seg_len == 0 && causal_q_offset == 0, SAB_ERR_UNSUPPORTED,
@@ -1049,6 +1069,34 @@ extern "C" int sab_qk_int8_sv_f8_attn_varlen_window(const int8_t* q_int8, const 
                                                o_stride_h, is_causal, q_gran, k_gran, sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v,
                                                cu_q_scale, cu_k_scale, max_seqlen_q, stream);
   tl_window = nullptr;
+  return st;
+}
+
+extern "C" int sab_qk_int8_sv_f8_attn_varlen_blocksparse(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out,
+                                                         float* lse, const float* q_scale, const float* k_scale,
+                                                         const float* v_scale, const float* v_mean, int out_dtype, int nseq, int Hq,
+                                                         int Hkv, int Tq, int Tk, int D, int64_t q_stride_t, int64_t q_stride_h,
+                                                         int64_t k_stride_t, int64_t k_stride_h, int64_t v_t_pad, int64_t o_stride_t,
+                                                         int64_t o_stride_h, int is_causal, int q_gran, int k_gran, float sm_scale,
+                                                         const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
+                                                         const int32_t* cu_pad_v, const int32_t* cu_q_scale, const int32_t* cu_k_scale,
+                                                         int max_seqlen_q, int max_seqlen_k, const uint8_t* block_mask,
+                                                         int64_t mask_stride_b, int64_t mask_stride_h, int64_t mask_stride_qb,
+                                                         int64_t mask_stride_kb, void* stream) {
+  if (int st = sab::check_block_mask_varlen(block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb, q_gran,
+                                            max_seqlen_q, max_seqlen_k))
+    return st;
+  SAB_REQUIRE(cu_seqlens_q && cu_seqlens_k && cu_pad_v && cu_q_scale && cu_k_scale && nseq > 0, SAB_ERR_INVALID,
+              "the packed block mask needs cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale and nseq > 0");
+  const sab::BlockMask m{block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb};
+  tl_block_mask = &m;
+  tl_block_mask_max_k = max_seqlen_k;
+  const int st = sab_qk_int8_sv_f8_attn_varlen(q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq,
+                                               Hkv, Tq, Tk, D, q_stride_t, q_stride_h, k_stride_t, k_stride_h, v_t_pad, o_stride_t,
+                                               o_stride_h, is_causal, q_gran, k_gran, sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v,
+                                               cu_q_scale, cu_k_scale, max_seqlen_q, stream);
+  tl_block_mask = nullptr;
+  tl_block_mask_max_k = 0;
   return st;
 }
 

@@ -472,6 +472,14 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_varlen_window_kernel(co
   bwd_dq_tile<D, kKT, T, true, 0, false, true, true>(p, nullptr, nullptr, &w);
 }
 
+// the packed block-sparse form with a per-sequence K mean: sequence blockIdx.z compacts row (sequence, h, its own Q tile) of the
+// [nseq,Hq,.,.] mask, as the forward does; its dynamic shared memory adds kv_list_bytes(ceil(max_seqlen_k/64))
+template <int D, bool kKT, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dq_varlen_blocksparse_kernel(const __grid_constant__ BwdParams p,
+                                                                                    const __grid_constant__ BlockMask bm) {
+  bwd_dq_tile<D, kKT, T, true, 0, true, false, true>(p, nullptr, &bm);
+}
+
 // ------------------------------------------------------------------------------------------------ dK, dV
 template <int D>
 constexpr size_t bwd_dkdv_smem_bytes() {
@@ -563,7 +571,9 @@ __device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p, const BlockMas
         const int r = q0 + threadIdx.x;
         const bool ok = r < sq.q_len;
         const int64_t li = (int64_t(sq.tb) * a.Hq + h) * a.Sq + sq.q_off + r;
-        s_qss[threadIdx.x] = ok ? q_dequant_log2(a, qs_base, sq.q_blk0 + r / 128, r % 128) : 0.f;
+        int q_blk0 = sq.q_blk0;
+        if constexpr (kVarlen && kSparse) q_blk0 = *reinterpret_cast<const volatile int32_t*>(a.cu_qs + b);   // as k_off below
+        s_qss[threadIdx.x] = ok ? q_dequant_log2(a, qs_base, q_blk0 + r / 128, r % 128) : 0.f;
         if constexpr (kMask != 0 || kSparse || kWindow) s_nlse[threadIdx.x] = ok ? masked_nlse(p.lse[li]) : -INFINITY;
         else s_nlse[threadIdx.x] = ok ? -p.lse[li] : 0.f;
         s_dlt[threadIdx.x] = ok ? p.delta[li] : 0.f;
@@ -621,8 +631,12 @@ __device__ __forceinline__ void bwd_dkdv_tile(const BwdParams& p, const BlockMas
     }
   }
 
-  T* kb = reinterpret_cast<T*>(p.dk) + b * p.k_sb + hk * p.k_sh + sq.k_off * p.k_ss;
-  T* vb = reinterpret_cast<T*>(p.dv) + b * p.v_sb + hk * p.v_sh + sq.k_off * p.v_ss;
+  // the packed block-sparse form reads its sequence's first key (and, per step, its first Q scale block) again instead of
+  // holding them through the loop: at D = 128 those registers keep the kernel within 255 without a spill
+  int k_off = sq.k_off;
+  if constexpr (kVarlen && kSparse) k_off = *reinterpret_cast<const volatile int32_t*>(a.cu_k + b);
+  T* kb = reinterpret_cast<T*>(p.dk) + b * p.k_sb + hk * p.k_sh + k_off * p.k_ss;
+  T* vb = reinterpret_cast<T*>(p.dv) + b * p.v_sb + hk * p.v_sh + k_off * p.v_ss;
   const bool ok0 = key[0] < sq.kv_len, ok1 = key[1] < sq.kv_len;
   store_rows<T, D>(dk, kb + int64_t(key[0]) * p.k_ss, kb + int64_t(key[1]) * p.k_ss, ok0, ok1, t, p.sm_scale);
   store_rows<T, D>(dv, vb + int64_t(key[0]) * p.v_ss, vb + int64_t(key[1]) * p.v_ss, ok0, ok1, t, 1.0f);
@@ -658,6 +672,13 @@ __global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_varlen_window_kernel(
   const int b = blockIdx.z;
   const Window w = seq_window(win, p.a.cu_q[b + 1] - p.a.cu_q[b], p.a.cu_k[b + 1] - p.a.cu_k[b]);
   bwd_dkdv_tile<D, kKT, T, true, 0, false, true>(p, nullptr, &w);
+}
+
+// the packed block-sparse form: the mask bits of (sequence blockIdx.z, Q head, its own Q tile, its own key blocks)
+template <int D, bool kKT, typename T>
+__global__ void __launch_bounds__(kBwdThreads, 1) bwd_dkdv_varlen_blocksparse_kernel(const __grid_constant__ BwdParams p,
+                                                                                      const __grid_constant__ BlockMask bm) {
+  bwd_dkdv_tile<D, kKT, T, true, 0, true>(p, &bm);
 }
 
 // delta, then the dQ kernel kq (smem_q bytes, arguments p, q_args...) and the dK/dV kernel kkv (smem_kv bytes); cfg_*: their
@@ -707,16 +728,18 @@ static int launch_bwd_masked(const BwdParams& p, void* dbias, cudaStream_t strea
                                bwd_dkdv_smem_bytes<D>() + kMaskTileBytes, cfg_kv, stream, dbias);
 }
 
-template <int D, bool kKT, typename T>
-static int launch_bwd_blocksparse(const BwdParams& p, const BlockMask& bm, cudaStream_t stream) {
+// kVarlen: the packed form (grids sized from the longest sequence by the caller).  max_k: the longest key range a dQ CTA compacts
+// (Skv dense, max_seqlen_k packed).
+template <int D, bool kKT, typename T, bool kVarlen = false>
+static int launch_bwd_blocksparse(const BwdParams& p, const BlockMask& bm, int max_k, cudaStream_t stream) {
   static bool cfg_q[64] = {}, cfg_kv[64] = {};
   if (int st = launch_bwd_delta<T>(p, D, stream)) return st;
-  auto kq = bwd_dq_blocksparse_kernel<D, kKT, T>;
-  const size_t smem_q = bwd_dq_smem_bytes<D>() + kv_list_bytes((p.a.Sk + BN - 1) / BN);
+  auto kq = kVarlen ? bwd_dq_varlen_blocksparse_kernel<D, kKT, T> : bwd_dq_blocksparse_kernel<D, kKT, T>;
+  const size_t smem_q = bwd_dq_smem_bytes<D>() + kv_list_bytes((max_k + BN - 1) / BN);
   if (int st = ensure_dynamic_smem(kq, bwd_dq_smem_bytes<D>() + kv_list_bytes(kMaxKvBlocks), cfg_q)) return st;
   kq<<<dim3(p.a.n_q_tiles, p.a.Hq, p.a.B), kBwdThreads, smem_q, stream>>>(p, bm);
   SAB_CUDA_OK(cudaGetLastError());
-  auto kkv = bwd_dkdv_blocksparse_kernel<D, kKT, T>;
+  auto kkv = kVarlen ? bwd_dkdv_varlen_blocksparse_kernel<D, kKT, T> : bwd_dkdv_blocksparse_kernel<D, kKT, T>;
   if (int st = ensure_dynamic_smem(kkv, bwd_dkdv_smem_bytes<D>(), cfg_kv)) return st;
   kkv<<<dim3(p.n_k_tiles, p.a.Hkv, p.a.B), kBwdThreads, bwd_dkdv_smem_bytes<D>(), stream>>>(p, bm);
   SAB_CUDA_OK(cudaGetLastError());
@@ -949,11 +972,11 @@ extern "C" int sab_qk_int8_attn_bwd_blocksparse(const int8_t* q_int8, const int8
   const bool kt = k_gran == SAB_GRAN_PER_THREAD;
   const bool bf = dtype == SAB_DTYPE_BF16;
   if (D == 128) {
-    if (kt) return bf ? launch_bwd_blocksparse<128, true, __nv_bfloat16>(p, bm, s) : launch_bwd_blocksparse<128, true, __half>(p, bm, s);
-    return bf ? launch_bwd_blocksparse<128, false, __nv_bfloat16>(p, bm, s) : launch_bwd_blocksparse<128, false, __half>(p, bm, s);
+    if (kt) return bf ? launch_bwd_blocksparse<128, true, __nv_bfloat16>(p, bm, Skv, s) : launch_bwd_blocksparse<128, true, __half>(p, bm, Skv, s);
+    return bf ? launch_bwd_blocksparse<128, false, __nv_bfloat16>(p, bm, Skv, s) : launch_bwd_blocksparse<128, false, __half>(p, bm, Skv, s);
   }
-  if (kt) return bf ? launch_bwd_blocksparse<64, true, __nv_bfloat16>(p, bm, s) : launch_bwd_blocksparse<64, true, __half>(p, bm, s);
-  return bf ? launch_bwd_blocksparse<64, false, __nv_bfloat16>(p, bm, s) : launch_bwd_blocksparse<64, false, __half>(p, bm, s);
+  if (kt) return bf ? launch_bwd_blocksparse<64, true, __nv_bfloat16>(p, bm, Skv, s) : launch_bwd_blocksparse<64, true, __half>(p, bm, Skv, s);
+  return bf ? launch_bwd_blocksparse<64, false, __nv_bfloat16>(p, bm, Skv, s) : launch_bwd_blocksparse<64, false, __half>(p, bm, Skv, s);
 }
 
 extern "C" int sab_qk_int8_attn_bwd_window(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
@@ -994,7 +1017,8 @@ extern "C" int sab_qk_int8_attn_bwd_window(const int8_t* q_int8, const int8_t* k
   return bf ? launch_bwd_window<64, false, __nv_bfloat16>(p, w, s) : launch_bwd_window<64, false, __half>(p, w, s);
 }
 
-// sab_qk_int8_attn_bwd_varlen_seq and, with a window w (already checked), sab_qk_int8_attn_bwd_varlen_window
+// sab_qk_int8_attn_bwd_varlen_seq and, with a window w or a block mask bm (already checked), sab_qk_int8_attn_bwd_varlen_window /
+// sab_qk_int8_attn_bwd_varlen_blocksparse
 static int bwd_varlen_seq(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale, const void* q,
                           const void* k, const void* v, const void* o, const void* dout, const float* lse, const void* k_mean, void* dq,
                           void* dk, void* dv, void* workspace, int dtype, int nseq, int Hq, int Hkv, int Tq, int Tk, int D,
@@ -1003,7 +1027,7 @@ static int bwd_varlen_seq(const int8_t* q_int8, const int8_t* k_int8, const floa
                           int64_t o_stride_t, int64_t o_stride_h, int64_t do_stride_t, int64_t do_stride_h,
                           const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k, const int32_t* cu_q_scale,
                           const int32_t* cu_k_scale, int max_seqlen_q, int max_seqlen_k, int is_causal, int q_gran, int k_gran,
-                          float sm_scale, const sab::Window* w, void* stream) {
+                          float sm_scale, const sab::Window* w, const sab::BlockMask* bm, void* stream) {
   using namespace sab;
   SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
               SAB_ERR_INVALID, "null tensor pointer");
@@ -1039,6 +1063,19 @@ static int bwd_varlen_seq(const int8_t* q_int8, const int8_t* k_int8, const floa
     if (kt) return bf ? launch_bwd_window<64, true, __nv_bfloat16, true>(p, *w, s) : launch_bwd_window<64, true, __half, true>(p, *w, s);
     return bf ? launch_bwd_window<64, false, __nv_bfloat16, true>(p, *w, s) : launch_bwd_window<64, false, __half, true>(p, *w, s);
   }
+  if (bm != nullptr) {
+    const int mk = max_seqlen_k;
+    if (D == 128) {
+      if (kt) return bf ? launch_bwd_blocksparse<128, true, __nv_bfloat16, true>(p, *bm, mk, s)
+                        : launch_bwd_blocksparse<128, true, __half, true>(p, *bm, mk, s);
+      return bf ? launch_bwd_blocksparse<128, false, __nv_bfloat16, true>(p, *bm, mk, s)
+                : launch_bwd_blocksparse<128, false, __half, true>(p, *bm, mk, s);
+    }
+    if (kt) return bf ? launch_bwd_blocksparse<64, true, __nv_bfloat16, true>(p, *bm, mk, s)
+                      : launch_bwd_blocksparse<64, true, __half, true>(p, *bm, mk, s);
+    return bf ? launch_bwd_blocksparse<64, false, __nv_bfloat16, true>(p, *bm, mk, s)
+              : launch_bwd_blocksparse<64, false, __half, true>(p, *bm, mk, s);
+  }
   if (D == 128) {
     if (kt) return bf ? launch_bwd_varlen_seq<128, true, __nv_bfloat16>(p, s) : launch_bwd_varlen_seq<128, true, __half>(p, s);
     return bf ? launch_bwd_varlen_seq<128, false, __nv_bfloat16>(p, s) : launch_bwd_varlen_seq<128, false, __half>(p, s);
@@ -1060,7 +1097,8 @@ extern "C" int sab_qk_int8_attn_bwd_varlen_seq(const int8_t* q_int8, const int8_
   return bwd_varlen_seq(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, dtype, nseq, Hq, Hkv, Tq,
                         Tk, D, q8_stride_t, q8_stride_h, k8_stride_t, k8_stride_h, q_stride_t, q_stride_h, k_stride_t, k_stride_h,
                         v_stride_t, v_stride_h, o_stride_t, o_stride_h, do_stride_t, do_stride_h, cu_seqlens_q, cu_seqlens_k,
-                        cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, is_causal, q_gran, k_gran, sm_scale, nullptr, stream);
+                        cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, is_causal, q_gran, k_gran, sm_scale, nullptr, nullptr,
+                        stream);
 }
 
 extern "C" int sab_qk_int8_attn_bwd_varlen_window(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale,
@@ -1079,5 +1117,28 @@ extern "C" int sab_qk_int8_attn_bwd_varlen_window(const int8_t* q_int8, const in
   return bwd_varlen_seq(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, dtype, nseq, Hq, Hkv, Tq,
                         Tk, D, q8_stride_t, q8_stride_h, k8_stride_t, k8_stride_h, q_stride_t, q_stride_h, k_stride_t, k_stride_h,
                         v_stride_t, v_stride_h, o_stride_t, o_stride_h, do_stride_t, do_stride_h, cu_seqlens_q, cu_seqlens_k,
-                        cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, is_causal, q_gran, k_gran, sm_scale, &w, stream);
+                        cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, is_causal, q_gran, k_gran, sm_scale, &w, nullptr, stream);
+}
+
+extern "C" int sab_qk_int8_attn_bwd_varlen_blocksparse(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale,
+                                                       const float* k_scale, const void* q, const void* k, const void* v, const void* o,
+                                                       const void* dout, const float* lse, const void* k_mean, void* dq, void* dk,
+                                                       void* dv, void* workspace, int dtype, int nseq, int Hq, int Hkv, int Tq, int Tk,
+                                                       int D, int64_t q8_stride_t, int64_t q8_stride_h, int64_t k8_stride_t,
+                                                       int64_t k8_stride_h, int64_t q_stride_t, int64_t q_stride_h, int64_t k_stride_t,
+                                                       int64_t k_stride_h, int64_t v_stride_t, int64_t v_stride_h, int64_t o_stride_t,
+                                                       int64_t o_stride_h, int64_t do_stride_t, int64_t do_stride_h,
+                                                       const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
+                                                       const int32_t* cu_q_scale, const int32_t* cu_k_scale, int max_seqlen_q,
+                                                       int max_seqlen_k, int is_causal, int q_gran, int k_gran, float sm_scale,
+                                                       const uint8_t* block_mask, int64_t mask_stride_b, int64_t mask_stride_h,
+                                                       int64_t mask_stride_qb, int64_t mask_stride_kb, void* stream) {
+  if (int e = sab::check_block_mask_varlen(block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb, q_gran,
+                                           max_seqlen_q, max_seqlen_k))
+    return e;
+  const sab::BlockMask bm{block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb};
+  return bwd_varlen_seq(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, dtype, nseq, Hq, Hkv, Tq,
+                        Tk, D, q8_stride_t, q8_stride_h, k8_stride_t, k8_stride_h, q_stride_t, q_stride_h, k_stride_t, k_stride_h,
+                        v_stride_t, v_stride_h, o_stride_t, o_stride_h, do_stride_t, do_stride_h, cu_seqlens_q, cu_seqlens_k,
+                        cu_q_scale, cu_k_scale, max_seqlen_q, max_seqlen_k, is_causal, q_gran, k_gran, sm_scale, nullptr, &bm, stream);
 }

@@ -138,6 +138,22 @@ inline int check_block_mask(const void* block_mask, int64_t sb, int64_t sh, int6
   return SAB_OK;
 }
 
+// Host: the packed block-sparse entries' checks (sab_qk_int8_sv_f8_attn_varlen_blocksparse / sab_qk_int8_attn_bwd_varlen_blocksparse):
+// those of check_block_mask, except that causal is top-left inside each sequence and needs no Lq == Lk, and that the key limit
+// applies to max_seqlen_k (it sizes each CTA's list of visible key blocks), not to the packed total.
+inline int check_block_mask_varlen(const void* block_mask, int64_t sb, int64_t sh, int64_t sqb, int64_t skb, int q_gran, int max_q,
+                                   int max_k) {
+  SAB_REQUIRE(block_mask != nullptr, SAB_ERR_INVALID, "block_mask: null pointer");
+  SAB_REQUIRE(sb >= 0 && sh >= 0 && sqb >= 0 && skb >= 0, SAB_ERR_INVALID, "block_mask strides must be >= 0 (0 broadcasts)");
+  SAB_REQUIRE(q_gran == SAB_GRAN_PER_WARP || q_gran == SAB_GRAN_PER_THREAD, SAB_ERR_UNSUPPORTED,
+              "the block-sparse path needs per-warp or per-thread Q scales (q_gran %d)", q_gran);
+  SAB_REQUIRE(max_q > 0 && max_k > 0, SAB_ERR_INVALID, "the packed block mask needs max_seqlen_q and max_seqlen_k > 0 (got %d, %d)",
+              max_q, max_k);
+  SAB_REQUIRE(max_k <= kMaxKvBlocks * BN, SAB_ERR_UNSUPPORTED, "the block-sparse path supports max_seqlen_k <= %d (got %d)",
+              kMaxKvBlocks * BN, max_k);
+  return SAB_OK;
+}
+
 // ---- sliding-window attention (sab_qk_int8_sv_f8_attn_window / sab_qk_int8_attn_bwd_window).  A kernel argument, not an
 // AttnParams field, so the parameter offsets of the other kernels do not move.
 struct Window {

@@ -29,18 +29,32 @@ template <>
 __device__ __forceinline__ float to_float<__nv_bfloat16>(__nv_bfloat16 v) { return __bfloat162float(v); }
 
 // Grid (nblk, H, B); DP = D rounded up to 64 or 128, each row read by DP/8 threads with one 16-byte load (lanes past D read 0).
-template <typename T, int DP>
+// kSeq: the packed form (sab_block_stats_varlen).  x is [T,H,D] (sb unused), b is the sequence, and its blocks restart at its first
+// token cu[b]: block nb of sequence b is the dense kernel's block nb of that sequence alone.  The grid is sized by the longest
+// sequence (nblk = ceil(max_seqlen/blk)); a block past the end of its sequence writes mean 0 and sim 0.
+template <typename T, int DP, bool kSeq = false>
 __global__ void __launch_bounds__(kStatsThreads) predict_stats_kernel(const T* __restrict__ x, float* __restrict__ mean,
                                                                      float* __restrict__ sim, int S, int D, int blk, int64_t sb,
-                                                                     int64_t sh, int64_t ss) {
+                                                                     int64_t sh, int64_t ss, const int32_t* __restrict__ cu = nullptr) {
   constexpr int TPR = DP / 8;                 // threads per row (8 or 16: a power of two inside one warp)
   constexpr int RPP = kStatsThreads / TPR;    // rows per pass
   const int nb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int tr = threadIdx.x / TPR, tc = threadIdx.x % TPR;
   const int r0 = nb * blk;
+  [[maybe_unused]] int64_t tok0 = 0;   // packed form: the sequence's first token
+  if constexpr (kSeq) {
+    tok0 = cu[b];
+    S = cu[b + 1] - cu[b];
+    if (r0 >= S) {
+      const int64_t blk_idx = (int64_t(b) * gridDim.y + h) * gridDim.x + nb;
+      for (int d = threadIdx.x; d < D; d += kStatsThreads) mean[blk_idx * D + d] = 0.f;
+      if (threadIdx.x == 0) sim[blk_idx] = 0.f;
+      return;
+    }
+  }
   const int n = min(blk, S - r0);
   const bool live = tc * 8 < D;
-  const T* base = x + b * sb + h * sh + int64_t(r0) * ss + tc * 8;
+  const T* base = kSeq ? x + h * sh + (tok0 + r0) * ss + tc * 8 : x + b * sb + h * sh + int64_t(r0) * ss + tc * 8;
   float sx[8], su[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) { sx[e] = 0.f; su[e] = 0.f; }
@@ -99,6 +113,10 @@ struct SelectParams {
   uint8_t* mask;     // [B,Hq,nq,nk]
   int Hq, Hkv, nq, nk, D, npow, rows, causal;
   float scale_log2, cdf, sim;
+  // packed form (predict_select_kernel<true>): B = nseq, nq / nk / npow are the bounds of the longest sequences (the tensors'
+  // extents), and sequence b's own are read from the sequence tables on the device
+  const int32_t* cu_q;
+  const int32_t* cu_k;
 };
 
 // Every thread gets the reduction of v over the CTA, in a fixed order.  red: kSelWarps floats, free on entry.
@@ -120,6 +138,11 @@ __device__ __forceinline__ float block_reduce(float v, float* red) {
 __device__ __forceinline__ float key_p(uint64_t key) { return __uint_as_float(uint32_t(key >> 32)); }
 
 // Grid (ceil(nq/rows), Hq, B).  Shared memory: npow sort keys, the rows' Q means, one chunk of K means, the rows' logits.
+// kSeq: the packed form (sab_predict_block_mask_varlen).  b is the sequence; its rows run the dense kernel's steps on its own
+// nq_b = ceil(Lq_b/128) rows and nk_b = ceil(Lk_b/64) key blocks, with its own sort length npow_b (the bitonic network and the
+// scan's per-thread chunks depend on it, and so does the fp32 order of the prefix mass), so slice [b, :, :nq_b, :nk_b] is the
+// dense kernel's mask of that sequence alone.  Every other byte of the sequence's [Hq, nq, nk] slab is written 0.
+template <bool kSeq = false>
 __global__ void __launch_bounds__(kSelThreads) predict_select_kernel(const SelectParams p) {
   extern __shared__ __align__(16) unsigned char smem[];
   uint64_t* keys = reinterpret_cast<uint64_t*>(smem);
@@ -130,12 +153,27 @@ __global__ void __launch_bounds__(kSelThreads) predict_select_kernel(const Selec
   __shared__ float scan[kSelWarps];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int h = blockIdx.y, b = blockIdx.z, hk = h / (p.Hq / p.Hkv);
-  const int D = p.D, nk = p.nk;
+  const int D = p.D;
+  int nk = p.nk, npow = p.npow;   // packed form: this sequence's; the tensors keep the strides p.nq, p.nk
   const int i0 = blockIdx.x * p.rows;
-  const int nr = min(p.rows, p.nq - i0);
+  int nr = min(p.rows, p.nq - i0);
   const int64_t qrow0 = (int64_t(b) * p.Hq + h) * p.nq + i0;
   const float* km = p.km + (int64_t(b) * p.Hkv + hk) * nk * D;
   const float* ks = p.ks + (int64_t(b) * p.Hkv + hk) * nk;
+  if constexpr (kSeq) {
+    const int lq = p.cu_q[b + 1] - p.cu_q[b], lk = p.cu_k[b + 1] - p.cu_k[b];
+    const int nq = lk > 0 ? (lq + 127) / 128 : 0;   // a sequence without keys has no visible block
+    nk = (lk + 63) / 64;
+    npow = 1;
+    while (npow < nk) npow <<= 1;
+    // the bytes outside the sequence's blocks: whole rows past nq_b, columns past nk_b
+    for (int r = 0; r < nr; ++r) {
+      uint8_t* out = p.mask + (qrow0 + r) * p.nk;
+      for (int j = (i0 + r < nq ? nk : 0) + tid; j < p.nk; j += kSelThreads) out[j] = 0;
+    }
+    if (i0 >= nq) return;
+    nr = min(nr, nq - i0);
+  }
   for (int t = tid; t < nr * D; t += kSelThreads) qmean[t] = p.qm[qrow0 * D + t];
 
   // 1. logits of every (row, key block) the CTA's rows can see, the K means staged once for all rows
@@ -160,7 +198,7 @@ __global__ void __launch_bounds__(kSelThreads) predict_select_kernel(const Selec
   __syncthreads();
 
   // 2. per row: softmax over the candidates, descending order (ties: ascending j), prefix mass, forced blocks, mask bytes
-  const int per = (p.npow + kSelThreads - 1) / kSelThreads;   // sorted positions scanned by each thread, contiguous
+  const int per = (npow + kSelThreads - 1) / kSelThreads;   // sorted positions scanned by each thread, contiguous
   for (int r = 0; r < nr; ++r) {
     const int i = i0 + r;
     const bool row_forced = p.qs[qrow0 + r] < p.sim;
@@ -178,16 +216,16 @@ __global__ void __launch_bounds__(kSelThreads) predict_select_kernel(const Selec
         if (ks[j] >= p.sim) sum += exp2f(lg[j] - mx);
       sum = block_reduce<false>(sum, red);
       // key = (p bits, ~j): p >= 0, so descending keys are descending p with ties in ascending j; non-candidates are 0
-      for (int t = tid; t < p.npow; t += kSelThreads) {
+      for (int t = tid; t < npow; t += kSelThreads) {
         uint64_t key = 0;
         if (t <= jmax && ks[t] >= p.sim)
           key = (uint64_t(__float_as_uint(__fdiv_rn(exp2f(lg[t] - mx), sum))) << 32) | uint32_t(~uint32_t(t));
         keys[t] = key;
       }
       __syncthreads();
-      for (int k = 2; k <= p.npow; k <<= 1) {
+      for (int k = 2; k <= npow; k <<= 1) {
         for (int j = k >> 1; j > 0; j >>= 1) {
-          for (int t = tid; t < (p.npow >> 1); t += kSelThreads) {
+          for (int t = tid; t < (npow >> 1); t += kSelThreads) {
             const int lo = ((t & ~(j - 1)) << 1) | (t & (j - 1));
             const int hi = lo + j;
             const uint64_t a = keys[lo], c = keys[hi];
@@ -201,7 +239,7 @@ __global__ void __launch_bounds__(kSelThreads) predict_select_kernel(const Selec
       const int t0 = tid * per;
       float local = 0.f;
       for (int u = 0; u < per; ++u)
-        if (t0 + u < p.npow) local += key_p(keys[t0 + u]);
+        if (t0 + u < npow) local += key_p(keys[t0 + u]);
       float inc = local;
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1) {
@@ -214,14 +252,14 @@ __global__ void __launch_bounds__(kSelThreads) predict_select_kernel(const Selec
       for (int w = 0; w < warp; ++w) run += scan[w];
       for (int u = 0; u < per; ++u) {
         const int t = t0 + u;
-        if (t >= p.npow) break;
+        if (t >= npow) break;
         const uint64_t key = keys[t];
         if (key != 0 && run < p.cdf) kept[~uint32_t(key)] = 1;
         run += key_p(key);
       }
       __syncthreads();
     }
-    uint8_t* out = p.mask + (qrow0 + r) * nk;
+    uint8_t* out = p.mask + (qrow0 + r) * p.nk;
     for (int j = tid; j < nk; j += kSelThreads) {
       bool v = false;
       if (j <= jmax) {
@@ -235,20 +273,19 @@ __global__ void __launch_bounds__(kSelThreads) predict_select_kernel(const Selec
   }
 }
 
-template <typename T, int DP>
+template <typename T, int DP, bool kSeq = false>
 int launch_stats(const void* x, float* mean, float* sim, int B, int H, int S, int D, int64_t sb, int64_t sh, int64_t ss, int blk,
-                 cudaStream_t stream) {
+                 const int32_t* cu, cudaStream_t stream) {
   const dim3 grid((S + blk - 1) / blk, H, B);
-  predict_stats_kernel<T, DP><<<grid, kStatsThreads, 0, stream>>>(reinterpret_cast<const T*>(x), mean, sim, S, D, blk, sb, sh, ss);
+  predict_stats_kernel<T, DP, kSeq><<<grid, kStatsThreads, 0, stream>>>(reinterpret_cast<const T*>(x), mean, sim, S, D, blk, sb, sh,
+                                                                        ss, cu);
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
 }
 
-}  // namespace sab
-
-extern "C" int sab_block_stats(const void* x, int dtype, float* mean, float* sim, int B, int H, int S, int D, int64_t stride_b,
-                               int64_t stride_h, int64_t stride_s, int blk, void* stream) {
-  using namespace sab;
+// The statistics entries' checks and launch.  Packed form (cu != nullptr): B = nseq, S = max_seqlen, no batch stride.
+static int block_stats(const void* x, int dtype, float* mean, float* sim, int B, int H, int S, int D, int64_t stride_b,
+                       int64_t stride_h, int64_t stride_s, int blk, const int32_t* cu, void* stream) {
   SAB_REQUIRE(x && mean && sim, SAB_ERR_INVALID, "null tensor pointer");
   SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "Only half and bfloat16 are supported");
   SAB_REQUIRE(D > 0 && D <= 128 && D % 8 == 0, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (a multiple of 8, at most 128)", D);
@@ -260,17 +297,25 @@ extern "C" int sab_block_stats(const void* x, int dtype, float* mean, float* sim
   if (int st = sab_check_device()) return st;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const bool bf = dtype == SAB_DTYPE_BF16;
+  if (cu != nullptr) {
+    if (D <= 64)
+      return bf ? launch_stats<__nv_bfloat16, 64, true>(x, mean, sim, B, H, S, D, 0, stride_h, stride_s, blk, cu, s)
+                : launch_stats<__half, 64, true>(x, mean, sim, B, H, S, D, 0, stride_h, stride_s, blk, cu, s);
+    return bf ? launch_stats<__nv_bfloat16, 128, true>(x, mean, sim, B, H, S, D, 0, stride_h, stride_s, blk, cu, s)
+              : launch_stats<__half, 128, true>(x, mean, sim, B, H, S, D, 0, stride_h, stride_s, blk, cu, s);
+  }
   if (D <= 64)
-    return bf ? launch_stats<__nv_bfloat16, 64>(x, mean, sim, B, H, S, D, stride_b, stride_h, stride_s, blk, s)
-              : launch_stats<__half, 64>(x, mean, sim, B, H, S, D, stride_b, stride_h, stride_s, blk, s);
-  return bf ? launch_stats<__nv_bfloat16, 128>(x, mean, sim, B, H, S, D, stride_b, stride_h, stride_s, blk, s)
-            : launch_stats<__half, 128>(x, mean, sim, B, H, S, D, stride_b, stride_h, stride_s, blk, s);
+    return bf ? launch_stats<__nv_bfloat16, 64>(x, mean, sim, B, H, S, D, stride_b, stride_h, stride_s, blk, nullptr, s)
+              : launch_stats<__half, 64>(x, mean, sim, B, H, S, D, stride_b, stride_h, stride_s, blk, nullptr, s);
+  return bf ? launch_stats<__nv_bfloat16, 128>(x, mean, sim, B, H, S, D, stride_b, stride_h, stride_s, blk, nullptr, s)
+            : launch_stats<__half, 128>(x, mean, sim, B, H, S, D, stride_b, stride_h, stride_s, blk, nullptr, s);
 }
 
-extern "C" int sab_predict_block_mask(const float* q_mean, const float* q_sim, const float* k_mean, const float* k_sim,
-                                      uint8_t* block_mask, int B, int Hq, int Hkv, int Sq, int Skv, int D, int is_causal,
-                                      float sm_scale, float cdf_threshold, float sim_threshold, void* stream) {
-  using namespace sab;
+// The selection entries' checks and launch.  Packed form (cu_q != nullptr): B = nseq, Sq / Skv = max_seqlen_q / max_seqlen_k, and
+// causal needs no Sq == Skv (top-left inside each sequence).
+static int predict_mask(const float* q_mean, const float* q_sim, const float* k_mean, const float* k_sim, uint8_t* block_mask, int B,
+                        int Hq, int Hkv, int Sq, int Skv, int D, int is_causal, float sm_scale, float cdf_threshold,
+                        float sim_threshold, const int32_t* cu_q, const int32_t* cu_k, void* stream) {
   SAB_REQUIRE(q_mean && q_sim && k_mean && k_sim && block_mask, SAB_ERR_INVALID, "null tensor pointer");
   SAB_REQUIRE(D > 0 && D <= 128 && D % 8 == 0, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (a multiple of 8, at most 128)", D);
   SAB_REQUIRE(B > 0 && Hq > 0 && Hkv > 0 && Sq > 0 && Skv > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", B, Hq,
@@ -278,7 +323,8 @@ extern "C" int sab_predict_block_mask(const float* q_mean, const float* q_sim, c
   SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
   SAB_REQUIRE(Skv <= 64 * kMaxKeyBlocks, SAB_ERR_UNSUPPORTED, "block mask prediction supports kv_len <= %d, got %d",
               64 * kMaxKeyBlocks, Skv);
-  SAB_REQUIRE(!is_causal || Sq == Skv, SAB_ERR_INVALID, "qo_len (%d) and kv_len (%d) must be equal for causal attention", Sq, Skv);
+  SAB_REQUIRE(!is_causal || Sq == Skv || cu_q != nullptr, SAB_ERR_INVALID,
+              "qo_len (%d) and kv_len (%d) must be equal for causal attention", Sq, Skv);
   SAB_REQUIRE(cdf_threshold > 0.f, SAB_ERR_INVALID, "cdf_threshold must be > 0, got %g", double(cdf_threshold));
   SAB_REQUIRE(!std::isnan(sim_threshold), SAB_ERR_INVALID, "sim_threshold must not be NaN");
   SAB_REQUIRE(std::isfinite(sm_scale), SAB_ERR_INVALID, "sm_scale must be finite, got %g", double(sm_scale));
@@ -289,6 +335,7 @@ extern "C" int sab_predict_block_mask(const float* q_mean, const float* q_sim, c
   p.causal = is_causal ? 1 : 0;
   p.scale_log2 = sm_scale * 1.44269504088896340736f;
   p.cdf = cdf_threshold; p.sim = sim_threshold;
+  p.cu_q = cu_q; p.cu_k = cu_k;
   p.npow = 1;
   while (p.npow < p.nk) p.npow <<= 1;
   const size_t fixed = size_t(p.npow) * 8 + size_t(kSelChunk) * (D + 1) * 4;
@@ -296,10 +343,41 @@ extern "C" int sab_predict_block_mask(const float* q_mean, const float* q_sim, c
   p.rows = int(std::min<size_t>(kSelMaxRows, (kSelSmemMax - fixed) / per_row));
   p.rows = std::max(1, std::min(p.rows, p.nq));
   const size_t smem = fixed + per_row * p.rows;
-  static bool configured[64] = {};
-  if (int st = ensure_dynamic_smem(predict_select_kernel, kSelSmemMax, configured)) return st;
+  static bool configured[64] = {}, configured_seq[64] = {};
+  auto kern = cu_q != nullptr ? predict_select_kernel<true> : predict_select_kernel<false>;
+  if (int st = ensure_dynamic_smem(kern, kSelSmemMax, cu_q != nullptr ? configured_seq : configured)) return st;
   const dim3 grid((p.nq + p.rows - 1) / p.rows, Hq, B);
-  predict_select_kernel<<<grid, kSelThreads, smem, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+  kern<<<grid, kSelThreads, smem, reinterpret_cast<cudaStream_t>(stream)>>>(p);
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
+}
+
+}  // namespace sab
+
+extern "C" int sab_block_stats(const void* x, int dtype, float* mean, float* sim, int B, int H, int S, int D, int64_t stride_b,
+                               int64_t stride_h, int64_t stride_s, int blk, void* stream) {
+  return sab::block_stats(x, dtype, mean, sim, B, H, S, D, stride_b, stride_h, stride_s, blk, nullptr, stream);
+}
+
+extern "C" int sab_predict_block_mask(const float* q_mean, const float* q_sim, const float* k_mean, const float* k_sim,
+                                      uint8_t* block_mask, int B, int Hq, int Hkv, int Sq, int Skv, int D, int is_causal,
+                                      float sm_scale, float cdf_threshold, float sim_threshold, void* stream) {
+  return sab::predict_mask(q_mean, q_sim, k_mean, k_sim, block_mask, B, Hq, Hkv, Sq, Skv, D, is_causal, sm_scale, cdf_threshold,
+                           sim_threshold, nullptr, nullptr, stream);
+}
+
+extern "C" int sab_block_stats_varlen(const void* x, int dtype, float* mean, float* sim, const int32_t* cu_seqlens, int nseq,
+                                      int max_seqlen, int H, int D, int64_t stride_t, int64_t stride_h, int blk, void* stream) {
+  SAB_REQUIRE(cu_seqlens != nullptr, SAB_ERR_INVALID, "the packed statistics need cu_seqlens");
+  return sab::block_stats(x, dtype, mean, sim, nseq, H, max_seqlen, D, 0, stride_h, stride_t, blk, cu_seqlens, stream);
+}
+
+extern "C" int sab_predict_block_mask_varlen(const float* q_mean, const float* q_sim, const float* k_mean, const float* k_sim,
+                                             uint8_t* block_mask, const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k, int nseq,
+                                             int Hq, int Hkv, int max_seqlen_q, int max_seqlen_k, int D, int is_causal,
+                                             float sm_scale, float cdf_threshold, float sim_threshold, void* stream) {
+  SAB_REQUIRE(cu_seqlens_q != nullptr && cu_seqlens_k != nullptr, SAB_ERR_INVALID,
+              "the packed prediction needs cu_seqlens_q and cu_seqlens_k");
+  return sab::predict_mask(q_mean, q_sim, k_mean, k_sim, block_mask, nseq, Hq, Hkv, max_seqlen_q, max_seqlen_k, D, is_causal, sm_scale,
+                           cdf_threshold, sim_threshold, cu_seqlens_q, cu_seqlens_k, stream);
 }

@@ -752,6 +752,81 @@ def _(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, d
     return None
 
 
+@torch.library.custom_op("sageattention_b200::qk_int8_sv_f8_attn_varlen_blocksparse", mutates_args=("output",), device_types="cuda")
+def qk_int8_sv_f8_attn_varlen_blocksparse(query: torch.Tensor, key: torch.Tensor, value: torch.Tensor, output: torch.Tensor,
+                                          query_scale: torch.Tensor, key_scale: torch.Tensor, value_scale: torch.Tensor,
+                                          value_mean: Optional[torch.Tensor], cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor,
+                                          cu_pad_v: torch.Tensor, cu_q_scale: torch.Tensor, cu_k_scale: torch.Tensor,
+                                          max_seqlen_q: int, max_seqlen_k: int, block_mask: torch.Tensor, is_causal: int,
+                                          q_quant_gran: int, k_quant_gran: int, sm_scale: float, return_lse: int) -> torch.Tensor:
+    """qk_int8_sv_f8_attn_varlen_seq restricted to the visible tiles of a block mask inside each sequence (include/sageattn_b200.h,
+    sab_qk_int8_sv_f8_attn_varlen_blocksparse): a bool view [nseq,Hq,ceil(max_seqlen_q/128),ceil(max_seqlen_k/64)], strides may be
+    0.  Returns the [Hq,Tq] log2 LSE when return_lse, else an empty tensor; a row with no visible key gets 0 and lse -inf."""
+    Tq, Hq, D = query.shape
+    Tk, Hkv, _ = key.shape
+    nseq = cu_seqlens_q.numel() - 1
+    mask = _block_mask_args(block_mask, nseq, Hq, max_seqlen_q, max_seqlen_k)
+    lse = torch.empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32, device=query.device)
+    with torch.cuda.device(query.device):
+        check(lib().sab_qk_int8_sv_f8_attn_varlen_blocksparse(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
+                                                              lse.data_ptr() if return_lse else None, query_scale.data_ptr(),
+                                                              key_scale.data_ptr(), value_scale.data_ptr(), _ptr(value_mean),
+                                                              _dt(output), nseq, Hq, Hkv, Tq, Tk, D, query.stride(0), query.stride(1),
+                                                              key.stride(0), key.stride(1), _v_pad(value), output.stride(0),
+                                                              output.stride(1), is_causal, q_quant_gran, k_quant_gran, float(sm_scale),
+                                                              cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), cu_pad_v.data_ptr(),
+                                                              cu_q_scale.data_ptr(), cu_k_scale.data_ptr(), max_seqlen_q, max_seqlen_k,
+                                                              *mask, _stream(query)))
+    return lse
+
+
+@qk_int8_sv_f8_attn_varlen_blocksparse.register_fake
+def _(query, key, value, output, query_scale, key_scale, value_scale, value_mean, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale,
+      cu_k_scale, max_seqlen_q, max_seqlen_k, block_mask, is_causal, q_quant_gran, k_quant_gran, sm_scale, return_lse):
+    Tq, Hq, _ = query.shape
+    return query.new_empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32)
+
+
+@torch.library.custom_op("sageattention_b200::qk_int8_attn_bwd_varlen_blocksparse", mutates_args=("dq", "dk", "dv"),
+                         device_types="cuda")
+def qk_int8_attn_bwd_varlen_blocksparse(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale: torch.Tensor, k_scale: torch.Tensor,
+                                        q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, o: torch.Tensor, dout: torch.Tensor,
+                                        lse: torch.Tensor, k_mean: Optional[torch.Tensor], dq: torch.Tensor, dk: torch.Tensor,
+                                        dv: torch.Tensor, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor,
+                                        cu_q_scale: torch.Tensor, cu_k_scale: torch.Tensor, max_seqlen_q: int, max_seqlen_k: int,
+                                        block_mask: torch.Tensor, is_causal: int, q_quant_gran: int, k_quant_gran: int,
+                                        sm_scale: float) -> None:
+    """Gradients of qk_int8_sv_f8_attn_varlen_blocksparse (include/sageattn_b200.h, sab_qk_int8_attn_bwd_varlen_blocksparse): the
+    arguments of qk_int8_attn_bwd_varlen_seq plus the block mask view the forward received."""
+    Tq, Hq, D = q.shape
+    Tk, Hkv, _ = k.shape
+    nseq = cu_seqlens_q.numel() - 1
+    for x, y in ((dq, q), (dk, k), (dv, v)):
+        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
+    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (Hq, Tq), "lse must be [Hq,Tq] fp32"
+    mask = _block_mask_args(block_mask, nseq, Hq, max_seqlen_q, max_seqlen_k)
+    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in (t.stride(0), t.stride(1))]
+    if k_mean is not None:
+        assert k_mean.numel() == nseq * Hkv * D and k_mean.dtype == k.dtype, "k_mean must have nseq*Hkv*D elements of k's dtype"
+        k_mean = k_mean.reshape(nseq, Hkv, D).contiguous()
+    with torch.cuda.device(q.device):
+        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(1, Hq, Tq), dtype=torch.uint8, device=q.device)
+        check(lib().sab_qk_int8_attn_bwd_varlen_blocksparse(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(),
+                                                            k_scale.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
+                                                            dout.data_ptr(), lse.data_ptr(), _ptr(k_mean), dq.data_ptr(), dk.data_ptr(),
+                                                            dv.data_ptr(), ws.data_ptr(), _dt(q), nseq, Hq, Hkv, Tq, Tk, D, *strides,
+                                                            cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), cu_q_scale.data_ptr(),
+                                                            cu_k_scale.data_ptr(), max_seqlen_q, max_seqlen_k, is_causal, q_quant_gran,
+                                                            k_quant_gran, float(sm_scale), *mask, _stream(q)))
+
+
+@qk_int8_attn_bwd_varlen_blocksparse.register_fake
+def _(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, cu_seqlens_q, cu_seqlens_k, cu_q_scale, cu_k_scale,
+      max_seqlen_q, max_seqlen_k, block_mask, is_causal, q_quant_gran, k_quant_gran, sm_scale):
+    return None
+
+
 # ----------------------------------------------------------------------------------------------- block-mask prediction
 @torch.library.custom_op("sageattention_b200::block_stats", mutates_args=("mean", "sim"), device_types="cuda")
 def block_stats(x: torch.Tensor, mean: torch.Tensor, sim: torch.Tensor, tensor_layout: int, block_size: int) -> None:
@@ -799,6 +874,59 @@ def predict_block_mask(q_mean: torch.Tensor, q_sim: torch.Tensor, k_mean: torch.
 
 @predict_block_mask.register_fake
 def _(q_mean, q_sim, k_mean, k_sim, block_mask, Sq, Skv, is_causal, sm_scale, cdf_threshold, sim_threshold):
+    return None
+
+
+@torch.library.custom_op("sageattention_b200::block_stats_varlen", mutates_args=("mean", "sim"), device_types="cuda")
+def block_stats_varlen(x: torch.Tensor, mean: torch.Tensor, sim: torch.Tensor, cu_seqlens: torch.Tensor, max_seqlen: int,
+                       block_size: int) -> None:
+    """block_stats of every sequence of packed x [T,H,D] on its own (include/sageattn_b200.h, sab_block_stats_varlen): mean
+    [nseq,H,ceil(max_seqlen/block_size),D] and sim [nseq,H,ceil(max_seqlen/block_size)], blocks past a sequence's end 0."""
+    T, H, D = x.shape
+    nseq = cu_seqlens.numel() - 1
+    if x.data_ptr() % 16 or any(s % 8 for s in x.stride()[:-1]):
+        x = x.contiguous()
+    nb = (max_seqlen + block_size - 1) // block_size
+    assert mean.dtype == torch.float32 and mean.is_contiguous() and tuple(mean.shape) == (nseq, H, nb, D), \
+        f"mean must be a contiguous fp32 [{nseq}, {H}, {nb}, {D}] tensor"
+    assert sim.dtype == torch.float32 and sim.is_contiguous() and tuple(sim.shape) == (nseq, H, nb), \
+        f"sim must be a contiguous fp32 [{nseq}, {H}, {nb}] tensor"
+    with torch.cuda.device(x.device):
+        check(lib().sab_block_stats_varlen(x.data_ptr(), _dt(x), mean.data_ptr(), sim.data_ptr(), cu_seqlens.data_ptr(), nseq,
+                                           max_seqlen, H, D, x.stride(0), x.stride(1), block_size, _stream(x)))
+
+
+@block_stats_varlen.register_fake
+def _(x, mean, sim, cu_seqlens, max_seqlen, block_size):
+    return None
+
+
+@torch.library.custom_op("sageattention_b200::predict_block_mask_varlen", mutates_args=("block_mask",), device_types="cuda")
+def predict_block_mask_varlen(q_mean: torch.Tensor, q_sim: torch.Tensor, k_mean: torch.Tensor, k_sim: torch.Tensor,
+                              block_mask: torch.Tensor, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor, max_seqlen_q: int,
+                              max_seqlen_k: int, is_causal: int, sm_scale: float, cdf_threshold: float, sim_threshold: float) -> None:
+    """Writes the bool [nseq,Hq,ceil(max_seqlen_q/128),ceil(max_seqlen_k/64)] block_mask predicted for each sequence from
+    block_stats_varlen of q (block 128) and k (block 64) (include/sageattn_b200.h, sab_predict_block_mask_varlen)."""
+    nseq, Hq, nq, D = q_mean.shape
+    Hkv, nk = k_mean.size(1), k_mean.size(2)
+    assert nseq == cu_seqlens_q.numel() - 1 == cu_seqlens_k.numel() - 1, "statistics and cu_seqlens disagree on nseq"
+    assert nq == (max_seqlen_q + 127) // 128 and nk == (max_seqlen_k + 63) // 64 and k_mean.size(3) == D and k_mean.size(0) == nseq, \
+        "q / k statistics do not match max_seqlen_q / max_seqlen_k"
+    for t in (q_mean, q_sim, k_mean, k_sim):
+        assert t.dtype == torch.float32 and t.is_contiguous(), "block statistics must be contiguous fp32"
+    assert tuple(q_sim.shape) == (nseq, Hq, nq) and tuple(k_sim.shape) == (nseq, Hkv, nk), "sim shapes do not match the means"
+    assert block_mask.dtype == torch.bool and block_mask.is_contiguous() and tuple(block_mask.shape) == (nseq, Hq, nq, nk), \
+        f"block_mask must be a contiguous bool [{nseq}, {Hq}, {nq}, {nk}] tensor"
+    with torch.cuda.device(q_mean.device):
+        check(lib().sab_predict_block_mask_varlen(q_mean.data_ptr(), q_sim.data_ptr(), k_mean.data_ptr(), k_sim.data_ptr(),
+                                                  block_mask.data_ptr(), cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), nseq, Hq,
+                                                  Hkv, max_seqlen_q, max_seqlen_k, D, is_causal, float(sm_scale), float(cdf_threshold),
+                                                  float(sim_threshold), _stream(q_mean)))
+
+
+@predict_block_mask_varlen.register_fake
+def _(q_mean, q_sim, k_mean, k_sim, block_mask, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, is_causal, sm_scale,
+      cdf_threshold, sim_threshold):
     return None
 
 

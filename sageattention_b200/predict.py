@@ -1,7 +1,8 @@
 """Block-sparse masks predicted from pooled Q/K statistics (no reference counterpart): predict_block_mask, whose output is the
 block_mask that sageattn_blocksparse takes.  Two sm_90a kernels (csrc/predict.cu): one pass over q and k for the per-block
 statistics, one that scores, orders and selects key blocks per 128-query block.  The definition is in include/sageattn_b200.h
-(sab_block_stats, sab_predict_block_mask)."""
+(sab_block_stats, sab_predict_block_mask).  predict_block_mask_varlen is the same for every packed sequence on its own, through
+the packed forms of the two kernels (sab_block_stats_varlen, sab_predict_block_mask_varlen), for sageattn_varlen_blocksparse."""
 import math
 from typing import Optional
 
@@ -77,4 +78,59 @@ def predict_block_mask(q: torch.Tensor, k: torch.Tensor, *, cdf_threshold: float
     ops.block_stats(k, k_mean, k_sim, lay, 64)
     ops.predict_block_mask(q_mean, q_sim, k_mean, k_sim, block_mask, Sq, Skv, 1 if is_causal else 0, sm_scale, cdf_threshold,
                            sim_threshold)
+    return block_mask
+
+
+def predict_block_mask_varlen(q: torch.Tensor, k: torch.Tensor, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor,
+                              max_seqlen_q: int, max_seqlen_k: int, *, cdf_threshold: float, sim_threshold: float,
+                              is_causal: bool = False, sm_scale: Optional[float] = None) -> torch.Tensor:
+    """predict_block_mask of every packed sequence on its own, in three launches whatever the number of sequences: the block mask
+    that sageattn_varlen_blocksparse takes.  q [Tq,Hq,D], k [Tk,Hkv,D] packed as for sageattn_varlen_qk_int8_pv_fp8_cuda
+    (cu_seqlens int32 or int64 on q's device, the same length; max_seqlen_* >= every length), max_seqlen_k <= 1048576.
+
+    Returns a contiguous torch.bool [nseq, Hq, ceil(max_seqlen_q/128), ceil(max_seqlen_k/64)] tensor on q's device.  Contract: slice
+    [b, :, :nq_b, :nk_b] (nq_b = ceil(Lq_b/128), nk_b = ceil(Lk_b/64)) is the bits of predict_block_mask(q_b[None], k_b[None],
+    tensor_layout="NHD", <same options>)[0]: the statistics blocks restart at each sequence's first token, and each sequence sorts
+    its candidates on its own power-of-two length, so its prefix masses are summed in the dense call's order.  Every entry outside
+    the slices is False, and so is every entry of a sequence without queries or keys.  is_causal is top-left inside each sequence,
+    with the rules of predict_block_mask, and allows Lq != Lk.  The lengths are read on the device (no host sync).  The inputs carry
+    no gradient here.  Deterministic."""
+    from .core import _check_cu_seqlens
+    assert q.is_cuda, "Input tensors must be on cuda."
+    assert q.dtype in [torch.float16, torch.bfloat16], "Input tensors must be in dtype of torch.float16 or torch.bfloat16"
+    assert q.device == k.device, "All tensors must be on the same device."
+    assert q.dtype == k.dtype, "All tensors must have the same dtype."
+    _check_cu_seqlens(q, k, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k)
+    head_dim_og = q.size(-1)
+    if head_dim_og > 128 or k.size(-1) != head_dim_og:
+        raise ValueError(f"Unsupported head_dim: {head_dim_og} (q) / {k.size(-1)} (k); at most 128 and equal")
+    assert q.stride(-1) == 1 and k.stride(-1) == 1, "Last dim of qkv must be contiguous."
+    Hq, Hkv = q.size(1), k.size(1)
+    if Hq % Hkv:
+        raise ValueError(f"num_qo_heads ({Hq}) must be divisible by num_kv_heads ({Hkv})")
+    max_seqlen_q, max_seqlen_k = int(max_seqlen_q), int(max_seqlen_k)
+    if max_seqlen_k > MAX_KV_LEN:
+        raise ValueError(f"predict_block_mask_varlen supports max_seqlen_k <= {MAX_KV_LEN}, got {max_seqlen_k}")
+    cdf_threshold, sim_threshold = float(cdf_threshold), float(sim_threshold)
+    if not cdf_threshold > 0.0:
+        raise ValueError(f"cdf_threshold must be > 0, got {cdf_threshold}")
+    if math.isnan(sim_threshold):
+        raise ValueError("sim_threshold must not be NaN")
+    if sm_scale is None:
+        sm_scale = head_dim_og ** -0.5
+    if not math.isfinite(sm_scale):
+        raise ValueError(f"sm_scale must be finite, got {sm_scale}")
+
+    q, k = _pad8(q.detach()), _pad8(k.detach())
+    cu_q, cu_k = cu_seqlens_q.to(torch.int32).contiguous(), cu_seqlens_k.to(torch.int32).contiguous()
+    nseq, D = cu_q.numel() - 1, q.size(-1)
+    nq, nk = (max_seqlen_q + 127) // 128, (max_seqlen_k + 63) // 64
+    f32 = dict(dtype=torch.float32, device=q.device)
+    q_mean, q_sim = torch.empty((nseq, Hq, nq, D), **f32), torch.empty((nseq, Hq, nq), **f32)
+    k_mean, k_sim = torch.empty((nseq, Hkv, nk, D), **f32), torch.empty((nseq, Hkv, nk), **f32)
+    block_mask = torch.empty((nseq, Hq, nq, nk), dtype=torch.bool, device=q.device)
+    ops.block_stats_varlen(q, q_mean, q_sim, cu_q, max_seqlen_q, 128)
+    ops.block_stats_varlen(k, k_mean, k_sim, cu_k, max_seqlen_k, 64)
+    ops.predict_block_mask_varlen(q_mean, q_sim, k_mean, k_sim, block_mask, cu_q, cu_k, max_seqlen_q, max_seqlen_k,
+                                  1 if is_causal else 0, sm_scale, cdf_threshold, sim_threshold)
     return block_mask

@@ -7,6 +7,8 @@ import pytest
 import torch
 
 from attn_blocksparse_oracle import attn_int8_fp8_blocksparse, expand_block_mask
+from attn_bwd_oracle import elementwise_ratio
+from attn_window_oracle import attn_int8_fp8_blocksparse_causal, attn_int8_fp8_tiles
 from oracle import sage_oracle as O
 
 
@@ -64,6 +66,56 @@ def test_broadcast_mask_equals_expanded():
     kw = dict(qk_quant_gran="per_warp", sm_scale=0.125, lazy_tau=4)
     assert torch.equal(attn_int8_fp8_blocksparse(q8, k8, v8, qs, ks, vs, bm, **kw),
                        attn_int8_fp8_blocksparse(q8, k8, v8, qs, ks, vs, bm.expand(B, Hq, -1, -1).clone(), **kw))
+
+
+@pytest.mark.parametrize("tau", [4, 0])
+@pytest.mark.parametrize("gran", ["per_thread", "per_warp"])
+def test_tile_list_restatement_on_all_visible_tiles_is_the_dense_restatement_bitwise(gran, tau):
+    """The tile-list restatement (attn_window_oracle.attn_int8_fp8_tiles) through its causal block-sparse caller with an all-True
+    mask is the dense causal restatement, and with every tile listed and nothing masked the dense non-causal one."""
+    B, Hq, Hkv, S, D = 2, 4, 2, 333, 64
+    _, _, _, q8, qs, k8, ks, v8, vs = _operands(B, Hq, Hkv, S, S, D, gran, seed=5)
+    kw = dict(qk_quant_gran=gran, sm_scale=D ** -0.5, lazy_tau=tau, return_lse=True)
+    for causal in (False, True):
+        ref = O.attn_int8_fp8_cuda(q8, k8, v8, qs, ks, vs, is_causal=causal, **kw)
+        if causal:
+            got = attn_int8_fp8_blocksparse_causal(q8, k8, v8, qs, ks, vs, torch.ones(1, 1, 3, 6, dtype=torch.bool), **kw)
+        else:
+            got = attn_int8_fp8_tiles(q8, k8, v8, qs, ks, vs, lambda b, h, i: range(6), torch.ones(1, 1, 1, 1, dtype=torch.bool), **kw)
+        assert torch.equal(got[0], ref[0]) and torch.equal(got[1], ref[1]), causal
+
+
+@pytest.mark.parametrize("gran", ["per_thread", "per_warp"])
+def test_tile_list_restatement_is_the_gathered_restatement_bitwise(gran):
+    """Non-causal, the tile-list loop over the visible tiles of each mask row with the expanded element mask gives the bits of the
+    gathered restatement (attn_int8_fp8_blocksparse), per (batch, head) masks, hidden rows and a partial last tile included."""
+    B, Hq, Hkv, Sq, Sk, D = 2, 4, 2, 300, 333, 64
+    _, _, _, q8, qs, k8, ks, v8, vs = _operands(B, Hq, Hkv, Sq, Sk, D, gran, seed=6)
+    bm = _mask(B, Hq, Sq, Sk, 0.5, 7)
+    bm[0, 0, 1] = False
+    bm[1, 3, :, -1] = True
+    kw = dict(qk_quant_gran=gran, sm_scale=D ** -0.5, lazy_tau=4, return_lse=True, v_mean=torch.randn(B, Hkv, D))
+    ref = attn_int8_fp8_blocksparse(q8, k8, v8, qs, ks, vs, bm, **kw)
+    got = attn_int8_fp8_tiles(q8, k8, v8, qs, ks, vs, lambda b, h, i: [j for j in range(bm.size(3)) if bm[b, h, i, j]],
+                              expand_block_mask(bm, Sq, Sk), **kw)
+    assert torch.equal(got[0], ref[0]) and torch.equal(got[1], ref[1])
+
+
+def test_bound_rejects_a_flipped_diagonal_tile():
+    """Causal: the restatement on a mask with one tile of a diagonal 64-key pair flipped, either way, is outside the bound of the
+    true mask's restatement."""
+    B, Hq, Hkv, S, D = 1, 2, 1, 384, 64
+    _, _, _, q8, qs, k8, ks, v8, vs = _operands(B, Hq, Hkv, S, S, D, "per_thread", seed=8)
+    bm = _mask(B, Hq, S, S, 0.6, 9)
+    bm[..., 0] = True
+    kw = dict(qk_quant_gran="per_thread", sm_scale=D ** -0.5, lazy_tau=4)
+    o, bd = attn_int8_fp8_blocksparse_causal(q8, k8, v8, qs, ks, vs, bm, bound=True, **kw)
+    assert float(elementwise_ratio(o, bd.o, bd.o_bound).max()) <= 1.0
+    for i, j in ((1, 2), (1, 3), (2, 5)):
+        flip = bm.clone()
+        flip[0, 1, i, j] = ~flip[0, 1, i, j]
+        bad = attn_int8_fp8_blocksparse_causal(q8, k8, v8, qs, ks, vs, flip, **kw)
+        assert float(elementwise_ratio(bad, bd.o, bd.o_bound).max()) > 1.0, (i, j)
 
 
 def _call_fwd(lib, mask, strides=(0, 0, 1, 1), is_causal=0, q_gran=3, Sq=128, Skv=128):

@@ -102,6 +102,9 @@ FWD_CASES = [  # gran, pv_accum_dtype, smooth_v, causal, Hq, Hkv, D, dtype, cu d
     ("per_warp", "fp32", True, True, 8, 2, 128, FP, torch.int32),
     ("per_thread", "fp32", False, True, 8, 2, 64, BF, torch.int32),
     ("per_warp", "fp32", False, False, 8, 8, 96, FP, torch.int32),
+    ("per_warp", "fp32+fp32", False, True, 4, 2, 64, FP, torch.int64),
+    ("per_warp", "fp32", True, False, 8, 2, 128, BF, torch.int32),
+    ("per_thread", "fp32+fp16", False, True, 4, 4, 128, FP, torch.int64),
 ]
 
 
@@ -234,6 +237,9 @@ BWD_CASES = [  # gran, causal, dtype, D, density
     ("per_thread", False, FP, 128, 0.5),
     ("per_warp", True, BF, 96, 0.3),
     ("per_thread", False, BF, 64, 0.1),
+    ("per_warp", True, BF, 64, 0.5),
+    ("per_thread", True, FP, 64, 0.3),
+    ("per_warp", False, FP, 128, 0.25),
 ]
 
 

@@ -166,6 +166,9 @@ FWD_CASES = [  # gran, pv_accum_dtype, smooth_v, causal, Hq, Hkv, D, dtype
     ("per_warp", "fp32", True, True, 8, 2, 128, FP),
     ("per_thread", "fp32", False, True, 32, 8, 64, BF),
     ("per_warp", "fp32", False, False, 8, 8, 96, FP),
+    ("per_warp", "fp32+fp32", False, True, 4, 2, 64, FP),
+    ("per_warp", "fp32", True, False, 8, 2, 128, BF),
+    ("per_thread", "fp32+fp16", False, True, 4, 4, 128, FP),
 ]
 
 
@@ -262,7 +265,8 @@ def _grads_varlen(q, k, v, do, lens_q, lens_k, **kw):
     return o.detach(), qg.grad, kg.grad, vg.grad
 
 
-BWD_CASES = [("per_thread", True, BF, 128), ("per_warp", False, FP, 64), ("per_thread", False, FP, 128), ("per_warp", True, BF, 96)]
+BWD_CASES = [("per_thread", True, BF, 128), ("per_warp", False, FP, 64), ("per_thread", False, FP, 128), ("per_warp", True, BF, 96),
+             ("per_warp", False, BF, 64), ("per_thread", True, FP, 64), ("per_thread", False, BF, 64), ("per_warp", True, FP, 128)]
 
 
 @pytest.mark.parametrize("case", BWD_CASES)

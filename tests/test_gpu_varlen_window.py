@@ -81,6 +81,9 @@ FWD_CASES = [  # gran, pv_accum_dtype, smooth_v, causal, Hq, Hkv, D, dtype, cu d
     ("per_warp", "fp32", True, True, 8, 2, 128, FP, torch.int32),
     ("per_thread", "fp32", False, True, 8, 2, 64, BF, torch.int32),
     ("per_warp", "fp32", False, False, 8, 8, 96, FP, torch.int32),
+    ("per_warp", "fp32+fp32", False, True, 4, 2, 64, FP, torch.int64),
+    ("per_warp", "fp32", True, False, 8, 2, 128, BF, torch.int32),
+    ("per_thread", "fp32+fp16", False, True, 4, 4, 128, FP, torch.int64),
 ]
 
 
@@ -200,6 +203,8 @@ BWD_CASES = [  # gran, causal, dtype, D, window
     ("per_thread", False, BF, 64, (1000, -1)),
     ("per_warp", False, BF, 128, (-1, 100)),
     ("per_thread", True, FP, 64, (100, 150)),
+    ("per_warp", False, BF, 64, (0, 0)),
+    ("per_warp", True, FP, 128, (130, 0)),
 ]
 
 

@@ -8,7 +8,8 @@ import re
 import pytest
 import torch
 
-from attn_window_oracle import attn_int8_fp8_window, window_mask, window_tiles
+from attn_bwd_oracle import elementwise_ratio
+from attn_window_oracle import E4M3, attn_int8_fp8_window, window_mask, window_tiles
 from oracle import sage_oracle as O
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -99,6 +100,61 @@ def test_bottom_rows_start_in_a_later_tile():
                                  lazy_tau=tau)
         ref = _exact(q, k, v, window_mask(S, S, 10, 0), D ** -0.5)
         assert torch.isfinite(o).all() and (o.double() - ref).abs().max().item() < 0.13 * v.abs().max().item()
+
+
+# ------------------------------------------------------------------------------------------------ the bound of the restatement
+def _bound_case(window=(200, 37), dt=torch.float16, gran="per_thread"):
+    """The restatement with its bound at 700 x 700, GQA 4:2, D=64, and the keyword arguments to call it again."""
+    _, _, _, q8, qs, k8, ks, v8, vs = _operands(1, 4, 2, 700, 700, 64, gran, seed=3)
+    kw = dict(qk_quant_gran=gran, sm_scale=0.125, lazy_tau=4, return_lse=True, out_dtype=dt)
+    o, lse, bd = attn_int8_fp8_window(q8, k8, v8, qs, ks, vs, window=window, bound=True, **kw)
+    return (q8, k8, v8, qs, ks, vs), kw, o, bd
+
+
+def _worst(o, bd):
+    return float(elementwise_ratio(o, bd.o, bd.o_bound).max())
+
+
+@pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16])
+def test_bound_accepts_every_ambiguous_p_flipped(dt):
+    """A kernel whose P8 takes the other candidate code on every ambiguous element (P within eps_P of an e4m3 rounding midpoint)
+    is within the bound; the case has such elements."""
+    ops_, kw, o, bd = _bound_case(dt=dt)
+    assert bd.ambiguous > 0 and _worst(o, bd) <= 1.0
+    flipped = attn_int8_fp8_window(*ops_, window=(200, 37), p8_fn=lambda p8, lo, hi: torch.where(p8 == lo, hi, lo), **kw)[0]
+    assert not torch.equal(flipped, o) and _worst(flipped, bd) <= 1.0
+
+
+@pytest.mark.parametrize("window", [(201, 37), (199, 37), (200, 38), (200, 36)])
+def test_bound_rejects_a_window_side_off_by_one(window):
+    ops_, kw, o, bd = _bound_case()
+    assert _worst(attn_int8_fp8_window(*ops_, window=window, **kw)[0], bd) > 1.0
+
+
+def test_bound_rejects_one_unambiguous_p_moved_by_one_code():
+    """The next e4m3 code on one element of one tile: the largest P below 448 (the last finite code) that is not ambiguous."""
+    ops_, kw, o, bd = _bound_case()
+    calls = []
+
+    def bump(p8, lo, hi):
+        calls.append(1)
+        if len(calls) != 3:
+            return p8
+        cand = torch.where((lo == hi) & (p8 < 448.0), p8, 0.0)
+        g, r, j = (int(x) for x in torch.unravel_index(cand.argmax(), cand.shape))
+        p8 = p8.clone()
+        p8[g, r, j] = (p8[g, r, j].to(E4M3).view(torch.uint8) + 1).view(E4M3).float()
+        return p8
+    moved = attn_int8_fp8_window(*ops_, window=(200, 37), p8_fn=bump, **kw)[0]
+    assert (moved != o).any(-1).sum() == 1 and _worst(moved, bd) > 1.0
+
+
+def test_bound_rejects_one_row_replaced_by_its_neighbour():
+    _, _, o, bd = _bound_case()
+    for r in (0, 127, 128, 350, 698):
+        bad = o.clone()
+        bad[0, 1, r] = o[0, 1, r + 1]
+        assert _worst(bad, bd) > 1.0, r
 
 
 # ------------------------------------------------------------------------------------------------ C entries and Python guards

@@ -511,6 +511,40 @@ int sab_qk_int8_attn_bwd_varlen_window(const int8_t* q_int8, const int8_t* k_int
                                        int max_seqlen_q, int max_seqlen_k, int is_causal, int q_gran, int k_gran, float sm_scale,
                                        int window_left, int window_right, void* stream);
 
+/* Attention against a paged KV cache (no reference counterpart): the building blocks of sageattn_varlen_kvcache.
+ *   The paged quantisers read K or V from a cache [num_pages, page_size, H, D] (`dtype`; page stride page_stride, slot stride
+ *   stride_t, head stride stride_h, in elements, each a multiple of 8, 16-byte aligned base) through block_table [nseq, *] int32
+ *   device (row stride table_stride): token t of sequence b is slot t % page_size of page block_table[b * table_stride + t /
+ *   page_size].  cu_seqlens [nseq+1] int32 device is the exclusive cumsum of the sequence lengths Lk_b (the tokens read) and places
+ *   sequence b of the outputs, which are exactly those of the packed entries above on the gathered tensor, bit for bit:
+ *   sab_k_mean_paged = sab_k_mean_varlen, sab_quant_int8_paged = sab_quant_int8_varlen with is_key = 1 (out [Tk,H,D] at row
+ *   cu_seqlens[b] + t), sab_per_channel_fp8_paged = sab_per_channel_fp8_varlen (v_fp8 [H,D,t_pad] at column cu_pad[b] + t).
+ *   Slots past Lk_b and pages the first ceil(Lk_b/page_size) table entries do not name are never read.  The table entries are
+ *   trusted: each must lie in [0, num_pages).  Workspaces: sab_k_mean_varlen_workspace_bytes / sab_per_channel_fp8_varlen_workspace_bytes.
+ * sab_qk_int8_sv_f8_attn_varlen_bottom_right: sab_qk_int8_sv_f8_attn_varlen with causal aligned bottom-right inside each sequence:
+ *   query i of sequence b sees key j iff j <= i + Lk_b - Lq_b (Lk_b < Lq_b allowed: its first Lq_b - Lk_b rows see no key and
+ *   return 0 and lse -inf).  For Lk_b >= Lq_b sequence b gets the bits of sab_qk_int8_sv_f8_attn_window on that sequence alone with
+ *   the window (-1, Lk_b - Lq_b), non-causal.  Non-causal (is_causal == 0) is sab_qk_int8_sv_f8_attn_varlen itself. */
+int sab_k_mean_paged(const void* k_cache, int dtype, void* mean, const int32_t* cu_seqlens, const int32_t* block_table,
+                     int64_t table_stride, int page_size, int nseq, int max_seqlen, int H, int D, int64_t page_stride, int64_t stride_t,
+                     int64_t stride_h, void* workspace, void* stream);
+int sab_quant_int8_paged(const void* k_cache, int dtype, const void* mean, int8_t* out, float* scale, const int32_t* cu_seqlens,
+                         const int32_t* cu_scale, const int32_t* block_table, int64_t table_stride, int page_size, int nseq,
+                         int max_seqlen, int H, int D, int64_t page_stride, int64_t stride_t, int64_t stride_h, int64_t o_stride_t,
+                         int64_t o_stride_h, int granularity, void* stream);
+int sab_per_channel_fp8_paged(const void* v_cache, int dtype, uint8_t* v_fp8, float* v_scale, float* v_mean, const int32_t* cu_seqlens,
+                              const int32_t* cu_pad, const int32_t* block_table, int64_t table_stride, int page_size, int nseq,
+                              int max_seqlen, int H, int D, int64_t page_stride, int64_t stride_t, int64_t stride_h, int64_t t_pad,
+                              float scale_max, void* workspace, void* stream);
+int sab_qk_int8_sv_f8_attn_varlen_bottom_right(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out, float* lse,
+                                               const float* q_scale, const float* k_scale, const float* v_scale, const float* v_mean,
+                                               int out_dtype, int nseq, int Hq, int Hkv, int Tq, int Tk, int D, int64_t q_stride_t,
+                                               int64_t q_stride_h, int64_t k_stride_t, int64_t k_stride_h, int64_t v_t_pad,
+                                               int64_t o_stride_t, int64_t o_stride_h, int is_causal, int q_gran, int k_gran,
+                                               float sm_scale, const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
+                                               const int32_t* cu_pad_v, const int32_t* cu_q_scale, const int32_t* cu_k_scale,
+                                               int max_seqlen_q, void* stream);
+
 /* Block-sparse forms of the packed per-sequence INT8+FP8 attention (no reference counterpart): sab_qk_int8_sv_f8_attn_varlen and
  * sab_qk_int8_attn_bwd_varlen_seq with the block mask of sab_qk_int8_sv_f8_attn_blocksparse, applied inside each sequence.
  *   block_mask : bool (uint8, 0 = hidden) [nseq or 1, Hq or 1, ceil(max_seqlen_q/128), ceil(max_seqlen_k/64)] read through the

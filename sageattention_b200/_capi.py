@@ -74,6 +74,13 @@ EXPORTS = {
                                                   [c_void_p] * 5 + [c_int, c_int, c_void_p] + [c_int64] * 4 + [c_void_p]),
     "sab_qk_int8_attn_bwd_varlen_blocksparse": (c_int, [c_void_p] * 15 + [c_int] * 7 + [c_int64] * 14 + [c_void_p] * 4 +
                                                 [c_int] * 5 + [c_float, c_void_p] + [c_int64] * 4 + [c_void_p]),
+    "sab_k_mean_paged": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int64] + [c_int] * 5 + [c_int64] * 3 +
+                         [c_void_p, c_void_p]),
+    "sab_quant_int8_paged": (c_int, [c_void_p, c_int] + [c_void_p] * 6 + [c_int64] + [c_int] * 5 + [c_int64] * 5 + [c_int, c_void_p]),
+    "sab_per_channel_fp8_paged": (c_int, [c_void_p, c_int] + [c_void_p] * 6 + [c_int64] + [c_int] * 5 + [c_int64] * 4 +
+                                  [c_float, c_void_p, c_void_p]),
+    "sab_qk_int8_sv_f8_attn_varlen_bottom_right": (c_int, [c_void_p] * 9 + [c_int] * 7 + [c_int64] * 7 + [c_int, c_int, c_int, c_float] +
+                                                   [c_void_p] * 5 + [c_int, c_void_p]),
     "sab_block_stats": (c_int, [c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 4 + [c_int64] * 3 + [c_int, c_void_p]),
     "sab_predict_block_mask": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_float] * 3 + [c_void_p]),
     "sab_block_stats_varlen": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 4 + [c_int64] * 2 + [c_int, c_void_p]),

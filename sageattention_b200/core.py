@@ -15,7 +15,8 @@ from . import ops
 from ._capi import SAB_GRAN_PER_BLOCK, SAB_GRAN_PER_WARP, SAB_GRAN_PER_THREAD
 from .quant import (k_mean, per_block_int8, per_warp_int8, per_thread_int8, per_channel_fp8, quant_q_int8, quant_k_int8, smooth_quant_k,
                     per_block_int8_varlen, per_channel_fp8_varlen, transpose_v_f16, transpose_v_f16_varlen, k_mean_varlen,
-                    quant_q_int8_varlen, quant_k_int8_varlen, per_channel_fp8_varlen_seq)
+                    quant_q_int8_varlen, quant_k_int8_varlen, per_channel_fp8_varlen_seq, k_mean_paged, quant_k_int8_paged,
+                    per_channel_fp8_paged)
 
 _LOG2E = 1.44269504
 _MAX_BLOCKSPARSE_KV = 1 << 20   # 64 * 16384 key blocks: the longest key range a block-sparse CTA compacts in shared memory
@@ -776,3 +777,117 @@ def _varlen_qk_int8_pv_fp8(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, ma
             return o, lse / _LOG2E + _lse_correction_varlen(q, km, cu_q) * sm_scale
         return o, lse / _LOG2E
     return o
+
+
+# ------------------------------------------------------------------------------------------------ paged KV cache
+def _check_on_cuda(q):
+    if not q.is_cuda:
+        raise ValueError("q must be a CUDA tensor: there is no CPU implementation")
+
+
+def _check_kvcache(q, k_cache, v_cache, cu_seqlens_q, seqused_k, block_table, max_seqlen_q):
+    """The shape, dtype and device rules of sageattn_varlen_kvcache, or ValueError (the CUDA device itself: _check_on_cuda)."""
+    if not isinstance(q, torch.Tensor) or q.dtype not in (torch.float16, torch.bfloat16) or q.dim() != 3:
+        raise ValueError("q must be a packed [Tq, Hq, D] fp16 / bf16 tensor")
+    _check_on_cuda(q)
+    for name, c in (("k_cache", k_cache), ("v_cache", v_cache)):
+        if not isinstance(c, torch.Tensor) or c.dim() != 4:
+            raise ValueError(f"{name} must be a [num_pages, page_size, Hkv, D] tensor")
+        if c.device != q.device or c.dtype != q.dtype:
+            raise ValueError(f"{name} must have q's device and dtype ({q.device}, {q.dtype}), got ({c.device}, {c.dtype})")
+        if c.stride(-1) != 1 or c.data_ptr() % 16 != 0 or any(s % 8 != 0 for s in c.stride()[:3]):
+            raise ValueError(f"{name} needs stride(-1) == 1 and 16-byte aligned rows (other strides multiples of 8 elements)")
+    if k_cache.shape != v_cache.shape:
+        raise ValueError(f"k_cache and v_cache must have the same shape (got {tuple(k_cache.shape)} and {tuple(v_cache.shape)})")
+    num_pages, page_size, Hkv, D = k_cache.shape
+    if D not in (64, 128) or q.size(2) != D:
+        raise ValueError(f"the head dim must be 64 or 128 and the same for q and the cache (q {q.size(2)}, cache {D})")
+    if num_pages < 1 or page_size < 1 or Hkv < 1 or q.size(1) % Hkv != 0:
+        raise ValueError(f"num_qo_heads ({q.size(1)}) must be divisible by num_kv_heads ({Hkv}), and the cache must not be empty")
+    if not isinstance(cu_seqlens_q, torch.Tensor) or cu_seqlens_q.dim() != 1 or cu_seqlens_q.dtype not in (torch.int32, torch.int64) \
+            or cu_seqlens_q.numel() < 2 or cu_seqlens_q.device != q.device:
+        raise ValueError("cu_seqlens_q must be a 1-D int32 or int64 tensor of nseq + 1 >= 2 offsets on q's device")
+    nseq = cu_seqlens_q.numel() - 1
+    if not isinstance(seqused_k, torch.Tensor) or tuple(seqused_k.shape) != (nseq,) or seqused_k.dtype != torch.int32 \
+            or seqused_k.device != q.device:
+        raise ValueError(f"seqused_k must be an int32 [{nseq}] tensor on q's device")
+    if not isinstance(block_table, torch.Tensor) or block_table.dim() != 2 or block_table.size(0) != nseq or block_table.size(1) < 1 \
+            or block_table.dtype != torch.int32 or block_table.device != q.device or block_table.stride(1) != 1:
+        raise ValueError(f"block_table must be an int32 [{nseq}, max_pages] tensor on q's device with contiguous rows")
+    if isinstance(max_seqlen_q, bool) or not isinstance(max_seqlen_q, numbers.Integral) or max_seqlen_q < 1:
+        raise ValueError(f"max_seqlen_q must be an int >= 1, got {max_seqlen_q!r}")
+    if q.size(0) == 0:
+        raise ValueError("the packed batch must hold at least one query")
+
+
+def sageattn_varlen_kvcache(q: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, cu_seqlens_q: torch.Tensor,
+                            seqused_k: torch.Tensor, block_table: torch.Tensor, max_seqlen_q: int, is_causal: bool = False,
+                            qk_quant_gran: str = "per_thread", sm_scale: Optional[float] = None, pv_accum_dtype: str = "fp32+fp16",
+                            smooth_k: bool = True, smooth_v: bool = False, return_lse: bool = False):
+    """Attention of packed queries against a paged KV cache (no reference counterpart): chunked prefill, prefix caching and
+    speculative verification, where each sequence's Lq_b new queries attend to Lk_b >= Lq_b keys of which the earlier ones are cached.
+
+    q: packed [Tq,Hq,D] with cu_seqlens_q (int32 or int64, nseq + 1 offsets) and max_seqlen_q, as in
+    sageattn_varlen_qk_int8_pv_fp8_cuda.  k_cache / v_cache: [num_pages, page_size, Hkv, D], the same shape, q's dtype, D 64 or 128
+    (no head-dim padding: it would copy the cache), Hq % Hkv == 0, stride(-1) == 1 and 16-byte aligned rows; other strides are free,
+    so a view such as kv_cache[0] of a [2, num_pages, ...] buffer is accepted.  block_table: int32 [nseq, max_pages]; token t of
+    sequence b is k_cache[block_table[b, t // page_size], t % page_size].  Pages may be shared between sequences (prefix sharing).
+    Entries past ceil(seqused_k[b] / page_size) are never read, nor are slots past seqused_k[b] in the last page.  Every entry read
+    must lie in [0, num_pages): like the cu_seqlens values, the table is trusted.  A padded, unpaged cache [nseq, S_cap, Hkv, D] is
+    the case page_size = S_cap, block_table = arange(nseq)[:, None].  seqused_k: int32 [nseq] on the device, Lk_b.
+
+    Synchronisation: the call copies seqused_k to the host once (the other packed entry points do not synchronise).  The host copy
+    checks 0 <= Lk_b <= max_pages * page_size (ValueError before any launch) and sizes the packed quantised K / V exactly.  The
+    quantisers read the pages directly: there is no gathered 16-bit copy of the cache.  Shape, dtype and device errors raise
+    ValueError before any launch; every other option (checks, warnings, V ranges, smooth_v rules) is that of
+    sageattn_varlen_qk_int8_pv_fp8_cuda.
+
+    Contract, with K_b / V_b the first Lk_b tokens of sequence b gathered from its pages:
+      * non-causal: the bits of sageattn_varlen_qk_int8_pv_fp8_cuda(q, Kp, Vp, cu_seqlens_q, [0, cumsum(seqused_k)], ...) on the
+        gathered sequences packed; every statistic (K mean, INT8 blocks, V scale and mean) is per sequence;
+      * is_causal: bottom-right, query i of sequence b sees key j iff j <= i + Lk_b - Lq_b.  For Lk_b >= Lq_b, sequence b's rows are
+        the bits of sageattn_window(q_b[None], K_b[None], V_b[None], window_size=(-1, Lk_b - Lq_b), tensor_layout="NHD",
+        is_causal=False, <same options>).  For Lk_b < Lq_b its first Lq_b - Lk_b rows see no key;
+      * a row that sees no key (Lk_b = 0, or the rows above) returns 0 and lse -inf; a sequence with Lq_b = 0 writes nothing, and rows
+        past cu_seqlens_q[-1] are not written.
+    return_lse: also returns the [Hq,Tq] fp32 LSE in natural-log units, with sageattn_varlen_qk_int8_pv_fp8_cuda's caveat on the
+    per-token K-mean correction.  Forward only: the output does not require grad."""
+    _check_kvcache(q, k_cache, v_cache, cu_seqlens_q, seqused_k, block_table, max_seqlen_q)
+    assert qk_quant_gran in ["per_warp", "per_thread"], "qk_quant_gran must be either 'per_warp' or 'per_thread'."
+    if pv_accum_dtype not in ("fp32", "fp32+fp32", "fp32+fp16"):
+        raise ValueError(f"Unsupported pv_accum_dtype: {pv_accum_dtype}")
+    page_size = k_cache.size(1)
+    lk = seqused_k.cpu().tolist()                       # the call's one device -> host copy
+    cap = block_table.size(1) * page_size
+    if any(n < 0 or n > cap for n in lk):
+        raise ValueError(f"seqused_k must lie in [0, max_pages * page_size] = [0, {cap}], got {lk}")
+    if sm_scale is None:
+        sm_scale = q.size(2) ** -0.5
+    if pv_accum_dtype in ("fp32+fp32", "fp32+fp16") and smooth_v:
+        warnings.warn(f"pv_accum_dtype is '{pv_accum_dtype}', smooth_v will be ignored.")
+        smooth_v = False
+    v_range = 2.25 if pv_accum_dtype == "fp32+fp16" else 448.0
+    max_seqlen_q = int(max_seqlen_q)
+    total_k, max_seqlen_k = sum(lk), max(lk)
+    with torch.no_grad():
+        if total_k == 0:                                # no sequence has a key: every row sees nothing
+            o = torch.zeros_like(q)
+            return (o, torch.full((q.size(1), q.size(0)), -float("inf"), dtype=torch.float32, device=q.device)) if return_lse else o
+        cu_q = cu_seqlens_q.to(torch.int32).contiguous()
+        cu_k = torch.nn.functional.pad(torch.cumsum(seqused_k, 0, dtype=torch.int32), (1, 0))
+        k_blocks = sum((n + 63) // 64 for n in lk)
+        t_pad = sum((n + 127) // 128 * 128 for n in lk)
+        km = k_mean_paged(k_cache, cu_k, block_table, max_seqlen_k) if smooth_k else None
+        q_int8, q_scale, cu_q_scale = quant_q_int8_varlen(q, cu_q, max_seqlen_q, qk_quant_gran)
+        k_int8, k_scale, cu_k_scale = quant_k_int8_paged(k_cache, km, cu_k, block_table, max_seqlen_k, total_k, k_blocks, qk_quant_gran)
+        v_fp8, v_scale, vm, cu_pad = per_channel_fp8_paged(v_cache, cu_k, block_table, max_seqlen_k, t_pad, v_range, smooth_v)
+        o = torch.empty(q.shape, dtype=q.dtype, device=q.device)
+        gran = SAB_GRAN_PER_WARP if qk_quant_gran == "per_warp" else SAB_GRAN_PER_THREAD
+        lse = ops.qk_int8_sv_f8_attn_varlen_bottom_right(q_int8, k_int8, v_fp8, o, q_scale, k_scale, v_scale, vm, cu_q, cu_k, cu_pad,
+                                                         cu_q_scale, cu_k_scale, max_seqlen_q, 1 if is_causal else 0, gran, gran,
+                                                         sm_scale, 1 if return_lse else 0)
+        if return_lse:
+            if smooth_k:
+                return o, lse / _LOG2E + _lse_correction_varlen(q, km, cu_q) * sm_scale
+            return o, lse / _LOG2E
+        return o

@@ -114,7 +114,10 @@ constexpr bool kSparse = kMask && !kPV16;     // block mask of the INT8+FP8 path
 // kMask (block-sparse) with kSeqV: the packed block-sparse form.  b is the sequence and qt its own Q tile, so the CTA compacts mask
 // row (b, h, qt) of a [nseq,Hq,ceil(max_seqlen_q/128),ceil(max_seqlen_k/64)] mask, cut at its sequence's n_kv and causal horizon:
 // the dense block-sparse kernel's path on that sequence alone.
-template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false, bool kWindow = false, bool kSeqV = false>
+// kBR with kWindow and kSeqV: the packed bottom-right causal form.  Sequence b's rows see the window (-1, Lk_b - Lq_b), derived
+// here instead of read from win_arg: the window kernel's path on that window, tile for tile.  The right side may be negative
+// (Lk_b < Lq_b: the first Lq_b - Lk_b rows see no key) and always bounds, so it is read as bounded whatever its sign.
+template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false, bool kWindow = false, bool kSeqV = false, bool kBR = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnParams p,
@@ -140,7 +143,7 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 
   // ---------------- work decode (uniform across the CTA)
   int qt = blockIdx.x;
-  if (p.causal) qt = p.n_q_tiles - 1 - qt;  // heaviest tiles first
+  if (p.causal || kBR) qt = p.n_q_tiles - 1 - qt;  // heaviest tiles first
   const int h = blockIdx.y;
   const int b = blockIdx.z;
   const int hk = h / (p.Hq / p.Hkv);
@@ -160,7 +163,7 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   }
   // the packed window form reads its sequence's clamped copy; every other form reads the kernel argument itself
   [[maybe_unused]] Window seq_win;
-  if constexpr (kWindow && kSeqV) seq_win = seq_window(win_arg, q_len, kv_len);
+  if constexpr (kWindow && kSeqV) seq_win = kBR ? Window{-1, kv_len - q_len} : seq_window(win_arg, q_len, kv_len);
   const Window& win = (kWindow && kSeqV) ? seq_win : win_arg;
   int n_kv = (kv_len + BN - 1) / BN;                 // 64-key tiles
   if (p.causal) n_kv = min(n_kv, (p.causal_q_offset + (qt + 1) * BM + BN - 1) / BN);
@@ -171,7 +174,7 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   [[maybe_unused]] int j0 = 0;   // window form: the first 64-key tile of the CTA's range
   if constexpr (kWindow) {
     int j1;
-    window_tiles(win, p.causal != 0, qt * BM, min(qt * BM + BM, q_len) - 1, kv_len, j0, j1);
+    window_tiles<kBR>(win, p.causal != 0, qt * BM, min(qt * BM + BM, q_len) - 1, kv_len, j0, j1);
     n_kv = j1 - j0;
   }
 
@@ -280,14 +283,14 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       if (p.causal) limit[i] = min(limit[i], p.causal_q_offset + q_row[i] - kj * BN + 1);
       if (kElemMask<kPV16, kMask> && q_row[i] >= q_len) limit[i] = 0;   // rows past the end: nothing visible, no mask bytes read
       if constexpr (kWindow) {
-        if (win.right >= 0) limit[i] = min(limit[i], q_row[i] + win.right + 1 - kj * BN);
+        if (kBR || win.right >= 0) limit[i] = min(limit[i], q_row[i] + win.right + 1 - kj * BN);
         lo[i] = win.left >= 0 ? q_row[i] - win.left - kj * BN : 0;
       }
     }
     masked_tile = kElemMask<kPV16, kMask> || (kv_len - kj * BN < BN) || (p.causal && (kj + 1) * BN > p.causal_q_offset + qt * BM + 1);
     if constexpr (kWindow) {
       // the top row's window ends inside the tile, or the bottom row's starts after its first key
-      masked_tile = masked_tile || (win.right >= 0 && (kj + 1) * BN - 1 > qt * BM + win.right) ||
+      masked_tile = masked_tile || ((kBR || win.right >= 0) && (kj + 1) * BN - 1 > qt * BM + win.right) ||
                     (win.left >= 0 && kj * BN < qt * BM + BM - 1 - win.left);
     }
   };
@@ -669,14 +672,14 @@ static int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUten
   return SAB_OK;
 }
 
-// the sliding-window form (sage_attn_fwd_kernel<D, kKT, OutT, false, false, true, kSeqV>); kSeqV: the packed form with
-// per-sequence V statistics
-template <int D, bool kKT, typename OutT, bool kSeqV = false>
+// the sliding-window form (sage_attn_fwd_kernel<D, kKT, OutT, false, false, true, kSeqV, kBR>); kSeqV: the packed form with
+// per-sequence V statistics; kBR (with kSeqV): the packed bottom-right causal form, whose kernel ignores w
+template <int D, bool kKT, typename OutT, bool kSeqV = false, bool kBR = false>
 static int launch_attn_window(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, AttnParams p, Window w,
                               dim3 grid, cudaStream_t stream) {
   p.lazy_tau = exact_max_mode() ? 0.0f : kLazyTau;
   constexpr size_t smem = attn_smem_bytes<D, false>();
-  auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, false, true, kSeqV>;
+  auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, false, true, kSeqV, kBR>;
   static bool configured[64] = {};
   if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
   kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p, w);
@@ -869,6 +872,19 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
     SAB_REQUIRE(!pv16 && (!varlen || tl_seq_v) && kv_seg_len == 0 && causal_q_offset == 0, SAB_ERR_UNSUPPORTED,
                 "the window is supported by the dense and the packed (per-sequence) single-GPU INT8/FP8 paths only");
     const Window w = *tl_window;
+    if (tl_seq_v && w.right == kWindowBottomRight) {
+      SAB_REQUIRE(!is_causal, SAB_ERR_INVALID, "the bottom-right causal form takes is_causal = 0");
+      if (D == 128) {
+        if (kt) return bf ? launch_attn_window<128, true, __nv_bfloat16, true, true>(tq, tk, tv, p, w, grid, s)
+                          : launch_attn_window<128, true, __half, true, true>(tq, tk, tv, p, w, grid, s);
+        return bf ? launch_attn_window<128, false, __nv_bfloat16, true, true>(tq, tk, tv, p, w, grid, s)
+                  : launch_attn_window<128, false, __half, true, true>(tq, tk, tv, p, w, grid, s);
+      }
+      if (kt) return bf ? launch_attn_window<64, true, __nv_bfloat16, true, true>(tq, tk, tv, p, w, grid, s)
+                        : launch_attn_window<64, true, __half, true, true>(tq, tk, tv, p, w, grid, s);
+      return bf ? launch_attn_window<64, false, __nv_bfloat16, true, true>(tq, tk, tv, p, w, grid, s)
+                : launch_attn_window<64, false, __half, true, true>(tq, tk, tv, p, w, grid, s);
+    }
     if (tl_seq_v) {
       if (D == 128) {
         if (kt) return bf ? launch_attn_window<128, true, __nv_bfloat16, true>(tq, tk, tv, p, w, grid, s)
@@ -1067,6 +1083,33 @@ extern "C" int sab_qk_int8_sv_f8_attn_varlen_window(const int8_t* q_int8, const 
   const int st = sab_qk_int8_sv_f8_attn_varlen(q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq,
                                                Hkv, Tq, Tk, D, q_stride_t, q_stride_h, k_stride_t, k_stride_h, v_t_pad, o_stride_t,
                                                o_stride_h, is_causal, q_gran, k_gran, sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v,
+                                               cu_q_scale, cu_k_scale, max_seqlen_q, stream);
+  tl_window = nullptr;
+  return st;
+}
+
+extern "C" int sab_qk_int8_sv_f8_attn_varlen_bottom_right(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out,
+                                                          float* lse, const float* q_scale, const float* k_scale,
+                                                          const float* v_scale, const float* v_mean, int out_dtype, int nseq, int Hq,
+                                                          int Hkv, int Tq, int Tk, int D, int64_t q_stride_t, int64_t q_stride_h,
+                                                          int64_t k_stride_t, int64_t k_stride_h, int64_t v_t_pad, int64_t o_stride_t,
+                                                          int64_t o_stride_h, int is_causal, int q_gran, int k_gran, float sm_scale,
+                                                          const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
+                                                          const int32_t* cu_pad_v, const int32_t* cu_q_scale,
+                                                          const int32_t* cu_k_scale, int max_seqlen_q, void* stream) {
+  SAB_REQUIRE(cu_seqlens_q && cu_seqlens_k && cu_pad_v && cu_q_scale && cu_k_scale && nseq > 0, SAB_ERR_INVALID,
+              "the packed bottom-right form needs cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale and nseq > 0");
+  // non-causal has no alignment: the packed form itself
+  if (!is_causal)
+    return sab_qk_int8_sv_f8_attn_varlen(q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq, Hkv,
+                                         Tq, Tk, D, q_stride_t, q_stride_h, k_stride_t, k_stride_h, v_t_pad, o_stride_t, o_stride_h, 0,
+                                         q_gran, k_gran, sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale,
+                                         max_seqlen_q, stream);
+  const sab::Window w{-1, sab::kWindowBottomRight};
+  tl_window = &w;
+  const int st = sab_qk_int8_sv_f8_attn_varlen(q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq,
+                                               Hkv, Tq, Tk, D, q_stride_t, q_stride_h, k_stride_t, k_stride_h, v_t_pad, o_stride_t,
+                                               o_stride_h, 0, q_gran, k_gran, sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v,
                                                cu_q_scale, cu_k_scale, max_seqlen_q, stream);
   tl_window = nullptr;
   return st;

@@ -160,12 +160,19 @@ struct Window {
   int left, right;                 // key j visible to query i iff i - left <= j <= i + right (top-left); -1: that side unbounded
 };
 
+// Window::right of the packed bottom-right causal form (sab_qk_int8_sv_f8_attn_varlen_kvcache), as handed to the launch: sequence
+// b's right side is Lk_b - Lq_b.  That side may be negative and is never unbounded, so the kernel derives it per sequence under
+// its own flag (kBR) and reads it with kRightBounded below; this value only selects that kernel.
+constexpr int kWindowBottomRight = -(1 << 30);
+
 // The 64-key tiles [j_lo, j_hi) that hold a key visible to some row of [r_lo, r_hi] (r_hi inclusive): the window, the causal
-// horizon and kv_len.  Empty (j_lo == j_hi) when no row of the range sees any key.
+// horizon and kv_len.  Empty (j_lo == j_hi) when no row of the range sees any key.  kRightBounded: w.right bounds the right side
+// whatever its sign (a negative right side hides keys up to |right| before the row's own position).
+template <bool kRightBounded = false>
 __device__ __forceinline__ void window_tiles(const Window& w, bool causal, int r_lo, int r_hi, int kv_len, int& j_lo, int& j_hi) {
   const int k_lo = w.left < 0 ? 0 : max(0, r_lo - w.left);
   int k_hi = kv_len - 1;
-  if (w.right >= 0) k_hi = min(k_hi, r_hi + w.right);
+  if (kRightBounded || w.right >= 0) k_hi = min(k_hi, r_hi + w.right);
   if (causal) k_hi = min(k_hi, r_hi);
   j_lo = k_lo / BN;
   j_hi = k_hi >= k_lo ? k_hi / BN + 1 : j_lo;

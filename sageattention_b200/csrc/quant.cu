@@ -5,6 +5,7 @@
 // 64/128-bit stores.  Semantics follow csrc/fused/fused.cu and sageattention/triton/quant_per_*.py of the
 // reference (see include/sageattn_b200.h for the per-entry citations).
 #include <cstdlib>
+#include <type_traits>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include "common.cuh"
@@ -77,6 +78,31 @@ __device__ __forceinline__ uint32_t pack_e4m3x4_q(float a, float b, float c, flo
   return r;
 }
 
+// How the per-sequence kernels address input row r (r < L_b) of sequence b, relative to the base of its head: `first` is the
+// offset of the sequence's first row, `row` the offset of row r from there (ss: the row stride of the input).
+// PackedRows: packed [T,H,D] (or one dense batch entry), row r at token t0 + r.  The contiguous kernels use it, and it spells the
+// same index arithmetic they had, so their code is unchanged.
+struct PackedRows {
+  __device__ __forceinline__ int64_t first(int t0, int64_t ss) const { return int64_t(t0) * ss; }
+  __device__ __forceinline__ int64_t row(int r, int64_t ss) const { return int64_t(r) * ss; }
+};
+// A paged cache [num_pages, page_size, H, D] (page stride page_stride, slot stride ss) with a block table: row r of sequence b
+// is slot r % page_size of page table[b][r / page_size].  Indexed in int64: a cache can hold more than 2^31 elements.
+struct PageTable {
+  const int32_t* table; int64_t table_stride;   // [nseq, max_pages] int32, row stride table_stride
+  int page_size; int64_t page_stride;
+};
+struct PagedRows {
+  const int32_t* table;   // this sequence's row of the block table
+  int page_size; int64_t page_stride;
+  __device__ __forceinline__ PagedRows(const PageTable& pt, int b)
+      : table(pt.table + int64_t(b) * pt.table_stride), page_size(pt.page_size), page_stride(pt.page_stride) {}
+  __device__ __forceinline__ int64_t first(int, int64_t) const { return 0; }
+  __device__ __forceinline__ int64_t row(int r, int64_t ss) const {
+    return int64_t(__ldg(table + r / page_size)) * page_stride + int64_t(r % page_size) * ss;
+  }
+};
+
 // =====================================================================================================
 // Channel statistics over the token dimension: per (b,h,d) sum / max / min.  Two deterministic stages
 // (no atomics): stage 1 reduces 1024-token chunks, stage 2 folds the chunk partials in order.
@@ -85,10 +111,10 @@ constexpr int kStatChunk = 1024;
 
 // kSeq: packed [T,H,D] input, blockIdx.z = sequence b = tokens [cu[b], cu[b+1]); its chunks start at the sequence's first token, so
 // the partials of a sequence are those of the dense call on that sequence alone.
-template <typename T, int D, bool kSeq = false>
-__global__ void __launch_bounds__(256) channel_stats_stage1(const T* __restrict__ x, float* __restrict__ part, int S,
-                                                             int64_t sb, int64_t sh, int64_t ss, int nchunk,
-                                                             const int32_t* __restrict__ cu = nullptr) {
+// Rows: how a row of sequence b is addressed (kSeq only; channel_stats_stage1_paged reads a paged cache).
+template <typename T, int D, bool kSeq, typename Rows = PackedRows>
+__device__ __forceinline__ void channel_stats_chunk(const T* __restrict__ x, float* __restrict__ part, int S, int64_t sb, int64_t sh,
+                                                    int64_t ss, int nchunk, const int32_t* __restrict__ cu, const Rows rows = Rows{}) {
   constexpr int TPR = D / 8;        // threads per token row
   constexpr int RPP = 256 / TPR;    // rows per pass
   const int chunk = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
@@ -98,7 +124,7 @@ __global__ void __launch_bounds__(256) channel_stats_stage1(const T* __restrict_
     const int t0 = cu[b];
     S = cu[b + 1] - t0;
     if (chunk * kStatChunk >= S) return;
-    base += int64_t(t0) * ss;
+    base += rows.first(t0, ss);
   }
   float sum[8], mx[8], mn[8];
 #pragma unroll
@@ -107,7 +133,7 @@ __global__ void __launch_bounds__(256) channel_stats_stage1(const T* __restrict_
   const int r1 = min(S, r0 + kStatChunk);
   for (int r = r0 + tr; r < r1; r += RPP) {
     float f[8];
-    load8<T>(base + int64_t(r) * ss, f);
+    load8<T>(base + rows.row(r, ss), f);
 #pragma unroll
     for (int i = 0; i < 8; ++i) { sum[i] += f[i]; mx[i] = fmaxf(mx[i], f[i]); mn[i] = fminf(mn[i], f[i]); }
   }
@@ -121,6 +147,20 @@ __global__ void __launch_bounds__(256) channel_stats_stage1(const T* __restrict_
     float* o = part + ((int64_t(b) * gridDim.y + h) * nchunk + chunk) * 3 * D;
     o[threadIdx.x] = a; o[D + threadIdx.x] = m1; o[2 * D + threadIdx.x] = m2;
   }
+}
+
+template <typename T, int D, bool kSeq = false>
+__global__ void __launch_bounds__(256) channel_stats_stage1(const T* __restrict__ x, float* __restrict__ part, int S,
+                                                             int64_t sb, int64_t sh, int64_t ss, int nchunk,
+                                                             const int32_t* __restrict__ cu = nullptr) {
+  channel_stats_chunk<T, D, kSeq>(x, part, S, sb, sh, ss, nchunk, cu);
+}
+// the kSeq form on a paged cache: sequence b's rows through its block-table row; cu: the packed offsets, i.e. the lengths
+template <typename T, int D>
+__global__ void __launch_bounds__(256) channel_stats_stage1_paged(const T* __restrict__ x, float* __restrict__ part, int64_t sh,
+                                                                   int64_t ss, int nchunk, const int32_t* __restrict__ cu,
+                                                                   const PageTable pt) {
+  channel_stats_chunk<T, D, true>(x, part, 0, 0, sh, ss, nchunk, cu, PagedRows(pt, blockIdx.z));
 }
 
 // mode 0: K mean -> T [B,H,D].  mode 1: V scale (+ mean) -> fp32.  mode 2: raw sum / max / min -> fp32.
@@ -240,8 +280,10 @@ __device__ __forceinline__ int seq_scale_mult(int blk) {
 //               half-integer (ties, or the 2.4e-5 error of x*RN(1/scale) against the IEEE quotient could matter);
 //               one |y - n| maximum per 8 elements decides, and those rare rows redo the exact reference sequence.
 // One 128-row tile of one (b,h).  `mean_bh`: the D per-channel means of this (b,h) (global or shared memory), or nullptr.
-template <typename T, int D, int MODE, int FLAGS>
-__device__ __forceinline__ void quant_int8_tile(const QuantParams& p, const int tile, const int h, const int b, const T* mean_bh) {
+// Rows: how a row of sequence b is addressed (varlen only; quant_int8_paged_kernel reads a paged cache).
+template <typename T, int D, int MODE, int FLAGS, typename Rows = PackedRows>
+__device__ __forceinline__ void quant_int8_tile(const QuantParams& p, const int tile, const int h, const int b, const T* mean_bh,
+                                                const Rows rows = Rows{}) {
   constexpr bool kTriton = (FLAGS & kQfTriton) != 0, kMean = (FLAGS & kQfMean) != 0, kSms = (FLAGS & kQfSmScale) != 0;
   constexpr int TPR = D / 8;
   constexpr int RPP = 256 / TPR;     // 16 (D=128) / 32 (D=64)
@@ -255,7 +297,7 @@ __device__ __forceinline__ void quant_int8_tile(const QuantParams& p, const int 
     const int t0 = p.cu[b];
     S = p.cu[b + 1] - t0;
     if (tile * 128 >= S) return;
-    x_off = int64_t(t0) * p.xss + int64_t(h) * p.xsh;
+    x_off = rows.first(t0, p.xss) + int64_t(h) * p.xsh;
     o_off = int64_t(t0) * p.oss + int64_t(h) * p.osh;
     scale_row0 = p.cu_scale[b];
     if constexpr ((FLAGS & kQfSeq) != 0) scale_row0 *= seq_scale_mult<MODE>(p.blk);
@@ -283,7 +325,7 @@ __device__ __forceinline__ void quant_int8_tile(const QuantParams& p, const int 
   for (int ps = 0; ps < NP; ++ps) {
     const int row = tile * 128 + ps * RPP + tr;
     raw[ps] = make_uint4(0, 0, 0, 0);
-    if (row < S) raw[ps] = *reinterpret_cast<const uint4*>(xb + int64_t(row) * p.xss);
+    if (row < S) raw[ps] = *reinterpret_cast<const uint4*>(xb + rows.row(row, p.xss));
   }
   // transform of one word before the sm_scale multiply: x - mean (Triton: `k - km` rounds to the input dtype)
   auto centred = [&](uint32_t w, int wi, float& lo, float& hi) {
@@ -459,6 +501,16 @@ __global__ void __launch_bounds__(256, 3) quant_int8_kernel(const QuantParams p)
     mean_bh = reinterpret_cast<const T*>(p.mean) + (int64_t((FLAGS & kQfSeq) == 0 && p.cu != nullptr ? 0 : b) * p.H + h) * D;
   quant_int8_tile<T, D, MODE, FLAGS>(p, blockIdx.x, h, b, mean_bh);
 }
+// the per-sequence form (kQfSeq) on a paged cache: sequence b's input rows through its block-table row; the output, the scales and
+// p.cu (the packed offsets) are those of the packed form
+template <typename T, int D, int MODE, int FLAGS>
+__global__ void __launch_bounds__(256, 3) quant_int8_paged_kernel(const QuantParams p, const PageTable pt) {
+  static_assert((FLAGS & kQfSeq) != 0, "the paged input exists for the per-sequence form only");
+  const int h = blockIdx.y, b = blockIdx.z;
+  const T* mean_bh = nullptr;
+  if constexpr ((FLAGS & kQfMean) != 0) mean_bh = reinterpret_cast<const T*>(p.mean) + (int64_t(b) * p.H + h) * D;
+  quant_int8_tile<T, D, MODE, FLAGS>(p, blockIdx.x, h, b, mean_bh, PagedRows(pt, b));
+}
 
 // =====================================================================================================
 // Single-pass K path: K smoothing mean + INT8 quantisation in ONE launch.  A thread-block cluster of
@@ -553,9 +605,10 @@ struct VQuantParams {
 };
 
 // One 128-token tile.  recp_bh / vmean_bh: the D per-channel values of this (b,h) (global or shared memory; vmean may be null).
-template <typename T, int D>
+// Rows: how a row of sequence b is addressed (varlen only; v_quant_transpose_paged_kernel reads a paged cache).
+template <typename T, int D, typename Rows = PackedRows>
 __device__ __forceinline__ void v_quant_transpose_tile(const VQuantParams& p, const int tile, const int h, const int b,
-                                                       const float* recp_bh, const float* vmean_bh) {
+                                                       const float* recp_bh, const float* vmean_bh, const Rows rows = Rows{}) {
   constexpr int TPR = D / 8;
   constexpr int RPP = 256 / TPR;
   int S = p.S, tok0 = 0;
@@ -569,12 +622,16 @@ __device__ __forceinline__ void v_quant_transpose_tile(const VQuantParams& p, co
   }
   __shared__ __align__(16) T s_in[128][D + 8];  // +8 elements: conflict-free column reads
   const int tr = threadIdx.x / TPR, tc = threadIdx.x % TPR;
-  const T* vb = reinterpret_cast<const T*>(p.v) + (varlen ? int64_t(tok0) * p.ss : int64_t(b) * p.sb) + int64_t(h) * p.sh + tc * 8;
+  // packed rows keep the plain conditional: with the call in it, the compiler schedules the dense caller v_scale_quant_kernel anew
+  int64_t seq0;
+  if constexpr (std::is_same_v<Rows, PackedRows>) seq0 = varlen ? int64_t(tok0) * p.ss : int64_t(b) * p.sb;
+  else seq0 = rows.first(tok0, p.ss);
+  const T* vb = reinterpret_cast<const T*>(p.v) + seq0 + int64_t(h) * p.sh + tc * 8;
 #pragma unroll
   for (int r = tr; r < 128; r += RPP) {
     const int row = tile * 128 + r;
     uint4 raw = make_uint4(0, 0, 0, 0);
-    if (row < S) raw = *reinterpret_cast<const uint4*>(vb + int64_t(row) * p.ss);
+    if (row < S) raw = *reinterpret_cast<const uint4*>(vb + rows.row(row, p.ss));
     *reinterpret_cast<uint4*>(&s_in[r][tc * 8]) = raw;
   }
   __syncthreads();
@@ -609,6 +666,13 @@ __global__ void __launch_bounds__(256) v_quant_transpose_kernel(const VQuantPara
   const int h = blockIdx.y, b = blockIdx.z;
   const int64_t bh = int64_t(!kSeq && p.cu != nullptr ? 0 : b) * p.H + h;
   v_quant_transpose_tile<T, D>(p, blockIdx.x, h, b, p.recp + bh * D, p.vmean ? p.vmean + bh * D : nullptr);
+}
+// the kSeq form on a paged cache: sequence b's input rows through its block-table row; v_fp8, p.cu and p.cu_pad as in the packed form
+template <typename T, int D>
+__global__ void __launch_bounds__(256) v_quant_transpose_paged_kernel(const VQuantParams p, const PageTable pt) {
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int64_t bh = int64_t(b) * p.H + h;
+  v_quant_transpose_tile<T, D>(p, blockIdx.x, h, b, p.recp + bh * D, p.vmean ? p.vmean + bh * D : nullptr, PagedRows(pt, b));
 }
 
 // Single-pass V path: per-channel |max| (+ mean for smooth_v) and the e4m3 quantisation + transpose in ONE launch, same cluster
@@ -768,11 +832,17 @@ static int launch_quant_t(const QuantParams& p, int mode, dim3 grid, cudaStream_
     default: return launch_quant_f<T, D, 7>(p, mode, grid, st);
   }
 }
-// the per-sequence varlen form: per-thread Q / K (Triton semantics) and per-warp Q / K (CUDA semantics); a mean on K only
+// the per-sequence varlen form: per-thread Q / K (Triton semantics) and per-warp Q / K (CUDA semantics); a mean on K only.
+// pg: K read from a paged cache (nullptr: packed input).
 template <typename T, int D>
-static int launch_quant_seq_t(const QuantParams& p, int mode, dim3 grid, cudaStream_t st) {
+static int launch_quant_seq_t(const QuantParams& p, int mode, dim3 grid, cudaStream_t st, const PageTable* pg) {
   const bool mean = p.mean != nullptr;
-  if (mode == kGroupThreadQ) quant_int8_kernel<T, D, kGroupThreadQ, kQfTriton | kQfSeq><<<grid, 256, 0, st>>>(p);
+  if (pg != nullptr) {
+    if (mode == kGroupThreadK && mean) quant_int8_paged_kernel<T, D, kGroupThreadK, kQfTriton | kQfMean | kQfSeq><<<grid, 256, 0, st>>>(p, *pg);
+    else if (mode == kGroupThreadK) quant_int8_paged_kernel<T, D, kGroupThreadK, kQfTriton | kQfSeq><<<grid, 256, 0, st>>>(p, *pg);
+    else if (mean) quant_int8_paged_kernel<T, D, kGroupBlock, kQfMean | kQfSeq><<<grid, 256, 0, st>>>(p, *pg);
+    else quant_int8_paged_kernel<T, D, kGroupBlock, kQfSeq><<<grid, 256, 0, st>>>(p, *pg);
+  } else if (mode == kGroupThreadQ) quant_int8_kernel<T, D, kGroupThreadQ, kQfTriton | kQfSeq><<<grid, 256, 0, st>>>(p);
   else if (mode == kGroupThreadK && mean) quant_int8_kernel<T, D, kGroupThreadK, kQfTriton | kQfMean | kQfSeq><<<grid, 256, 0, st>>>(p);
   else if (mode == kGroupThreadK) quant_int8_kernel<T, D, kGroupThreadK, kQfTriton | kQfSeq><<<grid, 256, 0, st>>>(p);
   else if (mean) quant_int8_kernel<T, D, kGroupBlock, kQfMean | kQfSeq><<<grid, 256, 0, st>>>(p);
@@ -780,9 +850,9 @@ static int launch_quant_seq_t(const QuantParams& p, int mode, dim3 grid, cudaStr
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
 }
-static int launch_quant_seq(const QuantParams& p, int dtype, int D, int mode, dim3 grid, cudaStream_t st) {
-  if (dtype == SAB_DTYPE_FP16) return D == 128 ? launch_quant_seq_t<__half, 128>(p, mode, grid, st) : launch_quant_seq_t<__half, 64>(p, mode, grid, st);
-  return D == 128 ? launch_quant_seq_t<__nv_bfloat16, 128>(p, mode, grid, st) : launch_quant_seq_t<__nv_bfloat16, 64>(p, mode, grid, st);
+static int launch_quant_seq(const QuantParams& p, int dtype, int D, int mode, dim3 grid, cudaStream_t st, const PageTable* pg) {
+  if (dtype == SAB_DTYPE_FP16) return D == 128 ? launch_quant_seq_t<__half, 128>(p, mode, grid, st, pg) : launch_quant_seq_t<__half, 64>(p, mode, grid, st, pg);
+  return D == 128 ? launch_quant_seq_t<__nv_bfloat16, 128>(p, mode, grid, st, pg) : launch_quant_seq_t<__nv_bfloat16, 64>(p, mode, grid, st, pg);
 }
 
 static int launch_quant(const QuantParams& p, int dtype, int D, int mode, dim3 grid, cudaStream_t st) {
@@ -1055,31 +1125,33 @@ extern "C" int64_t sab_per_channel_fp8_varlen_workspace_bytes(int nseq, int H, i
 
 template <typename T, int D>
 static void launch_stats_seq(const void* x, float* part, const int32_t* cu, int nseq, int H, int nchunk, int64_t sh, int64_t ss,
-                             cudaStream_t st) {
-  channel_stats_stage1<T, D, true><<<dim3(nchunk, H, nseq), 256, 0, st>>>(reinterpret_cast<const T*>(x), part, 0, 0, sh, ss, nchunk, cu);
+                             cudaStream_t st, const PageTable* pg) {
+  const dim3 grid(nchunk, H, nseq);
+  if (pg != nullptr) channel_stats_stage1_paged<T, D><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(x), part, sh, ss, nchunk, cu, *pg);
+  else channel_stats_stage1<T, D, true><<<grid, 256, 0, st>>>(reinterpret_cast<const T*>(x), part, 0, 0, sh, ss, nchunk, cu);
 }
 static int run_stats_seq(const void* x, int dtype, float* part, const int32_t* cu, int nseq, int H, int nchunk, int D, int64_t sh,
-                         int64_t ss, cudaStream_t st) {
+                         int64_t ss, cudaStream_t st, const PageTable* pg) {
   if (dtype == SAB_DTYPE_FP16) {
-    if (D == 128) launch_stats_seq<__half, 128>(x, part, cu, nseq, H, nchunk, sh, ss, st);
-    else launch_stats_seq<__half, 64>(x, part, cu, nseq, H, nchunk, sh, ss, st);
+    if (D == 128) launch_stats_seq<__half, 128>(x, part, cu, nseq, H, nchunk, sh, ss, st, pg);
+    else launch_stats_seq<__half, 64>(x, part, cu, nseq, H, nchunk, sh, ss, st, pg);
   } else {
-    if (D == 128) launch_stats_seq<__nv_bfloat16, 128>(x, part, cu, nseq, H, nchunk, sh, ss, st);
-    else launch_stats_seq<__nv_bfloat16, 64>(x, part, cu, nseq, H, nchunk, sh, ss, st);
+    if (D == 128) launch_stats_seq<__nv_bfloat16, 128>(x, part, cu, nseq, H, nchunk, sh, ss, st, pg);
+    else launch_stats_seq<__nv_bfloat16, 64>(x, part, cu, nseq, H, nchunk, sh, ss, st, pg);
   }
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
 }
 
-extern "C" int sab_k_mean_varlen(const void* k, int dtype, void* mean, const int32_t* cu_seqlens, int nseq, int max_seqlen, int H,
-                                 int D, int64_t stride_t, int64_t stride_h, void* workspace, void* stream) {
-  int st = check_common(k, dtype, D, 0, stride_h, stride_t);
-  if (st) return st;
+// The per-sequence front-end on packed input (pg == nullptr) or on a paged cache (pg: block table and page geometry).  The
+// sequences, their lengths and every output layout come from cu_seqlens in both cases; only the input rows are addressed differently.
+static int k_mean_seq(const void* k, int dtype, void* mean, const int32_t* cu_seqlens, int nseq, int max_seqlen, int H, int D,
+                      int64_t stride_t, int64_t stride_h, void* workspace, void* stream, const PageTable* pg) {
   SAB_REQUIRE(mean && workspace && cu_seqlens && nseq > 0 && max_seqlen > 0 && H > 0, SAB_ERR_INVALID, "bad arguments to sab_k_mean_varlen");
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const int nchunk = (max_seqlen + kStatChunk - 1) / kStatChunk;
   float* part = reinterpret_cast<float*>(workspace);
-  if ((st = run_stats_seq(k, dtype, part, cu_seqlens, nseq, H, nchunk, D, stride_h, stride_t, s))) return st;
+  if (int st = run_stats_seq(k, dtype, part, cu_seqlens, nseq, H, nchunk, D, stride_h, stride_t, s, pg)) return st;
   if (dtype == SAB_DTYPE_FP16)
     channel_stats_stage2<__half, true><<<dim3(H, nseq), 128, 0, s>>>(part, nchunk, D, 0, 0, reinterpret_cast<__half*>(mean), nullptr,
                                                                      nullptr, 0.f, nullptr, cu_seqlens);
@@ -1090,12 +1162,9 @@ extern "C" int sab_k_mean_varlen(const void* k, int dtype, void* mean, const int
   return SAB_OK;
 }
 
-extern "C" int sab_quant_int8_varlen(const void* x, int dtype, const void* mean, int8_t* out, float* scale, const int32_t* cu_seqlens,
-                                     const int32_t* cu_scale, int nseq, int max_seqlen, int H, int D, int64_t x_stride_t,
-                                     int64_t x_stride_h, int64_t o_stride_t, int64_t o_stride_h, int granularity, int is_key,
-                                     void* stream) {
-  int st = check_common(x, dtype, D, 0, x_stride_h, x_stride_t);
-  if (st) return st;
+static int quant_int8_seq(const void* x, int dtype, const void* mean, int8_t* out, float* scale, const int32_t* cu_seqlens,
+                          const int32_t* cu_scale, int nseq, int max_seqlen, int H, int D, int64_t x_stride_t, int64_t x_stride_h,
+                          int64_t o_stride_t, int64_t o_stride_h, int granularity, int is_key, void* stream, const PageTable* pg) {
   SAB_REQUIRE(out && scale && cu_seqlens && cu_scale && nseq > 0 && max_seqlen > 0 && H > 0, SAB_ERR_INVALID,
               "bad arguments to sab_quant_int8_varlen");
   SAB_REQUIRE(granularity == SAB_GRAN_PER_WARP || granularity == SAB_GRAN_PER_THREAD, SAB_ERR_INVALID,
@@ -1114,15 +1183,12 @@ extern "C" int sab_quant_int8_varlen(const void* x, int dtype, const void* mean,
   p.has_sm_scale = 0; p.sm_scale = 1.f;
   p.cu = cu_seqlens; p.cu_scale = cu_scale;
   const int mode = pt ? (is_key ? kGroupThreadK : kGroupThreadQ) : kGroupBlock;
-  return launch_quant_seq(p, dtype, D, mode, dim3((max_seqlen + 127) / 128, H, nseq), reinterpret_cast<cudaStream_t>(stream));
+  return launch_quant_seq(p, dtype, D, mode, dim3((max_seqlen + 127) / 128, H, nseq), reinterpret_cast<cudaStream_t>(stream), pg);
 }
 
-extern "C" int sab_per_channel_fp8_varlen(const void* v, int dtype, uint8_t* v_fp8, float* v_scale, float* v_mean,
-                                          const int32_t* cu_seqlens, const int32_t* cu_pad, int nseq, int max_seqlen, int H, int D,
-                                          int64_t stride_t, int64_t stride_h, int64_t t_pad, float scale_max, void* workspace,
-                                          void* stream) {
-  int st = check_common(v, dtype, D, 0, stride_h, stride_t);
-  if (st) return st;
+static int per_channel_fp8_seq(const void* v, int dtype, uint8_t* v_fp8, float* v_scale, float* v_mean, const int32_t* cu_seqlens,
+                               const int32_t* cu_pad, int nseq, int max_seqlen, int H, int D, int64_t stride_t, int64_t stride_h,
+                               int64_t t_pad, float scale_max, void* workspace, void* stream, const PageTable* pg) {
   SAB_REQUIRE(v_fp8 && v_scale && workspace && cu_seqlens && cu_pad && nseq > 0 && max_seqlen > 0 && H > 0, SAB_ERR_INVALID,
               "bad arguments to sab_per_channel_fp8_varlen");
   SAB_REQUIRE(t_pad % 128 == 0 && aligned16(v_fp8), SAB_ERR_INVALID, "t_pad must be a multiple of 128 and v_fp8 16-byte aligned");
@@ -1130,7 +1196,7 @@ extern "C" int sab_per_channel_fp8_varlen(const void* v, int dtype, uint8_t* v_f
   const int nchunk = (max_seqlen + kStatChunk - 1) / kStatChunk;
   float* part = reinterpret_cast<float*>(workspace);
   float* recp = part + int64_t(nseq) * H * nchunk * 3 * D;
-  if ((st = run_stats_seq(v, dtype, part, cu_seqlens, nseq, H, nchunk, D, stride_h, stride_t, s))) return st;
+  if (int st = run_stats_seq(v, dtype, part, cu_seqlens, nseq, H, nchunk, D, stride_h, stride_t, s, pg)) return st;
   channel_stats_stage2<__half, true><<<dim3(H, nseq), 128, 0, s>>>(part, nchunk, D, 0, 1, nullptr, v_scale, v_mean, scale_max, recp,
                                                                    cu_seqlens);
   SAB_CUDA_OK(cudaGetLastError());
@@ -1138,10 +1204,79 @@ extern "C" int sab_per_channel_fp8_varlen(const void* v, int dtype, uint8_t* v_f
   p.v = v; p.out = v_fp8; p.recp = recp; p.vmean = v_mean; p.H = H; p.S = 0;
   p.sb = 0; p.sh = stride_h; p.ss = stride_t; p.s_pad = t_pad; p.scale_max = scale_max; p.cu = cu_seqlens; p.cu_pad = cu_pad;
   const dim3 grid((max_seqlen + 127) / 128, H, nseq);
-#define SAB_VQ(T, DD) v_quant_transpose_kernel<T, DD, true><<<grid, 256, 0, s>>>(p)
+#define SAB_VQ(T, DD)                                                                                  \
+  do {                                                                                                 \
+    if (pg != nullptr) v_quant_transpose_paged_kernel<T, DD><<<grid, 256, 0, s>>>(p, *pg);             \
+    else v_quant_transpose_kernel<T, DD, true><<<grid, 256, 0, s>>>(p);                                \
+  } while (0)
   if (dtype == SAB_DTYPE_FP16) { if (D == 128) SAB_VQ(__half, 128); else SAB_VQ(__half, 64); }
   else { if (D == 128) SAB_VQ(__nv_bfloat16, 128); else SAB_VQ(__nv_bfloat16, 64); }
 #undef SAB_VQ
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
+}
+
+extern "C" int sab_k_mean_varlen(const void* k, int dtype, void* mean, const int32_t* cu_seqlens, int nseq, int max_seqlen, int H,
+                                 int D, int64_t stride_t, int64_t stride_h, void* workspace, void* stream) {
+  if (int st = check_common(k, dtype, D, 0, stride_h, stride_t)) return st;
+  return k_mean_seq(k, dtype, mean, cu_seqlens, nseq, max_seqlen, H, D, stride_t, stride_h, workspace, stream, nullptr);
+}
+
+extern "C" int sab_quant_int8_varlen(const void* x, int dtype, const void* mean, int8_t* out, float* scale, const int32_t* cu_seqlens,
+                                     const int32_t* cu_scale, int nseq, int max_seqlen, int H, int D, int64_t x_stride_t,
+                                     int64_t x_stride_h, int64_t o_stride_t, int64_t o_stride_h, int granularity, int is_key,
+                                     void* stream) {
+  if (int st = check_common(x, dtype, D, 0, x_stride_h, x_stride_t)) return st;
+  return quant_int8_seq(x, dtype, mean, out, scale, cu_seqlens, cu_scale, nseq, max_seqlen, H, D, x_stride_t, x_stride_h, o_stride_t,
+                        o_stride_h, granularity, is_key, stream, nullptr);
+}
+
+extern "C" int sab_per_channel_fp8_varlen(const void* v, int dtype, uint8_t* v_fp8, float* v_scale, float* v_mean,
+                                          const int32_t* cu_seqlens, const int32_t* cu_pad, int nseq, int max_seqlen, int H, int D,
+                                          int64_t stride_t, int64_t stride_h, int64_t t_pad, float scale_max, void* workspace,
+                                          void* stream) {
+  if (int st = check_common(v, dtype, D, 0, stride_h, stride_t)) return st;
+  return per_channel_fp8_seq(v, dtype, v_fp8, v_scale, v_mean, cu_seqlens, cu_pad, nseq, max_seqlen, H, D, stride_t, stride_h, t_pad,
+                             scale_max, workspace, stream, nullptr);
+}
+
+// ---------------------------------------------------------------------------------------------- per-sequence front-end, paged input
+// The per-sequence varlen front-end reading a paged cache [num_pages, page_size, H, D] through a block table: the outputs are the
+// packed form's, bit for bit those of the varlen entries on the gathered packed tensor.
+static int check_paged(const void* x, int dtype, int D, const int32_t* block_table, int64_t table_stride, int page_size,
+                       int64_t page_stride, int64_t stride_t, int64_t stride_h, PageTable& pg) {
+  if (int st = check_common(x, dtype, D, page_stride, stride_h, stride_t)) return st;
+  SAB_REQUIRE(block_table != nullptr && table_stride >= 0 && page_size > 0 && page_stride >= 0, SAB_ERR_INVALID,
+              "the paged form needs a block table, table_stride >= 0, page_size > 0 and page_stride >= 0");
+  pg = PageTable{block_table, table_stride, page_size, page_stride};
+  return SAB_OK;
+}
+
+extern "C" int sab_k_mean_paged(const void* k_cache, int dtype, void* mean, const int32_t* cu_seqlens, const int32_t* block_table,
+                                int64_t table_stride, int page_size, int nseq, int max_seqlen, int H, int D, int64_t page_stride,
+                                int64_t stride_t, int64_t stride_h, void* workspace, void* stream) {
+  PageTable pg;
+  if (int st = check_paged(k_cache, dtype, D, block_table, table_stride, page_size, page_stride, stride_t, stride_h, pg)) return st;
+  return k_mean_seq(k_cache, dtype, mean, cu_seqlens, nseq, max_seqlen, H, D, stride_t, stride_h, workspace, stream, &pg);
+}
+
+extern "C" int sab_quant_int8_paged(const void* k_cache, int dtype, const void* mean, int8_t* out, float* scale,
+                                    const int32_t* cu_seqlens, const int32_t* cu_scale, const int32_t* block_table, int64_t table_stride,
+                                    int page_size, int nseq, int max_seqlen, int H, int D, int64_t page_stride, int64_t stride_t,
+                                    int64_t stride_h, int64_t o_stride_t, int64_t o_stride_h, int granularity, void* stream) {
+  PageTable pg;
+  if (int st = check_paged(k_cache, dtype, D, block_table, table_stride, page_size, page_stride, stride_t, stride_h, pg)) return st;
+  return quant_int8_seq(k_cache, dtype, mean, out, scale, cu_seqlens, cu_scale, nseq, max_seqlen, H, D, stride_t, stride_h, o_stride_t,
+                        o_stride_h, granularity, 1, stream, &pg);
+}
+
+extern "C" int sab_per_channel_fp8_paged(const void* v_cache, int dtype, uint8_t* v_fp8, float* v_scale, float* v_mean,
+                                         const int32_t* cu_seqlens, const int32_t* cu_pad, const int32_t* block_table,
+                                         int64_t table_stride, int page_size, int nseq, int max_seqlen, int H, int D, int64_t page_stride,
+                                         int64_t stride_t, int64_t stride_h, int64_t t_pad, float scale_max, void* workspace,
+                                         void* stream) {
+  PageTable pg;
+  if (int st = check_paged(v_cache, dtype, D, block_table, table_stride, page_size, page_stride, stride_t, stride_h, pg)) return st;
+  return per_channel_fp8_seq(v_cache, dtype, v_fp8, v_scale, v_mean, cu_seqlens, cu_pad, nseq, max_seqlen, H, D, stride_t, stride_h,
+                             t_pad, scale_max, workspace, stream, &pg);
 }

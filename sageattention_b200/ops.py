@@ -646,6 +646,104 @@ def _(query, key, value, output, query_scale, key_scale, value_scale, value_mean
     return query.new_empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32)
 
 
+# ----------------------------------------------------------------------------------------------- paged KV cache
+def _paged(cache: torch.Tensor, block_table: torch.Tensor):
+    """(table_stride, page_size, page_stride, stride_t, stride_h) of a [num_pages, page_size, H, D] cache and its block table."""
+    return block_table.stride(0), cache.size(1), cache.stride(0), cache.stride(1), cache.stride(2)
+
+
+@torch.library.custom_op("sageattention_b200::k_mean_paged", mutates_args=("mean",), device_types="cuda")
+def k_mean_paged(k_cache: torch.Tensor, mean: torch.Tensor, cu_seqlens: torch.Tensor, block_table: torch.Tensor,
+                 max_seqlen: int) -> None:
+    """k_mean_varlen reading K from a paged cache (include/sageattn_b200.h, sab_k_mean_paged): mean [nseq,H,D] in the cache's dtype."""
+    _, _, H, D = k_cache.shape
+    nseq = cu_seqlens.numel() - 1
+    tstride, page_size, pstride, st, sh = _paged(k_cache, block_table)
+    with torch.cuda.device(k_cache.device):
+        ws = torch.empty(lib().sab_k_mean_varlen_workspace_bytes(nseq, H, max_seqlen, D), dtype=torch.uint8, device=k_cache.device)
+        check(lib().sab_k_mean_paged(k_cache.data_ptr(), _dt(k_cache), mean.data_ptr(), cu_seqlens.data_ptr(), block_table.data_ptr(),
+                                     tstride, page_size, nseq, max_seqlen, H, D, pstride, st, sh, ws.data_ptr(), _stream(k_cache)))
+
+
+@k_mean_paged.register_fake
+def _(k_cache, mean, cu_seqlens, block_table, max_seqlen):
+    return None
+
+
+@torch.library.custom_op("sageattention_b200::quant_int8_paged", mutates_args=("output", "scale"), device_types="cuda")
+def quant_int8_paged(k_cache: torch.Tensor, mean: Optional[torch.Tensor], output: torch.Tensor, scale: torch.Tensor,
+                     cu_seqlens: torch.Tensor, cu_scale: torch.Tensor, block_table: torch.Tensor, max_seqlen: int,
+                     granularity: int) -> None:
+    """quant_int8_varlen of K read from a paged cache (include/sageattn_b200.h, sab_quant_int8_paged): output [Tk,H,D] packed."""
+    _, _, H, D = k_cache.shape
+    tstride, page_size, pstride, st, sh = _paged(k_cache, block_table)
+    with torch.cuda.device(k_cache.device):
+        check(lib().sab_quant_int8_paged(k_cache.data_ptr(), _dt(k_cache), _ptr(mean), output.data_ptr(), scale.data_ptr(),
+                                         cu_seqlens.data_ptr(), cu_scale.data_ptr(), block_table.data_ptr(), tstride, page_size,
+                                         cu_seqlens.numel() - 1, max_seqlen, H, D, pstride, st, sh, output.stride(0), output.stride(1),
+                                         granularity, _stream(k_cache)))
+
+
+@quant_int8_paged.register_fake
+def _(k_cache, mean, output, scale, cu_seqlens, cu_scale, block_table, max_seqlen, granularity):
+    return None
+
+
+@torch.library.custom_op("sageattention_b200::per_channel_fp8_paged", mutates_args=("v_fp8", "v_scale", "v_mean"), device_types="cuda")
+def per_channel_fp8_paged(v_cache: torch.Tensor, v_fp8: torch.Tensor, v_scale: torch.Tensor, v_mean: Optional[torch.Tensor],
+                          cu_seqlens: torch.Tensor, cu_pad: torch.Tensor, block_table: torch.Tensor, max_seqlen: int,
+                          scale_max: float) -> None:
+    """per_channel_fp8_varlen_seq reading V from a paged cache (include/sageattn_b200.h, sab_per_channel_fp8_paged)."""
+    _, _, H, D = v_cache.shape
+    nseq = cu_seqlens.numel() - 1
+    tstride, page_size, pstride, st, sh = _paged(v_cache, block_table)
+    with torch.cuda.device(v_cache.device):
+        ws = torch.empty(lib().sab_per_channel_fp8_varlen_workspace_bytes(nseq, H, max_seqlen, D), dtype=torch.uint8,
+                         device=v_cache.device)
+        check(lib().sab_per_channel_fp8_paged(v_cache.data_ptr(), _dt(v_cache), v_fp8.data_ptr(), v_scale.data_ptr(), _ptr(v_mean),
+                                              cu_seqlens.data_ptr(), cu_pad.data_ptr(), block_table.data_ptr(), tstride, page_size,
+                                              nseq, max_seqlen, H, D, pstride, st, sh, v_fp8.size(-1), float(scale_max), ws.data_ptr(),
+                                              _stream(v_cache)))
+
+
+@per_channel_fp8_paged.register_fake
+def _(v_cache, v_fp8, v_scale, v_mean, cu_seqlens, cu_pad, block_table, max_seqlen, scale_max):
+    return None
+
+
+@torch.library.custom_op("sageattention_b200::qk_int8_sv_f8_attn_varlen_bottom_right", mutates_args=("output",), device_types="cuda")
+def qk_int8_sv_f8_attn_varlen_bottom_right(query: torch.Tensor, key: torch.Tensor, value: torch.Tensor, output: torch.Tensor,
+                                           query_scale: torch.Tensor, key_scale: torch.Tensor, value_scale: torch.Tensor,
+                                           value_mean: Optional[torch.Tensor], cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor,
+                                           cu_pad_v: torch.Tensor, cu_q_scale: torch.Tensor, cu_k_scale: torch.Tensor,
+                                           max_seqlen_q: int, is_causal: int, q_quant_gran: int, k_quant_gran: int, sm_scale: float,
+                                           return_lse: int) -> torch.Tensor:
+    """qk_int8_sv_f8_attn_varlen_seq with causal aligned bottom-right inside each sequence (include/sageattn_b200.h,
+    sab_qk_int8_sv_f8_attn_varlen_bottom_right).  Returns the [Hq,Tq] log2 LSE when return_lse, else an empty tensor; a row with
+    no visible key gets 0 and lse -inf."""
+    Tq, Hq, D = query.shape
+    Tk, Hkv, _ = key.shape
+    lse = torch.empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32, device=query.device)
+    with torch.cuda.device(query.device):
+        check(lib().sab_qk_int8_sv_f8_attn_varlen_bottom_right(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
+                                                               lse.data_ptr() if return_lse else None, query_scale.data_ptr(),
+                                                               key_scale.data_ptr(), value_scale.data_ptr(), _ptr(value_mean),
+                                                               _dt(output), cu_seqlens_q.numel() - 1, Hq, Hkv, Tq, Tk, D, query.stride(0),
+                                                               query.stride(1), key.stride(0), key.stride(1), _v_pad(value),
+                                                               output.stride(0), output.stride(1), is_causal, q_quant_gran, k_quant_gran,
+                                                               float(sm_scale), cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(),
+                                                               cu_pad_v.data_ptr(), cu_q_scale.data_ptr(), cu_k_scale.data_ptr(),
+                                                               max_seqlen_q, _stream(query)))
+    return lse
+
+
+@qk_int8_sv_f8_attn_varlen_bottom_right.register_fake
+def _(query, key, value, output, query_scale, key_scale, value_scale, value_mean, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale,
+      cu_k_scale, max_seqlen_q, is_causal, q_quant_gran, k_quant_gran, sm_scale, return_lse):
+    Tq, Hq, _ = query.shape
+    return query.new_empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32)
+
+
 @torch.library.custom_op("sageattention_b200::qk_int8_attn_bwd_varlen_seq", mutates_args=("dq", "dk", "dv"), device_types="cuda")
 def qk_int8_attn_bwd_varlen_seq(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale: torch.Tensor, k_scale: torch.Tensor,
                                 q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, o: torch.Tensor, dout: torch.Tensor,

@@ -287,3 +287,44 @@ def per_channel_fp8_varlen_seq(v: torch.Tensor, cu_seqlens_k: torch.Tensor, max_
     vm = torch.empty((nseq, h_kv, head_dim), dtype=torch.float32, device=v.device) if smooth_v else None
     ops.per_channel_fp8_varlen_seq(v, v_fp8, v_scale, vm, cu_seqlens_k.to(torch.int32), cu_pad, max_seqlen_k, scale_max)
     return v_fp8, v_scale, vm, cu_pad
+
+
+# ------------------------------------------------------------------------------------------------ per-sequence statistics, paged K / V
+# The inputs are a paged cache [num_pages, page_size, H, D] and a block table [nseq, max_pages] int32: token t of sequence b is
+# cache[block_table[b, t // page_size], t % page_size].  cu_seqlens_k holds the exclusive cumsum of the sequence lengths; the
+# outputs are those of the packed forms above on the gathered tensor, bit for bit.  The caller passes the exact packed sizes.
+def k_mean_paged(k_cache: torch.Tensor, cu_seqlens_k: torch.Tensor, block_table: torch.Tensor, max_seqlen_k: int) -> torch.Tensor:
+    """k_mean_varlen of the gathered K: [nseq,H,D] in the cache's dtype."""
+    nseq = cu_seqlens_k.numel() - 1
+    mean = torch.empty((nseq, k_cache.size(2), k_cache.size(3)), dtype=k_cache.dtype, device=k_cache.device)
+    ops.k_mean_paged(k_cache, mean, cu_seqlens_k, block_table, max_seqlen_k)
+    return mean
+
+
+def quant_k_int8_paged(k_cache: torch.Tensor, km: Optional[torch.Tensor], cu_seqlens_k: torch.Tensor, block_table: torch.Tensor,
+                       max_seqlen_k: int, total_k: int, k_blocks: int, qk_quant_gran: str = "per_thread"):
+    """quant_k_int8_varlen of the gathered K: (k_int8 [total_k,H,D], k_scale [k_blocks*mult,H], cu_k_scale), with total_k the number
+    of keys and k_blocks the number of 64-key blocks, sum_b ceil(L_b/64)."""
+    from ._capi import SAB_GRAN_PER_WARP, SAB_GRAN_PER_THREAD
+    mult = 1 if qk_quant_gran == "per_warp" else 4
+    cu_k_scale = varlen_block_table(cu_seqlens_k, 64)
+    H, D = k_cache.size(2), k_cache.size(3)
+    k_int8 = torch.empty((total_k, H, D), dtype=torch.int8, device=k_cache.device)
+    k_scale = torch.empty((k_blocks * mult, H), dtype=torch.float32, device=k_cache.device)
+    ops.quant_int8_paged(k_cache, None if km is None else km.contiguous(), k_int8, k_scale, cu_seqlens_k, cu_k_scale, block_table,
+                         max_seqlen_k, SAB_GRAN_PER_WARP if qk_quant_gran == "per_warp" else SAB_GRAN_PER_THREAD)
+    return k_int8, k_scale, cu_k_scale
+
+
+def per_channel_fp8_paged(v_cache: torch.Tensor, cu_seqlens_k: torch.Tensor, block_table: torch.Tensor, max_seqlen_k: int,
+                          t_pad: int, scale_max: float = 448.0, smooth_v: bool = False):
+    """per_channel_fp8_varlen_seq of the gathered V: (v_fp8 [H,D,t_pad], v_scale [nseq,H,D], vm [nseq,H,D] or None, cu_pad), with
+    t_pad = sum_b ceil(L_b/128)*128."""
+    nseq = cu_seqlens_k.numel() - 1
+    H, D = v_cache.size(2), v_cache.size(3)
+    cu_pad = varlen_block_table(cu_seqlens_k, 128) * 128
+    v_fp8 = torch.empty((H, D, t_pad), dtype=torch.float8_e4m3fn, device=v_cache.device)
+    v_scale = torch.empty((nseq, H, D), dtype=torch.float32, device=v_cache.device)
+    vm = torch.empty((nseq, H, D), dtype=torch.float32, device=v_cache.device) if smooth_v else None
+    ops.per_channel_fp8_paged(v_cache, v_fp8, v_scale, vm, cu_seqlens_k, cu_pad, block_table, max_seqlen_k, scale_max)
+    return v_fp8, v_scale, vm, cu_pad

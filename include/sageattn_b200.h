@@ -599,6 +599,40 @@ int sab_predict_block_mask_varlen(const float* q_mean, const float* q_sim, const
                                   int Hkv, int max_seqlen_q, int max_seqlen_k, int D, int is_causal, float sm_scale,
                                   float cdf_threshold, float sim_threshold, void* stream);
 
+/* 8-bit paged KV cache for decoding (no reference counterpart): the building blocks of PagedKVCache8 and sageattn_kvcache8.
+ *   The cache is token-major and contiguous: k_pages int8 and v_pages e4m3 [num_pages, page_size, Hkv, D], k_scale and v_scale fp32
+ *   [num_pages, page_size, Hkv], k_smooth fp32 [Hkv, D].  D is 64 or 128, page_size a multiple of 16, `dtype` the 16-bit type of
+ *   the tokens written and of q / out.  Slot s is token s % page_size of page s / page_size.
+ * sab_kvcache8_write: quantises T tokens k, v [T, Hkv, D] (element strides k_stride_t / k_stride_h, v_stride_t / v_stride_h, last
+ *   dim contiguous) into the slots slot_mapping[t] (int64 device, page * page_size + slot; a negative entry skips the token, and so
+ *   does an entry >= num_pages * page_size), one launch.  Per (token, head), in fp32: K x = k - k_smooth[h], amax = max|x|, k_scale
+ *   = amax / 127 (IEEE), k8 = cvt.rni.sat.s8(x * RN(127 / amax)); V amax = max|v|, v_scale = amax / 448, v8 =
+ *   cvt.rn.satfinite.e4m3(v * RN(448 / amax)).  amax == 0 stores scale 0 and zeros; when RN(qmax / amax) overflows (a denormal
+ *   amax) the quotient x / scale is used instead.  The result depends on the token alone; unmapped slots are never written.
+ * sab_kvcache8_attn: attention of packed q [Tq, Hq, D] (cu_seqlens_q [nseq+1] int32 device) against the cache: sequence b has
+ *   Lk_b = seqused_k[b] keys (int32 device, read only on the device; clamped to max_pages * page_size), key j at slot j % page_size
+ *   of page block_table[b * table_stride + j / page_size] (trusted, in [0, num_pages)).  Causal is bottom-right: query i sees key j
+ *   iff j <= i + Lk_b - Lq_b.  Q is quantised per (token, head) as K is, without smoothing; logits in log2 units are
+ *   float(dot(q8, k8)) * (q_scale * sm_scale * log2e) * k_scale.  Keys are cut into chunks of sab_kvcache8_chunk_keys() keys, one
+ *   CTA per (sequence, KV head, chunk) holding all max_seqlen_q * Hq / Hkv <= 64 query rows of that KV head (rows past
+ *   max_seqlen_q are not written); within a chunk an exact running max over 64-key tiles, P = bf16(p * v_scale) times bf16(v8)
+ *   with fp32 accumulation.  A second kernel merges the chunks of a row in ascending order (no atomics: bit-reproducible).  out
+ *   [Tq, Hq, D] (strides o_stride_t / o_stride_h) in `dtype`; lse (optional) [Hq, Tq] fp32 in natural-log units including
+ *   (q . k_smooth) * sm_scale.  A row that sees no key returns 0 and lse -inf.  workspace: sab_kvcache8_workspace_bytes(Tq, Hq, D,
+ *   max_pages * page_size) bytes.  No host synchronisation: the grid follows nseq, Hkv and max_pages * page_size.  Launch-grid
+ *   limits, refused with SAB_ERR_INVALID: Hq <= 65535, nseq * ceil(max_pages * page_size / chunk) < 2^31, nseq * max_seqlen_q
+ *   < 2^31 and max_pages * page_size < 2^31. */
+int sab_kvcache8_chunk_keys(void);
+int64_t sab_kvcache8_workspace_bytes(int Tq, int Hq, int D, int64_t max_keys);
+int sab_kvcache8_write(const void* k, const void* v, int dtype, const float* k_smooth, const int64_t* slot_mapping, int T, int Hkv,
+                       int D, int64_t k_stride_t, int64_t k_stride_h, int64_t v_stride_t, int64_t v_stride_h, int8_t* k_pages,
+                       float* k_scale, uint8_t* v_pages, float* v_scale, int64_t num_pages, int page_size, void* stream);
+int sab_kvcache8_attn(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
+                      const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
+                      const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq, int Tq,
+                      int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h, int64_t o_stride_t,
+                      int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale, void* workspace, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -81,6 +81,12 @@ EXPORTS = {
                                   [c_float, c_void_p, c_void_p]),
     "sab_qk_int8_sv_f8_attn_varlen_bottom_right": (c_int, [c_void_p] * 9 + [c_int] * 7 + [c_int64] * 7 + [c_int, c_int, c_int, c_float] +
                                                    [c_void_p] * 5 + [c_int, c_void_p]),
+    "sab_kvcache8_chunk_keys": (c_int, []),
+    "sab_kvcache8_workspace_bytes": (c_int64, [c_int] * 3 + [c_int64]),
+    "sab_kvcache8_write": (c_int, [c_void_p] * 2 + [c_int] + [c_void_p] * 2 + [c_int] * 3 + [c_int64] * 4 + [c_void_p] * 4 +
+                           [c_int64, c_int, c_void_p]),
+    "sab_kvcache8_attn": (c_int, [c_void_p, c_int] + [c_void_p] * 10 + [c_int64] + [c_int] * 7 + [c_int64] * 4 +
+                          [c_int, c_int, c_float, c_void_p, c_void_p]),
     "sab_block_stats": (c_int, [c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 4 + [c_int64] * 3 + [c_int, c_void_p]),
     "sab_predict_block_mask": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_float] * 3 + [c_void_p]),
     "sab_block_stats_varlen": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 4 + [c_int64] * 2 + [c_int, c_void_p]),

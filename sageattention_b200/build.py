@@ -8,8 +8,8 @@ import os, subprocess, sys, hashlib
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libsageattn_b200.so")
-SOURCES = ["attn.cu", "attn_bwd.cu", "quant.cu", "predict.cu", "capi.cu"]
-HEADERS = ["ptx.cuh", "common.cuh", "attn_common.cuh", os.path.join("..", "..", "include", "sageattn_b200.h")]
+SOURCES = ["attn.cu", "attn_bwd.cu", "quant.cu", "predict.cu", "kvcache8.cu", "capi.cu"]
+HEADERS = ["ptx.cuh", "common.cuh", "attn_common.cuh", "quant_common.cuh", os.path.join("..", "..", "include", "sageattn_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 # per-source extra nvcc flags (none at present)

@@ -1,0 +1,570 @@
+// 8-bit paged KV cache for decoding on sm_90a (H100): the write kernel that quantises each token once, per (token, head), into
+// INT8 K / e4m3 V pages, and split-KV attention that reads those pages directly.
+//   kv8_write_kernel   one warp per (token, head): K - k_smooth -> INT8 with an fp32 scale, V -> e4m3 with an fp32 scale.
+//   kv8_attn_kernel    one CTA per (sequence, KV head, chunk of kChunk keys) holding every query row of that KV head (GQA head
+//                      packing, <= 64 rows): Q quantised in the prologue, 64-key tiles loaded through the block table with 16-byte
+//                      cp.async (double-buffered), QK^T on mma.sync s8, an exact running max, P = bf16(p * v_scale) times
+//                      bf16(v8) on mma.sync bf16 with fp32 accumulators.  Writes the chunk's unnormalised O, max and sum.
+//   kv8_combine_kernel one CTA per (query row, Q head): folds the row's chunks in ascending order, O / L and the natural-log lse.
+// Decode is bound by the bytes of the cache, so the kernels aim at one read of each K / V byte per chunk, not at tensor-core rate.
+#include <atomic>
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include "common.cuh"
+#include "ptx.cuh"
+#include "quant_common.cuh"
+
+#ifndef SAB_KV8_CHUNK
+#define SAB_KV8_CHUNK 1024
+#endif
+
+namespace sab {
+namespace {
+
+constexpr int kChunk = SAB_KV8_CHUNK;   // keys per split-KV chunk: a multiple of 64, fixed so a row's bits depend on its own keys
+static_assert(kChunk % 64 == 0, "the chunk is a whole number of 64-key tiles");
+constexpr int kRows = 64;               // query rows per CTA: max_seqlen_q * Hq / Hkv
+constexpr int kTile = 64;               // keys per tile
+constexpr int kThreads = 128;
+constexpr float kLog2e = 1.4426950408889634f;
+
+// Per-row quantisation to [-qmax, qmax]: scale = amax / qmax, x * RN(qmax / amax) rounded by the caller's instruction.  amax == 0
+// gives scale 0 and zeros; a denormal amax, whose RN(qmax / amax) overflows, takes the IEEE quotient x / scale instead.
+struct RowQuant {
+  float scale, mult;
+  bool exact;
+  __device__ __forceinline__ RowQuant(float amax, float qmax) {
+    scale = amax > 0.f ? __fdiv_rn(amax, qmax) : 0.f;
+    mult = amax > 0.f ? __fdiv_rn(qmax, amax) : 0.f;
+    exact = !(mult <= 3.402823466e+38f);
+  }
+  __device__ __forceinline__ float operator()(float x) const { return exact ? __fdiv_rn(x, scale) : __fmul_rn(x, mult); }
+};
+
+template <typename T, int E>
+__device__ __forceinline__ void load_row(const T* p, float (&f)[E]) {
+  static_assert(E == 2 || E == 4, "2 or 4 elements per lane");
+  if constexpr (E == 4) {
+    const uint2 raw = *reinterpret_cast<const uint2*>(p);
+    const T* e = reinterpret_cast<const T*>(&raw);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) f[i] = to_f<T>(e[i]);
+  } else {
+    const uint32_t raw = *reinterpret_cast<const uint32_t*>(p);
+    const T* e = reinterpret_cast<const T*>(&raw);
+    f[0] = to_f<T>(e[0]);
+    f[1] = to_f<T>(e[1]);
+  }
+}
+
+template <int E>
+__device__ __forceinline__ float warp_amax(const float (&x)[E]) {
+  float a = 0.f;
+#pragma unroll
+  for (int i = 0; i < E; ++i) a = fmaxf(a, fabsf(x[i]));
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) a = fmaxf(a, __shfl_xor_sync(0xffffffffu, a, o));
+  return a;
+}
+
+template <int E>
+__device__ __forceinline__ uint32_t pack_s8(const float (&x)[E], const RowQuant& rq) {
+  uint32_t r = 0;
+#pragma unroll
+  for (int i = 0; i < E; ++i) r |= uint32_t(uint8_t(cvt_rni_sat_s8(rq(x[i])))) << (8 * i);
+  return r;
+}
+
+// ------------------------------------------------------------------------------------------------ write
+template <typename T, int D>
+__global__ void __launch_bounds__(256) kv8_write_kernel(const T* __restrict__ k, const T* __restrict__ v,
+                                                        const float* __restrict__ k_smooth, const int64_t* __restrict__ slot_mapping,
+                                                        int T_, int Hkv, int64_t kst, int64_t ksh, int64_t vst, int64_t vsh,
+                                                        int8_t* __restrict__ k_pages, float* __restrict__ k_scale,
+                                                        uint8_t* __restrict__ v_pages, float* __restrict__ v_scale, int64_t num_slots) {
+  constexpr int E = D / 32;
+  const int lane = threadIdx.x % 32;
+  const int64_t item = int64_t(blockIdx.x) * 8 + threadIdx.x / 32;
+  if (item >= int64_t(T_) * Hkv) return;
+  const int t = int(item / Hkv), h = int(item % Hkv);
+  const int64_t slot = slot_mapping[t];
+  if (slot < 0 || slot >= num_slots) return;
+  const int64_t row = slot * Hkv + h;   // [num_slots, Hkv] rows of the cache
+  float x[E];
+  load_row<T, E>(k + int64_t(t) * kst + int64_t(h) * ksh + lane * E, x);
+#pragma unroll
+  for (int i = 0; i < E; ++i) x[i] = __fsub_rn(x[i], k_smooth[h * D + lane * E + i]);
+  const RowQuant kq(warp_amax<E>(x), 127.f);
+  const uint32_t k8 = pack_s8<E>(x, kq);
+  load_row<T, E>(v + int64_t(t) * vst + int64_t(h) * vsh + lane * E, x);
+  const RowQuant vq(warp_amax<E>(x), 448.f);
+  uint32_t v8;
+  if constexpr (E == 4) v8 = pack_e4m3x4_q(vq(x[0]), vq(x[1]), vq(x[2]), vq(x[3]));
+  else v8 = pack_e4m3x4_q(vq(x[0]), vq(x[1]), 0.f, 0.f);
+  if constexpr (E == 4) {
+    reinterpret_cast<uint32_t*>(k_pages + row * D)[lane] = k8;
+    reinterpret_cast<uint32_t*>(v_pages + row * D)[lane] = v8;
+  } else {
+    reinterpret_cast<uint16_t*>(k_pages + row * D)[lane] = uint16_t(k8);
+    reinterpret_cast<uint16_t*>(v_pages + row * D)[lane] = uint16_t(v8);
+  }
+  if (lane == 0) {
+    k_scale[row] = kq.scale;
+    v_scale[row] = vq.scale;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ attention
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool valid) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async4(uint32_t dst, const void* src, bool valid) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(valid ? 4 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
+
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
+}
+// D[16 x 8] += A[16 x 32 s8] * B[32 x 8 s8], int32
+__device__ __forceinline__ void mma_s8(int (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// D[16 x 8] += A[16 x 16 bf16] * B[16 x 8 bf16], fp32
+__device__ __forceinline__ void mma_bf16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+// two e4m3 bytes (lo, hi) -> bf16x2, exactly (every e4m3 value is an f16 and a bf16)
+__device__ __forceinline__ uint32_t e4m3x2_to_bf16x2(uint32_t lo, uint32_t hi) {
+  const uint16_t pair = uint16_t(lo | (hi << 8));
+  uint32_t h2;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h2) : "h"(pair));
+  const __half2 hv = *reinterpret_cast<const __half2*>(&h2);
+  const __nv_bfloat162 b = __floats2bfloat162_rn(__low2float(hv), __high2float(hv));
+  return *reinterpret_cast<const uint32_t*>(&b);
+}
+
+struct Kv8Params {
+  const void* q; const int8_t* k_pages; const float* k_scale; const uint8_t* v_pages; const float* v_scale;
+  const int32_t* cu_q; const int32_t* seqused_k; const int32_t* table; int64_t table_stride;
+  int max_pages, page_size, Hq, Hkv, max_chunks, max_seqlen_q;
+  int64_t q_st, q_sh;
+  float scale_log2;     // sm_scale * log2(e)
+  float* o_part;        // [Tq, Hq, max_chunks, D]
+  float2* ml_part;      // [Tq, Hq, max_chunks]: (running max in log2 units, sum of p)
+};
+
+template <int D>
+struct Kv8Smem {
+  static constexpr int kRowB = D + 16;                   // int8 / e4m3 row pitch in bytes: conflict-free ldmatrix and byte reads
+  static constexpr int kPB = kTile * 2 + 16;             // bf16 P row pitch in bytes
+  alignas(128) int8_t q8[kRows * kRowB];
+  alignas(128) int8_t k8[2][kTile * kRowB];
+  alignas(128) uint8_t v8[2][kTile * kRowB];
+  alignas(128) uint8_t p[kRows * kPB];
+  float ks[2][kTile], vs[2][kTile];
+  float qc[kRows];                                       // q_scale * sm_scale * log2(e)
+  float red_max[4][kRows], red_sum[4][kRows];            // per-warp partial row max / sum of the tile
+};
+
+template <typename T, int D, bool kCausal>
+__global__ void __launch_bounds__(kThreads) kv8_attn_kernel(const Kv8Params p) {
+  using S = Kv8Smem<D>;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  S& sm = *reinterpret_cast<S*>(smem_raw);
+  const int b = blockIdx.x / p.max_chunks, chunk = blockIdx.x % p.max_chunks, h = blockIdx.y;
+  const int G = p.Hq / p.Hkv;
+  const int q0 = p.cu_q[b];
+  const int Lq = min(p.cu_q[b + 1] - q0, p.max_seqlen_q);
+  const int Lk = min(p.seqused_k[b], p.max_pages * p.page_size);
+  const int kbeg = chunk * kChunk;
+  if (Lq <= 0 || kbeg >= Lk) return;
+  const int kend = min(Lk, kbeg + kChunk);
+  const int R = Lq * G;                 // rows r = i * G + g: query i, Q head h * G + g
+  const int nM = (R + 15) / 16;
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32, g8 = lane / 4, c4 = lane % 4;
+  const int32_t* table = p.table + int64_t(b) * p.table_stride;
+  const int64_t hD = int64_t(h) * D;
+
+  // ---- tile loader: keys kbeg + 64 t .. of this KV head, zero-filled past kend
+  auto load_tile = [&](int t, int buf) {
+    constexpr int CPR = D / 16;   // 16-byte chunks per row
+    for (int i = threadIdx.x; i < kTile * CPR; i += kThreads) {
+      const int r = i / CPR, cc = i % CPR;
+      const int key = kbeg + t * kTile + r;
+      const bool ok = key < kend;
+      const int64_t slot = ok ? int64_t(__ldg(table + key / p.page_size)) * p.page_size + key % p.page_size : 0;
+      const int64_t off = (slot * p.Hkv) * D + hD + cc * 16;
+      cp_async16(smem_u32(&sm.k8[buf][r * S::kRowB + cc * 16]), p.k_pages + off, ok);
+      cp_async16(smem_u32(&sm.v8[buf][r * S::kRowB + cc * 16]), p.v_pages + off, ok);
+    }
+    if (threadIdx.x < kTile) {
+      const int key = kbeg + t * kTile + threadIdx.x;
+      const bool ok = key < kend;
+      const int64_t slot = ok ? int64_t(__ldg(table + key / p.page_size)) * p.page_size + key % p.page_size : 0;
+      cp_async4(smem_u32(&sm.ks[buf][threadIdx.x]), p.k_scale + slot * p.Hkv + h, ok);
+      cp_async4(smem_u32(&sm.vs[buf][threadIdx.x]), p.v_scale + slot * p.Hkv + h, ok);
+    }
+  };
+  const int ntiles = (kend - kbeg + kTile - 1) / kTile;
+  load_tile(0, 0);
+  cp_async_commit();
+
+  // ---- Q prologue: per (token, head) INT8, one warp per row
+  {
+    constexpr int E = D / 32;
+    const T* q = reinterpret_cast<const T*>(p.q);
+    for (int r = warp; r < nM * 16; r += 4) {
+      uint32_t q8 = 0;
+      float qc = 0.f;
+      if (r < R) {
+        const int i = r / G, hq = h * G + r % G;
+        float x[E];
+        load_row<T, E>(q + int64_t(q0 + i) * p.q_st + int64_t(hq) * p.q_sh + lane * E, x);
+        const RowQuant rq(warp_amax<E>(x), 127.f);
+        q8 = pack_s8<E>(x, rq);
+        qc = __fmul_rn(rq.scale, p.scale_log2);
+      }
+      if constexpr (E == 4) *reinterpret_cast<uint32_t*>(&sm.q8[r * S::kRowB + lane * 4]) = q8;
+      else *reinterpret_cast<uint16_t*>(&sm.q8[r * S::kRowB + lane * 2]) = uint16_t(q8);
+      if (lane == 0) sm.qc[r] = qc;
+    }
+  }
+
+  // per thread: rows 16 mt + g8 (+8); QK keys 16 warp + 8 nt + 2 c4 (+1); PV columns (D / 4) warp + 8 nt + 2 c4 (+1)
+  constexpr int NO = D / 32;            // PV n-tiles per warp
+  float o[4][NO][4];
+  float m_run[4][2], l_run[4][2];
+#pragma unroll
+  for (int mt = 0; mt < 4; ++mt) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j) { m_run[mt][j] = -INFINITY; l_run[mt][j] = 0.f; }
+#pragma unroll
+    for (int nt = 0; nt < NO; ++nt)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) o[mt][nt][e] = 0.f;
+  }
+  // the last key row r may see: causal is bottom-right inside the sequence
+  int lim[4][2];
+#pragma unroll
+  for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int r = mt * 16 + g8 + 8 * j;
+      lim[mt][j] = r >= R ? -1 : (kCausal ? min(kend - 1, r / G + Lk - Lq) : kend - 1);
+    }
+
+  for (int t = 0; t < ntiles; ++t) {
+    const int buf = t & 1;
+    // Tile t is the only group in flight.  Past the barrier it is visible to every warp, and every warp has finished the P V of
+    // tile t - 1, the last reader of buffer buf ^ 1, so only now may the loads of tile t + 1 overwrite that buffer.
+    cp_async_wait<0>();
+    __syncthreads();
+    if (t + 1 < ntiles) load_tile(t + 1, buf ^ 1);
+    cp_async_commit();
+
+    // ---- S = Q K^T for this warp's 16 keys, in log2 units
+    const int key0 = kbeg + t * kTile + warp * 16;
+    float s[4][2][4];
+    {
+      int acc[4][2][4];
+#pragma unroll
+      for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) acc[mt][nt][e] = 0;
+#pragma unroll
+      for (int ks = 0; ks < D / 32; ++ks) {
+        uint32_t bk[4];
+        ldsm_x4(smem_u32(&sm.k8[buf][(warp * 16 + (lane / 16) * 8 + lane % 8) * S::kRowB + ks * 32 + ((lane / 8) & 1) * 16]), bk);
+#pragma unroll
+        for (int mt = 0; mt < 4; ++mt) {
+          if (mt < nM) {
+            uint32_t a[4];
+            ldsm_x4(smem_u32(&sm.q8[(mt * 16 + lane % 8 + ((lane / 8) & 1) * 8) * S::kRowB + ks * 32 + (lane / 16) * 16]), a);
+            mma_s8(acc[mt][0], a, bk[0], bk[1]);
+            mma_s8(acc[mt][1], a, bk[2], bk[3]);
+          }
+        }
+      }
+#pragma unroll
+      for (int mt = 0; mt < 4; ++mt) {
+        float rmax[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const float qc = sm.qc[mt * 16 + g8 + 8 * j];
+#pragma unroll
+          for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int kl = warp * 16 + nt * 8 + 2 * c4 + e;
+              float x = __fmul_rn(__fmul_rn(float(acc[mt][nt][2 * j + e]), qc), sm.ks[buf][kl]);
+              if (key0 + nt * 8 + 2 * c4 + e > lim[mt][j]) x = -INFINITY;
+              s[mt][nt][2 * j + e] = x;
+              rmax[j] = fmaxf(rmax[j], x);
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          rmax[j] = fmaxf(rmax[j], __shfl_xor_sync(0xffffffffu, rmax[j], 1));
+          rmax[j] = fmaxf(rmax[j], __shfl_xor_sync(0xffffffffu, rmax[j], 2));
+          if (c4 == 0) sm.red_max[warp][mt * 16 + g8 + 8 * j] = rmax[j];
+        }
+      }
+    }
+    __syncthreads();
+
+    // ---- exact running max, p = 2^(s - m), P = bf16(p * v_scale) to shared memory, partial row sums
+    float alpha[4][2];
+#pragma unroll
+    for (int mt = 0; mt < 4; ++mt) {
+      float rsum[2] = {0.f, 0.f};
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int r = mt * 16 + g8 + 8 * j;
+        const float m_new = fmaxf(fmaxf(m_run[mt][j], fmaxf(sm.red_max[0][r], sm.red_max[1][r])),
+                                  fmaxf(sm.red_max[2][r], sm.red_max[3][r]));
+        alpha[mt][j] = m_run[mt][j] == -INFINITY ? 0.f : ex2_approx(__fsub_rn(m_run[mt][j], m_new));
+        m_run[mt][j] = m_new;
+#pragma unroll
+        for (int nt = 0; nt < 2; ++nt) {
+          float pe[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float x = s[mt][nt][2 * j + e];
+            pe[e] = x == -INFINITY ? 0.f : ex2_approx(__fsub_rn(x, m_new));
+            rsum[j] += pe[e];
+          }
+          const int kl = warp * 16 + nt * 8 + 2 * c4;
+          const __nv_bfloat162 pv = __floats2bfloat162_rn(__fmul_rn(pe[0], sm.vs[buf][kl]), __fmul_rn(pe[1], sm.vs[buf][kl + 1]));
+          if (mt < nM) *reinterpret_cast<__nv_bfloat162*>(&sm.p[r * S::kPB + kl * 2]) = pv;
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        rsum[j] += __shfl_xor_sync(0xffffffffu, rsum[j], 1);
+        rsum[j] += __shfl_xor_sync(0xffffffffu, rsum[j], 2);
+        if (c4 == 0) sm.red_sum[warp][mt * 16 + g8 + 8 * j] = rsum[j];
+      }
+    }
+    __syncthreads();
+
+    // ---- l = alpha l + sum p;  O = alpha O + P V for this warp's D / 4 columns
+#pragma unroll
+    for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const int r = mt * 16 + g8 + 8 * j;
+        l_run[mt][j] = __fmaf_rn(alpha[mt][j], l_run[mt][j],
+                                 __fadd_rn(__fadd_rn(sm.red_sum[0][r], sm.red_sum[1][r]), __fadd_rn(sm.red_sum[2][r], sm.red_sum[3][r])));
+#pragma unroll
+        for (int nt = 0; nt < NO; ++nt) {
+          o[mt][nt][2 * j] *= alpha[mt][j];
+          o[mt][nt][2 * j + 1] *= alpha[mt][j];
+        }
+      }
+    const uint8_t* vt = sm.v8[buf];
+#pragma unroll
+    for (int kk = 0; kk < kTile / 16; ++kk) {
+      uint32_t bv[NO][2];
+#pragma unroll
+      for (int nt = 0; nt < NO; ++nt) {
+        const int col = warp * (D / 4) + nt * 8 + g8;
+        const int k0 = kk * 16 + 2 * c4;
+        bv[nt][0] = e4m3x2_to_bf16x2(vt[k0 * S::kRowB + col], vt[(k0 + 1) * S::kRowB + col]);
+        bv[nt][1] = e4m3x2_to_bf16x2(vt[(k0 + 8) * S::kRowB + col], vt[(k0 + 9) * S::kRowB + col]);
+      }
+#pragma unroll
+      for (int mt = 0; mt < 4; ++mt) {
+        if (mt < nM) {
+          uint32_t a[4];
+          ldsm_x4(smem_u32(&sm.p[(mt * 16 + lane % 8 + ((lane / 8) & 1) * 8) * S::kPB + (kk * 16 + (lane / 16) * 8) * 2]), a);
+#pragma unroll
+          for (int nt = 0; nt < NO; ++nt) mma_bf16(o[mt][nt], a, bv[nt][0], bv[nt][1]);
+        }
+      }
+    }
+  }
+
+  // ---- the chunk's partials of rows r < R
+#pragma unroll
+  for (int mt = 0; mt < 4; ++mt)
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int r = mt * 16 + g8 + 8 * j;
+      if (r >= R) continue;
+      const int64_t idx = (int64_t(q0 + r / G) * p.Hq + h * G + r % G) * p.max_chunks + chunk;
+#pragma unroll
+      for (int nt = 0; nt < NO; ++nt)
+        *reinterpret_cast<float2*>(p.o_part + idx * D + warp * (D / 4) + nt * 8 + 2 * c4) = make_float2(o[mt][nt][2 * j], o[mt][nt][2 * j + 1]);
+      if (warp == 0 && c4 == 0) p.ml_part[idx] = make_float2(m_run[mt][j], l_run[mt][j]);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ combine
+struct Kv8CombineParams {
+  const void* q; const float* k_smooth; const int32_t* cu_q; const int32_t* seqused_k;
+  const float* o_part; const float2* ml_part;
+  void* out; float* lse;
+  int Tq, Hq, Hkv, max_chunks, max_seqlen_q, max_keys;
+  int64_t q_st, q_sh, o_st, o_sh;
+  float sm_scale;
+};
+
+template <typename T, int D>
+__global__ void __launch_bounds__(D) kv8_combine_kernel(const Kv8CombineParams p) {
+  const int b = blockIdx.x / p.max_seqlen_q, i = blockIdx.x % p.max_seqlen_q, hq = blockIdx.y, d = threadIdx.x;
+  const int q0 = p.cu_q[b];
+  if (i >= p.cu_q[b + 1] - q0) return;
+  const int t = q0 + i;
+  const int nc = (min(p.seqused_k[b], p.max_keys) + kChunk - 1) / kChunk;
+  const int64_t base = (int64_t(t) * p.Hq + hq) * p.max_chunks;
+  float M = -INFINITY;
+  for (int c = 0; c < nc; ++c) M = fmaxf(M, p.ml_part[base + c].x);
+  float L = 0.f, acc = 0.f;
+  if (M != -INFINITY) {
+    for (int c = 0; c < nc; ++c) {
+      const float2 ml = p.ml_part[base + c];
+      const float w = ml.x == -INFINITY ? 0.f : ex2_approx(__fsub_rn(ml.x, M));
+      L = __fmaf_rn(w, ml.y, L);
+      acc = __fmaf_rn(w, p.o_part[(base + c) * D + d], acc);
+    }
+  }
+  T* out = reinterpret_cast<T*>(p.out) + int64_t(t) * p.o_st + int64_t(hq) * p.o_sh;
+  out[d] = from_f<T>(M == -INFINITY ? 0.f : __fdiv_rn(acc, L));
+  if (p.lse == nullptr) return;
+  // lse = (M + log2 L) / log2(e) + (q . k_smooth) * sm_scale: the softmax ran on q . (k - k_smooth)
+  __shared__ float red[D / 32];
+  const T* q = reinterpret_cast<const T*>(p.q) + int64_t(t) * p.q_st + int64_t(hq) * p.q_sh;
+  float dot = to_f<T>(q[d]) * p.k_smooth[(hq / (p.Hq / p.Hkv)) * D + d];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+  if (d % 32 == 0) red[d / 32] = dot;
+  __syncthreads();
+  if (d == 0) {
+    float qk = 0.f;
+#pragma unroll
+    for (int w = 0; w < D / 32; ++w) qk += red[w];
+    p.lse[int64_t(hq) * p.Tq + t] = M == -INFINITY ? -INFINITY : (M + log2f(L)) / kLog2e + qk * p.sm_scale;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ host
+int check_dtype_dim(int dtype, int D) {
+  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "Only half and bfloat16 are supported");
+  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d", D);
+  return SAB_OK;
+}
+
+template <typename T, int D>
+int launch_write(const void* k, const void* v, const float* k_smooth, const int64_t* slots, int T_, int Hkv, int64_t kst, int64_t ksh,
+                 int64_t vst, int64_t vsh, int8_t* kp, float* ksc, uint8_t* vp, float* vsc, int64_t num_slots, cudaStream_t st) {
+  const int64_t blocks = (int64_t(T_) * Hkv + 7) / 8;
+  kv8_write_kernel<T, D><<<dim3(unsigned(blocks)), 256, 0, st>>>(reinterpret_cast<const T*>(k), reinterpret_cast<const T*>(v), k_smooth,
+                                                                slots, T_, Hkv, kst, ksh, vst, vsh, kp, ksc, vp, vsc, num_slots);
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
+}
+
+template <typename T, int D, bool kCausal>
+int launch_attn_t(const Kv8Params& p, int nseq, cudaStream_t st) {
+  auto kern = kv8_attn_kernel<T, D, kCausal>;
+  const int bytes = int(sizeof(Kv8Smem<D>));
+  // once per device, so a launch inside CUDA-graph capture makes no attribute call
+  static std::atomic<uint64_t> configured{0};
+  int dev = 0;
+  SAB_CUDA_OK(cudaGetDevice(&dev));
+  const uint64_t bit = uint64_t(1) << (dev & 63);
+  if (!(configured.load() & bit)) {
+    SAB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    configured.fetch_or(bit);
+  }
+  kern<<<dim3(unsigned(nseq * p.max_chunks), unsigned(p.Hkv)), kThreads, bytes, st>>>(p);
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
+}
+
+template <typename T, int D>
+int launch_attn(const Kv8Params& p, const Kv8CombineParams& c, int nseq, bool causal, cudaStream_t st) {
+  if (int r = causal ? launch_attn_t<T, D, true>(p, nseq, st) : launch_attn_t<T, D, false>(p, nseq, st)) return r;
+  kv8_combine_kernel<T, D><<<dim3(unsigned(nseq * c.max_seqlen_q), unsigned(c.Hq)), D, 0, st>>>(c);
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
+}
+
+}  // namespace
+}  // namespace sab
+
+using namespace sab;
+
+extern "C" int sab_kvcache8_chunk_keys(void) { return kChunk; }
+
+extern "C" int64_t sab_kvcache8_workspace_bytes(int Tq, int Hq, int D, int64_t max_keys) {
+  const int64_t chunks = (max_keys + kChunk - 1) / kChunk;
+  return int64_t(Tq) * Hq * chunks * (int64_t(D) + 2) * 4;
+}
+
+extern "C" int sab_kvcache8_write(const void* k, const void* v, int dtype, const float* k_smooth, const int64_t* slot_mapping, int T,
+                                  int Hkv, int D, int64_t k_stride_t, int64_t k_stride_h, int64_t v_stride_t, int64_t v_stride_h,
+                                  int8_t* k_pages, float* k_scale, uint8_t* v_pages, float* v_scale, int64_t num_pages, int page_size,
+                                  void* stream) {
+  SAB_REQUIRE(k && v && k_smooth && slot_mapping && k_pages && k_scale && v_pages && v_scale, SAB_ERR_INVALID, "null pointer argument");
+  if (int r = check_dtype_dim(dtype, D)) return r;
+  SAB_REQUIRE(T >= 0 && Hkv > 0 && num_pages > 0 && page_size > 0 && page_size % 16 == 0, SAB_ERR_INVALID,
+              "need T >= 0, Hkv > 0, num_pages > 0 and page_size a positive multiple of 16");
+  SAB_REQUIRE(k_stride_t >= 0 && k_stride_h >= 0 && v_stride_t >= 0 && v_stride_h >= 0 && (k_stride_t | k_stride_h | v_stride_t | v_stride_h) % 4 == 0 &&
+                  (reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v)) % 8 == 0,
+              SAB_ERR_INVALID, "k and v need 8-byte aligned rows (non-negative strides, multiples of 4 elements)");
+  SAB_REQUIRE(int64_t(T) * Hkv < (int64_t(1) << 33), SAB_ERR_INVALID, "too many tokens in one write");
+  if (T == 0) return SAB_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int64_t ns = num_pages * page_size;
+  if (dtype == SAB_DTYPE_FP16)
+    return D == 128 ? launch_write<__half, 128>(k, v, k_smooth, slot_mapping, T, Hkv, k_stride_t, k_stride_h, v_stride_t, v_stride_h, k_pages, k_scale, v_pages, v_scale, ns, st)
+                    : launch_write<__half, 64>(k, v, k_smooth, slot_mapping, T, Hkv, k_stride_t, k_stride_h, v_stride_t, v_stride_h, k_pages, k_scale, v_pages, v_scale, ns, st);
+  return D == 128 ? launch_write<__nv_bfloat16, 128>(k, v, k_smooth, slot_mapping, T, Hkv, k_stride_t, k_stride_h, v_stride_t, v_stride_h, k_pages, k_scale, v_pages, v_scale, ns, st)
+                  : launch_write<__nv_bfloat16, 64>(k, v, k_smooth, slot_mapping, T, Hkv, k_stride_t, k_stride_h, v_stride_t, v_stride_h, k_pages, k_scale, v_pages, v_scale, ns, st);
+}
+
+extern "C" int sab_kvcache8_attn(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
+                                 const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
+                                 const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq,
+                                 int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h,
+                                 int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale,
+                                 void* workspace, void* stream) {
+  SAB_REQUIRE(q && k_pages && k_scale && v_pages && v_scale && k_smooth && out && cu_seqlens_q && seqused_k && block_table && workspace,
+              SAB_ERR_INVALID, "null pointer argument");
+  if (int r = check_dtype_dim(dtype, D)) return r;
+  SAB_REQUIRE(Hkv > 0 && Hq > 0 && Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
+  SAB_REQUIRE(nseq > 0 && Tq > 0 && max_seqlen_q > 0 && max_pages > 0 && page_size > 0 && page_size % 16 == 0 && table_stride >= max_pages,
+              SAB_ERR_INVALID, "need nseq, Tq, max_seqlen_q, max_pages > 0, page_size a positive multiple of 16 and table_stride >= max_pages");
+  SAB_REQUIRE(int64_t(max_seqlen_q) * (Hq / Hkv) <= kRows, SAB_ERR_INVALID,
+              "max_seqlen_q * Hq / Hkv = %lld exceeds %d query rows per KV head", (long long)max_seqlen_q * (Hq / Hkv), kRows);
+  SAB_REQUIRE(q_stride_t >= 0 && q_stride_h >= 0 && (q_stride_t | q_stride_h) % 4 == 0 && reinterpret_cast<uintptr_t>(q) % 8 == 0,
+              SAB_ERR_INVALID, "q needs 8-byte aligned rows (non-negative strides, multiples of 4 elements)");
+  const int64_t max_keys = int64_t(max_pages) * page_size;
+  const int64_t chunks = (max_keys + kChunk - 1) / kChunk;
+  // grid y is Hkv (attention) and Hq (combine); grid x is nseq * chunks and nseq * max_seqlen_q; key indices are int
+  SAB_REQUIRE(Hq <= 65535 && chunks * nseq < (int64_t(1) << 31) && int64_t(nseq) * max_seqlen_q < (int64_t(1) << 31),
+              SAB_ERR_INVALID, "launch grid too large: need Hq <= 65535, nseq * chunks < 2^31 and nseq * max_seqlen_q < 2^31");
+  SAB_REQUIRE(max_keys < (int64_t(1) << 31), SAB_ERR_INVALID, "max_pages * page_size must be < 2^31 keys");
+  Kv8Params p{q, k_pages, k_scale, v_pages, v_scale, cu_seqlens_q, seqused_k, block_table, table_stride, max_pages, page_size, Hq, Hkv,
+              int(chunks), max_seqlen_q, q_stride_t, q_stride_h, float(double(sm_scale) * 1.4426950408889634),
+              static_cast<float*>(workspace), nullptr};
+  p.ml_part = reinterpret_cast<float2*>(p.o_part + int64_t(Tq) * Hq * chunks * D);
+  Kv8CombineParams c{q, k_smooth, cu_seqlens_q, seqused_k, p.o_part, p.ml_part, out, lse, Tq, Hq, Hkv, int(chunks), max_seqlen_q,
+                     int(max_keys), q_stride_t, q_stride_h, o_stride_t, o_stride_h, sm_scale};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool causal = is_causal != 0;
+  if (dtype == SAB_DTYPE_FP16)
+    return D == 128 ? launch_attn<__half, 128>(p, c, nseq, causal, st) : launch_attn<__half, 64>(p, c, nseq, causal, st);
+  return D == 128 ? launch_attn<__nv_bfloat16, 128>(p, c, nseq, causal, st) : launch_attn<__nv_bfloat16, 64>(p, c, nseq, causal, st);
+}

@@ -1152,3 +1152,55 @@ def _(query, key, value, output, query_scale, key_scale, cu_seqlens_q, cu_seqlen
     if return_lse:
         return torch.empty((query.size(1), query.size(0)), dtype=torch.float32, device=query.device)
     return torch.empty((0,), dtype=torch.float32, device=query.device)
+
+
+# ----------------------------------------------------------------------------------------------- 8-bit paged KV cache
+def kvcache8_chunk_keys() -> int:
+    """Keys per split-KV chunk of sageattn_kvcache8 (a compile-time constant of the library)."""
+    return lib().sab_kvcache8_chunk_keys()
+
+
+@torch.library.custom_op("sageattention_b200::kvcache8_write", mutates_args=("k_pages", "k_scale", "v_pages", "v_scale"),
+                         device_types="cuda")
+def kvcache8_write(k: torch.Tensor, v: torch.Tensor, k_smooth: torch.Tensor, slot_mapping: torch.Tensor, k_pages: torch.Tensor,
+                   k_scale: torch.Tensor, v_pages: torch.Tensor, v_scale: torch.Tensor) -> None:
+    """Quantise tokens k, v [T,Hkv,D] into the slots slot_mapping [T] of an 8-bit paged cache (include/sageattn_b200.h,
+    sab_kvcache8_write)."""
+    T, Hkv, D = k.shape
+    num_pages, page_size = k_pages.shape[:2]
+    with torch.cuda.device(k.device):
+        check(lib().sab_kvcache8_write(k.data_ptr(), v.data_ptr(), _dt(k), k_smooth.data_ptr(), slot_mapping.data_ptr(), T, Hkv, D,
+                                       k.stride(0), k.stride(1), v.stride(0), v.stride(1), k_pages.data_ptr(), k_scale.data_ptr(),
+                                       v_pages.data_ptr(), v_scale.data_ptr(), num_pages, page_size, _stream(k)))
+
+
+@kvcache8_write.register_fake
+def _(k, v, k_smooth, slot_mapping, k_pages, k_scale, v_pages, v_scale):
+    return None
+
+
+@torch.library.custom_op("sageattention_b200::kvcache8_attn", mutates_args=("output",), device_types="cuda")
+def kvcache8_attn(q: torch.Tensor, k_pages: torch.Tensor, k_scale: torch.Tensor, v_pages: torch.Tensor, v_scale: torch.Tensor,
+                  k_smooth: torch.Tensor, output: torch.Tensor, cu_seqlens_q: torch.Tensor, seqused_k: torch.Tensor,
+                  block_table: torch.Tensor, max_seqlen_q: int, is_causal: int, sm_scale: float, return_lse: int) -> torch.Tensor:
+    """Split-KV attention of packed q [Tq,Hq,D] against an 8-bit paged cache (include/sageattn_b200.h, sab_kvcache8_attn).  Returns
+    the [Hq,Tq] natural-log LSE when return_lse, else an empty tensor."""
+    Tq, Hq, D = q.shape
+    page_size, Hkv = k_pages.size(1), k_pages.size(2)
+    nseq, max_pages = block_table.shape
+    lse = torch.empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32, device=q.device)
+    with torch.cuda.device(q.device):
+        ws = torch.empty(lib().sab_kvcache8_workspace_bytes(Tq, Hq, D, max_pages * page_size), dtype=torch.uint8, device=q.device)
+        check(lib().sab_kvcache8_attn(q.data_ptr(), _dt(q), k_pages.data_ptr(), k_scale.data_ptr(), v_pages.data_ptr(),
+                                      v_scale.data_ptr(), k_smooth.data_ptr(), output.data_ptr(), lse.data_ptr() if return_lse else None,
+                                      cu_seqlens_q.data_ptr(), seqused_k.data_ptr(), block_table.data_ptr(), block_table.stride(0),
+                                      max_pages, nseq, Tq, Hq, Hkv, D, page_size, q.stride(0), q.stride(1), output.stride(0),
+                                      output.stride(1), max_seqlen_q, is_causal, float(sm_scale), ws.data_ptr(), _stream(q)))
+    return lse
+
+
+@kvcache8_attn.register_fake
+def _(q, k_pages, k_scale, v_pages, v_scale, k_smooth, output, cu_seqlens_q, seqused_k, block_table, max_seqlen_q, is_causal,
+      sm_scale, return_lse):
+    Tq, Hq, _ = q.shape
+    return q.new_empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32)

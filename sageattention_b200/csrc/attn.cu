@@ -3,7 +3,8 @@
 //
 // Serves (a) the INT8+FP8 path (sageattn_qk_int8_pv_fp8_cuda and everything built on it) and (b) the FP16-PV numerics of the
 // reference's Triton kernels (kPV16: sageattn_varlen, sageattn_qk_int8_pv_fp16_triton incl. attn_mask,
-// sageattn_qk_int8_pv_fp16_cuda).  One CTA = one 128-row Q tile of one (batch, head), 384 threads:
+// sageattn_qk_int8_pv_fp16_cuda).  One CTA = one 128-row Q tile of one (batch, head), 384 threads (the dense INT8+FP8 kernel at
+// D = 128: one 192-row tile, 512 threads, a third consumer warpgroup; see kNC below):
 //   warps 0-3 / 4-7 : two consumer warpgroups, 64 Q rows each.  Per 64-key tile: S = Q K^T (wgmma s8, int32 accumulators in
 //                     registers), online softmax in registers, P (e4m3 or f16) handed to the PV wgmma as its register A operand,
 //                     O (fp32, 64 x D) accumulated in registers.  The loop is rotated so that each warpgroup issues PV(j-1)
@@ -29,13 +30,14 @@
 
 namespace sab {
 
-constexpr int kConsumerWGs = 2;                           // 64 Q rows each
-constexpr int kNumThreads = (kConsumerWGs + 1) * 128;     // + the producer warpgroup (one TMA warp; setmaxnreg is per warpgroup)
-constexpr int kStages = 6;                                // K / V^T ring depth (64-key tiles)
+// kNC consumer warpgroups of 64 Q rows each: 2 (a 128-row Q tile), or 3 (192 rows) in the dense INT8+FP8 kernel at D = 128
+template <int kNC>
+constexpr int kNumThreads = (kNC + 1) * 128;   // + the producer warpgroup (one TMA warp; setmaxnreg is per warpgroup)
+constexpr int kStages = 6;                     // K / V^T ring depth (64-key tiles)
 
-template <int D, bool kPV16>
+template <int D, bool kPV16, int kNC = 2>
 constexpr size_t attn_smem_bytes() {
-  return size_t(BM) * D + size_t(kStages) * (BN * D + BN * D * (kPV16 ? 2 : 1)) + (1 + 2 * kStages) * 8 + 1024;
+  return size_t(kNC * 64) * D + size_t(kStages) * (BN * D + BN * D * (kPV16 ? 2 : 1)) + (1 + 2 * kStages) * 8 + 1024;
 }
 
 // Shared memory of the block-sparse form behind the INT8+FP8 kernel's barriers: build_kv_list's 64 bytes of counts, then the list
@@ -117,8 +119,15 @@ constexpr bool kSparse = kMask && !kPV16;     // block mask of the INT8+FP8 path
 // kBR with kWindow and kSeqV: the packed bottom-right causal form.  Sequence b's rows see the window (-1, Lk_b - Lq_b), derived
 // here instead of read from win_arg: the window kernel's path on that window, tile for tile.  The right side may be negative
 // (Lk_b < Lq_b: the first Lq_b - Lk_b rows see no key) and always bounds, so it is read as bounded whatever its sign.
-template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false, bool kWindow = false, bool kSeqV = false, bool kBR = false>
-__global__ void __launch_bounds__(kNumThreads, 1)
+// kNC = 3 (dense INT8+FP8 at D = 128 only): three consumer warpgroups on a 192-row Q tile, so each SM sub-partition has more
+// independent warps to hide the softmax's latency, and each K/V tile serves 192 rows.  160 registers per consumer thread hold
+// O (64) but not a 64-register tile product next to S: the FP8 PV runs as two m64n64 halves into 32 registers, each folded
+// into O before the next (a column's product does not depend on N, so O is the same to the bit), and softmax(j) runs under
+// the second half.  The turn passes round the three warpgroups (see the main loop).  At 160 registers ptxas keeps three values
+// (a turn barrier id and the two rows' Q scales) in 12 bytes of local memory, reloaded once per 64-key step.
+template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false, bool kWindow = false, bool kSeqV = false, bool kBR = false,
+          int kNC = 2>
+__global__ void __launch_bounds__(kNumThreads<kNC>, 1)
 sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                      const __grid_constant__ CUtensorMap tmV, const __grid_constant__ AttnParams p,
                      const __grid_constant__ Window win_arg) {
@@ -126,8 +135,11 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   constexpr uint32_t V_TILE = D * BN * (kPV16 ? 2 : 1);
   constexpr int SWQK = D;                        // swizzle span of the Q/K tiles (= row bytes)
   constexpr int SWV = kPV16 ? 128 : 64;          // V^T rows: 64 keys = 64 B (fp8) / 128 B (fp16)
-  constexpr uint32_t Q_BYTES = BM * D;
+  static_assert(kNC == 2 || (kNC == 3 && D == 128 && !kPV16 && !kMask && !kWindow && !kSeqV), "three consumers: dense INT8+FP8, D = 128");
+  constexpr int QM = kNC * 64;                   // Q rows per CTA
+  constexpr uint32_t Q_BYTES = QM * D;
   constexpr int NO = D / 2;                      // fp32 O accumulators per thread (64 x D over 128 threads)
+  constexpr bool kHalfPV = kNC == 3;             // the FP8 PV as two m64n64 halves (see above)
 
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* sQ = smem;
@@ -159,22 +171,22 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     q_blk0 = p.cu_qs[b];
     k_blk0 = p.cu_ks[b];
     tb = 0;
-    if (qt * BM >= q_len) return;  // attn_qk_int8_block_varlen.py:84-85
+    if (qt * QM >= q_len) return;  // attn_qk_int8_block_varlen.py:84-85
   }
   // the packed window form reads its sequence's clamped copy; every other form reads the kernel argument itself
   [[maybe_unused]] Window seq_win;
   if constexpr (kWindow && kSeqV) seq_win = kBR ? Window{-1, kv_len - q_len} : seq_window(win_arg, q_len, kv_len);
   const Window& win = (kWindow && kSeqV) ? seq_win : win_arg;
   int n_kv = (kv_len + BN - 1) / BN;                 // 64-key tiles
-  if (p.causal) n_kv = min(n_kv, (p.causal_q_offset + (qt + 1) * BM + BN - 1) / BN);
+  if (p.causal) n_kv = min(n_kv, (p.causal_q_offset + (qt + 1) * QM + BN - 1) / BN);
   if constexpr (kSparse<kPV16, kMask>) {
     const BlockMask bm{static_cast<const uint8_t*>(p.mask), p.mask_sb, p.mask_sh, p.mask_sm, p.mask_sn};
-    n_kv = build_kv_list<kNumThreads>(bm, b, h, qt, n_kv, kv_list<D>(smem), kv_scratch<D>(smem));
+    n_kv = build_kv_list<kNumThreads<kNC>>(bm, b, h, qt, n_kv, kv_list<D>(smem), kv_scratch<D>(smem));
   }
   [[maybe_unused]] int j0 = 0;   // window form: the first 64-key tile of the CTA's range
   if constexpr (kWindow) {
     int j1;
-    window_tiles<kBR>(win, p.causal != 0, qt * BM, min(qt * BM + BM, q_len) - 1, kv_len, j0, j1);
+    window_tiles<kBR>(win, p.causal != 0, qt * QM, min(qt * QM + QM, q_len) - 1, kv_len, j0, j1);
     n_kv = j1 - j0;
   }
 
@@ -183,21 +195,21 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     mbar_init(q_full, 1);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(kv_full + i, 1);
-      mbar_init(kv_empty + i, kConsumerWGs);
+      mbar_init(kv_empty + i, kNC);
     }
     fence_barrier_init();
   }
   __syncthreads();
 
-  if (warp >= kConsumerWGs * 4) {
+  if (warp >= kNC * 4) {
     // =============================== TMA producer ===============================
     setmaxnreg_dec<24>();
-    if (warp == kConsumerWGs * 4 && lane == 0 && n_kv > 0) {
+    if (warp == kNC * 4 && lane == 0 && n_kv > 0) {
       tma_prefetch_desc(&tmQ);
       tma_prefetch_desc(&tmK);
       tma_prefetch_desc(&tmV);
       mbar_expect_tx(q_full, Q_BYTES);
-      tma_load_4d(sQ, &tmQ, q_full, 0, q_off + qt * BM, h, tb);
+      tma_load_4d(sQ, &tmQ, q_full, 0, q_off + qt * QM, h, tb);   // the host's Q box is QM rows
       int ready_seg = -1;
       for (int j = 0; j < n_kv; ++j) {
         const int s = j % kStages;
@@ -232,7 +244,7 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   }
 
   // =============================== consumer warpgroups ===============================
-  setmaxnreg_inc<240>();
+  setmaxnreg_inc<kNC == 2 ? 240 : 160>();   // 3 x 128 x 160 + 128 x 24 = 64512 of the SM's 65536
   // wgmma accumulator layout (m64nN): warp w of the warpgroup owns rows 16w..16w+15; lane = 4 g + t holds rows 16w+g (registers
   // 4i, 4i+1) and 16w+g+8 (4i+2, 4i+3) at columns 8i+2t, 8i+2t+1.  A row is spread over the 4 lanes of a quad.
   const int wg = warp >> 2;
@@ -245,8 +257,15 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     const int row = row0 + 8 * i;
-    q_row[i] = qt * BM + row;  // row index inside the sequence
-    qss[i] = q_dequant_log2(p, qs_base, q_blk0 + qt, row);
+    q_row[i] = qt * QM + row;  // row index inside the sequence
+    if constexpr (kNC == 2) {
+      qss[i] = q_dequant_log2(p, qs_base, q_blk0 + qt, row);
+    } else {
+      // a 192-row tile covers parts of two 128-row scale blocks; a row past the end (never stored) reads the last row's scale,
+      // which exists
+      const int r = min(q_row[i], q_len - 1);
+      qss[i] = q_dequant_log2(p, qs_base, q_blk0 + r / BM, r % BM);
+    }
   }
   const float tau = p.lazy_tau;
   float m[2] = {kMaskValue, kMaskValue};   // running max (log2 units, includes the -8.807 offset on the fp8 path)
@@ -287,18 +306,19 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         lo[i] = win.left >= 0 ? q_row[i] - win.left - kj * BN : 0;
       }
     }
-    masked_tile = kElemMask<kPV16, kMask> || (kv_len - kj * BN < BN) || (p.causal && (kj + 1) * BN > p.causal_q_offset + qt * BM + 1);
+    masked_tile = kElemMask<kPV16, kMask> || (kv_len - kj * BN < BN) || (p.causal && (kj + 1) * BN > p.causal_q_offset + qt * QM + 1);
     if constexpr (kWindow) {
       // the top row's window ends inside the tile, or the bottom row's starts after its first key
-      masked_tile = masked_tile || ((kBR || win.right >= 0) && (kj + 1) * BN - 1 > qt * BM + win.right) ||
-                    (win.left >= 0 && kj * BN < qt * BM + BM - 1 - win.left);
+      masked_tile = masked_tile || ((kBR || win.right >= 0) && (kj + 1) * BN - 1 > qt * QM + win.right) ||
+                    (win.left >= 0 && kj * BN < qt * QM + QM - 1 - win.left);
     }
   };
 
   uint32_t s[32];                   // S of the tile in flight (int32)
   float alpha[2];                   // O rescale factor of the last softmax'd tile
   uint32_t a[kPV16 ? 4 : 2][4];     // P of the tile whose PV comes next, as the PV A operand
-  [[maybe_unused]] float ot[NO];    // FP8 path: its P V, from zero
+  constexpr int NOT = kHalfPV ? NO / 2 : NO;
+  [[maybe_unused]] float ot[NOT];   // FP8 path: its P V (kHalfPV: one half of it), from zero
 
   // ---- S (registers, int32) -> P: running max m, sum d, rescale factor alpha, P as A fragments
   float e[32];                      // P of the last softmax in fp32, same register order as S
@@ -486,9 +506,21 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     } else {
       fence_regs(ot);
 #pragma unroll
-      for (int i = 0; i < NO; ++i) o[i] += ot[i];
+      for (int i = 0; i < NOT; ++i) o[i] += ot[i];
     }
     if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty + j % kStages);   // K(j) and V(j) consumed by this warpgroup
+  };
+  // kHalfPV: ot = P V(j) for output columns 64 hh .. 64 hh + 63 (V^T rows from 64 hh: 64 rows of 64 B, a whole number of 64-B
+  // swizzle atoms), and its fold into those columns of O
+  auto issue_pv_half = [&](int j, int hh) {
+    const uint64_t dV = dV0 + uint64_t(j % kStages) * (V_TILE >> 4) + uint64_t(hh) * ((64 * SWV) >> 4);
+#pragma unroll
+    for (int c = 0; c < 2; ++c) wgmma_pv_f8(ot, a[c], dV + 2 * c, c > 0);
+  };
+  auto fold_half = [&](int hh) {
+    fence_regs(ot);
+#pragma unroll
+    for (int i = 0; i < NOT; ++i) o[NOT * hh + i] += ot[i];
   };
 
   // ---- main loop, rotated so each warpgroup has ONE tensor-core phase per tile: QK(j) and PV(j-1) issued back to back, then
@@ -504,70 +536,140 @@ sage_attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   // touched.  Slot j-1 is released one phase later than it was consumed; the ring absorbs it.
   constexpr bool kSoftmaxUnderPV = D == 128;
   constexpr uint32_t kTurnThreads = 2 * 128;
-  const uint32_t my_turn = 1 + wg, their_turn = 2 - wg;
+  const uint32_t my_turn = 1 + wg;
+  [[maybe_unused]] const uint32_t their_turn = 2 - wg;   // two warpgroups
   PhaseClocks clk;
   clk.loop_start();
-  if (n_kv > 0) {
-    mbar_wait_wd(q_full, 0);
-    if (wg == 1) named_bar_arrive(their_turn, kTurnThreads);
-    tile_setup(0);
-    mbar_wait_wd(kv_full, 0);                  // never hold the turn while waiting on TMA
-    named_bar_sync(my_turn, kTurnThreads);
-    wgmma_fence();
-    issue_qk(0);
-    wgmma_commit();
-    named_bar_arrive(their_turn, kTurnThreads);
-    wgmma_wait<0>();
-    fence_regs(s);
-    softmax(0);
-    pack_p();
-  }
-  for (int j = 1; j < n_kv; ++j) {
-    tile_setup(j);
-    mbar_wait_wd(kv_full + j % kStages, (j / kStages) & 1);
-    named_bar_sync(my_turn, kTurnThreads);
-    clk.turn();
-    if constexpr (kPV16) rescale_o();          // before the in-place PV
-    wgmma_fence();
-    if constexpr (kSoftmaxUnderPV) {
-      issue_qk(j);
+  if constexpr (kHalfPV) {
+    // Three warpgroups: the turn goes round them (warpgroup w waits on barrier 1 + w and hands the turn to barrier
+    // 1 + (w + 1) % 3, each barrier counting its owner and its predecessor).  Warpgroup 2 hands the first turn to warpgroup 0
+    // and skips the hand-over after its last phase, so each barrier sees n_kv + 1 arrivals and n_kv + 1 waits and none is left
+    // over.  Warpgroups whose rows all lie past Sq run the same phases (n_kv is uniform per CTA), so the rotation never skips
+    // one.  A phase is PV(j-1) half 0 and QK(j), two commit groups; half 0 is folded into O as soon as it lands (under QK(j)) and
+    // half 1 is issued before the turn passes, so the phase reaches the tensor cores in one piece; softmax(j) then runs under
+    // half 1.  O's per-element sequence stays o *= alpha(j-1), o += PV(j-1).
+    const uint32_t next_turn = 1 + (wg + 1) % kNC;
+    if (n_kv > 0) {
+      mbar_wait_wd(q_full, 0);
+      if (wg == kNC - 1) named_bar_arrive(next_turn, kTurnThreads);
+      tile_setup(0);
+      mbar_wait_wd(kv_full, 0);                // never hold the turn while waiting on TMA
+      named_bar_sync(my_turn, kTurnThreads);
+      wgmma_fence();
+      issue_qk(0);
       wgmma_commit();
-      issue_pv(j - 1);
-      wgmma_commit();
-    } else {
-      issue_pv(j - 1);
-      issue_qk(j);
-      wgmma_commit();
+      named_bar_arrive(next_turn, kTurnThreads);
+      wgmma_wait<0>();
+      fence_regs(s);
+      softmax(0);
+      pack_p();
     }
-    named_bar_arrive(their_turn, kTurnThreads);
-    if constexpr (!kPV16) rescale_o();         // overlaps the MMAs
-    if constexpr (kSoftmaxUnderPV) {
-      wgmma_wait<1>();                         // S(j) is ready; PV(j-1) may still run
+    for (int j = 1; j < n_kv; ++j) {
+      tile_setup(j);
+      mbar_wait_wd(kv_full + j % kStages, (j / kStages) & 1);
+      named_bar_sync(my_turn, kTurnThreads);
+      clk.turn();
+      wgmma_fence();
+      issue_pv_half(j - 1, 0);
+      wgmma_commit();
+      issue_qk(j);
+      wgmma_commit();
+      rescale_o();
+      wgmma_wait<1>();                         // PV(j-1) half 0 is ready; QK(j) may still run
+      fold_half(0);
+      wgmma_fence();
+      issue_pv_half(j - 1, 1);
+      wgmma_commit();
+      named_bar_arrive(next_turn, kTurnThreads);
+      wgmma_wait<1>();                         // S(j) is ready; half 1 may still run
       fence_regs(s);
       clk.mma_done();
       softmax(j);
       wgmma_wait<0>();
-      finish_pv(j - 1);
-    } else {
+      fold_half(1);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty + (j - 1) % kStages);
+      pack_p();
+      clk.soft_done();
+    }
+    if (n_kv > 0) {
+      named_bar_sync(my_turn, kTurnThreads);
+      wgmma_fence();
+      issue_pv_half(n_kv - 1, 0);
+      wgmma_commit();
+      rescale_o();
+      wgmma_wait<0>();
+      fold_half(0);
+      wgmma_fence();
+      issue_pv_half(n_kv - 1, 1);
+      wgmma_commit();
+      if (wg != kNC - 1) named_bar_arrive(next_turn, kTurnThreads);
+      wgmma_wait<0>();
+      fold_half(1);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(kv_empty + (n_kv - 1) % kStages);
+    }
+  } else {
+    if (n_kv > 0) {
+      mbar_wait_wd(q_full, 0);
+      if (wg == 1) named_bar_arrive(their_turn, kTurnThreads);
+      tile_setup(0);
+      mbar_wait_wd(kv_full, 0);                  // never hold the turn while waiting on TMA
+      named_bar_sync(my_turn, kTurnThreads);
+      wgmma_fence();
+      issue_qk(0);
+      wgmma_commit();
+      named_bar_arrive(their_turn, kTurnThreads);
       wgmma_wait<0>();
       fence_regs(s);
-      clk.mma_done();
-      finish_pv(j - 1);
-      softmax(j);
+      softmax(0);
+      pack_p();
     }
-    pack_p();
-    clk.soft_done();
-  }
-  if (n_kv > 0) {
-    named_bar_sync(my_turn, kTurnThreads);
-    if constexpr (kPV16) rescale_o();
-    wgmma_fence();
-    issue_pv(n_kv - 1);
-    wgmma_commit();
-    if (wg == 0) named_bar_arrive(their_turn, kTurnThreads);
-    if constexpr (!kPV16) rescale_o();
-    wgmma_wait<0>();
-    finish_pv(n_kv - 1);
+    for (int j = 1; j < n_kv; ++j) {
+      tile_setup(j);
+      mbar_wait_wd(kv_full + j % kStages, (j / kStages) & 1);
+      named_bar_sync(my_turn, kTurnThreads);
+      clk.turn();
+      if constexpr (kPV16) rescale_o();          // before the in-place PV
+      wgmma_fence();
+      if constexpr (kSoftmaxUnderPV) {
+        issue_qk(j);
+        wgmma_commit();
+        issue_pv(j - 1);
+        wgmma_commit();
+      } else {
+        issue_pv(j - 1);
+        issue_qk(j);
+        wgmma_commit();
+      }
+      named_bar_arrive(their_turn, kTurnThreads);
+      if constexpr (!kPV16) rescale_o();         // overlaps the MMAs
+      if constexpr (kSoftmaxUnderPV) {
+        wgmma_wait<1>();                         // S(j) is ready; PV(j-1) may still run
+        fence_regs(s);
+        clk.mma_done();
+        softmax(j);
+        wgmma_wait<0>();
+        finish_pv(j - 1);
+      } else {
+        wgmma_wait<0>();
+        fence_regs(s);
+        clk.mma_done();
+        finish_pv(j - 1);
+        softmax(j);
+      }
+      pack_p();
+      clk.soft_done();
+    }
+    if (n_kv > 0) {
+      named_bar_sync(my_turn, kTurnThreads);
+      if constexpr (kPV16) rescale_o();
+      wgmma_fence();
+      issue_pv(n_kv - 1);
+      wgmma_commit();
+      if (wg == 0) named_bar_arrive(their_turn, kTurnThreads);
+      if constexpr (!kPV16) rescale_o();
+      wgmma_wait<0>();
+      finish_pv(n_kv - 1);
+    }
   }
   clk.flush();
 
@@ -658,16 +760,40 @@ static bool exact_max_mode() {
   return v == 1;
 }
 constexpr float kLazyTau = 4.0f;
+// The dense INT8+FP8 kernel at D = 128 runs three consumer warpgroups on 192-row Q tiles.  SAB_ATTN_CONSUMERS=2 keeps it on two
+// (128-row tiles, as every other form), so the two forms can be compared; they compute the same bits.
+static int dense_consumers() {
+  static int v = -1;
+  if (v < 0) {
+    const char* e = getenv("SAB_ATTN_CONSUMERS");
+    v = (e != nullptr && e[0] == '2') ? 2 : 3;
+  }
+  return v;
+}
 
+// nc: consumer warpgroups, 3 only for the dense INT8+FP8 instantiations at D = 128 (the tensor map of Q has nc * 64-row boxes
+// and the grid nc * 64-row tiles)
 template <int D, bool kKT, typename OutT, bool kPV16, bool kMask = false>
 static int launch_attn(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, AttnParams p,
-                       dim3 grid, cudaStream_t stream) {
+                       dim3 grid, cudaStream_t stream, int nc = 2) {
   p.lazy_tau = (kPV16 || exact_max_mode()) ? 0.0f : kLazyTau;
+  if constexpr (D == 128 && !kPV16 && !kMask) {
+    if (nc == 3) {
+      constexpr size_t smem = attn_smem_bytes<D, false, 3>();
+      auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, false, false, false, false, 3>;
+      static bool configured[64] = {};
+      if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
+      kern<<<grid, kNumThreads<3>, smem, stream>>>(tq, tk, tv, p, Window{-1, -1});
+      SAB_CUDA_OK(cudaGetLastError());
+      return SAB_OK;
+    }
+  }
+  SAB_REQUIRE(nc == 2, SAB_ERR_INVALID, "three consumer warpgroups need the dense INT8+FP8 kernel at head dim 128");
   constexpr size_t smem = attn_smem_bytes<D, kPV16>();
   auto kern = sage_attn_fwd_kernel<D, kKT, OutT, kPV16, kMask>;
   static bool configured[64] = {};
   if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
-  kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p, Window{-1, -1});
+  kern<<<grid, kNumThreads<2>, smem, stream>>>(tq, tk, tv, p, Window{-1, -1});
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
 }
@@ -682,7 +808,7 @@ static int launch_attn_window(const CUtensorMap& tq, const CUtensorMap& tk, cons
   auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, false, true, kSeqV, kBR>;
   static bool configured[64] = {};
   if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
-  kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p, w);
+  kern<<<grid, kNumThreads<2>, smem, stream>>>(tq, tk, tv, p, w);
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
 }
@@ -696,7 +822,7 @@ static int launch_attn_seqv(const CUtensorMap& tq, const CUtensorMap& tk, const 
   auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, false, false, true>;
   static bool configured[64] = {};
   if (int st = ensure_dynamic_smem(kern, smem, configured)) return st;
-  kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p, Window{-1, -1});
+  kern<<<grid, kNumThreads<2>, smem, stream>>>(tq, tk, tv, p, Window{-1, -1});
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
 }
@@ -712,7 +838,7 @@ static int launch_attn_blocksparse(const CUtensorMap& tq, const CUtensorMap& tk,
   auto kern = sage_attn_fwd_kernel<D, kKT, OutT, false, true, false, kSeqV>;
   static bool configured[64] = {};
   if (int st = ensure_dynamic_smem(kern, smem_max, configured)) return st;
-  kern<<<grid, kNumThreads, smem, stream>>>(tq, tk, tv, p, Window{-1, -1});
+  kern<<<grid, kNumThreads<2>, smem, stream>>>(tq, tk, tv, p, Window{-1, -1});
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
 }
@@ -773,6 +899,10 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
   int st = sab_check_device();
   if (st != SAB_OK) return st;
 
+  // the dense INT8+FP8 kernel at D = 128 (also sequence-parallel): three consumer warpgroups unless SAB_ATTN_CONSUMERS=2
+  const int nc = (D == 128 && !pv16 && !varlen && tl_mask == nullptr && tl_block_mask == nullptr && tl_window == nullptr &&
+                  !tl_seq_v) ? dense_consumers() : 2;
+  const uint32_t qbox = uint32_t(nc) * 64;   // Q rows per CTA
   CUtensorMap tq, tk, tv;
   const int swqk = D == 128 ? 128 : 64;
   const uint32_t kbox = BN;                 // 64-key tiles
@@ -780,11 +910,11 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
   const int swv = pv16 ? 128 : 64;
   if (kv_seg_len > 0) {
     const int P = Skv / kv_seg_len;
-    if ((st = make_map_u8(&tq, q_int8, D, Sq, Hq, B, q_stride_s, q_stride_h, q_stride_b, D, BM, swqk))) return st;
+    if ((st = make_map_u8(&tq, q_int8, D, Sq, Hq, B, q_stride_s, q_stride_h, q_stride_b, D, qbox, swqk))) return st;
     if ((st = make_map_u8(&tk, k_int8, D, kv_seg_len, Hkv, uint64_t(B) * P, k_stride_s, k_stride_h, k_stride_b, D, kbox, swqk))) return st;
     if ((st = make_map_u8(&tv, v_fp8, v_s_pad * vb, D, Hkv, uint64_t(B) * P, v_s_pad * vb, uint64_t(v_s_pad) * D * vb, uint64_t(v_s_pad) * D * Hkv * vb, vbox, D, swv))) return st;
   } else if (!varlen) {
-    if ((st = make_map_u8(&tq, q_int8, D, Sq, Hq, B, q_stride_s, q_stride_h, q_stride_b, D, BM, swqk))) return st;
+    if ((st = make_map_u8(&tq, q_int8, D, Sq, Hq, B, q_stride_s, q_stride_h, q_stride_b, D, qbox, swqk))) return st;
     if ((st = make_map_u8(&tk, k_int8, D, Skv > 0 ? Skv : 1, Hkv, B, k_stride_s, k_stride_h, k_stride_b, D, kbox, swqk))) return st;
     if ((st = make_map_u8(&tv, v_fp8, v_s_pad * vb, D, Hkv, B, v_s_pad * vb, uint64_t(v_s_pad) * D * vb, uint64_t(v_s_pad) * D * Hkv * vb, vbox, D, swv))) return st;
   } else {
@@ -800,7 +930,7 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
   p.o_stride_b = o_stride_b; p.o_stride_h = o_stride_h; p.o_stride_s = o_stride_s;
   p.B = B; p.Hq = Hq; p.Hkv = Hkv; p.Sq = Sq; p.Sk = Skv;
   const int max_q = varlen ? max_seqlen_q : Sq;
-  p.n_q_tiles = (max_q + BM - 1) / BM;
+  p.n_q_tiles = (max_q + int(qbox) - 1) / int(qbox);
   p.causal = is_causal ? 1 : 0;
   p.sm_scale_log2 = fold_sm_scale ? 1.0f : sm_scale * 1.44269504088896340736f;
   p.q_gran = q_gran;
@@ -925,7 +1055,7 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
 #define SAB_LAUNCH(DD, KT, T)                                                      \
   do {                                                                             \
     if (pv16) return launch_attn<DD, KT, T, true>(tq, tk, tv, p, grid, s);         \
-    return launch_attn<DD, KT, T, false>(tq, tk, tv, p, grid, s);                  \
+    return launch_attn<DD, KT, T, false>(tq, tk, tv, p, grid, s, nc);              \
   } while (0)
   if (D == 128) {
     if (kt) { if (bf) SAB_LAUNCH(128, true, __nv_bfloat16); else SAB_LAUNCH(128, true, __half); }

@@ -632,6 +632,20 @@ int sab_kvcache8_attn(const void* q, int dtype, const int8_t* k_pages, const flo
                       const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq, int Tq,
                       int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h, int64_t o_stride_t,
                       int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale, void* workspace, void* stream);
+/* sab_kvcache8_prefill: attention of packed query chunks of any length against the same cache (chunked prefill, prefix caching):
+ *   the arguments, checks and causal rule of sab_kvcache8_attn without its row limit and without a workspace.  One CTA per
+ *   (sequence, 128-row Q tile, Q head), grid nseq * ceil(max_seqlen_q / 128) x Hq, so no host synchronisation.  Numerics: those of
+ *   sab_kvcache8_attn with one chunk: Q quantised per (token, head) to INT8, logits in log2 units float(dot(q8, k8)) * (q_scale *
+ *   sm_scale * log2e) * k_scale, one exact running max per row over 64-key tiles from key 0, P = bf16(p * v_scale) times bf16(v8)
+ *   with fp32 accumulation (wgmma), O / l.  A row's bits depend only on its own q, keys and values.  out [Tq, Hq, D] (strides
+ *   o_stride_t / o_stride_h, even, 4-byte aligned) in `dtype`; lse (optional) [Hq, Tq] fp32 as in sab_kvcache8_attn.  A row that
+ *   sees no key returns 0 and lse -inf; rows past max_seqlen_q are not written.  Launch-grid limits, refused with SAB_ERR_INVALID:
+ *   Hq <= 65535, nseq * ceil(max_seqlen_q / 128) < 2^31 and max_pages * page_size < 2^31. */
+int sab_kvcache8_prefill(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
+                         const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
+                         const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq, int Tq,
+                         int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h, int64_t o_stride_t,
+                         int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale, void* stream);
 
 #ifdef __cplusplus
 }

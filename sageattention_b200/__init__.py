@@ -10,7 +10,7 @@ from .quant import per_block_int8, per_warp_int8, per_thread_int8, per_channel_f
 from .cache import QuantizedKV, quantize_kv, sageattn_prequantized
 from .host import sageattn_host
 from .predict import predict_block_mask, predict_block_mask_varlen
-from .kvcache8 import PagedKVCache8, sageattn_kvcache8
+from .kvcache8 import PagedKVCache8, sageattn_kvcache8, sageattn_kvcache8_prefill
 
 __all__ = ["sageattn", "sageattn_varlen", "sageattn_qk_int8_pv_fp16_triton", "sageattn_qk_int8_pv_fp16_cuda",
            "sageattn_qk_int8_pv_fp8_cuda", "sageattn_qk_int8_pv_fp8_cuda_sm90", "sageattn_blocksparse", "sageattn_window",
@@ -18,4 +18,4 @@ __all__ = ["sageattn", "sageattn_varlen", "sageattn_qk_int8_pv_fp16_triton", "sa
            "sageattn_varlen_kvcache",
            "per_block_int8", "per_warp_int8", "per_thread_int8", "per_channel_fp8", "k_mean", "transpose_v_f16",
            "QuantizedKV", "quantize_kv", "sageattn_prequantized", "sageattn_host", "predict_block_mask",
-           "predict_block_mask_varlen", "PagedKVCache8", "sageattn_kvcache8"]
+           "predict_block_mask_varlen", "PagedKVCache8", "sageattn_kvcache8", "sageattn_kvcache8_prefill"]

@@ -7,6 +7,8 @@
 //                      bf16(v8) on mma.sync bf16 with fp32 accumulators.  Writes the chunk's unnormalised O, max and sum.
 //   kv8_combine_kernel one CTA per (query row, Q head): folds the row's chunks in ascending order, O / L and the natural-log lse.
 // Decode is bound by the bytes of the cache, so the kernels aim at one read of each K / V byte per chunk, not at tensor-core rate.
+//   kv8_prefill_kernel one CTA per (sequence, 128-row Q tile, Q head) for query chunks of any length (chunked prefill): the decode
+//                      numerics without chunks, on the warpgroup tensor cores (see its section below).
 #include <atomic>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -457,6 +459,306 @@ __global__ void __launch_bounds__(D) kv8_combine_kernel(const Kv8CombineParams p
   }
 }
 
+// ------------------------------------------------------------------------------------------------ chunked prefill
+// kv8_prefill_kernel: one CTA per (sequence, 128-row Q tile, Q head), three warpgroups.
+//   warpgroups 0-1  consumers, 64 query rows each.  Q is quantised per (token, head) into a swizzled s8 tile; per 64-key tile, S =
+//                   Q K^T on wgmma m64n64k32 s8, the decode kernel's exact running max, P = bf16(p * v_scale) as the register A
+//                   operand of wgmma bf16 against V^T, O in fp32 registers.  A row folds all its keys: no chunks, no combine.
+//   warpgroup 2     producer.  16-byte cp.async of each tile's K (int8) and V (e4m3) rows through the block table into a
+//                   kPfStages-deep ring, zero-filled past Lk_b (no slot past the sequence is read), with the tile's 64 k / v scales;
+//                   kPfLag tiles behind its loads it converts V exactly to bf16 into the swizzled V^T tile the PV wgmma reads, so
+//                   the consumers' serial path holds no conversion.
+// Every row runs over the same tile grid from key 0, and a tile past a row's horizon adds p = 0 with alpha = 1, so a row's bits do
+// not depend on which other rows share its CTA: prefilling a prompt in chunks of any size gives the same bits.
+constexpr int kPfRows = 128;       // query rows per CTA
+constexpr int kPfStages = 4;       // K / V ring depth (64-key tiles)
+constexpr int kPfLag = 2;          // tiles the producer's loads run ahead of its V conversion
+constexpr int kPfThreads = 384;
+
+template <int D>
+struct PfSmem {
+  alignas(1024) int8_t q8[kPfRows * D];              // s8 Q, K-major, swizzled (span D bytes)
+  alignas(1024) int8_t k8[kPfStages][kTile * D];     // s8 K rows, K-major, swizzled (span D bytes)
+  alignas(1024) uint16_t vt[kPfStages][D * kTile];   // bf16 V^T [D][64 keys], 128-B swizzle
+  alignas(16) uint8_t v8[kPfStages][kTile * D];      // e4m3 V rows as loaded
+  float ks[kPfStages][kTile], vs[kPfStages][kTile];
+  float qc[kPfRows];                                 // q_scale * sm_scale * log2(e)
+  float qk[kPfRows];                                 // q . k_smooth (lse only)
+  uint64_t full[kPfStages], empty[kPfStages];
+};
+
+// 16-byte chunk c of row r of a K-major tile of D-byte rows under the D-byte hardware swizzle (128 B: c ^ r % 8; 64 B: c ^ r / 2 % 4)
+template <int D>
+__device__ __forceinline__ int pf_swz(int r, int c) { return c ^ ((r * D >> 7) & (D / 16 - 1)); }
+
+struct PfParams {
+  const void* q; const int8_t* k_pages; const float* k_scale; const uint8_t* v_pages; const float* v_scale; const float* k_smooth;
+  const int32_t* cu_q; const int32_t* seqused_k; const int32_t* table; int64_t table_stride;
+  void* out; float* lse;
+  int max_pages, page_size, Hq, Hkv, n_qt, max_seqlen_q, Tq;
+  int64_t q_st, q_sh, o_st, o_sh;
+  float sm_scale, scale_log2;   // scale_log2 = sm_scale * log2(e)
+};
+
+template <typename T, int D, bool kCausal>
+__global__ void __launch_bounds__(kPfThreads, 1) kv8_prefill_kernel(const PfParams p) {
+  using S = PfSmem<D>;
+  extern __shared__ __align__(1024) unsigned char pf_smem[];
+  S& sm = *reinterpret_cast<S*>(pf_smem + ((1024u - (smem_u32(pf_smem) & 1023u)) & 1023u));   // 1 KB-aligned swizzled tiles
+  const int b = blockIdx.x / p.n_qt, qt = p.n_qt - 1 - blockIdx.x % p.n_qt, hq = blockIdx.y;   // longest rows first
+  const int hk = hq / (p.Hq / p.Hkv);
+  const int q0 = p.cu_q[b];
+  const int Lq = min(p.cu_q[b + 1] - q0, p.max_seqlen_q);
+  const int Lk = max(0, min(p.seqused_k[b], p.max_pages * p.page_size));
+  const int r0 = qt * kPfRows;          // the CTA's first row inside the sequence
+  if (r0 >= Lq) return;
+  // keys [0, kmax) hold every key a row of the CTA sees; tiles past `first_h` (the first row's last key) take the masked path
+  const int last = min(r0 + kPfRows, Lq) - 1;
+  const int kmax = kCausal ? max(0, min(Lk, last + Lk - Lq + 1)) : Lk;
+  const int first_h = kCausal ? min(Lk - 1, r0 + Lk - Lq) : Lk - 1;
+  const int n = (kmax + kTile - 1) / kTile;
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < kPfStages; ++i) {
+      mbar_init(&sm.full[i], 128);      // every producer thread, after its copies and its part of V^T
+      mbar_init(&sm.empty[i], 2);       // one thread per consumer warpgroup, after its P V of the tile
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp >= 8) {
+    // =============================== producer ===============================
+    const int pt = threadIdx.x - 256;
+    const int32_t* table = p.table + int64_t(b) * p.table_stride;
+    auto slot_of = [&](int key) { return int64_t(__ldg(table + key / p.page_size)) * p.page_size + key % p.page_size; };
+    auto load_tile = [&](int t) {
+      const int s = t % kPfStages;
+      constexpr int CPR = D / 16;       // 16-byte chunks per row; two threads per row
+      const int r = pt >> 1, key = t * kTile + r;
+      const bool ok = key < Lk;
+      const int64_t off = ((ok ? slot_of(key) : 0) * p.Hkv + hk) * D;
+#pragma unroll
+      for (int i = 0; i < CPR / 2; ++i) {
+        const int c = (pt & 1) * (CPR / 2) + i;
+        cp_async16(smem_u32(&sm.k8[s][r * D + pf_swz<D>(r, c) * 16]), p.k_pages + off + c * 16, ok);
+        cp_async16(smem_u32(&sm.v8[s][r * D + c * 16]), p.v_pages + off + c * 16, ok);
+      }
+      const int sk = t * kTile + (pt & (kTile - 1));
+      const bool sok = sk < Lk;
+      const int64_t si = (sok ? slot_of(sk) : 0) * p.Hkv + hk;
+      if (pt < kTile) cp_async4(smem_u32(&sm.ks[s][pt]), p.k_scale + si, sok);
+      else cp_async4(smem_u32(&sm.vs[s][pt - kTile]), p.v_scale + si, sok);
+    };
+    // V^T element (d, key) of a tile: 16-byte chunk key / 8 of row d, swizzled.  Item (key octet ko, column quad dg) reads 8 words
+    // of V8 and writes 4 chunks; the column order is rotated by dg to spread the stores over the banks.
+    auto convert = [&](int t) {
+      const int s = t % kPfStages;
+      constexpr int NQ = D / 4;
+#pragma unroll
+      for (int it = 0; it < (8 * NQ) / 128; ++it) {
+        const int w = it * 128 + pt, ko = w / NQ, dg = w % NQ;
+        uint32_t x[8];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) x[j] = *reinterpret_cast<const uint32_t*>(&sm.v8[s][(8 * ko + j) * D + 4 * dg]);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int e = (i + dg) & 3, d = 4 * dg + e, sh = 8 * e;
+          uint32_t y[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) y[j] = e4m3x2_to_bf16x2((x[2 * j] >> sh) & 0xffu, (x[2 * j + 1] >> sh) & 0xffu);
+          st_shared_v4(smem_u32(&sm.vt[s][d * kTile]) + ((ko ^ (d & 7)) * 16), y[0], y[1], y[2], y[3]);
+        }
+      }
+    };
+    for (int t = 0; t < n + kPfLag; ++t) {
+      if (t < n) {
+        mbar_wait(&sm.empty[t % kPfStages], ((t / kPfStages) & 1) ^ 1);
+        load_tile(t);
+      }
+      cp_async_commit();
+      const int c = t - kPfLag;
+      if (c >= 0) {
+        cp_async_wait<kPfLag>();          // this thread's copies of tile c have landed
+        named_bar_sync(2, 128);           // ... and every producer thread's
+        convert(c);
+        fence_proxy_async_smem();         // the cp.async and V^T writes, before the consumers' wgmma reads them
+        mbar_arrive(&sm.full[c % kPfStages]);
+      }
+    }
+    return;
+  }
+
+  // =============================== consumers ===============================
+  // ---- Q prologue: one warp per row, per (token, head) INT8 as the decode kernel's
+  {
+    constexpr int E = D / 32;
+    const T* q = reinterpret_cast<const T*>(p.q);
+    for (int r = warp; r < kPfRows; r += 8) {
+      uint32_t q8 = 0;
+      float qc = 0.f, qk = 0.f;
+      if (r0 + r < Lq) {
+        const int64_t tok = q0 + r0 + r;
+        float x[E];
+        load_row<T, E>(q + tok * p.q_st + int64_t(hq) * p.q_sh + lane * E, x);
+        const RowQuant rq(warp_amax<E>(x), 127.f);
+        q8 = pack_s8<E>(x, rq);
+        qc = __fmul_rn(rq.scale, p.scale_log2);
+        if (p.lse != nullptr) {
+#pragma unroll
+          for (int i = 0; i < E; ++i) qk += x[i] * p.k_smooth[hk * D + lane * E + i];
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) qk += __shfl_xor_sync(0xffffffffu, qk, o);
+        }
+      }
+      int8_t* dst = &sm.q8[r * D + pf_swz<D>(r, lane * E / 16) * 16 + (lane * E) % 16];
+      if constexpr (E == 4) *reinterpret_cast<uint32_t*>(dst) = q8;
+      else *reinterpret_cast<uint16_t*>(dst) = uint16_t(q8);
+      if (lane == 0) {
+        sm.qc[r] = qc;
+        sm.qk[r] = qk;
+      }
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(1, 256);
+  }
+
+  // wgmma accumulator layout (m64nN): warp w of the warpgroup owns rows 16w..16w+15; lane = 4 g + t4 holds rows 16w+g (registers
+  // 4i, 4i+1) and 16w+g+8 (4i+2, 4i+3) at columns 8i+2t4, 8i+2t4+1.  A row is spread over the 4 lanes of a quad.
+  const int wg = warp / 4, t4 = lane % 4;
+  const int row0 = wg * 64 + (warp % 4) * 16 + lane / 4;   // rows row0 and row0 + 8 of the CTA
+  float qcr[2];
+  int lim[2];                           // the last key each row sees (-1: a row past Lq)
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int i = r0 + row0 + 8 * r;
+    qcr[r] = sm.qc[row0 + 8 * r];
+    lim[r] = i >= Lq ? -1 : (kCausal ? min(Lk - 1, i + Lk - Lq) : Lk - 1);
+  }
+  constexpr int NO = D / 2;
+  float o[NO];
+#pragma unroll
+  for (int i = 0; i < NO; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};   // l: this thread's part of the row sum
+  uint32_t acc[32];
+  uint32_t a[4][4];                     // P of the tile, as the A operand of four k16 steps
+  const uint64_t dQ = make_wgmma_desc<D>(smem_u32(sm.q8 + wg * 64 * D));
+  const uint64_t dK0 = make_wgmma_desc<D>(smem_u32(sm.k8[0]));
+  const uint64_t dV0 = make_wgmma_desc<128>(smem_u32(sm.vt[0]));
+  auto issue_qk = [&](int t) {
+    const uint64_t dK = dK0 + uint64_t(t % kPfStages) * ((kTile * D) >> 4);
+#pragma unroll
+    for (int k = 0; k < D / 32; ++k) wgmma_qk_i8(acc, dQ + 2 * k, dK + 2 * k, k > 0);
+  };
+  auto issue_pv = [&](int t) {
+    const uint64_t dV = dV0 + uint64_t(t % kPfStages) * ((D * kTile * 2) >> 4);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_rs_bf16(o, a[kk], dV + 2 * kk, 1);
+  };
+
+  // Each step: S = Q K(t)^T, softmax, O += P V(t), each product waited for before the next (QK(t + 1) queued behind PV(t) makes
+  // ptxas serialise every wgmma of the loop).  The two consumer warpgroups overlap each other's softmax and products.  Slot t - 1
+  // is released once PV(t - 1) has completed.
+  for (int t = 0; t < n; ++t) {
+    const int s = t % kPfStages;
+    mbar_wait(&sm.full[s], (t / kPfStages) & 1);
+    wgmma_fence();
+    issue_qk(t);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(acc);
+    fence_regs(o);
+    if (t > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&sm.empty[(t - 1) % kPfStages]);
+    // ---- logits in log2 units, the exact running max, p = 2^(s - m), P = bf16(p * v_scale)
+    const bool masked = t * kTile + kTile - 1 > first_h;
+    float2 ksv[8], vsv[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      ksv[i] = *reinterpret_cast<const float2*>(&sm.ks[s][8 * i + 2 * t4]);
+      vsv[i] = *reinterpret_cast<const float2*>(&sm.vs[s][8 * i + 2 * t4]);
+    }
+    float e[32];
+    float alpha[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      float x[16];
+      float mx = -INFINITY;
+#pragma unroll
+      for (int c = 0; c < 16; ++c) {
+        const int idx = 4 * (c >> 1) + 2 * r + (c & 1);
+        const float kscale = (c & 1) ? ksv[c >> 1].y : ksv[c >> 1].x;
+        float v = __fmul_rn(__fmul_rn(float(int(acc[idx])), qcr[r]), kscale);
+        if (masked && t * kTile + 8 * (c >> 1) + 2 * t4 + (c & 1) > lim[r]) v = -INFINITY;
+        x[c] = v;
+        mx = fmaxf(mx, v);
+      }
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m[r], mx);
+      alpha[r] = m[r] == -INFINITY ? 0.f : ex2_approx(__fsub_rn(m[r], m_new));
+      m[r] = m_new;
+      float sum = 0.f;
+#pragma unroll
+      for (int c = 0; c < 16; ++c) {
+        const int idx = 4 * (c >> 1) + 2 * r + (c & 1);
+        const float pe = x[c] == -INFINITY ? 0.f : ex2_approx(__fsub_rn(x[c], m_new));
+        sum += pe;
+        e[idx] = __fmul_rn(pe, (c & 1) ? vsv[c >> 1].y : vsv[c >> 1].x);
+      }
+      l[r] = __fmaf_rn(alpha[r], l[r], sum);
+    }
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const __nv_bfloat162 pv = __floats2bfloat162_rn(e[8 * kk + 2 * j], e[8 * kk + 2 * j + 1]);
+        a[kk][j] = *reinterpret_cast<const uint32_t*>(&pv);
+      }
+#pragma unroll
+    for (int i = 0; i < NO; i += 4) {
+      o[i] *= alpha[0];
+      o[i + 1] *= alpha[0];
+      o[i + 2] *= alpha[1];
+      o[i + 3] *= alpha[1];
+    }
+    // ---- O += P V(t)
+    fence_regs(o);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) fence_regs(a[kk]);
+    wgmma_fence();
+    issue_pv(t);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(o);
+  }
+  if (n > 0) {
+    wgmma_wait<0>();
+    fence_regs(o);
+  }
+
+  // ---- epilogue: O / l in the output type; lse = (m + log2 l) / log2(e) + (q . k_smooth) * sm_scale
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    float L = l[r];
+    L += __shfl_xor_sync(0xffffffffu, L, 1);
+    L += __shfl_xor_sync(0xffffffffu, L, 2);
+    const int row = row0 + 8 * r, i = r0 + row;
+    if (i >= Lq) continue;
+    const bool seen = m[r] != -INFINITY;
+    T* orow = reinterpret_cast<T*>(p.out) + int64_t(q0 + i) * p.o_st + int64_t(hq) * p.o_sh;
+#pragma unroll
+    for (int nb = 0; nb < D / 8; ++nb) {
+      T pair[2];
+      pair[0] = from_f<T>(seen ? __fdiv_rn(o[4 * nb + 2 * r], L) : 0.f);
+      pair[1] = from_f<T>(seen ? __fdiv_rn(o[4 * nb + 2 * r + 1], L) : 0.f);
+      *reinterpret_cast<uint32_t*>(orow + 8 * nb + 2 * t4) = *reinterpret_cast<const uint32_t*>(pair);
+    }
+    if (p.lse != nullptr && t4 == 0)
+      p.lse[int64_t(hq) * p.Tq + q0 + i] = seen ? (m[r] + log2f(L)) / kLog2e + sm.qk[row] * p.sm_scale : -INFINITY;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ host
 int check_dtype_dim(int dtype, int D) {
   SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "Only half and bfloat16 are supported");
@@ -498,6 +800,29 @@ int launch_attn(const Kv8Params& p, const Kv8CombineParams& c, int nseq, bool ca
   kv8_combine_kernel<T, D><<<dim3(unsigned(nseq * c.max_seqlen_q), unsigned(c.Hq)), D, 0, st>>>(c);
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
+}
+
+template <typename T, int D, bool kCausal>
+int launch_prefill_t(const PfParams& p, int nseq, cudaStream_t st) {
+  auto kern = kv8_prefill_kernel<T, D, kCausal>;
+  const int bytes = int(sizeof(PfSmem<D>)) + 1024;   // + the alignment of the swizzled tiles
+  // once per device, so a launch inside CUDA-graph capture makes no attribute call
+  static std::atomic<uint64_t> configured{0};
+  int dev = 0;
+  SAB_CUDA_OK(cudaGetDevice(&dev));
+  const uint64_t bit = uint64_t(1) << (dev & 63);
+  if (!(configured.load() & bit)) {
+    SAB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    configured.fetch_or(bit);
+  }
+  kern<<<dim3(unsigned(int64_t(nseq) * p.n_qt), unsigned(p.Hq)), kPfThreads, bytes, st>>>(p);
+  SAB_CUDA_OK(cudaGetLastError());
+  return SAB_OK;
+}
+
+template <typename T, int D>
+int launch_prefill(const PfParams& p, int nseq, bool causal, cudaStream_t st) {
+  return causal ? launch_prefill_t<T, D, true>(p, nseq, st) : launch_prefill_t<T, D, false>(p, nseq, st);
 }
 
 }  // namespace
@@ -567,4 +892,35 @@ extern "C" int sab_kvcache8_attn(const void* q, int dtype, const int8_t* k_pages
   if (dtype == SAB_DTYPE_FP16)
     return D == 128 ? launch_attn<__half, 128>(p, c, nseq, causal, st) : launch_attn<__half, 64>(p, c, nseq, causal, st);
   return D == 128 ? launch_attn<__nv_bfloat16, 128>(p, c, nseq, causal, st) : launch_attn<__nv_bfloat16, 64>(p, c, nseq, causal, st);
+}
+
+extern "C" int sab_kvcache8_prefill(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
+                                    const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
+                                    const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq,
+                                    int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h,
+                                    int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale,
+                                    void* stream) {
+  SAB_REQUIRE(q && k_pages && k_scale && v_pages && v_scale && k_smooth && out && cu_seqlens_q && seqused_k && block_table,
+              SAB_ERR_INVALID, "null pointer argument");
+  if (int r = check_dtype_dim(dtype, D)) return r;
+  SAB_REQUIRE(Hkv > 0 && Hq > 0 && Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
+  SAB_REQUIRE(nseq > 0 && Tq > 0 && max_seqlen_q > 0 && max_pages > 0 && page_size > 0 && page_size % 16 == 0 && table_stride >= max_pages,
+              SAB_ERR_INVALID, "need nseq, Tq, max_seqlen_q, max_pages > 0, page_size a positive multiple of 16 and table_stride >= max_pages");
+  SAB_REQUIRE(q_stride_t >= 0 && q_stride_h >= 0 && (q_stride_t | q_stride_h) % 4 == 0 && reinterpret_cast<uintptr_t>(q) % 8 == 0,
+              SAB_ERR_INVALID, "q needs 8-byte aligned rows (non-negative strides, multiples of 4 elements)");
+  SAB_REQUIRE(o_stride_t >= 0 && o_stride_h >= 0 && (o_stride_t | o_stride_h) % 2 == 0 && reinterpret_cast<uintptr_t>(out) % 4 == 0,
+              SAB_ERR_INVALID, "out needs 4-byte aligned element pairs (non-negative, even strides)");
+  const int64_t n_qt = (int64_t(max_seqlen_q) + kPfRows - 1) / kPfRows;
+  // grid y is Hq, grid x is nseq * ceil(max_seqlen_q / 128); key indices are int
+  SAB_REQUIRE(Hq <= 65535 && n_qt * nseq < (int64_t(1) << 31), SAB_ERR_INVALID,
+              "launch grid too large: need Hq <= 65535 and nseq * ceil(max_seqlen_q / 128) < 2^31");
+  SAB_REQUIRE(int64_t(max_pages) * page_size < (int64_t(1) << 31), SAB_ERR_INVALID, "max_pages * page_size must be < 2^31 keys");
+  PfParams p{q, k_pages, k_scale, v_pages, v_scale, k_smooth, cu_seqlens_q, seqused_k, block_table, table_stride, out, lse,
+             max_pages, page_size, Hq, Hkv, int(n_qt), max_seqlen_q, Tq, q_stride_t, q_stride_h, o_stride_t, o_stride_h,
+             sm_scale, float(double(sm_scale) * 1.4426950408889634)};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool causal = is_causal != 0;
+  if (dtype == SAB_DTYPE_FP16)
+    return D == 128 ? launch_prefill<__half, 128>(p, nseq, causal, st) : launch_prefill<__half, 64>(p, nseq, causal, st);
+  return D == 128 ? launch_prefill<__nv_bfloat16, 128>(p, nseq, causal, st) : launch_prefill<__nv_bfloat16, 64>(p, nseq, causal, st);
 }

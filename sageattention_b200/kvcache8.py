@@ -4,7 +4,8 @@
 reads and quantises the whole cache again.  Here the statistics belong to the token: K and V get one fp32 scale per (token, head),
 and the K smoothing vector belongs to the cache.  A token written once is never touched again, and a decode step reads about 0.52x
 the bytes of a bf16 cache at D = 128 with no quantiser pass and no host synchronisation, so write + attention can be captured in
-a CUDA graph.
+a CUDA graph.  sageattn_kvcache8 serves decode-sized queries; sageattn_kvcache8_prefill serves query chunks of any length
+(chunked prefill, prefix caching) from the same cache.
 """
 import numbers
 from typing import Optional
@@ -111,29 +112,8 @@ class PagedKVCache8:
                            self.v_pages.view(torch.uint8), self.v_scale)
 
 
-def sageattn_kvcache8(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_q: torch.Tensor, seqused_k: torch.Tensor,
-                      block_table: torch.Tensor, max_seqlen_q: int, is_causal: bool = True, sm_scale: Optional[float] = None,
-                      return_lse: bool = False):
-    """Attention of packed queries against a PagedKVCache8, for decoding and speculative verification.
-
-    q: packed [Tq, Hq, D] in the cache's dtype with cu_seqlens_q (int32 or int64, nseq + 1 offsets) and max_seqlen_q, as in
-    sageattn_varlen_kvcache; Hq % Hkv == 0.  seqused_k: int32 [nseq], Lk_b.  block_table: int32 [nseq, max_pages]; key j of
-    sequence b is slot j % page_size of page block_table[b, j // page_size].  Table entries are trusted: each one read must lie in
-    [0, num_pages).  Pages may be shared between sequences.  Lk_b is read on the device only and clamped to max_pages * page_size;
-    the call never synchronises with the host, so cache.write + this call can be captured in a CUDA graph and replayed with
-    seqused_k and the slot mapping advanced in place.
-
-    Limits: max_seqlen_q * Hq / Hkv <= 64 (decode and speculative verification; one CTA holds every query row of a KV head), else
-    ValueError: use sageattn_varlen_kvcache for longer query chunks.  Rows of a sequence past max_seqlen_q, and rows past
-    cu_seqlens_q[-1], are not written.  Forward only.
-
-    Causal is bottom-right: query i of sequence b sees key j iff j <= i + Lk_b - Lq_b.  A row that sees no key returns 0 and lse
-    -inf.  Numerics: Q is quantised per (token, head) to INT8 as K is (without smoothing); logits in log2 units are
-    float(dot(q8, k8)) * (q_scale * sm_scale * log2e) * k_scale.  Keys are cut into fixed chunks of ops.kvcache8_chunk_keys() keys;
-    within a chunk an exact running max over 64-key tiles, p = 2^(s - m), P = bf16(p * v_scale) times the e4m3 V with fp32
-    accumulation; a second kernel merges a row's chunks in ascending order with no atomics.  A sequence's bits depend only on its
-    own q, keys and values, not on the rest of the batch or on the table width.  return_lse also returns the [Hq, Tq] fp32 LSE in
-    natural-log units of the logits q . k * sm_scale."""
+def _attn_args(q, cache, cu_seqlens_q, seqused_k, block_table, max_seqlen_q):
+    """The argument checks both cache calls share; returns (Hq, D, cu_seqlens_q as int32)."""
     if not isinstance(cache, PagedKVCache8):
         raise ValueError("cache must be a PagedKVCache8")
     dev = cache.device
@@ -159,15 +139,73 @@ def sageattn_kvcache8(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_q: torch
         raise ValueError(f"block_table must be an int32 [{nseq}, max_pages] tensor on q's device with contiguous rows")
     if isinstance(max_seqlen_q, bool) or not isinstance(max_seqlen_q, numbers.Integral) or max_seqlen_q < 1:
         raise ValueError(f"max_seqlen_q must be an int >= 1, got {max_seqlen_q!r}")
+    cu_q = cu_seqlens_q if cu_seqlens_q.dtype == torch.int32 else cu_seqlens_q.to(torch.int32)
+    return Hq, D, cu_q
+
+
+def sageattn_kvcache8(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_q: torch.Tensor, seqused_k: torch.Tensor,
+                      block_table: torch.Tensor, max_seqlen_q: int, is_causal: bool = True, sm_scale: Optional[float] = None,
+                      return_lse: bool = False):
+    """Attention of packed queries against a PagedKVCache8, for decoding and speculative verification.
+
+    q: packed [Tq, Hq, D] in the cache's dtype with cu_seqlens_q (int32 or int64, nseq + 1 offsets) and max_seqlen_q, as in
+    sageattn_varlen_kvcache; Hq % Hkv == 0.  seqused_k: int32 [nseq], Lk_b.  block_table: int32 [nseq, max_pages]; key j of
+    sequence b is slot j % page_size of page block_table[b, j // page_size].  Table entries are trusted: each one read must lie in
+    [0, num_pages).  Pages may be shared between sequences.  Lk_b is read on the device only and clamped to max_pages * page_size;
+    the call never synchronises with the host, so cache.write + this call can be captured in a CUDA graph and replayed with
+    seqused_k and the slot mapping advanced in place.
+
+    Limits: max_seqlen_q * Hq / Hkv <= 64 (decode and speculative verification; one CTA holds every query row of a KV head), else
+    ValueError: use sageattn_kvcache8_prefill for longer query chunks.  Rows of a sequence past max_seqlen_q, and rows past
+    cu_seqlens_q[-1], are not written.  Forward only.
+
+    Causal is bottom-right: query i of sequence b sees key j iff j <= i + Lk_b - Lq_b.  A row that sees no key returns 0 and lse
+    -inf.  Numerics: Q is quantised per (token, head) to INT8 as K is (without smoothing); logits in log2 units are
+    float(dot(q8, k8)) * (q_scale * sm_scale * log2e) * k_scale.  Keys are cut into fixed chunks of ops.kvcache8_chunk_keys() keys;
+    within a chunk an exact running max over 64-key tiles, p = 2^(s - m), P = bf16(p * v_scale) times the e4m3 V with fp32
+    accumulation; a second kernel merges a row's chunks in ascending order with no atomics.  A sequence's bits depend only on its
+    own q, keys and values, not on the rest of the batch or on the table width.  return_lse also returns the [Hq, Tq] fp32 LSE in
+    natural-log units of the logits q . k * sm_scale."""
+    Hq, D, cu_q = _attn_args(q, cache, cu_seqlens_q, seqused_k, block_table, max_seqlen_q)
+    Hkv = cache.num_kv_heads
     if max_seqlen_q * (Hq // Hkv) > _ROW_LIMIT:
         raise ValueError(f"max_seqlen_q * Hq / Hkv = {max_seqlen_q * (Hq // Hkv)} exceeds the {_ROW_LIMIT} query rows the split-KV "
-                         "kernel holds per KV head; use sageattn_varlen_kvcache for longer query chunks")
+                         "kernel holds per KV head; use sageattn_kvcache8_prefill for longer query chunks on this cache (or "
+                         "sageattn_varlen_kvcache on a 16-bit cache)")
     if sm_scale is None:
         sm_scale = D ** -0.5
-    cu_q = cu_seqlens_q if cu_seqlens_q.dtype == torch.int32 else cu_seqlens_q.to(torch.int32)
     with torch.no_grad():
-        o = torch.empty(q.shape, dtype=q.dtype, device=dev)
+        o = torch.empty(q.shape, dtype=q.dtype, device=cache.device)
         lse = ops.kvcache8_attn(q, cache.k_pages, cache.k_scale, cache.v_pages.view(torch.uint8), cache.v_scale, cache.k_smooth, o,
                                 cu_q.contiguous(), seqused_k.contiguous(), block_table, int(max_seqlen_q), 1 if is_causal else 0,
                                 float(sm_scale), 1 if return_lse else 0)
+    return (o, lse) if return_lse else o
+
+
+def sageattn_kvcache8_prefill(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_q: torch.Tensor, seqused_k: torch.Tensor,
+                              block_table: torch.Tensor, max_seqlen_q: int, is_causal: bool = True, sm_scale: Optional[float] = None,
+                              return_lse: bool = False):
+    """Attention of packed query chunks of any length against a PagedKVCache8: chunked prefill, prefix caching and long
+    speculative verification on the 8-bit cache alone.
+
+    Arguments, checks and the causal rule are those of sageattn_kvcache8, without its row limit: q packed [Tq, Hq, D] in the cache's
+    dtype, cu_seqlens_q int32 or int64, seqused_k int32 [nseq] (read on the device only), block_table int32 [nseq, max_pages] with
+    contiguous rows and trusted entries.  The call never synchronises with the host and allocates nothing but o (and lse), so
+    cache.write + this call can be captured in a CUDA graph.  Causal is bottom-right: query i of sequence b sees key j iff
+    j <= i + Lk_b - Lq_b; a row that sees no key returns 0 and lse -inf.  Rows of a sequence past max_seqlen_q, and rows past
+    cu_seqlens_q[-1], are not written.  Forward only.
+
+    Numerics: those of sageattn_kvcache8 without chunks.  Q is quantised per (token, head) to INT8; logits in log2 units are
+    float(dot(q8, k8)) * (q_scale * sm_scale * log2e) * k_scale; one exact running max per row over 64-key tiles from key 0,
+    p = 2^(s - m), P = bf16(p * v_scale) times the e4m3 V with fp32 accumulation, O / l.  A row's bits depend only on its own
+    q, keys and values: not on the batch, the table width, or the size of the chunk it was prefilled in.  return_lse also returns
+    the [Hq, Tq] fp32 LSE in natural-log units of the logits q . k * sm_scale."""
+    Hq, D, cu_q = _attn_args(q, cache, cu_seqlens_q, seqused_k, block_table, max_seqlen_q)
+    if sm_scale is None:
+        sm_scale = D ** -0.5
+    with torch.no_grad():
+        o = torch.empty(q.shape, dtype=q.dtype, device=cache.device)
+        lse = ops.kvcache8_prefill(q, cache.k_pages, cache.k_scale, cache.v_pages.view(torch.uint8), cache.v_scale, cache.k_smooth,
+                                   o, cu_q.contiguous(), seqused_k.contiguous(), block_table, int(max_seqlen_q),
+                                   1 if is_causal else 0, float(sm_scale), 1 if return_lse else 0)
     return (o, lse) if return_lse else o

@@ -646,6 +646,26 @@ int sab_kvcache8_prefill(const void* q, int dtype, const int8_t* k_pages, const 
                          const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq, int Tq,
                          int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h, int64_t o_stride_t,
                          int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale, void* stream);
+/* sab_kvcache8_attn_window / sab_kvcache8_prefill_window: sab_kvcache8_attn / sab_kvcache8_prefill with a sliding window, the same
+ *   arguments plus window_left / window_right (>= -1, else SAB_ERR_INVALID before any launch; -1 leaves a side unbounded) and the
+ *   same workspace size.  With off_b = Lk_b - Lq_b, query i sees key j iff i + off_b - window_left <= j <= i + off_b +
+ *   window_right, and j <= i + off_b as well when is_causal.  Table entries read: only keys j >= max(0, Lk_b - Lq_b -
+ *   window_left) are ever loaded; the table entries, K / V bytes and scales of keys below that bound are never read, so those
+ *   entries may name any page in [0, num_pages) (a shared null page, or pages reused for newer tokens).  Numerics and the bits
+ *   of a row are those of the call without a window on the visible keys: tiles left of the window are skipped, and a tile in
+ *   which a row sees nothing leaves it unchanged.  A row that sees no key returns 0 and lse -inf. */
+int sab_kvcache8_attn_window(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
+                             const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
+                             const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq,
+                             int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h,
+                             int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale,
+                             void* workspace, int window_left, int window_right, void* stream);
+int sab_kvcache8_prefill_window(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
+                                const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
+                                const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq,
+                                int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h,
+                                int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale,
+                                int window_left, int window_right, void* stream);
 
 #ifdef __cplusplus
 }

@@ -161,6 +161,7 @@ struct Kv8Params {
   float scale_log2;     // sm_scale * log2(e)
   float* o_part;        // [Tq, Hq, max_chunks, D]
   float2* ml_part;      // [Tq, Hq, max_chunks]: (running max in log2 units, sum of p)
+  int window_left, window_right;   // kWindow: query i sees keys [i + off - left, i + off + right], off = Lk - Lq (-1: unbounded)
 };
 
 template <int D>
@@ -176,8 +177,12 @@ struct Kv8Smem {
   float red_max[4][kRows], red_sum[4][kRows];            // per-warp partial row max / sum of the tile
 };
 
-template <typename T, int D, bool kCausal>
-__global__ void __launch_bounds__(kThreads) kv8_attn_kernel(const Kv8Params p) {
+// kWindow: the sliding-window form.  The causal rule arrives folded into window_right (0), so kCausal is false.  Tiles left of the
+// CTA's first visible key are skipped (a tile in which a row sees nothing is an exact identity on its m, l and O), and keys left of
+// it are zero-filled without reading their table entry.  Three CTAs per SM (168 registers, no spill) as the D = 128 forms; the
+// D = 64 forms' 128 registers would spill here.  The minimum of 0 leaves the other forms as they were.
+template <typename T, int D, bool kCausal, bool kWindow = false>
+__global__ void __launch_bounds__(kThreads, kWindow ? 3 : 0) kv8_attn_kernel(const Kv8Params p) {
   using S = Kv8Smem<D>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   S& sm = *reinterpret_cast<S*>(smem_raw);
@@ -194,29 +199,48 @@ __global__ void __launch_bounds__(kThreads) kv8_attn_kernel(const Kv8Params p) {
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32, g8 = lane / 4, c4 = lane % 4;
   const int32_t* table = p.table + int64_t(b) * p.table_stride;
   const int64_t hD = int64_t(h) * D;
+  // keys [klo, kend) hold every key a row of the CTA sees: klo is row 0's first key (the lower bounds rise with the row).  The
+  // last row's upper bound, Lk - 1 + max(right, 0), never falls below kend - 1, so the range ends at kend.  The tiles visited
+  // start at kb, the 64-key tile (of the grid from key 0) holding klo.
+  int klo = kbeg, kb = kbeg;
+  if constexpr (kWindow) {
+    if (p.window_left >= 0) klo = int(max(int64_t(kbeg), int64_t(Lk) - Lq - p.window_left));
+    if (klo >= kend) {
+      // nothing to read: the empty partials (m = -inf, l = 0, O = 0) the combine folds with weight 0
+      for (int e = threadIdx.x; e < R * D; e += kThreads) {
+        const int r = e / D;
+        p.o_part[((int64_t(q0 + r / G) * p.Hq + h * G + r % G) * p.max_chunks + chunk) * D + e % D] = 0.f;
+      }
+      for (int r = threadIdx.x; r < R; r += kThreads)
+        p.ml_part[(int64_t(q0 + r / G) * p.Hq + h * G + r % G) * p.max_chunks + chunk] = make_float2(-INFINITY, 0.f);
+      return;
+    }
+    kb = klo - (klo - kbeg) % kTile;
+  }
 
-  // ---- tile loader: keys kbeg + 64 t .. of this KV head, zero-filled past kend
-  auto load_tile = [&](int t, int buf) {
+  // ---- tile loader: keys kb + 64 t .. of this KV head, zero-filled outside [klo, kend); only the first tile (first) holds keys
+  // below klo
+  auto load_tile = [&](int t, int buf, bool first) {
     constexpr int CPR = D / 16;   // 16-byte chunks per row
     for (int i = threadIdx.x; i < kTile * CPR; i += kThreads) {
       const int r = i / CPR, cc = i % CPR;
-      const int key = kbeg + t * kTile + r;
-      const bool ok = key < kend;
+      const int key = kb + t * kTile + r;
+      const bool ok = key < kend && (!kWindow || !first || key >= klo);
       const int64_t slot = ok ? int64_t(__ldg(table + key / p.page_size)) * p.page_size + key % p.page_size : 0;
       const int64_t off = (slot * p.Hkv) * D + hD + cc * 16;
       cp_async16(smem_u32(&sm.k8[buf][r * S::kRowB + cc * 16]), p.k_pages + off, ok);
       cp_async16(smem_u32(&sm.v8[buf][r * S::kRowB + cc * 16]), p.v_pages + off, ok);
     }
     if (threadIdx.x < kTile) {
-      const int key = kbeg + t * kTile + threadIdx.x;
-      const bool ok = key < kend;
+      const int key = kb + t * kTile + threadIdx.x;
+      const bool ok = key < kend && (!kWindow || !first || key >= klo);
       const int64_t slot = ok ? int64_t(__ldg(table + key / p.page_size)) * p.page_size + key % p.page_size : 0;
       cp_async4(smem_u32(&sm.ks[buf][threadIdx.x]), p.k_scale + slot * p.Hkv + h, ok);
       cp_async4(smem_u32(&sm.vs[buf][threadIdx.x]), p.v_scale + slot * p.Hkv + h, ok);
     }
   };
-  const int ntiles = (kend - kbeg + kTile - 1) / kTile;
-  load_tile(0, 0);
+  const int ntiles = (kend - kb + kTile - 1) / kTile;
+  load_tile(0, 0, true);
   cp_async_commit();
 
   // ---- Q prologue: per (token, head) INT8, one warp per row
@@ -253,14 +277,21 @@ __global__ void __launch_bounds__(kThreads) kv8_attn_kernel(const Kv8Params p) {
 #pragma unroll
       for (int e = 0; e < 4; ++e) o[mt][nt][e] = 0.f;
   }
-  // the last key row r may see: causal is bottom-right inside the sequence
+  // the last key row r may see: causal is bottom-right inside the sequence.  kWindow, in one register per row as lim: row r sees
+  // key < kend iff unsigned(key - lo) <= span, with lo = i + off - left and span = left + right.  A side past what the sequence
+  // can reach (left > Lk, right > Lq: rows are i < Lq <= 64) sees as much as -1 and is clamped to it, so the key - lo of every
+  // key < kend lies in (-2^31, 2^32) and the unsigned test is exact.  Rows r >= R take lo = kend and see nothing.
   int lim[4][2];
+  const int wl = p.window_left < 0 || p.window_left > Lk ? Lk : p.window_left;
+  const int wr = p.window_right < 0 || p.window_right > Lq ? Lq : p.window_right;
+  const unsigned span = unsigned(wl) + unsigned(wr);
 #pragma unroll
   for (int mt = 0; mt < 4; ++mt)
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       const int r = mt * 16 + g8 + 8 * j;
-      lim[mt][j] = r >= R ? -1 : (kCausal ? min(kend - 1, r / G + Lk - Lq) : kend - 1);
+      if constexpr (kWindow) lim[mt][j] = r >= R ? kend : r / G + Lk - Lq - wl;
+      else lim[mt][j] = r >= R ? -1 : (kCausal ? min(kend - 1, r / G + Lk - Lq) : kend - 1);
     }
 
   for (int t = 0; t < ntiles; ++t) {
@@ -269,11 +300,11 @@ __global__ void __launch_bounds__(kThreads) kv8_attn_kernel(const Kv8Params p) {
     // tile t - 1, the last reader of buffer buf ^ 1, so only now may the loads of tile t + 1 overwrite that buffer.
     cp_async_wait<0>();
     __syncthreads();
-    if (t + 1 < ntiles) load_tile(t + 1, buf ^ 1);
+    if (t + 1 < ntiles) load_tile(t + 1, buf ^ 1, false);
     cp_async_commit();
 
     // ---- S = Q K^T for this warp's 16 keys, in log2 units
-    const int key0 = kbeg + t * kTile + warp * 16;
+    const int key0 = kb + t * kTile + warp * 16;
     float s[4][2][4];
     {
       int acc[4][2][4];
@@ -309,7 +340,8 @@ __global__ void __launch_bounds__(kThreads) kv8_attn_kernel(const Kv8Params p) {
             for (int e = 0; e < 2; ++e) {
               const int kl = warp * 16 + nt * 8 + 2 * c4 + e;
               float x = __fmul_rn(__fmul_rn(float(acc[mt][nt][2 * j + e]), qc), sm.ks[buf][kl]);
-              if (key0 + nt * 8 + 2 * c4 + e > lim[mt][j]) x = -INFINITY;
+              const int key = key0 + nt * 8 + 2 * c4 + e;
+              if (kWindow ? key >= kend || unsigned(key - lim[mt][j]) > span : key > lim[mt][j]) x = -INFINITY;
               s[mt][nt][2 * j + e] = x;
               rmax[j] = fmaxf(rmax[j], x);
             }
@@ -498,9 +530,12 @@ struct PfParams {
   int max_pages, page_size, Hq, Hkv, n_qt, max_seqlen_q, Tq;
   int64_t q_st, q_sh, o_st, o_sh;
   float sm_scale, scale_log2;   // scale_log2 = sm_scale * log2(e)
+  int window_left, window_right;   // kWindow: as Kv8Params
 };
 
-template <typename T, int D, bool kCausal>
+// kWindow: the sliding-window form, the causal rule folded into window_right (0) as in kv8_attn_kernel.  The CTA visits the tiles
+// from the one holding its first row's first key; loop index t counts visited tiles, tile tf + t of the grid from key 0.
+template <typename T, int D, bool kCausal, bool kWindow = false>
 __global__ void __launch_bounds__(kPfThreads, 1) kv8_prefill_kernel(const PfParams p) {
   using S = PfSmem<D>;
   extern __shared__ __align__(1024) unsigned char pf_smem[];
@@ -512,11 +547,25 @@ __global__ void __launch_bounds__(kPfThreads, 1) kv8_prefill_kernel(const PfPara
   const int Lk = max(0, min(p.seqused_k[b], p.max_pages * p.page_size));
   const int r0 = qt * kPfRows;          // the CTA's first row inside the sequence
   if (r0 >= Lq) return;
-  // keys [0, kmax) hold every key a row of the CTA sees; tiles past `first_h` (the first row's last key) take the masked path
+  // keys [klo, kmax) hold every key a row of the CTA sees; tiles past `first_h` (the first row's last key), and kWindow: tiles
+  // starting before `lo_last` (the last row's first key), take the masked path
   const int last = min(r0 + kPfRows, Lq) - 1;
-  const int kmax = kCausal ? max(0, min(Lk, last + Lk - Lq + 1)) : Lk;
-  const int first_h = kCausal ? min(Lk - 1, r0 + Lk - Lq) : Lk - 1;
-  const int n = (kmax + kTile - 1) / kTile;
+  int kmax = kCausal ? max(0, min(Lk, last + Lk - Lq + 1)) : Lk;
+  int first_h = kCausal ? min(Lk - 1, r0 + Lk - Lq) : Lk - 1;
+  int klo = 0, lo_last = 0, tf = 0;
+  if constexpr (kWindow) {
+    const int64_t off = int64_t(Lk) - Lq;
+    if (p.window_right >= 0) {
+      kmax = int(max(int64_t(0), min(int64_t(Lk), last + off + p.window_right + 1)));
+      first_h = int(min(int64_t(Lk - 1), r0 + off + p.window_right));
+    }
+    if (p.window_left >= 0) {
+      klo = int(max(int64_t(0), min(int64_t(Lk), r0 + off - p.window_left)));
+      lo_last = int(max(int64_t(0), min(int64_t(Lk), last + off - p.window_left)));
+    }
+    tf = klo / kTile;
+  }
+  const int n = kWindow ? max(0, (kmax + kTile - 1) / kTile - tf) : (kmax + kTile - 1) / kTile;
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
 
   if (threadIdx.x == 0) {
@@ -536,8 +585,8 @@ __global__ void __launch_bounds__(kPfThreads, 1) kv8_prefill_kernel(const PfPara
     auto load_tile = [&](int t) {
       const int s = t % kPfStages;
       constexpr int CPR = D / 16;       // 16-byte chunks per row; two threads per row
-      const int r = pt >> 1, key = t * kTile + r;
-      const bool ok = key < Lk;
+      const int r = pt >> 1, key = (tf + t) * kTile + r;
+      const bool ok = kWindow ? key >= klo && key < kmax : key < Lk;
       const int64_t off = ((ok ? slot_of(key) : 0) * p.Hkv + hk) * D;
 #pragma unroll
       for (int i = 0; i < CPR / 2; ++i) {
@@ -545,8 +594,8 @@ __global__ void __launch_bounds__(kPfThreads, 1) kv8_prefill_kernel(const PfPara
         cp_async16(smem_u32(&sm.k8[s][r * D + pf_swz<D>(r, c) * 16]), p.k_pages + off + c * 16, ok);
         cp_async16(smem_u32(&sm.v8[s][r * D + c * 16]), p.v_pages + off + c * 16, ok);
       }
-      const int sk = t * kTile + (pt & (kTile - 1));
-      const bool sok = sk < Lk;
+      const int sk = (tf + t) * kTile + (pt & (kTile - 1));
+      const bool sok = kWindow ? sk >= klo && sk < kmax : sk < Lk;
       const int64_t si = (sok ? slot_of(sk) : 0) * p.Hkv + hk;
       if (pt < kTile) cp_async4(smem_u32(&sm.ks[s][pt]), p.k_scale + si, sok);
       else cp_async4(smem_u32(&sm.vs[s][pt - kTile]), p.v_scale + si, sok);
@@ -629,12 +678,17 @@ __global__ void __launch_bounds__(kPfThreads, 1) kv8_prefill_kernel(const PfPara
   const int wg = warp / 4, t4 = lane % 4;
   const int row0 = wg * 64 + (warp % 4) * 16 + lane / 4;   // rows row0 and row0 + 8 of the CTA
   float qcr[2];
-  int lim[2];                           // the last key each row sees (-1: a row past Lq)
+  int lim[2], lo[2];                    // the last key each row sees (-1: a row past Lq); kWindow: the first
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int i = r0 + row0 + 8 * r;
     qcr[r] = sm.qc[row0 + 8 * r];
     lim[r] = i >= Lq ? -1 : (kCausal ? min(Lk - 1, i + Lk - Lq) : Lk - 1);
+    if constexpr (kWindow) {
+      const int64_t diag = int64_t(i) + Lk - Lq;
+      if (i < Lq && p.window_right >= 0) lim[r] = int(max(int64_t(-1), min(int64_t(Lk - 1), diag + p.window_right)));
+      lo[r] = p.window_left < 0 ? 0 : int(max(int64_t(0), min(int64_t(Lk), diag - p.window_left)));
+    }
   }
   constexpr int NO = D / 2;
   float o[NO];
@@ -671,7 +725,8 @@ __global__ void __launch_bounds__(kPfThreads, 1) kv8_prefill_kernel(const PfPara
     fence_regs(o);
     if (t > 0 && (threadIdx.x & 127) == 0) mbar_arrive(&sm.empty[(t - 1) % kPfStages]);
     // ---- logits in log2 units, the exact running max, p = 2^(s - m), P = bf16(p * v_scale)
-    const bool masked = t * kTile + kTile - 1 > first_h;
+    const int kt = (tf + t) * kTile;    // the tile's first key
+    const bool masked = kt + kTile - 1 > first_h || (kWindow && kt < lo_last);
     float2 ksv[8], vsv[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -689,7 +744,8 @@ __global__ void __launch_bounds__(kPfThreads, 1) kv8_prefill_kernel(const PfPara
         const int idx = 4 * (c >> 1) + 2 * r + (c & 1);
         const float kscale = (c & 1) ? ksv[c >> 1].y : ksv[c >> 1].x;
         float v = __fmul_rn(__fmul_rn(float(int(acc[idx])), qcr[r]), kscale);
-        if (masked && t * kTile + 8 * (c >> 1) + 2 * t4 + (c & 1) > lim[r]) v = -INFINITY;
+        const int key = kt + 8 * (c >> 1) + 2 * t4 + (c & 1);
+        if (masked && (key > lim[r] || (kWindow && key < lo[r]))) v = -INFINITY;
         x[c] = v;
         mx = fmaxf(mx, v);
       }
@@ -776,9 +832,9 @@ int launch_write(const void* k, const void* v, const float* k_smooth, const int6
   return SAB_OK;
 }
 
-template <typename T, int D, bool kCausal>
+template <typename T, int D, bool kCausal, bool kWindow = false>
 int launch_attn_t(const Kv8Params& p, int nseq, cudaStream_t st) {
-  auto kern = kv8_attn_kernel<T, D, kCausal>;
+  auto kern = kv8_attn_kernel<T, D, kCausal, kWindow>;
   const int bytes = int(sizeof(Kv8Smem<D>));
   // once per device, so a launch inside CUDA-graph capture makes no attribute call
   static std::atomic<uint64_t> configured{0};
@@ -794,17 +850,20 @@ int launch_attn_t(const Kv8Params& p, int nseq, cudaStream_t st) {
   return SAB_OK;
 }
 
+// window: the kWindow kernel, with the causal rule already folded into p.window_right
 template <typename T, int D>
-int launch_attn(const Kv8Params& p, const Kv8CombineParams& c, int nseq, bool causal, cudaStream_t st) {
-  if (int r = causal ? launch_attn_t<T, D, true>(p, nseq, st) : launch_attn_t<T, D, false>(p, nseq, st)) return r;
+int launch_attn(const Kv8Params& p, const Kv8CombineParams& c, int nseq, bool causal, bool window, cudaStream_t st) {
+  if (int r = window ? launch_attn_t<T, D, false, true>(p, nseq, st)
+                     : causal ? launch_attn_t<T, D, true>(p, nseq, st) : launch_attn_t<T, D, false>(p, nseq, st))
+    return r;
   kv8_combine_kernel<T, D><<<dim3(unsigned(nseq * c.max_seqlen_q), unsigned(c.Hq)), D, 0, st>>>(c);
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
 }
 
-template <typename T, int D, bool kCausal>
+template <typename T, int D, bool kCausal, bool kWindow = false>
 int launch_prefill_t(const PfParams& p, int nseq, cudaStream_t st) {
-  auto kern = kv8_prefill_kernel<T, D, kCausal>;
+  auto kern = kv8_prefill_kernel<T, D, kCausal, kWindow>;
   const int bytes = int(sizeof(PfSmem<D>)) + 1024;   // + the alignment of the swizzled tiles
   // once per device, so a launch inside CUDA-graph capture makes no attribute call
   static std::atomic<uint64_t> configured{0};
@@ -821,8 +880,16 @@ int launch_prefill_t(const PfParams& p, int nseq, cudaStream_t st) {
 }
 
 template <typename T, int D>
-int launch_prefill(const PfParams& p, int nseq, bool causal, cudaStream_t st) {
+int launch_prefill(const PfParams& p, int nseq, bool causal, bool window, cudaStream_t st) {
+  if (window) return launch_prefill_t<T, D, false, true>(p, nseq, st);
   return causal ? launch_prefill_t<T, D, true>(p, nseq, st) : launch_prefill_t<T, D, false>(p, nseq, st);
+}
+
+// The window rule the kernels take: < -1 is refused; causal makes the right side 0 (j <= i + off whatever right is).
+int window_args(int window_left, int window_right, int is_causal, int& right) {
+  SAB_REQUIRE(window_left >= -1 && window_right >= -1, SAB_ERR_INVALID, "window_left and window_right must be >= -1 (-1: unbounded)");
+  right = is_causal ? 0 : window_right;
+  return SAB_OK;
 }
 
 }  // namespace
@@ -859,12 +926,13 @@ extern "C" int sab_kvcache8_write(const void* k, const void* v, int dtype, const
                   : launch_write<__nv_bfloat16, 64>(k, v, k_smooth, slot_mapping, T, Hkv, k_stride_t, k_stride_h, v_stride_t, v_stride_h, k_pages, k_scale, v_pages, v_scale, ns, st);
 }
 
-extern "C" int sab_kvcache8_attn(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
-                                 const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
-                                 const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq,
-                                 int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h,
-                                 int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale,
-                                 void* workspace, void* stream) {
+// sab_kvcache8_attn and, with window, sab_kvcache8_attn_window (window_right with the causal rule folded in)
+static int kvcache8_attn(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
+                         const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
+                         const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq,
+                         int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h,
+                         int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale,
+                         void* workspace, bool window, int window_left, int window_right, void* stream) {
   SAB_REQUIRE(q && k_pages && k_scale && v_pages && v_scale && k_smooth && out && cu_seqlens_q && seqused_k && block_table && workspace,
               SAB_ERR_INVALID, "null pointer argument");
   if (int r = check_dtype_dim(dtype, D)) return r;
@@ -883,23 +951,49 @@ extern "C" int sab_kvcache8_attn(const void* q, int dtype, const int8_t* k_pages
   SAB_REQUIRE(max_keys < (int64_t(1) << 31), SAB_ERR_INVALID, "max_pages * page_size must be < 2^31 keys");
   Kv8Params p{q, k_pages, k_scale, v_pages, v_scale, cu_seqlens_q, seqused_k, block_table, table_stride, max_pages, page_size, Hq, Hkv,
               int(chunks), max_seqlen_q, q_stride_t, q_stride_h, float(double(sm_scale) * 1.4426950408889634),
-              static_cast<float*>(workspace), nullptr};
+              static_cast<float*>(workspace), nullptr, window_left, window_right};
   p.ml_part = reinterpret_cast<float2*>(p.o_part + int64_t(Tq) * Hq * chunks * D);
   Kv8CombineParams c{q, k_smooth, cu_seqlens_q, seqused_k, p.o_part, p.ml_part, out, lse, Tq, Hq, Hkv, int(chunks), max_seqlen_q,
                      int(max_keys), q_stride_t, q_stride_h, o_stride_t, o_stride_h, sm_scale};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool causal = is_causal != 0;
   if (dtype == SAB_DTYPE_FP16)
-    return D == 128 ? launch_attn<__half, 128>(p, c, nseq, causal, st) : launch_attn<__half, 64>(p, c, nseq, causal, st);
-  return D == 128 ? launch_attn<__nv_bfloat16, 128>(p, c, nseq, causal, st) : launch_attn<__nv_bfloat16, 64>(p, c, nseq, causal, st);
+    return D == 128 ? launch_attn<__half, 128>(p, c, nseq, causal, window, st) : launch_attn<__half, 64>(p, c, nseq, causal, window, st);
+  return D == 128 ? launch_attn<__nv_bfloat16, 128>(p, c, nseq, causal, window, st)
+                  : launch_attn<__nv_bfloat16, 64>(p, c, nseq, causal, window, st);
 }
 
-extern "C" int sab_kvcache8_prefill(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
-                                    const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
-                                    const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq,
-                                    int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h,
-                                    int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale,
-                                    void* stream) {
+extern "C" int sab_kvcache8_attn(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
+                                 const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
+                                 const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq,
+                                 int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h,
+                                 int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale,
+                                 void* workspace, void* stream) {
+  return kvcache8_attn(q, dtype, k_pages, k_scale, v_pages, v_scale, k_smooth, out, lse, cu_seqlens_q, seqused_k, block_table,
+                       table_stride, max_pages, nseq, Tq, Hq, Hkv, D, page_size, q_stride_t, q_stride_h, o_stride_t, o_stride_h,
+                       max_seqlen_q, is_causal, sm_scale, workspace, false, -1, -1, stream);
+}
+
+extern "C" int sab_kvcache8_attn_window(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
+                                        const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
+                                        const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages,
+                                        int nseq, int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t,
+                                        int64_t q_stride_h, int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal,
+                                        float sm_scale, void* workspace, int window_left, int window_right, void* stream) {
+  int right = -1;
+  if (int r = window_args(window_left, window_right, is_causal, right)) return r;
+  return kvcache8_attn(q, dtype, k_pages, k_scale, v_pages, v_scale, k_smooth, out, lse, cu_seqlens_q, seqused_k, block_table,
+                       table_stride, max_pages, nseq, Tq, Hq, Hkv, D, page_size, q_stride_t, q_stride_h, o_stride_t, o_stride_h,
+                       max_seqlen_q, is_causal, sm_scale, workspace, true, window_left, right, stream);
+}
+
+// sab_kvcache8_prefill and, with window, sab_kvcache8_prefill_window (window_right with the causal rule folded in)
+static int kvcache8_prefill(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
+                            const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
+                            const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq,
+                            int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h,
+                            int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale,
+                            bool window, int window_left, int window_right, void* stream) {
   SAB_REQUIRE(q && k_pages && k_scale && v_pages && v_scale && k_smooth && out && cu_seqlens_q && seqused_k && block_table,
               SAB_ERR_INVALID, "null pointer argument");
   if (int r = check_dtype_dim(dtype, D)) return r;
@@ -917,10 +1011,36 @@ extern "C" int sab_kvcache8_prefill(const void* q, int dtype, const int8_t* k_pa
   SAB_REQUIRE(int64_t(max_pages) * page_size < (int64_t(1) << 31), SAB_ERR_INVALID, "max_pages * page_size must be < 2^31 keys");
   PfParams p{q, k_pages, k_scale, v_pages, v_scale, k_smooth, cu_seqlens_q, seqused_k, block_table, table_stride, out, lse,
              max_pages, page_size, Hq, Hkv, int(n_qt), max_seqlen_q, Tq, q_stride_t, q_stride_h, o_stride_t, o_stride_h,
-             sm_scale, float(double(sm_scale) * 1.4426950408889634)};
+             sm_scale, float(double(sm_scale) * 1.4426950408889634), window_left, window_right};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool causal = is_causal != 0;
   if (dtype == SAB_DTYPE_FP16)
-    return D == 128 ? launch_prefill<__half, 128>(p, nseq, causal, st) : launch_prefill<__half, 64>(p, nseq, causal, st);
-  return D == 128 ? launch_prefill<__nv_bfloat16, 128>(p, nseq, causal, st) : launch_prefill<__nv_bfloat16, 64>(p, nseq, causal, st);
+    return D == 128 ? launch_prefill<__half, 128>(p, nseq, causal, window, st) : launch_prefill<__half, 64>(p, nseq, causal, window, st);
+  return D == 128 ? launch_prefill<__nv_bfloat16, 128>(p, nseq, causal, window, st)
+                  : launch_prefill<__nv_bfloat16, 64>(p, nseq, causal, window, st);
+}
+
+extern "C" int sab_kvcache8_prefill(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
+                                    const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
+                                    const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq,
+                                    int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h,
+                                    int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale,
+                                    void* stream) {
+  return kvcache8_prefill(q, dtype, k_pages, k_scale, v_pages, v_scale, k_smooth, out, lse, cu_seqlens_q, seqused_k, block_table,
+                          table_stride, max_pages, nseq, Tq, Hq, Hkv, D, page_size, q_stride_t, q_stride_h, o_stride_t, o_stride_h,
+                          max_seqlen_q, is_causal, sm_scale, false, -1, -1, stream);
+}
+
+extern "C" int sab_kvcache8_prefill_window(const void* q, int dtype, const int8_t* k_pages, const float* k_scale,
+                                           const uint8_t* v_pages, const float* v_scale, const float* k_smooth, void* out, float* lse,
+                                           const int32_t* cu_seqlens_q, const int32_t* seqused_k, const int32_t* block_table,
+                                           int64_t table_stride, int max_pages, int nseq, int Tq, int Hq, int Hkv, int D, int page_size,
+                                           int64_t q_stride_t, int64_t q_stride_h, int64_t o_stride_t, int64_t o_stride_h,
+                                           int max_seqlen_q, int is_causal, float sm_scale, int window_left, int window_right,
+                                           void* stream) {
+  int right = -1;
+  if (int r = window_args(window_left, window_right, is_causal, right)) return r;
+  return kvcache8_prefill(q, dtype, k_pages, k_scale, v_pages, v_scale, k_smooth, out, lse, cu_seqlens_q, seqused_k, block_table,
+                          table_stride, max_pages, nseq, Tq, Hq, Hkv, D, page_size, q_stride_t, q_stride_h, o_stride_t, o_stride_h,
+                          max_seqlen_q, is_causal, sm_scale, true, window_left, right, stream);
 }

@@ -13,6 +13,7 @@ from typing import Optional
 import torch
 
 from . import ops
+from .core import _check_window_size
 
 _ROW_LIMIT = 64     # query rows per (sequence, KV head): max_seqlen_q * Hq / Hkv
 
@@ -143,9 +144,17 @@ def _attn_args(q, cache, cu_seqlens_q, seqused_k, block_table, max_seqlen_q):
     return Hq, D, cu_q
 
 
+def _window_arg(window_size, block_table, cache):
+    """window_size checked as sageattn_window's, each side clamped at the table's max_pages * page_size keys (no row sees more),
+    so a Python int of any size reaches the C ABI as an int32."""
+    left, right = _check_window_size(window_size)
+    max_keys = block_table.size(1) * cache.page_size
+    return min(left, max_keys), min(right, max_keys)
+
+
 def sageattn_kvcache8(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_q: torch.Tensor, seqused_k: torch.Tensor,
                       block_table: torch.Tensor, max_seqlen_q: int, is_causal: bool = True, sm_scale: Optional[float] = None,
-                      return_lse: bool = False):
+                      return_lse: bool = False, window_size=(-1, -1)):
     """Attention of packed queries against a PagedKVCache8, for decoding and speculative verification.
 
     q: packed [Tq, Hq, D] in the cache's dtype with cu_seqlens_q (int32 or int64, nseq + 1 offsets) and max_seqlen_q, as in
@@ -165,8 +174,16 @@ def sageattn_kvcache8(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_q: torch
     within a chunk an exact running max over 64-key tiles, p = 2^(s - m), P = bf16(p * v_scale) times the e4m3 V with fp32
     accumulation; a second kernel merges a row's chunks in ascending order with no atomics.  A sequence's bits depend only on its
     own q, keys and values, not on the rest of the batch or on the table width.  return_lse also returns the [Hq, Tq] fp32 LSE in
-    natural-log units of the logits q . k * sm_scale."""
+    natural-log units of the logits q . k * sm_scale.
+
+    window_size = (left, right), a pair of ints >= -1 (ValueError otherwise, before any launch), makes a sliding window aligned as
+    the causal rule: with off_b = Lk_b - Lq_b, query i sees key j iff i + off_b - left <= j <= i + off_b + right (-1 leaves a side
+    unbounded), and j <= i + off_b as well when is_causal.  Only keys j >= max(0, Lk_b - Lq_b - left) are ever loaded: their
+    table entries, K / V bytes and scales are the only ones read, so the entries below that bound may name any page in
+    [0, num_pages) (a shared null page, or pages reused for newer tokens).  Skipping keys left of the window changes no bit of what
+    a row computes, and (-1, -1) is the call without a window."""
     Hq, D, cu_q = _attn_args(q, cache, cu_seqlens_q, seqused_k, block_table, max_seqlen_q)
+    window = _window_arg(window_size, block_table, cache)
     Hkv = cache.num_kv_heads
     if max_seqlen_q * (Hq // Hkv) > _ROW_LIMIT:
         raise ValueError(f"max_seqlen_q * Hq / Hkv = {max_seqlen_q * (Hq // Hkv)} exceeds the {_ROW_LIMIT} query rows the split-KV "
@@ -176,15 +193,15 @@ def sageattn_kvcache8(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_q: torch
         sm_scale = D ** -0.5
     with torch.no_grad():
         o = torch.empty(q.shape, dtype=q.dtype, device=cache.device)
-        lse = ops.kvcache8_attn(q, cache.k_pages, cache.k_scale, cache.v_pages.view(torch.uint8), cache.v_scale, cache.k_smooth, o,
-                                cu_q.contiguous(), seqused_k.contiguous(), block_table, int(max_seqlen_q), 1 if is_causal else 0,
-                                float(sm_scale), 1 if return_lse else 0)
+        args = (q, cache.k_pages, cache.k_scale, cache.v_pages.view(torch.uint8), cache.v_scale, cache.k_smooth, o, cu_q.contiguous(),
+                seqused_k.contiguous(), block_table, int(max_seqlen_q), 1 if is_causal else 0, float(sm_scale), 1 if return_lse else 0)
+        lse = ops.kvcache8_attn(*args) if window == (-1, -1) else ops.kvcache8_attn_window(*args, *window)
     return (o, lse) if return_lse else o
 
 
 def sageattn_kvcache8_prefill(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_q: torch.Tensor, seqused_k: torch.Tensor,
                               block_table: torch.Tensor, max_seqlen_q: int, is_causal: bool = True, sm_scale: Optional[float] = None,
-                              return_lse: bool = False):
+                              return_lse: bool = False, window_size=(-1, -1)):
     """Attention of packed query chunks of any length against a PagedKVCache8: chunked prefill, prefix caching and long
     speculative verification on the 8-bit cache alone.
 
@@ -199,13 +216,17 @@ def sageattn_kvcache8_prefill(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_
     float(dot(q8, k8)) * (q_scale * sm_scale * log2e) * k_scale; one exact running max per row over 64-key tiles from key 0,
     p = 2^(s - m), P = bf16(p * v_scale) times the e4m3 V with fp32 accumulation, O / l.  A row's bits depend only on its own
     q, keys and values: not on the batch, the table width, or the size of the chunk it was prefilled in.  return_lse also returns
-    the [Hq, Tq] fp32 LSE in natural-log units of the logits q . k * sm_scale."""
+    the [Hq, Tq] fp32 LSE in natural-log units of the logits q . k * sm_scale.
+
+    window_size: the sliding window of sageattn_kvcache8, with the same rule and the same promise: only keys
+    j >= max(0, Lk_b - Lq_b - left) are ever loaded, and a row's bits do not change with the chunk size."""
     Hq, D, cu_q = _attn_args(q, cache, cu_seqlens_q, seqused_k, block_table, max_seqlen_q)
+    window = _window_arg(window_size, block_table, cache)
     if sm_scale is None:
         sm_scale = D ** -0.5
     with torch.no_grad():
         o = torch.empty(q.shape, dtype=q.dtype, device=cache.device)
-        lse = ops.kvcache8_prefill(q, cache.k_pages, cache.k_scale, cache.v_pages.view(torch.uint8), cache.v_scale, cache.k_smooth,
-                                   o, cu_q.contiguous(), seqused_k.contiguous(), block_table, int(max_seqlen_q),
-                                   1 if is_causal else 0, float(sm_scale), 1 if return_lse else 0)
+        args = (q, cache.k_pages, cache.k_scale, cache.v_pages.view(torch.uint8), cache.v_scale, cache.k_smooth, o, cu_q.contiguous(),
+                seqused_k.contiguous(), block_table, int(max_seqlen_q), 1 if is_causal else 0, float(sm_scale), 1 if return_lse else 0)
+        lse = ops.kvcache8_prefill(*args) if window == (-1, -1) else ops.kvcache8_prefill_window(*args, *window)
     return (o, lse) if return_lse else o

@@ -612,7 +612,8 @@ int sab_predict_block_mask_varlen(const float* q_mean, const float* q_sim, const
  * sab_kvcache8_attn: attention of packed q [Tq, Hq, D] (cu_seqlens_q [nseq+1] int32 device) against the cache: sequence b has
  *   Lk_b = seqused_k[b] keys (int32 device, read only on the device; clamped to max_pages * page_size), key j at slot j % page_size
  *   of page block_table[b * table_stride + j / page_size] (trusted, in [0, num_pages)).  Causal is bottom-right: query i sees key j
- *   iff j <= i + Lk_b - Lq_b.  Q is quantised per (token, head) as K is, without smoothing; logits in log2 units are
+ *   iff j <= i + Lk_b - Lq_b, with Lq_b = cu_seqlens_q[b + 1] - cu_seqlens_q[b] even when it exceeds max_seqlen_q (only the
+ *   first max_seqlen_q rows are then written, each seeing what it sees in the whole sequence).  Q is quantised per (token, head) as K is, without smoothing; logits in log2 units are
  *   float(dot(q8, k8)) * (q_scale * sm_scale * log2e) * k_scale.  Keys are cut into chunks of sab_kvcache8_chunk_keys() keys, one
  *   CTA per (sequence, KV head, chunk) holding all max_seqlen_q * Hq / Hkv <= 64 query rows of that KV head (rows past
  *   max_seqlen_q are not written); within a chunk an exact running max over 64-key tiles, P = bf16(p * v_scale) times bf16(v8)
@@ -639,7 +640,8 @@ int sab_kvcache8_attn(const void* q, int dtype, const int8_t* k_pages, const flo
  *   sm_scale * log2e) * k_scale, one exact running max per row over 64-key tiles from key 0, P = bf16(p * v_scale) times bf16(v8)
  *   with fp32 accumulation (wgmma), O / l.  A row's bits depend only on its own q, keys and values.  out [Tq, Hq, D] (strides
  *   o_stride_t / o_stride_h, even, 4-byte aligned) in `dtype`; lse (optional) [Hq, Tq] fp32 as in sab_kvcache8_attn.  A row that
- *   sees no key returns 0 and lse -inf; rows past max_seqlen_q are not written.  Launch-grid limits, refused with SAB_ERR_INVALID:
+ *   sees no key returns 0 and lse -inf; rows past max_seqlen_q are not written, and the rows written take Lq_b from
+ *   cu_seqlens_q as in sab_kvcache8_attn.  Launch-grid limits, refused with SAB_ERR_INVALID:
  *   Hq <= 65535, nseq * ceil(max_seqlen_q / 128) < 2^31 and max_pages * page_size < 2^31. */
 int sab_kvcache8_prefill(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
                          const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,

@@ -161,7 +161,7 @@ struct Kv8Params {
   float scale_log2;     // sm_scale * log2(e)
   float* o_part;        // [Tq, Hq, max_chunks, D]
   float2* ml_part;      // [Tq, Hq, max_chunks]: (running max in log2 units, sum of p)
-  int window_left, window_right;   // kWindow: query i sees keys [i + off - left, i + off + right], off = Lk - Lq (-1: unbounded)
+  int window_left, window_right;   // kWindow: query i sees keys [i + off - left, i + off + right], off = Lk - Lq_b (-1: unbounded)
 };
 
 template <int D>
@@ -189,8 +189,10 @@ __global__ void __launch_bounds__(kThreads, kWindow ? 3 : 0) kv8_attn_kernel(con
   const int b = blockIdx.x / p.max_chunks, chunk = blockIdx.x % p.max_chunks, h = blockIdx.y;
   const int G = p.Hq / p.Hkv;
   const int q0 = p.cu_q[b];
-  const int Lq = min(p.cu_q[b + 1] - q0, p.max_seqlen_q);
+  const int Lqb = p.cu_q[b + 1] - q0;   // the sequence's queries: the causal and window offsets are taken from it
+  const int Lq = min(Lqb, p.max_seqlen_q);   // the rows held and written
   const int Lk = min(p.seqused_k[b], p.max_pages * p.page_size);
+  const int off = Lk - Lqb;             // query i's diagonal key is i + off
   const int kbeg = chunk * kChunk;
   if (Lq <= 0 || kbeg >= Lk) return;
   const int kend = min(Lk, kbeg + kChunk);
@@ -199,12 +201,12 @@ __global__ void __launch_bounds__(kThreads, kWindow ? 3 : 0) kv8_attn_kernel(con
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32, g8 = lane / 4, c4 = lane % 4;
   const int32_t* table = p.table + int64_t(b) * p.table_stride;
   const int64_t hD = int64_t(h) * D;
-  // keys [klo, kend) hold every key a row of the CTA sees: klo is row 0's first key (the lower bounds rise with the row).  The
-  // last row's upper bound, Lk - 1 + max(right, 0), never falls below kend - 1, so the range ends at kend.  The tiles visited
-  // start at kb, the 64-key tile (of the grid from key 0) holding klo.
+  // keys [klo, kend) hold every key a row of the CTA sees: klo is row 0's first key (the lower bounds rise with the row), and no
+  // row sees a key at or past Lk.  Keys of [klo, kend) that no row sees (past the last held row's upper bound) are masked.  The
+  // tiles visited start at kb, the 64-key tile (of the grid from key 0) holding klo.
   int klo = kbeg, kb = kbeg;
   if constexpr (kWindow) {
-    if (p.window_left >= 0) klo = int(max(int64_t(kbeg), int64_t(Lk) - Lq - p.window_left));
+    if (p.window_left >= 0) klo = int(max(int64_t(kbeg), int64_t(off) - p.window_left));
     if (klo >= kend) {
       // nothing to read: the empty partials (m = -inf, l = 0, O = 0) the combine folds with weight 0
       for (int e = threadIdx.x; e < R * D; e += kThreads) {
@@ -279,19 +281,21 @@ __global__ void __launch_bounds__(kThreads, kWindow ? 3 : 0) kv8_attn_kernel(con
   }
   // the last key row r may see: causal is bottom-right inside the sequence.  kWindow, in one register per row as lim: row r sees
   // key < kend iff unsigned(key - lo) <= span, with lo = i + off - left and span = left + right.  A side past what the sequence
-  // can reach (left > Lk, right > Lq: rows are i < Lq <= 64) sees as much as -1 and is clamped to it, so the key - lo of every
-  // key < kend lies in (-2^31, 2^32) and the unsigned test is exact.  Rows r >= R take lo = kend and see nothing.
+  // can reach (left > Lk, right > Lq_b: rows are i < Lq_b) sees as much as -1 and is clamped to it, so 0 <= wl <= Lk and
+  // 0 <= wr <= Lq_b.  For every key in [0, kend) and row i < Lq_b, key - lo = key - i + Lq_b - Lk + wl then lies in
+  // [wl - Lk + 1, Lq_b + wl - 1]: a key left of lo maps to an unsigned value of at least 2^32 + wl - Lk + 1, above
+  // span <= wl + Lq_b because Lk + Lq_b < 2^32, so the unsigned test is exact.  Rows r >= R take lo = kend and see nothing.
   int lim[4][2];
   const int wl = p.window_left < 0 || p.window_left > Lk ? Lk : p.window_left;
-  const int wr = p.window_right < 0 || p.window_right > Lq ? Lq : p.window_right;
+  const int wr = p.window_right < 0 || p.window_right > Lqb ? Lqb : p.window_right;
   const unsigned span = unsigned(wl) + unsigned(wr);
 #pragma unroll
   for (int mt = 0; mt < 4; ++mt)
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       const int r = mt * 16 + g8 + 8 * j;
-      if constexpr (kWindow) lim[mt][j] = r >= R ? kend : r / G + Lk - Lq - wl;
-      else lim[mt][j] = r >= R ? -1 : (kCausal ? min(kend - 1, r / G + Lk - Lq) : kend - 1);
+      if constexpr (kWindow) lim[mt][j] = r >= R ? kend : r / G + off - wl;
+      else lim[mt][j] = r >= R ? -1 : (kCausal ? min(kend - 1, r / G + off) : kend - 1);
     }
 
   for (int t = 0; t < ntiles; ++t) {
@@ -543,25 +547,26 @@ __global__ void __launch_bounds__(kPfThreads, 1) kv8_prefill_kernel(const PfPara
   const int b = blockIdx.x / p.n_qt, qt = p.n_qt - 1 - blockIdx.x % p.n_qt, hq = blockIdx.y;   // longest rows first
   const int hk = hq / (p.Hq / p.Hkv);
   const int q0 = p.cu_q[b];
-  const int Lq = min(p.cu_q[b + 1] - q0, p.max_seqlen_q);
+  const int Lqb = p.cu_q[b + 1] - q0;   // the sequence's queries: the causal and window offsets are taken from it
+  const int Lq = min(Lqb, p.max_seqlen_q);   // the rows held and written
   const int Lk = max(0, min(p.seqused_k[b], p.max_pages * p.page_size));
+  const int off = Lk - Lqb;             // query i's diagonal key is i + off
   const int r0 = qt * kPfRows;          // the CTA's first row inside the sequence
   if (r0 >= Lq) return;
   // keys [klo, kmax) hold every key a row of the CTA sees; tiles past `first_h` (the first row's last key), and kWindow: tiles
   // starting before `lo_last` (the last row's first key), take the masked path
   const int last = min(r0 + kPfRows, Lq) - 1;
-  int kmax = kCausal ? max(0, min(Lk, last + Lk - Lq + 1)) : Lk;
-  int first_h = kCausal ? min(Lk - 1, r0 + Lk - Lq) : Lk - 1;
+  int kmax = kCausal ? max(0, min(Lk, last + off + 1)) : Lk;
+  int first_h = kCausal ? min(Lk - 1, r0 + off) : Lk - 1;
   int klo = 0, lo_last = 0, tf = 0;
   if constexpr (kWindow) {
-    const int64_t off = int64_t(Lk) - Lq;
     if (p.window_right >= 0) {
-      kmax = int(max(int64_t(0), min(int64_t(Lk), last + off + p.window_right + 1)));
-      first_h = int(min(int64_t(Lk - 1), r0 + off + p.window_right));
+      kmax = int(max(int64_t(0), min(int64_t(Lk), last + int64_t(off) + p.window_right + 1)));
+      first_h = int(min(int64_t(Lk - 1), r0 + int64_t(off) + p.window_right));
     }
     if (p.window_left >= 0) {
-      klo = int(max(int64_t(0), min(int64_t(Lk), r0 + off - p.window_left)));
-      lo_last = int(max(int64_t(0), min(int64_t(Lk), last + off - p.window_left)));
+      klo = int(max(int64_t(0), min(int64_t(Lk), r0 + int64_t(off) - p.window_left)));
+      lo_last = int(max(int64_t(0), min(int64_t(Lk), last + int64_t(off) - p.window_left)));
     }
     tf = klo / kTile;
   }
@@ -683,9 +688,9 @@ __global__ void __launch_bounds__(kPfThreads, 1) kv8_prefill_kernel(const PfPara
   for (int r = 0; r < 2; ++r) {
     const int i = r0 + row0 + 8 * r;
     qcr[r] = sm.qc[row0 + 8 * r];
-    lim[r] = i >= Lq ? -1 : (kCausal ? min(Lk - 1, i + Lk - Lq) : Lk - 1);
+    lim[r] = i >= Lq ? -1 : (kCausal ? min(Lk - 1, i + off) : Lk - 1);
     if constexpr (kWindow) {
-      const int64_t diag = int64_t(i) + Lk - Lq;
+      const int64_t diag = int64_t(i) + off;
       if (i < Lq && p.window_right >= 0) lim[r] = int(max(int64_t(-1), min(int64_t(Lk - 1), diag + p.window_right)));
       lo[r] = p.window_left < 0 ? 0 : int(max(int64_t(0), min(int64_t(Lk), diag - p.window_left)));
     }

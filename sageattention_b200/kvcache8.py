@@ -168,8 +168,9 @@ def sageattn_kvcache8(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_q: torch
     ValueError: use sageattn_kvcache8_prefill for longer query chunks.  Rows of a sequence past max_seqlen_q, and rows past
     cu_seqlens_q[-1], are not written.  Forward only.
 
-    Causal is bottom-right: query i of sequence b sees key j iff j <= i + Lk_b - Lq_b.  A row that sees no key returns 0 and lse
-    -inf.  Numerics: Q is quantised per (token, head) to INT8 as K is (without smoothing); logits in log2 units are
+    Causal is bottom-right: query i of sequence b sees key j iff j <= i + Lk_b - Lq_b, Lq_b = cu_seqlens_q[b + 1] - cu_seqlens_q[b]
+    even when it exceeds max_seqlen_q: the rows written then see what they see in the whole sequence, with and without a window.
+    A row that sees no key returns 0 and lse -inf.  Numerics: Q is quantised per (token, head) to INT8 as K is (without smoothing); logits in log2 units are
     float(dot(q8, k8)) * (q_scale * sm_scale * log2e) * k_scale.  Keys are cut into fixed chunks of ops.kvcache8_chunk_keys() keys;
     within a chunk an exact running max over 64-key tiles, p = 2^(s - m), P = bf16(p * v_scale) times the e4m3 V with fp32
     accumulation; a second kernel merges a row's chunks in ascending order with no atomics.  A sequence's bits depend only on its
@@ -210,7 +211,7 @@ def sageattn_kvcache8_prefill(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_
     contiguous rows and trusted entries.  The call never synchronises with the host and allocates nothing but o (and lse), so
     cache.write + this call can be captured in a CUDA graph.  Causal is bottom-right: query i of sequence b sees key j iff
     j <= i + Lk_b - Lq_b; a row that sees no key returns 0 and lse -inf.  Rows of a sequence past max_seqlen_q, and rows past
-    cu_seqlens_q[-1], are not written.  Forward only.
+    cu_seqlens_q[-1], are not written; the rows written take Lq_b from cu_seqlens_q, as in sageattn_kvcache8.  Forward only.
 
     Numerics: those of sageattn_kvcache8 without chunks.  Q is quantised per (token, head) to INT8; logits in log2 units are
     float(dot(q8, k8)) * (q_scale * sm_scale * log2e) * k_scale; one exact running max per row over 64-key tiles from key 0,

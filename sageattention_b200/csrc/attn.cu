@@ -855,10 +855,7 @@ static thread_local const sab::Window* tl_window = nullptr;
 // set by sab_qk_int8_sv_f8_attn_varlen (same thread): v_scale / v_mean are per sequence
 static thread_local bool tl_seq_v = false;
 // attention mask of the masked entry point, handed to attn_entry by sab_qk_int8_sv_f16_attn_masked (same thread)
-struct MaskArgs {
-  const void* ptr; int kind; int64_t sb, sh, sm, sn;
-};
-static thread_local const MaskArgs* tl_mask = nullptr;
+static thread_local const sab::MaskArgs* tl_mask = nullptr;
 // segment flags of the fused sequence-parallel entry point, handed to attn_entry by sab_qk_int8_sv_f8_attn_sp (same thread)
 struct SegArgs {
   const uint32_t* flags;
@@ -1123,7 +1120,7 @@ extern "C" int sab_qk_int8_sv_f16_attn_masked(const int8_t* q_int8, const int8_t
                                               float sm_scale, int fold_sm_scale, const void* attn_mask, int mask_kind,
                                               int64_t mask_stride_b, int64_t mask_stride_h, int64_t mask_stride_m,
                                               int64_t mask_stride_n, void* stream) {
-  const MaskArgs m{attn_mask, mask_kind, mask_stride_b, mask_stride_h, mask_stride_m, mask_stride_n};
+  const sab::MaskArgs m{attn_mask, mask_kind, mask_stride_b, mask_stride_h, mask_stride_m, mask_stride_n};
   tl_mask = &m;
   const int st = attn_entry(1, q_int8, k_int8, reinterpret_cast<const uint8_t*>(v_f16t), out, lse, q_scale, k_scale, nullptr,
                             nullptr, out_dtype, B, Hq, Hkv, Sq, Skv, D, q_stride_b, q_stride_h, q_stride_s, k_stride_b,

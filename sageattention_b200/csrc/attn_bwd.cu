@@ -762,8 +762,22 @@ static int launch_bwd_window(const BwdParams& p, const Window& w, cudaStream_t s
   return SAB_OK;
 }
 
-// Checks shared by the dense and the varlen entry, after the pointer / size checks: the forward's codes and messages (attn.cu).
-// st: (b, h, s) element strides of q8, k8, q, k, v, o, dout.
+// The first checks of every entry, after its window / block-mask checks: the forward's codes and messages (attn.cu).  B / Sq / Skv
+// are nseq / Tq / Tk for the packed entries.
+static int check_bwd_args(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale, const void* q,
+                          const void* k, const void* v, const void* o, const void* dout, const float* lse, const void* dq,
+                          const void* dk, const void* dv, const void* workspace, int dtype, int B, int Hq, int Hkv, int Sq, int Skv,
+                          int D) {
+  SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
+              SAB_ERR_INVALID, "null tensor pointer");
+  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
+  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "dtype must be fp16 or bf16");
+  SAB_REQUIRE(B > 0 && Hq > 0 && Hkv > 0 && Sq > 0 && Skv > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", B, Hq, Hkv, Sq, Skv);
+  SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
+  return SAB_OK;
+}
+
+// The last checks of every entry, then the device check.  st: (b, h, s) element strides of q8, k8, q, k, v, o, dout.
 static int check_bwd_layout(const int8_t* q_int8, const int8_t* k_int8, const void* q, const void* k, const void* v,
                             const void* o, const void* dout, void* dq, void* dk, void* dv, const int64_t (&st)[21]) {
   bool ok16 = aligned16(q) && aligned16(k) && aligned16(v) && aligned16(o) && aligned16(dout) && aligned16(dq) && aligned16(dk) && aligned16(dv);
@@ -775,7 +789,7 @@ static int check_bwd_layout(const int8_t* q_int8, const int8_t* k_int8, const vo
   return sab_check_device();
 }
 
-// The parameters both entries fill; the varlen entry then adds its sequence tables
+// The parameters every entry fills; the packed entries then add their sequence tables
 static BwdParams bwd_params(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale, const void* q,
                             const void* k, const void* v, const void* o, const void* dout, const float* lse, const void* k_mean,
                             void* dq, void* dk, void* dv, void* workspace, int B, int Hq, int Hkv, int Sq, int Skv,
@@ -834,6 +848,65 @@ extern "C" int64_t sab_attn_bwd_workspace_bytes(int B, int Hq, int Sq) {
   return (int64_t(B) * Hq * Sq * 4 + 255) / 256 * 256;
 }
 
+// sab_qk_int8_attn_bwd and, with a window w or a block mask bm (already checked) or an attention mask m and its nullable dbias,
+// sab_qk_int8_attn_bwd_window / sab_qk_int8_attn_bwd_blocksparse / sab_qk_int8_attn_bwd_masked
+static int bwd_dense(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale, const void* q,
+                     const void* k, const void* v, const void* o, const void* dout, const float* lse, const void* k_mean, void* dq,
+                     void* dk, void* dv, void* workspace, int dtype, int B, int Hq, int Hkv, int Sq, int Skv, int D,
+                     int64_t q8_stride_b, int64_t q8_stride_h, int64_t q8_stride_s, int64_t k8_stride_b, int64_t k8_stride_h,
+                     int64_t k8_stride_s, int64_t q_stride_b, int64_t q_stride_h, int64_t q_stride_s, int64_t k_stride_b,
+                     int64_t k_stride_h, int64_t k_stride_s, int64_t v_stride_b, int64_t v_stride_h, int64_t v_stride_s,
+                     int64_t o_stride_b, int64_t o_stride_h, int64_t o_stride_s, int64_t do_stride_b, int64_t do_stride_h,
+                     int64_t do_stride_s, int is_causal, int q_gran, int k_gran, float sm_scale, int fold_sm_scale,
+                     const sab::Window* w, const sab::BlockMask* bm, const sab::MaskArgs* m, void* dbias, void* stream) {
+  using namespace sab;
+  if (int e = check_bwd_args(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, dq, dk, dv, workspace, dtype, B, Hq, Hkv, Sq, Skv, D))
+    return e;
+  SAB_REQUIRE(q_gran >= 1 && q_gran <= 3 && k_gran >= 1 && k_gran <= 3, SAB_ERR_INVALID, "unknown quant granularity q=%d k=%d", q_gran, k_gran);
+  SAB_REQUIRE(!is_causal || Sq == Skv, SAB_ERR_INVALID, "qo_len and kv_len must be equal for causal attention.");
+  if (m != nullptr) {
+    // the masked forward's checks (attn.cu), then the gradient's own
+    SAB_REQUIRE(k_gran != SAB_GRAN_PER_THREAD, SAB_ERR_UNSUPPORTED,
+                "attn_mask is supported by the dense non-causal fp16-PV path with per-block / per-warp K scales only");
+    SAB_REQUIRE(m->ptr != nullptr && (m->kind == SAB_MASK_BOOL || m->kind == SAB_MASK_BIAS), SAB_ERR_INVALID,
+                "attn_mask: null pointer or unknown kind %d", m->kind);
+    SAB_REQUIRE(dbias == nullptr || m->kind == SAB_MASK_BIAS, SAB_ERR_INVALID, "dbias needs an additive bias mask (SAB_MASK_BIAS)");
+    SAB_REQUIRE(aligned16(dbias), SAB_ERR_INVALID, "dbias must be 16-byte aligned");
+  }
+  const int64_t st[21] = {q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s, q_stride_b, q_stride_h, q_stride_s,
+                          k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s, o_stride_b, o_stride_h, o_stride_s,
+                          do_stride_b, do_stride_h, do_stride_s};
+  if (int e = check_bwd_layout(q_int8, k_int8, q, k, v, o, dout, dq, dk, dv, st)) return e;
+  BwdParams p = bwd_params(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, B, Hq, Hkv, Sq, Skv,
+                           st, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const bool kt = k_gran == SAB_GRAN_PER_THREAD;
+  const bool bf = dtype == SAB_DTYPE_BF16;
+  if (m != nullptr) {
+    p.a.mask = m->ptr; p.a.mask_kind = m->kind;
+    p.a.mask_sb = m->sb; p.a.mask_sh = m->sh; p.a.mask_sm = m->sm; p.a.mask_sn = m->sn;
+    if (D == 128) return bf ? launch_bwd_masked<128, __nv_bfloat16>(p, dbias, s) : launch_bwd_masked<128, __half>(p, dbias, s);
+    return bf ? launch_bwd_masked<64, __nv_bfloat16>(p, dbias, s) : launch_bwd_masked<64, __half>(p, dbias, s);
+  }
+  if (w != nullptr) {
+    if (D == 128) {
+      if (kt) return bf ? launch_bwd_window<128, true, __nv_bfloat16>(p, *w, s) : launch_bwd_window<128, true, __half>(p, *w, s);
+      return bf ? launch_bwd_window<128, false, __nv_bfloat16>(p, *w, s) : launch_bwd_window<128, false, __half>(p, *w, s);
+    }
+    if (kt) return bf ? launch_bwd_window<64, true, __nv_bfloat16>(p, *w, s) : launch_bwd_window<64, true, __half>(p, *w, s);
+    return bf ? launch_bwd_window<64, false, __nv_bfloat16>(p, *w, s) : launch_bwd_window<64, false, __half>(p, *w, s);
+  }
+  if (bm != nullptr) {
+    if (D == 128) {
+      if (kt) return bf ? launch_bwd_blocksparse<128, true, __nv_bfloat16>(p, *bm, Skv, s) : launch_bwd_blocksparse<128, true, __half>(p, *bm, Skv, s);
+      return bf ? launch_bwd_blocksparse<128, false, __nv_bfloat16>(p, *bm, Skv, s) : launch_bwd_blocksparse<128, false, __half>(p, *bm, Skv, s);
+    }
+    if (kt) return bf ? launch_bwd_blocksparse<64, true, __nv_bfloat16>(p, *bm, Skv, s) : launch_bwd_blocksparse<64, true, __half>(p, *bm, Skv, s);
+    return bf ? launch_bwd_blocksparse<64, false, __nv_bfloat16>(p, *bm, Skv, s) : launch_bwd_blocksparse<64, false, __half>(p, *bm, Skv, s);
+  }
+  return dispatch_bwd(p, D, dtype, k_gran, stream);
+}
+
 extern "C" int sab_qk_int8_attn_bwd(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
                                     const void* q, const void* k, const void* v, const void* o, const void* dout, const float* lse,
                                     const void* k_mean, void* dq, void* dk, void* dv, void* workspace, int dtype, int B, int Hq, int Hkv, int Sq,
@@ -844,22 +917,11 @@ extern "C" int sab_qk_int8_attn_bwd(const int8_t* q_int8, const int8_t* k_int8, 
                                     int64_t o_stride_b, int64_t o_stride_h, int64_t o_stride_s, int64_t do_stride_b,
                                     int64_t do_stride_h, int64_t do_stride_s, int is_causal, int q_gran, int k_gran,
                                     float sm_scale, int fold_sm_scale, void* stream) {
-  using namespace sab;
-  SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
-              SAB_ERR_INVALID, "null tensor pointer");
-  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
-  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "dtype must be fp16 or bf16");
-  SAB_REQUIRE(B > 0 && Hq > 0 && Hkv > 0 && Sq > 0 && Skv > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", B, Hq, Hkv, Sq, Skv);
-  SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
-  SAB_REQUIRE(q_gran >= 1 && q_gran <= 3 && k_gran >= 1 && k_gran <= 3, SAB_ERR_INVALID, "unknown quant granularity q=%d k=%d", q_gran, k_gran);
-  SAB_REQUIRE(!is_causal || Sq == Skv, SAB_ERR_INVALID, "qo_len and kv_len must be equal for causal attention.");
-  const int64_t st[21] = {q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s, q_stride_b, q_stride_h, q_stride_s,
-                          k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s, o_stride_b, o_stride_h, o_stride_s,
-                          do_stride_b, do_stride_h, do_stride_s};
-  if (int e = check_bwd_layout(q_int8, k_int8, q, k, v, o, dout, dq, dk, dv, st)) return e;
-  const BwdParams p = bwd_params(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, B, Hq, Hkv, Sq,
-                                 Skv, st, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale);
-  return dispatch_bwd(p, D, dtype, k_gran, stream);
+  return bwd_dense(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, dtype, B, Hq, Hkv, Sq, Skv, D,
+                   q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s, q_stride_b, q_stride_h, q_stride_s,
+                   k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s, o_stride_b, o_stride_h, o_stride_s,
+                   do_stride_b, do_stride_h, do_stride_s, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale, nullptr, nullptr, nullptr,
+                   nullptr, stream);
 }
 
 extern "C" int sab_qk_int8_attn_bwd_varlen(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
@@ -873,12 +935,8 @@ extern "C" int sab_qk_int8_attn_bwd_varlen(const int8_t* q_int8, const int8_t* k
                                            const int32_t* cu_q_scale, const int32_t* cu_k_scale, int max_seqlen_q,
                                            int max_seqlen_k, int is_causal, float sm_scale, int fold_sm_scale, void* stream) {
   using namespace sab;
-  SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
-              SAB_ERR_INVALID, "null tensor pointer");
-  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
-  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "dtype must be fp16 or bf16");
-  SAB_REQUIRE(nseq > 0 && Hq > 0 && Hkv > 0 && Tq > 0 && Tk > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", nseq, Hq, Hkv, Tq, Tk);
-  SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
+  if (int e = check_bwd_args(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, dq, dk, dv, workspace, dtype, nseq, Hq, Hkv, Tq, Tk, D))
+    return e;
   SAB_REQUIRE(cu_seqlens_q && cu_seqlens_k && cu_q_scale && cu_k_scale && max_seqlen_q > 0 && max_seqlen_k > 0, SAB_ERR_INVALID,
               "varlen needs cu_seqlens_q, cu_seqlens_k, cu_q_scale, cu_k_scale, max_seqlen_q and max_seqlen_k");
   // packed [T,H,D]: no batch stride
@@ -909,34 +967,12 @@ extern "C" int sab_qk_int8_attn_bwd_masked(const int8_t* q_int8, const int8_t* k
                                            int q_gran, int k_gran, float sm_scale, int fold_sm_scale, const void* attn_mask,
                                            int mask_kind, int64_t mask_stride_b, int64_t mask_stride_h, int64_t mask_stride_m,
                                            int64_t mask_stride_n, void* dbias, void* stream) {
-  using namespace sab;
-  SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
-              SAB_ERR_INVALID, "null tensor pointer");
-  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
-  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "dtype must be fp16 or bf16");
-  SAB_REQUIRE(B > 0 && Hq > 0 && Hkv > 0 && Sq > 0 && Skv > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", B, Hq, Hkv, Sq, Skv);
-  SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
-  SAB_REQUIRE(q_gran >= 1 && q_gran <= 3 && k_gran >= 1 && k_gran <= 3, SAB_ERR_INVALID, "unknown quant granularity q=%d k=%d", q_gran, k_gran);
-  // the masked forward's checks (attn.cu), then the gradient's own
-  SAB_REQUIRE(k_gran != SAB_GRAN_PER_THREAD, SAB_ERR_UNSUPPORTED,
-              "attn_mask is supported by the dense non-causal fp16-PV path with per-block / per-warp K scales only");
-  SAB_REQUIRE(attn_mask != nullptr && (mask_kind == SAB_MASK_BOOL || mask_kind == SAB_MASK_BIAS), SAB_ERR_INVALID,
-              "attn_mask: null pointer or unknown kind %d", mask_kind);
-  SAB_REQUIRE(dbias == nullptr || mask_kind == SAB_MASK_BIAS, SAB_ERR_INVALID, "dbias needs an additive bias mask (SAB_MASK_BIAS)");
-  SAB_REQUIRE(aligned16(dbias), SAB_ERR_INVALID, "dbias must be 16-byte aligned");
-  const int64_t st[21] = {q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s, q_stride_b, q_stride_h, q_stride_s,
-                          k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s, o_stride_b, o_stride_h, o_stride_s,
-                          do_stride_b, do_stride_h, do_stride_s};
-  if (int e = check_bwd_layout(q_int8, k_int8, q, k, v, o, dout, dq, dk, dv, st)) return e;
-  BwdParams p = bwd_params(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, B, Hq, Hkv, Sq, Skv,
-                           st, 0, q_gran, k_gran, sm_scale, fold_sm_scale);
-  AttnParams& a = p.a;
-  a.mask = attn_mask; a.mask_kind = mask_kind;
-  a.mask_sb = mask_stride_b; a.mask_sh = mask_stride_h; a.mask_sm = mask_stride_m; a.mask_sn = mask_stride_n;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const bool bf = dtype == SAB_DTYPE_BF16;
-  if (D == 128) return bf ? launch_bwd_masked<128, __nv_bfloat16>(p, dbias, s) : launch_bwd_masked<128, __half>(p, dbias, s);
-  return bf ? launch_bwd_masked<64, __nv_bfloat16>(p, dbias, s) : launch_bwd_masked<64, __half>(p, dbias, s);
+  const sab::MaskArgs m{attn_mask, mask_kind, mask_stride_b, mask_stride_h, mask_stride_m, mask_stride_n};
+  return bwd_dense(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, dtype, B, Hq, Hkv, Sq, Skv, D,
+                   q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s, q_stride_b, q_stride_h, q_stride_s,
+                   k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s, o_stride_b, o_stride_h, o_stride_s,
+                   do_stride_b, do_stride_h, do_stride_s, 0, q_gran, k_gran, sm_scale, fold_sm_scale, nullptr, nullptr, &m, dbias,
+                   stream);
 }
 
 extern "C" int sab_qk_int8_attn_bwd_blocksparse(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale,
@@ -951,32 +987,14 @@ extern "C" int sab_qk_int8_attn_bwd_blocksparse(const int8_t* q_int8, const int8
                                                 int64_t do_stride_s, int is_causal, int q_gran, int k_gran, float sm_scale,
                                                 int fold_sm_scale, const uint8_t* block_mask, int64_t mask_stride_b,
                                                 int64_t mask_stride_h, int64_t mask_stride_qb, int64_t mask_stride_kb, void* stream) {
-  using namespace sab;
-  if (int e = check_block_mask(block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb, q_gran, is_causal, Sq, Skv))
+  if (int e = sab::check_block_mask(block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb, q_gran, is_causal, Sq, Skv))
     return e;
-  SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
-              SAB_ERR_INVALID, "null tensor pointer");
-  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
-  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "dtype must be fp16 or bf16");
-  SAB_REQUIRE(B > 0 && Hq > 0 && Hkv > 0 && Sq > 0 && Skv > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", B, Hq, Hkv, Sq, Skv);
-  SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
-  SAB_REQUIRE(k_gran >= 1 && k_gran <= 3, SAB_ERR_INVALID, "unknown quant granularity q=%d k=%d", q_gran, k_gran);
-  const int64_t st[21] = {q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s, q_stride_b, q_stride_h, q_stride_s,
-                          k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s, o_stride_b, o_stride_h, o_stride_s,
-                          do_stride_b, do_stride_h, do_stride_s};
-  if (int e = check_bwd_layout(q_int8, k_int8, q, k, v, o, dout, dq, dk, dv, st)) return e;
-  const BwdParams p = bwd_params(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, B, Hq, Hkv, Sq,
-                                 Skv, st, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale);
-  const BlockMask bm{block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb};
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const bool kt = k_gran == SAB_GRAN_PER_THREAD;
-  const bool bf = dtype == SAB_DTYPE_BF16;
-  if (D == 128) {
-    if (kt) return bf ? launch_bwd_blocksparse<128, true, __nv_bfloat16>(p, bm, Skv, s) : launch_bwd_blocksparse<128, true, __half>(p, bm, Skv, s);
-    return bf ? launch_bwd_blocksparse<128, false, __nv_bfloat16>(p, bm, Skv, s) : launch_bwd_blocksparse<128, false, __half>(p, bm, Skv, s);
-  }
-  if (kt) return bf ? launch_bwd_blocksparse<64, true, __nv_bfloat16>(p, bm, Skv, s) : launch_bwd_blocksparse<64, true, __half>(p, bm, Skv, s);
-  return bf ? launch_bwd_blocksparse<64, false, __nv_bfloat16>(p, bm, Skv, s) : launch_bwd_blocksparse<64, false, __half>(p, bm, Skv, s);
+  const sab::BlockMask bm{block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb};
+  return bwd_dense(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, dtype, B, Hq, Hkv, Sq, Skv, D,
+                   q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s, q_stride_b, q_stride_h, q_stride_s,
+                   k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s, o_stride_b, o_stride_h, o_stride_s,
+                   do_stride_b, do_stride_h, do_stride_s, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale, nullptr, &bm, nullptr,
+                   nullptr, stream);
 }
 
 extern "C" int sab_qk_int8_attn_bwd_window(const int8_t* q_int8, const int8_t* k_int8, const float* q_scale, const float* k_scale,
@@ -990,31 +1008,13 @@ extern "C" int sab_qk_int8_attn_bwd_window(const int8_t* q_int8, const int8_t* k
                                            int64_t o_stride_s, int64_t do_stride_b, int64_t do_stride_h, int64_t do_stride_s,
                                            int is_causal, int q_gran, int k_gran, float sm_scale, int fold_sm_scale,
                                            int window_left, int window_right, void* stream) {
-  using namespace sab;
-  if (int e = check_window(window_left, window_right, is_causal, Sq, Skv)) return e;
-  SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
-              SAB_ERR_INVALID, "null tensor pointer");
-  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
-  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "dtype must be fp16 or bf16");
-  SAB_REQUIRE(B > 0 && Hq > 0 && Hkv > 0 && Sq > 0 && Skv > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", B, Hq, Hkv, Sq, Skv);
-  SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
-  SAB_REQUIRE(q_gran >= 1 && q_gran <= 3 && k_gran >= 1 && k_gran <= 3, SAB_ERR_INVALID, "unknown quant granularity q=%d k=%d", q_gran, k_gran);
-  const int64_t st[21] = {q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s, q_stride_b, q_stride_h, q_stride_s,
-                          k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s, o_stride_b, o_stride_h, o_stride_s,
-                          do_stride_b, do_stride_h, do_stride_s};
-  if (int e = check_bwd_layout(q_int8, k_int8, q, k, v, o, dout, dq, dk, dv, st)) return e;
-  const BwdParams p = bwd_params(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, B, Hq, Hkv, Sq,
-                                 Skv, st, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale);
-  const Window w{window_left, window_right};
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const bool kt = k_gran == SAB_GRAN_PER_THREAD;
-  const bool bf = dtype == SAB_DTYPE_BF16;
-  if (D == 128) {
-    if (kt) return bf ? launch_bwd_window<128, true, __nv_bfloat16>(p, w, s) : launch_bwd_window<128, true, __half>(p, w, s);
-    return bf ? launch_bwd_window<128, false, __nv_bfloat16>(p, w, s) : launch_bwd_window<128, false, __half>(p, w, s);
-  }
-  if (kt) return bf ? launch_bwd_window<64, true, __nv_bfloat16>(p, w, s) : launch_bwd_window<64, true, __half>(p, w, s);
-  return bf ? launch_bwd_window<64, false, __nv_bfloat16>(p, w, s) : launch_bwd_window<64, false, __half>(p, w, s);
+  if (int e = sab::check_window(window_left, window_right, is_causal, Sq, Skv)) return e;
+  const sab::Window w{window_left, window_right};
+  return bwd_dense(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, k_mean, dq, dk, dv, workspace, dtype, B, Hq, Hkv, Sq, Skv, D,
+                   q8_stride_b, q8_stride_h, q8_stride_s, k8_stride_b, k8_stride_h, k8_stride_s, q_stride_b, q_stride_h, q_stride_s,
+                   k_stride_b, k_stride_h, k_stride_s, v_stride_b, v_stride_h, v_stride_s, o_stride_b, o_stride_h, o_stride_s,
+                   do_stride_b, do_stride_h, do_stride_s, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale, &w, nullptr, nullptr,
+                   nullptr, stream);
 }
 
 // sab_qk_int8_attn_bwd_varlen_seq and, with a window w or a block mask bm (already checked), sab_qk_int8_attn_bwd_varlen_window /
@@ -1029,12 +1029,8 @@ static int bwd_varlen_seq(const int8_t* q_int8, const int8_t* k_int8, const floa
                           const int32_t* cu_k_scale, int max_seqlen_q, int max_seqlen_k, int is_causal, int q_gran, int k_gran,
                           float sm_scale, const sab::Window* w, const sab::BlockMask* bm, void* stream) {
   using namespace sab;
-  SAB_REQUIRE(q_int8 && k_int8 && q_scale && k_scale && q && k && v && o && dout && lse && dq && dk && dv && workspace,
-              SAB_ERR_INVALID, "null tensor pointer");
-  SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
-  SAB_REQUIRE(dtype == SAB_DTYPE_FP16 || dtype == SAB_DTYPE_BF16, SAB_ERR_UNSUPPORTED, "dtype must be fp16 or bf16");
-  SAB_REQUIRE(nseq > 0 && Hq > 0 && Hkv > 0 && Tq > 0 && Tk > 0, SAB_ERR_INVALID, "bad sizes B=%d Hq=%d Hkv=%d Sq=%d Skv=%d", nseq, Hq, Hkv, Tq, Tk);
-  SAB_REQUIRE(Hq % Hkv == 0, SAB_ERR_INVALID, "num_qo_heads (%d) must be divisible by num_kv_heads (%d)", Hq, Hkv);
+  if (int e = check_bwd_args(q_int8, k_int8, q_scale, k_scale, q, k, v, o, dout, lse, dq, dk, dv, workspace, dtype, nseq, Hq, Hkv, Tq, Tk, D))
+    return e;
   SAB_REQUIRE((q_gran == SAB_GRAN_PER_WARP || q_gran == SAB_GRAN_PER_THREAD) && (k_gran == SAB_GRAN_PER_WARP || k_gran == SAB_GRAN_PER_THREAD),
               SAB_ERR_INVALID, "q_gran / k_gran must be SAB_GRAN_PER_WARP or SAB_GRAN_PER_THREAD (got %d, %d)", q_gran, k_gran);
   SAB_REQUIRE(cu_seqlens_q && cu_seqlens_k && cu_q_scale && cu_k_scale && max_seqlen_q > 0 && max_seqlen_k > 0, SAB_ERR_INVALID,

@@ -91,6 +91,12 @@ __device__ __forceinline__ void mbar_wait_wd(uint64_t* bar, uint32_t parity) {
 #endif
 }
 
+// ---- attention mask of the masked entries (sab_qk_int8_sv_f16_attn_masked / sab_qk_int8_attn_bwd_masked): AttnParams::mask,
+// mask_kind and the mask_s* strides
+struct MaskArgs {
+  const void* ptr; int kind; int64_t sb, sh, sm, sn;
+};
+
 // ---- block-sparse attention (sab_qk_int8_sv_f8_attn_blocksparse / sab_qk_int8_attn_bwd_blocksparse).  A kernel argument, not an
 // AttnParams field, so the parameter offsets of the other kernels do not move.
 struct BlockMask {

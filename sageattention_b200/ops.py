@@ -4,6 +4,7 @@ reference: ops mutate pre-allocated outputs and have fake impls so they trace un
 PyTorch is plumbing here: it owns device memory and the current stream; every op body is a single
 call into libsageattn_b200.so through ctypes with raw pointers, sizes and strides.
 """
+import math
 from typing import Optional
 import torch
 
@@ -376,13 +377,30 @@ def _(query, key, value, output, query_scale, key_scale, value_scale, cu_seqlens
 
 
 # ----------------------------------------------------------------------------------------------- backward
-def _check_bwd_operands(q_int8, k_int8, q, k, o, dout):
-    """The kernels read o and dout at q's sizes as 16-bit words, and q_int8 / k_int8 at q's / k's sizes as bytes: a smaller
-    tensor would be read out of bounds, another dtype as the wrong words."""
+def _bwd_operands(q_int8, k_int8, q, k, v, o, dout, lse, k_mean, dq, dk, dv, tensor_layout, lse_shape, k_mean_shape, k_mean_label):
+    """The operand checks of every backward op.  The kernels read o and dout at q's sizes as 16-bit words, and q_int8 / k_int8 at
+    q's / k's sizes as bytes: a smaller tensor would be read out of bounds, another dtype as the wrong words.  tensor_layout None:
+    packed [T,H,D] tensors and lse_shape (Hq, Tq), else lse_shape (B, Hq, Sq).  k_mean_label: the element count of k_mean_shape
+    as the message names it.  Returns the (b, h, s) strides ((t, h) packed) of q_int8, k_int8, q, k, v, o, dout, k_mean reshaped
+    to k_mean_shape and the delta workspace."""
+    for x, y in ((dq, q), (dk, k), (dv, v)):
+        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
     for name, t in (("o", o), ("dout", dout)):
         assert t.shape == q.shape and t.dtype == q.dtype, f"{name} must have q's shape and dtype"
     for name, t, ref in (("q_int8", q_int8, q), ("k_int8", k_int8, k)):
         assert t.shape == ref.shape and t.dtype == torch.int8, f"{name} must be int8 with the shape of {name[0]}"
+    packed = tensor_layout is None
+    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == lse_shape, \
+        f"lse must be {'[Hq,Tq]' if packed else '[B,Hq,Sq]'} fp32"
+    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout)
+               for s in ((t.stride(0), t.stride(1)) if packed else _bhs_strides(t, tensor_layout))]
+    if k_mean is not None:
+        assert k_mean.numel() == math.prod(k_mean_shape) and k_mean.dtype == k.dtype, \
+            f"k_mean must have {k_mean_label} elements of k's dtype"
+        k_mean = k_mean.reshape(k_mean_shape).contiguous()
+    ws_shape = (1, *lse_shape) if packed else lse_shape
+    ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(*ws_shape), dtype=torch.uint8, device=q.device)
+    return strides, k_mean, ws
 
 
 @torch.library.custom_op("sageattention_b200::qk_int8_attn_bwd", mutates_args=("dq", "dk", "dv"), device_types="cuda")
@@ -396,16 +414,9 @@ def qk_int8_attn_bwd(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale: torch.
     with B*Hkv*D elements, k's dtype; None without smoothing).  dq / dk / dv must have the strides of q / k / v."""
     B, Hq, Sq, D = _bhsd(q, tensor_layout)
     _, Hkv, Skv, _ = _bhsd(k, tensor_layout)
-    for x, y in ((dq, q), (dk, k), (dv, v)):
-        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
-    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
-    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (B, Hq, Sq), "lse must be [B,Hq,Sq] fp32"
-    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in _bhs_strides(t, tensor_layout)]
-    if k_mean is not None:
-        assert k_mean.numel() == B * Hkv * D and k_mean.dtype == k.dtype, "k_mean must have B*Hkv*D elements of k's dtype"
-        k_mean = k_mean.reshape(B, Hkv, D).contiguous()
+    strides, k_mean, ws = _bwd_operands(q_int8, k_int8, q, k, v, o, dout, lse, k_mean, dq, dk, dv, tensor_layout, (B, Hq, Sq),
+                                        (B, Hkv, D), "B*Hkv*D")
     with torch.cuda.device(q.device):
-        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(B, Hq, Sq), dtype=torch.uint8, device=q.device)
         check(lib().sab_qk_int8_attn_bwd(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(), k_scale.data_ptr(), q.data_ptr(),
                                          k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(), lse.data_ptr(), _ptr(k_mean), dq.data_ptr(),
                                          dk.data_ptr(), dv.data_ptr(), ws.data_ptr(), _dt(q), B, Hq, Hkv, Sq, Skv, D, *strides,
@@ -430,22 +441,15 @@ def qk_int8_attn_bwd_masked(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale:
     ln2 * dS."""
     B, Hq, Sq, D = _bhsd(q, tensor_layout)
     _, Hkv, Skv, _ = _bhsd(k, tensor_layout)
-    for x, y in ((dq, q), (dk, k), (dv, v)):
-        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
-    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
-    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (B, Hq, Sq), "lse must be [B,Hq,Sq] fp32"
+    strides, k_mean, ws = _bwd_operands(q_int8, k_int8, q, k, v, o, dout, lse, k_mean, dq, dk, dv, tensor_layout, (B, Hq, Sq),
+                                        (B, Hkv, D), "B*Hkv*D")
     assert attn_mask.dim() == 4 and tuple(attn_mask.shape) == (B, Hq, Sq, Skv), "attn_mask must be expanded to [B,Hq,Sq,Skv]"
     kind = SAB_MASK_BOOL if attn_mask.dtype == torch.bool else SAB_MASK_BIAS
     assert kind == SAB_MASK_BOOL or attn_mask.dtype == q.dtype, "attn_mask must be bool or the q dtype"
     if dbias is not None:
         assert dbias.dtype == attn_mask.dtype and dbias.is_contiguous() and tuple(dbias.shape) == (B, Hq, Sq, Skv), \
             "dbias must be a contiguous [B,Hq,Sq,Skv] tensor of the mask dtype"
-    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in _bhs_strides(t, tensor_layout)]
-    if k_mean is not None:
-        assert k_mean.numel() == B * Hkv * D and k_mean.dtype == k.dtype, "k_mean must have B*Hkv*D elements of k's dtype"
-        k_mean = k_mean.reshape(B, Hkv, D).contiguous()
     with torch.cuda.device(q.device):
-        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(B, Hq, Sq), dtype=torch.uint8, device=q.device)
         check(lib().sab_qk_int8_attn_bwd_masked(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(), k_scale.data_ptr(),
                                                 q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(), lse.data_ptr(),
                                                 _ptr(k_mean), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), ws.data_ptr(), _dt(q), B, Hq,
@@ -469,17 +473,10 @@ def qk_int8_attn_bwd_blocksparse(q_int8: torch.Tensor, k_int8: torch.Tensor, q_s
     qk_int8_attn_bwd plus the block mask view the forward received (qk_int8_sv_f8_attn_blocksparse)."""
     B, Hq, Sq, D = _bhsd(q, tensor_layout)
     _, Hkv, Skv, _ = _bhsd(k, tensor_layout)
-    for x, y in ((dq, q), (dk, k), (dv, v)):
-        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
-    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
-    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (B, Hq, Sq), "lse must be [B,Hq,Sq] fp32"
+    strides, k_mean, ws = _bwd_operands(q_int8, k_int8, q, k, v, o, dout, lse, k_mean, dq, dk, dv, tensor_layout, (B, Hq, Sq),
+                                        (B, Hkv, D), "B*Hkv*D")
     mask = _block_mask_args(block_mask, B, Hq, Sq, Skv)
-    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in _bhs_strides(t, tensor_layout)]
-    if k_mean is not None:
-        assert k_mean.numel() == B * Hkv * D and k_mean.dtype == k.dtype, "k_mean must have B*Hkv*D elements of k's dtype"
-        k_mean = k_mean.reshape(B, Hkv, D).contiguous()
     with torch.cuda.device(q.device):
-        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(B, Hq, Sq), dtype=torch.uint8, device=q.device)
         check(lib().sab_qk_int8_attn_bwd_blocksparse(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(), k_scale.data_ptr(),
                                                      q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(),
                                                      lse.data_ptr(), _ptr(k_mean), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
@@ -503,16 +500,9 @@ def qk_int8_attn_bwd_window(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale:
     qk_int8_attn_bwd plus the window the forward received (qk_int8_sv_f8_attn_window)."""
     B, Hq, Sq, D = _bhsd(q, tensor_layout)
     _, Hkv, Skv, _ = _bhsd(k, tensor_layout)
-    for x, y in ((dq, q), (dk, k), (dv, v)):
-        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
-    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
-    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (B, Hq, Sq), "lse must be [B,Hq,Sq] fp32"
-    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in _bhs_strides(t, tensor_layout)]
-    if k_mean is not None:
-        assert k_mean.numel() == B * Hkv * D and k_mean.dtype == k.dtype, "k_mean must have B*Hkv*D elements of k's dtype"
-        k_mean = k_mean.reshape(B, Hkv, D).contiguous()
+    strides, k_mean, ws = _bwd_operands(q_int8, k_int8, q, k, v, o, dout, lse, k_mean, dq, dk, dv, tensor_layout, (B, Hq, Sq),
+                                        (B, Hkv, D), "B*Hkv*D")
     with torch.cuda.device(q.device):
-        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(B, Hq, Sq), dtype=torch.uint8, device=q.device)
         check(lib().sab_qk_int8_attn_bwd_window(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(), k_scale.data_ptr(),
                                                 q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(),
                                                 lse.data_ptr(), _ptr(k_mean), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
@@ -539,16 +529,9 @@ def qk_int8_attn_bwd_varlen(q_int8: torch.Tensor, k_int8: torch.Tensor, q_scale:
     smoothing).  dq / dk / dv must have the strides of q / k / v; rows past cu_seqlens_*[-1] are not written."""
     Tq, Hq, D = q.shape
     Tk, Hkv, _ = k.shape
-    for x, y in ((dq, q), (dk, k), (dv, v)):
-        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
-    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
-    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (Hq, Tq), "lse must be [Hq,Tq] fp32"
-    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in (t.stride(0), t.stride(1))]
-    if k_mean is not None:
-        assert k_mean.numel() == Hkv * D and k_mean.dtype == k.dtype, "k_mean must have Hkv*D elements of k's dtype"
-        k_mean = k_mean.reshape(Hkv, D).contiguous()
+    strides, k_mean, ws = _bwd_operands(q_int8, k_int8, q, k, v, o, dout, lse, k_mean, dq, dk, dv, None, (Hq, Tq), (Hkv, D),
+                                        "Hkv*D")
     with torch.cuda.device(q.device):
-        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(1, Hq, Tq), dtype=torch.uint8, device=q.device)
         check(lib().sab_qk_int8_attn_bwd_varlen(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(), k_scale.data_ptr(),
                                                 q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(), lse.data_ptr(),
                                                 _ptr(k_mean), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), ws.data_ptr(), _dt(q),
@@ -757,16 +740,9 @@ def qk_int8_attn_bwd_varlen_seq(q_int8: torch.Tensor, k_int8: torch.Tensor, q_sc
     Tq, Hq, D = q.shape
     Tk, Hkv, _ = k.shape
     nseq = cu_seqlens_q.numel() - 1
-    for x, y in ((dq, q), (dk, k), (dv, v)):
-        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
-    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
-    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (Hq, Tq), "lse must be [Hq,Tq] fp32"
-    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in (t.stride(0), t.stride(1))]
-    if k_mean is not None:
-        assert k_mean.numel() == nseq * Hkv * D and k_mean.dtype == k.dtype, "k_mean must have nseq*Hkv*D elements of k's dtype"
-        k_mean = k_mean.reshape(nseq, Hkv, D).contiguous()
+    strides, k_mean, ws = _bwd_operands(q_int8, k_int8, q, k, v, o, dout, lse, k_mean, dq, dk, dv, None, (Hq, Tq), (nseq, Hkv, D),
+                                        "nseq*Hkv*D")
     with torch.cuda.device(q.device):
-        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(1, Hq, Tq), dtype=torch.uint8, device=q.device)
         check(lib().sab_qk_int8_attn_bwd_varlen_seq(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(), k_scale.data_ptr(),
                                                     q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(),
                                                     lse.data_ptr(), _ptr(k_mean), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
@@ -825,16 +801,9 @@ def qk_int8_attn_bwd_varlen_window(q_int8: torch.Tensor, k_int8: torch.Tensor, q
     Tq, Hq, D = q.shape
     Tk, Hkv, _ = k.shape
     nseq = cu_seqlens_q.numel() - 1
-    for x, y in ((dq, q), (dk, k), (dv, v)):
-        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
-    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
-    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (Hq, Tq), "lse must be [Hq,Tq] fp32"
-    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in (t.stride(0), t.stride(1))]
-    if k_mean is not None:
-        assert k_mean.numel() == nseq * Hkv * D and k_mean.dtype == k.dtype, "k_mean must have nseq*Hkv*D elements of k's dtype"
-        k_mean = k_mean.reshape(nseq, Hkv, D).contiguous()
+    strides, k_mean, ws = _bwd_operands(q_int8, k_int8, q, k, v, o, dout, lse, k_mean, dq, dk, dv, None, (Hq, Tq), (nseq, Hkv, D),
+                                        "nseq*Hkv*D")
     with torch.cuda.device(q.device):
-        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(1, Hq, Tq), dtype=torch.uint8, device=q.device)
         check(lib().sab_qk_int8_attn_bwd_varlen_window(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(), k_scale.data_ptr(),
                                                        q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), dout.data_ptr(),
                                                        lse.data_ptr(), _ptr(k_mean), dq.data_ptr(), dk.data_ptr(), dv.data_ptr(),
@@ -899,17 +868,10 @@ def qk_int8_attn_bwd_varlen_blocksparse(q_int8: torch.Tensor, k_int8: torch.Tens
     Tq, Hq, D = q.shape
     Tk, Hkv, _ = k.shape
     nseq = cu_seqlens_q.numel() - 1
-    for x, y in ((dq, q), (dk, k), (dv, v)):
-        assert x.stride() == y.stride() and x.dtype == y.dtype, "dq / dk / dv must have the strides and dtype of q / k / v"
-    _check_bwd_operands(q_int8, k_int8, q, k, o, dout)
-    assert lse.dtype == torch.float32 and lse.is_contiguous() and tuple(lse.shape) == (Hq, Tq), "lse must be [Hq,Tq] fp32"
+    strides, k_mean, ws = _bwd_operands(q_int8, k_int8, q, k, v, o, dout, lse, k_mean, dq, dk, dv, None, (Hq, Tq), (nseq, Hkv, D),
+                                        "nseq*Hkv*D")
     mask = _block_mask_args(block_mask, nseq, Hq, max_seqlen_q, max_seqlen_k)
-    strides = [s for t in (q_int8, k_int8, q, k, v, o, dout) for s in (t.stride(0), t.stride(1))]
-    if k_mean is not None:
-        assert k_mean.numel() == nseq * Hkv * D and k_mean.dtype == k.dtype, "k_mean must have nseq*Hkv*D elements of k's dtype"
-        k_mean = k_mean.reshape(nseq, Hkv, D).contiguous()
     with torch.cuda.device(q.device):
-        ws = torch.empty(lib().sab_attn_bwd_workspace_bytes(1, Hq, Tq), dtype=torch.uint8, device=q.device)
         check(lib().sab_qk_int8_attn_bwd_varlen_blocksparse(q_int8.data_ptr(), k_int8.data_ptr(), q_scale.data_ptr(),
                                                             k_scale.data_ptr(), q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
                                                             dout.data_ptr(), lse.data_ptr(), _ptr(k_mean), dq.data_ptr(), dk.data_ptr(),

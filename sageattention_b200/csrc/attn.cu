@@ -845,25 +845,17 @@ static int launch_attn_blocksparse(const CUtensorMap& tq, const CUtensorMap& tk,
 
 }  // namespace sab
 
-// block mask of the block-sparse entry point, handed to attn_entry by sab_qk_int8_sv_f8_attn_blocksparse (same thread)
-static thread_local const sab::BlockMask* tl_block_mask = nullptr;
-// with tl_block_mask, set by sab_qk_int8_sv_f8_attn_varlen_blocksparse (same thread): max_seqlen_k, which sizes each CTA's list of
-// visible key blocks (the packed Skv is the total key count)
-static thread_local int tl_block_mask_max_k = 0;
-// window of the sliding-window entry point, handed to attn_entry by sab_qk_int8_sv_f8_attn_window (same thread)
-static thread_local const sab::Window* tl_window = nullptr;
-// set by sab_qk_int8_sv_f8_attn_varlen (same thread): v_scale / v_mean are per sequence
-static thread_local bool tl_seq_v = false;
-// attention mask of the masked entry point, handed to attn_entry by sab_qk_int8_sv_f16_attn_masked (same thread)
-static thread_local const sab::MaskArgs* tl_mask = nullptr;
-// segment flags of the fused sequence-parallel entry point, handed to attn_entry by sab_qk_int8_sv_f8_attn_sp (same thread)
+// segment flags of the fused sequence-parallel entry point (sab_qk_int8_sv_f8_attn_sp)
 struct SegArgs {
   const uint32_t* flags;
   uint32_t epoch;
   int heads_per_flag;
 };
-static thread_local const SegArgs* tl_seg = nullptr;
 
+// Every forward entry.  The variant, each null / false when absent: a window (sab_qk_int8_sv_f8_attn_window and, through
+// attn_varlen_seq, the packed window and bottom-right forms); a block mask bm, already checked (the block-sparse entries), with
+// bm_max_k the packed max_seqlen_k; an attention mask m (sab_qk_int8_sv_f16_attn_masked); segment flags seg
+// (sab_qk_int8_sv_f8_attn_sp); seq_v: v_scale / v_mean are per sequence (attn_varlen_seq).
 static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out,
                                       float* lse, const float* q_scale, const float* k_scale, const float* v_scale,
                                       const float* v_mean, int out_dtype, int B, int Hq, int Hkv, int Sq, int Skv,
@@ -874,7 +866,8 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
                                       const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
                                       const int32_t* cu_pad_v, const int32_t* cu_q_scale, const int32_t* cu_k_scale,
                                       int max_seqlen_q, int causal_q_offset, int kv_seg_len, int32_t* debug_dump,
-                                      void* stream) {
+                                      void* stream, const sab::Window* window, const sab::BlockMask* bm, int bm_max_k,
+                                      const sab::MaskArgs* m, const SegArgs* seg, bool seq_v) {
   using namespace sab;
   SAB_REQUIRE(q_int8 && k_int8 && v_fp8 && out && q_scale && k_scale, SAB_ERR_INVALID, "null tensor pointer");
   SAB_REQUIRE(D == 64 || D == 128, SAB_ERR_UNSUPPORTED, "Unsupported head dim: %d (64 or 128 after padding)", D);
@@ -897,8 +890,7 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
   if (st != SAB_OK) return st;
 
   // the dense INT8+FP8 kernel at D = 128 (also sequence-parallel): three consumer warpgroups unless SAB_ATTN_CONSUMERS=2
-  const int nc = (D == 128 && !pv16 && !varlen && tl_mask == nullptr && tl_block_mask == nullptr && tl_window == nullptr &&
-                  !tl_seq_v) ? dense_consumers() : 2;
+  const int nc = (D == 128 && !pv16 && !varlen && !m && !bm && !window && !seq_v) ? dense_consumers() : 2;
   const uint32_t qbox = uint32_t(nc) * 64;   // Q rows per CTA
   CUtensorMap tq, tk, tv;
   const int swqk = D == 128 ? 128 : 64;
@@ -944,14 +936,14 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   const bool kt = k_gran == SAB_GRAN_PER_THREAD;
   const bool bf = out_dtype == SAB_DTYPE_BF16;
-  if (tl_mask != nullptr) {
+  if (m != nullptr) {
     // attn_qk_int8_per_block.py:33-52 (non-causal kernel only; sageattention/core.py:310-325 asserts mask is None when causal)
-    SAB_REQUIRE(pv16 && !kt && !varlen && !is_causal, SAB_ERR_UNSUPPORTED,
+    SAB_REQUIRE(!kt, SAB_ERR_UNSUPPORTED,
                 "attn_mask is supported by the dense non-causal fp16-PV path with per-block / per-warp K scales only");
-    SAB_REQUIRE(tl_mask->ptr != nullptr && (tl_mask->kind == SAB_MASK_BOOL || tl_mask->kind == SAB_MASK_BIAS), SAB_ERR_INVALID,
-                "attn_mask: null pointer or unknown kind %d", tl_mask->kind);
-    p.mask = tl_mask->ptr; p.mask_kind = tl_mask->kind;
-    p.mask_sb = tl_mask->sb; p.mask_sh = tl_mask->sh; p.mask_sm = tl_mask->sm; p.mask_sn = tl_mask->sn;
+    SAB_REQUIRE(m->ptr != nullptr && (m->kind == SAB_MASK_BOOL || m->kind == SAB_MASK_BIAS), SAB_ERR_INVALID,
+                "attn_mask: null pointer or unknown kind %d", m->kind);
+    p.mask = m->ptr; p.mask_kind = m->kind;
+    p.mask_sb = m->sb; p.mask_sh = m->sh; p.mask_sm = m->sm; p.mask_sn = m->sn;
     if (D == 128) {
       if (bf) return launch_attn<128, false, __nv_bfloat16, true, true>(tq, tk, tv, p, grid, s);
       return launch_attn<128, false, __half, true, true>(tq, tk, tv, p, grid, s);
@@ -959,20 +951,18 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
     if (bf) return launch_attn<64, false, __nv_bfloat16, true, true>(tq, tk, tv, p, grid, s);
     return launch_attn<64, false, __half, true, true>(tq, tk, tv, p, grid, s);
   }
-  if (tl_seg != nullptr) {
-    SAB_REQUIRE(!pv16 && kv_seg_len > 0 && !is_causal, SAB_ERR_UNSUPPORTED,
+  if (seg != nullptr) {
+    SAB_REQUIRE(kv_seg_len > 0, SAB_ERR_UNSUPPORTED,
                 "segment flags need the sequence-parallel INT8/FP8 form (kv_seg_len > 0), non-causal");
-    SAB_REQUIRE(tl_seg->flags != nullptr && tl_seg->heads_per_flag > 0 && Hkv % tl_seg->heads_per_flag == 0, SAB_ERR_INVALID,
-                "segment flags: null pointer or heads_per_flag (%d) does not divide num_kv_heads (%d)", tl_seg->heads_per_flag, Hkv);
-    p.seg_flags = tl_seg->flags; p.seg_epoch = tl_seg->epoch; p.seg_heads = tl_seg->heads_per_flag;   // polled by the producer
+    SAB_REQUIRE(seg->flags != nullptr && seg->heads_per_flag > 0 && Hkv % seg->heads_per_flag == 0, SAB_ERR_INVALID,
+                "segment flags: null pointer or heads_per_flag (%d) does not divide num_kv_heads (%d)", seg->heads_per_flag, Hkv);
+    p.seg_flags = seg->flags; p.seg_epoch = seg->epoch; p.seg_heads = seg->heads_per_flag;   // polled by the producer
   }
-  if (tl_block_mask != nullptr) {
-    SAB_REQUIRE(!pv16 && (!varlen || tl_seq_v) && kv_seg_len == 0 && causal_q_offset == 0, SAB_ERR_UNSUPPORTED,
-                "the block mask is supported by the dense and the packed (per-sequence) single-GPU INT8/FP8 paths only");
-    p.mask = tl_block_mask->ptr;
-    p.mask_sb = tl_block_mask->sb; p.mask_sh = tl_block_mask->sh; p.mask_sm = tl_block_mask->sqb; p.mask_sn = tl_block_mask->skb;
-    if (tl_seq_v) {
-      const int mk = tl_block_mask_max_k;
+  if (bm != nullptr) {
+    p.mask = bm->ptr;
+    p.mask_sb = bm->sb; p.mask_sh = bm->sh; p.mask_sm = bm->sqb; p.mask_sn = bm->skb;
+    if (seq_v) {
+      const int mk = bm_max_k;
       if (D == 128) {
         if (kt) return bf ? launch_attn_blocksparse<128, true, __nv_bfloat16, true>(tq, tk, tv, p, mk, grid, s)
                           : launch_attn_blocksparse<128, true, __half, true>(tq, tk, tv, p, mk, grid, s);
@@ -995,12 +985,9 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
     return bf ? launch_attn_blocksparse<64, false, __nv_bfloat16>(tq, tk, tv, p, Skv, grid, s)
               : launch_attn_blocksparse<64, false, __half>(tq, tk, tv, p, Skv, grid, s);
   }
-  if (tl_window != nullptr) {
-    SAB_REQUIRE(!pv16 && (!varlen || tl_seq_v) && kv_seg_len == 0 && causal_q_offset == 0, SAB_ERR_UNSUPPORTED,
-                "the window is supported by the dense and the packed (per-sequence) single-GPU INT8/FP8 paths only");
-    const Window w = *tl_window;
-    if (tl_seq_v && w.right == kWindowBottomRight) {
-      SAB_REQUIRE(!is_causal, SAB_ERR_INVALID, "the bottom-right causal form takes is_causal = 0");
+  if (window != nullptr) {
+    const Window w = *window;
+    if (seq_v && w.right == kWindowBottomRight) {
       if (D == 128) {
         if (kt) return bf ? launch_attn_window<128, true, __nv_bfloat16, true, true>(tq, tk, tv, p, w, grid, s)
                           : launch_attn_window<128, true, __half, true, true>(tq, tk, tv, p, w, grid, s);
@@ -1012,7 +999,7 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
       return bf ? launch_attn_window<64, false, __nv_bfloat16, true, true>(tq, tk, tv, p, w, grid, s)
                 : launch_attn_window<64, false, __half, true, true>(tq, tk, tv, p, w, grid, s);
     }
-    if (tl_seq_v) {
+    if (seq_v) {
       if (D == 128) {
         if (kt) return bf ? launch_attn_window<128, true, __nv_bfloat16, true>(tq, tk, tv, p, w, grid, s)
                           : launch_attn_window<128, true, __half, true>(tq, tk, tv, p, w, grid, s);
@@ -1035,9 +1022,7 @@ static int attn_entry(int pv16, const int8_t* q_int8, const int8_t* k_int8, cons
     return bf ? launch_attn_window<64, false, __nv_bfloat16>(tq, tk, tv, p, w, grid, s)
               : launch_attn_window<64, false, __half>(tq, tk, tv, p, w, grid, s);
   }
-  if (tl_seq_v) {
-    SAB_REQUIRE(!pv16 && varlen && kv_seg_len == 0 && causal_q_offset == 0, SAB_ERR_UNSUPPORTED,
-                "per-sequence V statistics need the packed single-GPU INT8/FP8 path");
+  if (seq_v) {
     if (D == 128) {
       if (kt) return bf ? launch_attn_seqv<128, true, __nv_bfloat16>(tq, tk, tv, p, grid, s)
                         : launch_attn_seqv<128, true, __half>(tq, tk, tv, p, grid, s);
@@ -1078,7 +1063,8 @@ extern "C" int sab_qk_int8_sv_f8_attn(const int8_t* q_int8, const int8_t* k_int8
   return attn_entry(0, q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, B, Hq, Hkv, Sq, Skv, D,
                     q_stride_b, q_stride_h, q_stride_s, k_stride_b, k_stride_h, k_stride_s, v_s_pad, o_stride_b, o_stride_h,
                     o_stride_s, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v,
-                    cu_q_scale, cu_k_scale, max_seqlen_q, causal_q_offset, kv_seg_len, debug_dump, stream);
+                    cu_q_scale, cu_k_scale, max_seqlen_q, causal_q_offset, kv_seg_len, debug_dump, stream, nullptr, nullptr, 0,
+                    nullptr, nullptr, false);
 }
 
 extern "C" int sab_qk_int8_sv_f8_attn_sp(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out,
@@ -1089,13 +1075,10 @@ extern "C" int sab_qk_int8_sv_f8_attn_sp(const int8_t* q_int8, const int8_t* k_i
                                          int64_t o_stride_s, int q_gran, int k_gran, float sm_scale, int kv_seg_len,
                                          const uint32_t* seg_flags, uint32_t seg_epoch, int heads_per_flag, void* stream) {
   const SegArgs a{seg_flags, seg_epoch, heads_per_flag};
-  tl_seg = &a;
-  const int st = attn_entry(0, q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, nullptr, out_dtype, B, Hq, Hkv, Sq, Skv,
-                            D, q_stride_b, q_stride_h, q_stride_s, k_stride_b, k_stride_h, k_stride_s, v_s_pad, o_stride_b,
-                            o_stride_h, o_stride_s, 0, q_gran, k_gran, sm_scale, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0,
-                            0, kv_seg_len, nullptr, stream);
-  tl_seg = nullptr;
-  return st;
+  return attn_entry(0, q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, nullptr, out_dtype, B, Hq, Hkv, Sq, Skv, D,
+                    q_stride_b, q_stride_h, q_stride_s, k_stride_b, k_stride_h, k_stride_s, v_s_pad, o_stride_b, o_stride_h,
+                    o_stride_s, 0, q_gran, k_gran, sm_scale, 0, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, kv_seg_len,
+                    nullptr, stream, nullptr, nullptr, 0, nullptr, &a, false);
 }
 
 extern "C" int sab_qk_int8_sv_f16_attn(const int8_t* q_int8, const int8_t* k_int8, const void* v_f16t, void* out, float* lse,
@@ -1109,7 +1092,8 @@ extern "C" int sab_qk_int8_sv_f16_attn(const int8_t* q_int8, const int8_t* k_int
   return attn_entry(1, q_int8, k_int8, reinterpret_cast<const uint8_t*>(v_f16t), out, lse, q_scale, k_scale, nullptr, nullptr,
                     out_dtype, B, Hq, Hkv, Sq, Skv, D, q_stride_b, q_stride_h, q_stride_s, k_stride_b, k_stride_h, k_stride_s,
                     v_s_pad, o_stride_b, o_stride_h, o_stride_s, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale,
-                    cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale, max_seqlen_q, 0, 0, nullptr, stream);
+                    cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale, max_seqlen_q, 0, 0, nullptr, stream, nullptr,
+                    nullptr, 0, nullptr, nullptr, false);
 }
 
 extern "C" int sab_qk_int8_sv_f16_attn_masked(const int8_t* q_int8, const int8_t* k_int8, const void* v_f16t, void* out, float* lse,
@@ -1121,13 +1105,10 @@ extern "C" int sab_qk_int8_sv_f16_attn_masked(const int8_t* q_int8, const int8_t
                                               int64_t mask_stride_b, int64_t mask_stride_h, int64_t mask_stride_m,
                                               int64_t mask_stride_n, void* stream) {
   const sab::MaskArgs m{attn_mask, mask_kind, mask_stride_b, mask_stride_h, mask_stride_m, mask_stride_n};
-  tl_mask = &m;
-  const int st = attn_entry(1, q_int8, k_int8, reinterpret_cast<const uint8_t*>(v_f16t), out, lse, q_scale, k_scale, nullptr,
-                            nullptr, out_dtype, B, Hq, Hkv, Sq, Skv, D, q_stride_b, q_stride_h, q_stride_s, k_stride_b,
-                            k_stride_h, k_stride_s, v_s_pad, o_stride_b, o_stride_h, o_stride_s, 0, q_gran, k_gran, sm_scale,
-                            fold_sm_scale, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0, nullptr, stream);
-  tl_mask = nullptr;
-  return st;
+  return attn_entry(1, q_int8, k_int8, reinterpret_cast<const uint8_t*>(v_f16t), out, lse, q_scale, k_scale, nullptr, nullptr,
+                    out_dtype, B, Hq, Hkv, Sq, Skv, D, q_stride_b, q_stride_h, q_stride_s, k_stride_b, k_stride_h, k_stride_s,
+                    v_s_pad, o_stride_b, o_stride_h, o_stride_s, 0, q_gran, k_gran, sm_scale, fold_sm_scale, nullptr, nullptr,
+                    nullptr, nullptr, nullptr, 0, 0, 0, nullptr, stream, nullptr, nullptr, 0, &m, nullptr, false);
 }
 
 extern "C" int sab_qk_int8_sv_f8_attn_blocksparse(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out,
@@ -1141,14 +1122,11 @@ extern "C" int sab_qk_int8_sv_f8_attn_blocksparse(const int8_t* q_int8, const in
                                                   int64_t mask_stride_qb, int64_t mask_stride_kb, void* stream) {
   if (int st = sab::check_block_mask(block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb, q_gran, is_causal, Sq, Skv))
     return st;
-  const sab::BlockMask m{block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb};
-  tl_block_mask = &m;
-  const int st = attn_entry(0, q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, B, Hq, Hkv, Sq, Skv, D,
-                            q_stride_b, q_stride_h, q_stride_s, k_stride_b, k_stride_h, k_stride_s, v_s_pad, o_stride_b, o_stride_h,
-                            o_stride_s, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale, nullptr, nullptr, nullptr, nullptr,
-                            nullptr, 0, 0, 0, nullptr, stream);
-  tl_block_mask = nullptr;
-  return st;
+  const sab::BlockMask bm{block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb};
+  return attn_entry(0, q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, B, Hq, Hkv, Sq, Skv, D,
+                    q_stride_b, q_stride_h, q_stride_s, k_stride_b, k_stride_h, k_stride_s, v_s_pad, o_stride_b, o_stride_h,
+                    o_stride_s, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale, nullptr, nullptr, nullptr, nullptr, nullptr, 0,
+                    0, 0, nullptr, stream, nullptr, &bm, 0, nullptr, nullptr, false);
 }
 
 extern "C" int sab_qk_int8_sv_f8_attn_window(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out, float* lse,
@@ -1160,13 +1138,32 @@ extern "C" int sab_qk_int8_sv_f8_attn_window(const int8_t* q_int8, const int8_t*
                                              int fold_sm_scale, int window_left, int window_right, void* stream) {
   if (int st = sab::check_window(window_left, window_right, is_causal, Sq, Skv)) return st;
   const sab::Window w{window_left, window_right};
-  tl_window = &w;
-  const int st = attn_entry(0, q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, B, Hq, Hkv, Sq, Skv, D,
-                            q_stride_b, q_stride_h, q_stride_s, k_stride_b, k_stride_h, k_stride_s, v_s_pad, o_stride_b, o_stride_h,
-                            o_stride_s, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale, nullptr, nullptr, nullptr, nullptr,
-                            nullptr, 0, 0, 0, nullptr, stream);
-  tl_window = nullptr;
-  return st;
+  return attn_entry(0, q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, B, Hq, Hkv, Sq, Skv, D,
+                    q_stride_b, q_stride_h, q_stride_s, k_stride_b, k_stride_h, k_stride_s, v_s_pad, o_stride_b, o_stride_h,
+                    o_stride_s, is_causal, q_gran, k_gran, sm_scale, fold_sm_scale, nullptr, nullptr, nullptr, nullptr, nullptr, 0,
+                    0, 0, nullptr, stream, &w, nullptr, 0, nullptr, nullptr, false);
+}
+
+// sab_qk_int8_sv_f8_attn_varlen and, with a window w or a block mask bm (already checked; bm_max_k: max_seqlen_k),
+// sab_qk_int8_sv_f8_attn_varlen_window / _varlen_bottom_right / _varlen_blocksparse
+static int attn_varlen_seq(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out, float* lse,
+                           const float* q_scale, const float* k_scale, const float* v_scale, const float* v_mean, int out_dtype,
+                           int nseq, int Hq, int Hkv, int Tq, int Tk, int D, int64_t q_stride_t, int64_t q_stride_h,
+                           int64_t k_stride_t, int64_t k_stride_h, int64_t v_t_pad, int64_t o_stride_t, int64_t o_stride_h,
+                           int is_causal, int q_gran, int k_gran, float sm_scale, const int32_t* cu_seqlens_q,
+                           const int32_t* cu_seqlens_k, const int32_t* cu_pad_v, const int32_t* cu_q_scale,
+                           const int32_t* cu_k_scale, int max_seqlen_q, const sab::Window* w, const sab::BlockMask* bm, int bm_max_k,
+                           void* stream) {
+  SAB_REQUIRE(q_gran == SAB_GRAN_PER_WARP || q_gran == SAB_GRAN_PER_THREAD, SAB_ERR_INVALID,
+              "q_gran must be SAB_GRAN_PER_WARP or SAB_GRAN_PER_THREAD (got %d)", q_gran);
+  SAB_REQUIRE(k_gran == SAB_GRAN_PER_WARP || k_gran == SAB_GRAN_PER_THREAD, SAB_ERR_INVALID,
+              "k_gran must be SAB_GRAN_PER_WARP or SAB_GRAN_PER_THREAD (got %d)", k_gran);
+  SAB_REQUIRE(v_scale != nullptr && cu_seqlens_q != nullptr && nseq > 0 && Tk > 0, SAB_ERR_INVALID,
+              "the packed INT8/FP8 form needs v_scale, cu_seqlens_q, nseq > 0 and Tk > 0");
+  return attn_entry(0, q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq, Hkv, Tq, Tk, D, 0,
+                    q_stride_h, q_stride_t, 0, k_stride_h, k_stride_t, v_t_pad, 0, o_stride_h, o_stride_t, is_causal, q_gran, k_gran,
+                    sm_scale, 0, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale, max_seqlen_q, 0, 0, nullptr, stream,
+                    w, bm, bm_max_k, nullptr, nullptr, true);
 }
 
 extern "C" int sab_qk_int8_sv_f8_attn_varlen(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out, float* lse,
@@ -1177,19 +1174,10 @@ extern "C" int sab_qk_int8_sv_f8_attn_varlen(const int8_t* q_int8, const int8_t*
                                              float sm_scale, const int32_t* cu_seqlens_q, const int32_t* cu_seqlens_k,
                                              const int32_t* cu_pad_v, const int32_t* cu_q_scale, const int32_t* cu_k_scale,
                                              int max_seqlen_q, void* stream) {
-  SAB_REQUIRE(q_gran == SAB_GRAN_PER_WARP || q_gran == SAB_GRAN_PER_THREAD, SAB_ERR_INVALID,
-              "q_gran must be SAB_GRAN_PER_WARP or SAB_GRAN_PER_THREAD (got %d)", q_gran);
-  SAB_REQUIRE(k_gran == SAB_GRAN_PER_WARP || k_gran == SAB_GRAN_PER_THREAD, SAB_ERR_INVALID,
-              "k_gran must be SAB_GRAN_PER_WARP or SAB_GRAN_PER_THREAD (got %d)", k_gran);
-  SAB_REQUIRE(v_scale != nullptr && cu_seqlens_q != nullptr && nseq > 0 && Tk > 0, SAB_ERR_INVALID,
-              "the packed INT8/FP8 form needs v_scale, cu_seqlens_q, nseq > 0 and Tk > 0");
-  tl_seq_v = true;
-  const int st = attn_entry(0, q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq, Hkv, Tq, Tk, D,
-                            0, q_stride_h, q_stride_t, 0, k_stride_h, k_stride_t, v_t_pad, 0, o_stride_h, o_stride_t, is_causal, q_gran,
-                            k_gran, sm_scale, 0, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale, max_seqlen_q, 0, 0,
-                            nullptr, stream);
-  tl_seq_v = false;
-  return st;
+  return attn_varlen_seq(q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq, Hkv, Tq, Tk, D,
+                         q_stride_t, q_stride_h, k_stride_t, k_stride_h, v_t_pad, o_stride_t, o_stride_h, is_causal, q_gran, k_gran,
+                         sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale, max_seqlen_q, nullptr, nullptr, 0,
+                         stream);
 }
 
 extern "C" int sab_qk_int8_sv_f8_attn_varlen_window(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out,
@@ -1206,13 +1194,9 @@ extern "C" int sab_qk_int8_sv_f8_attn_varlen_window(const int8_t* q_int8, const 
   SAB_REQUIRE(cu_seqlens_q && cu_seqlens_k && cu_pad_v && cu_q_scale && cu_k_scale && nseq > 0, SAB_ERR_INVALID,
               "the packed window needs cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale and nseq > 0");
   const sab::Window w{window_left, window_right};
-  tl_window = &w;
-  const int st = sab_qk_int8_sv_f8_attn_varlen(q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq,
-                                               Hkv, Tq, Tk, D, q_stride_t, q_stride_h, k_stride_t, k_stride_h, v_t_pad, o_stride_t,
-                                               o_stride_h, is_causal, q_gran, k_gran, sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v,
-                                               cu_q_scale, cu_k_scale, max_seqlen_q, stream);
-  tl_window = nullptr;
-  return st;
+  return attn_varlen_seq(q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq, Hkv, Tq, Tk, D,
+                         q_stride_t, q_stride_h, k_stride_t, k_stride_h, v_t_pad, o_stride_t, o_stride_h, is_causal, q_gran, k_gran,
+                         sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale, max_seqlen_q, &w, nullptr, 0, stream);
 }
 
 extern "C" int sab_qk_int8_sv_f8_attn_varlen_bottom_right(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out,
@@ -1226,20 +1210,12 @@ extern "C" int sab_qk_int8_sv_f8_attn_varlen_bottom_right(const int8_t* q_int8, 
                                                           const int32_t* cu_k_scale, int max_seqlen_q, void* stream) {
   SAB_REQUIRE(cu_seqlens_q && cu_seqlens_k && cu_pad_v && cu_q_scale && cu_k_scale && nseq > 0, SAB_ERR_INVALID,
               "the packed bottom-right form needs cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale and nseq > 0");
-  // non-causal has no alignment: the packed form itself
-  if (!is_causal)
-    return sab_qk_int8_sv_f8_attn_varlen(q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq, Hkv,
-                                         Tq, Tk, D, q_stride_t, q_stride_h, k_stride_t, k_stride_h, v_t_pad, o_stride_t, o_stride_h, 0,
-                                         q_gran, k_gran, sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale,
-                                         max_seqlen_q, stream);
+  // non-causal has no alignment: the packed form itself.  Causal: the bottom-right window, whose kernel takes is_causal = 0.
   const sab::Window w{-1, sab::kWindowBottomRight};
-  tl_window = &w;
-  const int st = sab_qk_int8_sv_f8_attn_varlen(q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq,
-                                               Hkv, Tq, Tk, D, q_stride_t, q_stride_h, k_stride_t, k_stride_h, v_t_pad, o_stride_t,
-                                               o_stride_h, 0, q_gran, k_gran, sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v,
-                                               cu_q_scale, cu_k_scale, max_seqlen_q, stream);
-  tl_window = nullptr;
-  return st;
+  return attn_varlen_seq(q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq, Hkv, Tq, Tk, D,
+                         q_stride_t, q_stride_h, k_stride_t, k_stride_h, v_t_pad, o_stride_t, o_stride_h, 0, q_gran, k_gran, sm_scale,
+                         cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale, max_seqlen_q, is_causal ? &w : nullptr, nullptr,
+                         0, stream);
 }
 
 extern "C" int sab_qk_int8_sv_f8_attn_varlen_blocksparse(const int8_t* q_int8, const int8_t* k_int8, const uint8_t* v_fp8, void* out,
@@ -1258,16 +1234,11 @@ extern "C" int sab_qk_int8_sv_f8_attn_varlen_blocksparse(const int8_t* q_int8, c
     return st;
   SAB_REQUIRE(cu_seqlens_q && cu_seqlens_k && cu_pad_v && cu_q_scale && cu_k_scale && nseq > 0, SAB_ERR_INVALID,
               "the packed block mask needs cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale and nseq > 0");
-  const sab::BlockMask m{block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb};
-  tl_block_mask = &m;
-  tl_block_mask_max_k = max_seqlen_k;
-  const int st = sab_qk_int8_sv_f8_attn_varlen(q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq,
-                                               Hkv, Tq, Tk, D, q_stride_t, q_stride_h, k_stride_t, k_stride_h, v_t_pad, o_stride_t,
-                                               o_stride_h, is_causal, q_gran, k_gran, sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v,
-                                               cu_q_scale, cu_k_scale, max_seqlen_q, stream);
-  tl_block_mask = nullptr;
-  tl_block_mask_max_k = 0;
-  return st;
+  const sab::BlockMask bm{block_mask, mask_stride_b, mask_stride_h, mask_stride_qb, mask_stride_kb};
+  return attn_varlen_seq(q_int8, k_int8, v_fp8, out, lse, q_scale, k_scale, v_scale, v_mean, out_dtype, nseq, Hq, Hkv, Tq, Tk, D,
+                         q_stride_t, q_stride_h, k_stride_t, k_stride_h, v_t_pad, o_stride_t, o_stride_h, is_causal, q_gran, k_gran,
+                         sm_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale, max_seqlen_q, nullptr, &bm,
+                         max_seqlen_k, stream);
 }
 
 #ifdef SAB_PHASE_CLOCKS

@@ -50,6 +50,12 @@ def _bhsd(t: torch.Tensor, tensor_layout: int):
     return t.size(0), t.size(2), t.size(1), t.size(3)
 
 
+def _lse(query: torch.Tensor, rows, return_lse: int) -> torch.Tensor:
+    """The lse a forward op returns, real and fake alike: fp32 of shape `rows` ((B, Hq, Sq) dense, (Hq, Tq) packed), or an
+    empty tensor when return_lse == 0."""
+    return query.new_empty(rows if return_lse else (0,), dtype=torch.float32)
+
+
 # ----------------------------------------------------------------------------------------------- K mean
 @torch.library.custom_op("sageattention_b200::k_mean", mutates_args=("mean",), device_types="cuda")
 def k_mean(k: torch.Tensor, mean: torch.Tensor, tensor_layout: int) -> None:
@@ -229,8 +235,7 @@ def qk_int8_sv_f8_attn(query: torch.Tensor, key: torch.Tensor, value: torch.Tens
     if kv_seg_len > 0:
         Skv = (key.size(0) // B) * kv_seg_len
     qs, ks, os_ = _bhs_strides(query, tensor_layout), _bhs_strides(key, tensor_layout), _bhs_strides(output, tensor_layout)
-    lse = torch.empty((B, Hq, Sq), dtype=torch.float32, device=query.device) if return_lse else \
-        torch.empty((0,), dtype=torch.float32, device=query.device)
+    lse = _lse(query, (B, Hq, Sq), return_lse)
     with torch.cuda.device(query.device):
         check(lib().sab_qk_int8_sv_f8_attn(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
                                            lse.data_ptr() if return_lse else None, query_scale.data_ptr(), key_scale.data_ptr(),
@@ -245,9 +250,7 @@ def qk_int8_sv_f8_attn(query: torch.Tensor, key: torch.Tensor, value: torch.Tens
 def _(query, key, value, output, query_scale, key_scale, value_scale, value_mean, tensor_layout, is_causal,
       q_quant_gran, k_quant_gran, sm_scale, fold_sm_scale, return_lse, causal_q_offset=0, kv_seg_len=0):
     B, Hq, Sq, D = _bhsd(query, tensor_layout)
-    if return_lse:
-        return torch.empty((B, Hq, Sq), dtype=torch.float32, device=query.device)
-    return torch.empty((0,), dtype=torch.float32, device=query.device)
+    return _lse(query, (B, Hq, Sq), return_lse)
 
 
 def _block_mask_args(block_mask: torch.Tensor, B: int, Hq: int, Sq: int, Skv: int):
@@ -271,8 +274,7 @@ def qk_int8_sv_f8_attn_blocksparse(query: torch.Tensor, key: torch.Tensor, value
     _, Hkv, Skv, _ = _bhsd(key, tensor_layout)
     mask = _block_mask_args(block_mask, B, Hq, Sq, Skv)
     qs, ks, os_ = _bhs_strides(query, tensor_layout), _bhs_strides(key, tensor_layout), _bhs_strides(output, tensor_layout)
-    lse = torch.empty((B, Hq, Sq), dtype=torch.float32, device=query.device) if return_lse else \
-        torch.empty((0,), dtype=torch.float32, device=query.device)
+    lse = _lse(query, (B, Hq, Sq), return_lse)
     with torch.cuda.device(query.device):
         check(lib().sab_qk_int8_sv_f8_attn_blocksparse(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
                                                        lse.data_ptr() if return_lse else None, query_scale.data_ptr(),
@@ -286,9 +288,7 @@ def qk_int8_sv_f8_attn_blocksparse(query: torch.Tensor, key: torch.Tensor, value
 def _(query, key, value, output, query_scale, key_scale, value_scale, value_mean, block_mask, tensor_layout, is_causal,
       q_quant_gran, k_quant_gran, sm_scale, fold_sm_scale, return_lse):
     B, Hq, Sq, D = _bhsd(query, tensor_layout)
-    if return_lse:
-        return torch.empty((B, Hq, Sq), dtype=torch.float32, device=query.device)
-    return torch.empty((0,), dtype=torch.float32, device=query.device)
+    return _lse(query, (B, Hq, Sq), return_lse)
 
 
 @torch.library.custom_op("sageattention_b200::qk_int8_sv_f8_attn_window", mutates_args=("output",), device_types="cuda")
@@ -303,8 +303,7 @@ def qk_int8_sv_f8_attn_window(query: torch.Tensor, key: torch.Tensor, value: tor
     B, Hq, Sq, D = _bhsd(query, tensor_layout)
     _, Hkv, Skv, _ = _bhsd(key, tensor_layout)
     qs, ks, os_ = _bhs_strides(query, tensor_layout), _bhs_strides(key, tensor_layout), _bhs_strides(output, tensor_layout)
-    lse = torch.empty((B, Hq, Sq), dtype=torch.float32, device=query.device) if return_lse else \
-        torch.empty((0,), dtype=torch.float32, device=query.device)
+    lse = _lse(query, (B, Hq, Sq), return_lse)
     with torch.cuda.device(query.device):
         check(lib().sab_qk_int8_sv_f8_attn_window(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
                                                   lse.data_ptr() if return_lse else None, query_scale.data_ptr(), key_scale.data_ptr(),
@@ -318,9 +317,7 @@ def qk_int8_sv_f8_attn_window(query: torch.Tensor, key: torch.Tensor, value: tor
 def _(query, key, value, output, query_scale, key_scale, value_scale, value_mean, window_left, window_right, tensor_layout,
       is_causal, q_quant_gran, k_quant_gran, sm_scale, fold_sm_scale, return_lse):
     B, Hq, Sq, D = _bhsd(query, tensor_layout)
-    if return_lse:
-        return torch.empty((B, Hq, Sq), dtype=torch.float32, device=query.device)
-    return torch.empty((0,), dtype=torch.float32, device=query.device)
+    return _lse(query, (B, Hq, Sq), return_lse)
 
 
 @torch.library.custom_op("sageattention_b200::qk_int8_sv_f8_attn_sp", mutates_args=("output",), device_types="cuda")
@@ -609,7 +606,7 @@ def qk_int8_sv_f8_attn_varlen_seq(query: torch.Tensor, key: torch.Tensor, value:
     the [Hq,Tq] log2 LSE when return_lse, else an empty tensor."""
     Tq, Hq, D = query.shape
     Tk, Hkv, _ = key.shape
-    lse = torch.empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32, device=query.device)
+    lse = _lse(query, (Hq, Tq), return_lse)
     with torch.cuda.device(query.device):
         check(lib().sab_qk_int8_sv_f8_attn_varlen(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
                                                   lse.data_ptr() if return_lse else None, query_scale.data_ptr(), key_scale.data_ptr(),
@@ -626,7 +623,7 @@ def qk_int8_sv_f8_attn_varlen_seq(query: torch.Tensor, key: torch.Tensor, value:
 def _(query, key, value, output, query_scale, key_scale, value_scale, value_mean, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale,
       cu_k_scale, max_seqlen_q, is_causal, q_quant_gran, k_quant_gran, sm_scale, return_lse):
     Tq, Hq, _ = query.shape
-    return query.new_empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32)
+    return _lse(query, (Hq, Tq), return_lse)
 
 
 # ----------------------------------------------------------------------------------------------- paged KV cache
@@ -706,7 +703,7 @@ def qk_int8_sv_f8_attn_varlen_bottom_right(query: torch.Tensor, key: torch.Tenso
     no visible key gets 0 and lse -inf."""
     Tq, Hq, D = query.shape
     Tk, Hkv, _ = key.shape
-    lse = torch.empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32, device=query.device)
+    lse = _lse(query, (Hq, Tq), return_lse)
     with torch.cuda.device(query.device):
         check(lib().sab_qk_int8_sv_f8_attn_varlen_bottom_right(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
                                                                lse.data_ptr() if return_lse else None, query_scale.data_ptr(),
@@ -724,7 +721,7 @@ def qk_int8_sv_f8_attn_varlen_bottom_right(query: torch.Tensor, key: torch.Tenso
 def _(query, key, value, output, query_scale, key_scale, value_scale, value_mean, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale,
       cu_k_scale, max_seqlen_q, is_causal, q_quant_gran, k_quant_gran, sm_scale, return_lse):
     Tq, Hq, _ = query.shape
-    return query.new_empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32)
+    return _lse(query, (Hq, Tq), return_lse)
 
 
 @torch.library.custom_op("sageattention_b200::qk_int8_attn_bwd_varlen_seq", mutates_args=("dq", "dk", "dv"), device_types="cuda")
@@ -769,7 +766,7 @@ def qk_int8_sv_f8_attn_varlen_window(query: torch.Tensor, key: torch.Tensor, val
     Returns the [Hq,Tq] log2 LSE when return_lse, else an empty tensor; a row with no visible key gets 0 and lse -inf."""
     Tq, Hq, D = query.shape
     Tk, Hkv, _ = key.shape
-    lse = torch.empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32, device=query.device)
+    lse = _lse(query, (Hq, Tq), return_lse)
     with torch.cuda.device(query.device):
         check(lib().sab_qk_int8_sv_f8_attn_varlen_window(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
                                                          lse.data_ptr() if return_lse else None, query_scale.data_ptr(),
@@ -786,7 +783,7 @@ def qk_int8_sv_f8_attn_varlen_window(query: torch.Tensor, key: torch.Tensor, val
 def _(query, key, value, output, query_scale, key_scale, value_scale, value_mean, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale,
       cu_k_scale, max_seqlen_q, window_left, window_right, is_causal, q_quant_gran, k_quant_gran, sm_scale, return_lse):
     Tq, Hq, _ = query.shape
-    return query.new_empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32)
+    return _lse(query, (Hq, Tq), return_lse)
 
 
 @torch.library.custom_op("sageattention_b200::qk_int8_attn_bwd_varlen_window", mutates_args=("dq", "dk", "dv"), device_types="cuda")
@@ -833,7 +830,7 @@ def qk_int8_sv_f8_attn_varlen_blocksparse(query: torch.Tensor, key: torch.Tensor
     Tk, Hkv, _ = key.shape
     nseq = cu_seqlens_q.numel() - 1
     mask = _block_mask_args(block_mask, nseq, Hq, max_seqlen_q, max_seqlen_k)
-    lse = torch.empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32, device=query.device)
+    lse = _lse(query, (Hq, Tq), return_lse)
     with torch.cuda.device(query.device):
         check(lib().sab_qk_int8_sv_f8_attn_varlen_blocksparse(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
                                                               lse.data_ptr() if return_lse else None, query_scale.data_ptr(),
@@ -851,7 +848,7 @@ def qk_int8_sv_f8_attn_varlen_blocksparse(query: torch.Tensor, key: torch.Tensor
 def _(query, key, value, output, query_scale, key_scale, value_scale, value_mean, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale,
       cu_k_scale, max_seqlen_q, max_seqlen_k, block_mask, is_causal, q_quant_gran, k_quant_gran, sm_scale, return_lse):
     Tq, Hq, _ = query.shape
-    return query.new_empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32)
+    return _lse(query, (Hq, Tq), return_lse)
 
 
 @torch.library.custom_op("sageattention_b200::qk_int8_attn_bwd_varlen_blocksparse", mutates_args=("dq", "dk", "dv"),
@@ -1029,8 +1026,7 @@ def qk_int8_sv_f16_attn(query: torch.Tensor, key: torch.Tensor, value: torch.Ten
     B, Hq, Sq, D = _bhsd(query, tensor_layout)
     _, Hkv, Skv, _ = _bhsd(key, tensor_layout)
     qs, ks, os_ = _bhs_strides(query, tensor_layout), _bhs_strides(key, tensor_layout), _bhs_strides(output, tensor_layout)
-    lse = torch.empty((B, Hq, Sq), dtype=torch.float32, device=query.device) if return_lse else \
-        torch.empty((0,), dtype=torch.float32, device=query.device)
+    lse = _lse(query, (B, Hq, Sq), return_lse)
     with torch.cuda.device(query.device):
         check(lib().sab_qk_int8_sv_f16_attn(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
                                             lse.data_ptr() if return_lse else None, query_scale.data_ptr(), key_scale.data_ptr(),
@@ -1044,9 +1040,7 @@ def qk_int8_sv_f16_attn(query: torch.Tensor, key: torch.Tensor, value: torch.Ten
 def _(query, key, value, output, query_scale, key_scale, tensor_layout, is_causal, q_quant_gran, k_quant_gran, sm_scale,
       fold_sm_scale, return_lse):
     B, Hq, Sq, D = _bhsd(query, tensor_layout)
-    if return_lse:
-        return torch.empty((B, Hq, Sq), dtype=torch.float32, device=query.device)
-    return torch.empty((0,), dtype=torch.float32, device=query.device)
+    return _lse(query, (B, Hq, Sq), return_lse)
 
 
 @torch.library.custom_op("sageattention_b200::qk_int8_sv_f16_attn_masked", mutates_args=("output",), device_types="cuda")
@@ -1062,8 +1056,7 @@ def qk_int8_sv_f16_attn_masked(query: torch.Tensor, key: torch.Tensor, value: to
     kind = SAB_MASK_BOOL if attn_mask.dtype == torch.bool else SAB_MASK_BIAS
     assert kind == SAB_MASK_BOOL or attn_mask.dtype == output.dtype, "attn_mask must be bool or the q / output dtype"
     qs, ks, os_ = _bhs_strides(query, tensor_layout), _bhs_strides(key, tensor_layout), _bhs_strides(output, tensor_layout)
-    lse = torch.empty((B, Hq, Sq), dtype=torch.float32, device=query.device) if return_lse else \
-        torch.empty((0,), dtype=torch.float32, device=query.device)
+    lse = _lse(query, (B, Hq, Sq), return_lse)
     with torch.cuda.device(query.device):
         check(lib().sab_qk_int8_sv_f16_attn_masked(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
                                                    lse.data_ptr() if return_lse else None, query_scale.data_ptr(),
@@ -1078,9 +1071,7 @@ def qk_int8_sv_f16_attn_masked(query: torch.Tensor, key: torch.Tensor, value: to
 def _(query, key, value, output, query_scale, key_scale, attn_mask, tensor_layout, q_quant_gran, k_quant_gran, sm_scale,
       fold_sm_scale, return_lse):
     B, Hq, Sq, D = _bhsd(query, tensor_layout)
-    if return_lse:
-        return torch.empty((B, Hq, Sq), dtype=torch.float32, device=query.device)
-    return torch.empty((0,), dtype=torch.float32, device=query.device)
+    return _lse(query, (B, Hq, Sq), return_lse)
 
 
 @torch.library.custom_op("sageattention_b200::qk_int8_sv_f16_attn_varlen", mutates_args=("output",), device_types="cuda")
@@ -1094,8 +1085,7 @@ def qk_int8_sv_f16_attn_varlen(query: torch.Tensor, key: torch.Tensor, value: to
     Tq, Hq, D = query.shape
     Tk, Hkv, _ = key.shape
     nseq = cu_seqlens_q.numel() - 1
-    lse = torch.empty((Hq, Tq), dtype=torch.float32, device=query.device) if return_lse else \
-        torch.empty((0,), dtype=torch.float32, device=query.device)
+    lse = _lse(query, (Hq, Tq), return_lse)
     with torch.cuda.device(query.device):
         check(lib().sab_qk_int8_sv_f16_attn(query.data_ptr(), key.data_ptr(), value.data_ptr(), output.data_ptr(),
                                             lse.data_ptr() if return_lse else None,
@@ -1111,9 +1101,7 @@ def qk_int8_sv_f16_attn_varlen(query: torch.Tensor, key: torch.Tensor, value: to
 @qk_int8_sv_f16_attn_varlen.register_fake
 def _(query, key, value, output, query_scale, key_scale, cu_seqlens_q, cu_seqlens_k, cu_pad_v, cu_q_scale, cu_k_scale,
       max_seqlen_q, is_causal, sm_scale, fold_sm_scale, return_lse=0):
-    if return_lse:
-        return torch.empty((query.size(1), query.size(0)), dtype=torch.float32, device=query.device)
-    return torch.empty((0,), dtype=torch.float32, device=query.device)
+    return _lse(query, (query.size(1), query.size(0)), return_lse)
 
 
 # ----------------------------------------------------------------------------------------------- 8-bit paged KV cache

@@ -668,6 +668,24 @@ int sab_kvcache8_prefill_window(const void* q, int dtype, const int8_t* k_pages,
                                 int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h,
                                 int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale,
                                 int window_left, int window_right, void* stream);
+/* sab_kvcache8_attn_shared: sab_kvcache8_attn with a prefix every sequence shares, read once for many sequences (parallel
+ *   sampling, beam search, requests behind one system prompt).  The same arguments plus shared_prefix_len (>= 0, else
+ *   SAB_ERR_INVALID before any launch) and the same workspace size.  Only whole chunks are shared: with C =
+ *   sab_kvcache8_chunk_keys() and P = min(shared_prefix_len, max_pages * page_size), P' = (P / C) * C; P' = 0 runs
+ *   sab_kvcache8_attn's kernels.  Promise (trusted, as table entries are): keys j < P' of every sequence are the same tokens,
+ *   stored in the pages block_table[0 .. P' / page_size - 1] name; row 0 is the only table row read for a shared chunk.
+ *   Chunk c < P' / C of sequence b goes to a shared CTA iff Lq_b >= 1 and (c + 1) * C <= Lk_b (non-causal) or
+ *   (c + 1) * C <= Lk_b - Lq_b + 1 (causal), decided on the device (no host synchronisation); such a CTA holds the rows of
+ *   S = 64 / (max_seqlen_q * Hq / Hkv) sequences and writes each row's partial for the chunk with the arithmetic of that row's
+ *   own CTA.  Every other chunk runs as in sab_kvcache8_attn.  Where the promise holds, out and lse are bit for bit those of
+ *   sab_kvcache8_attn.  Launch-grid limits: those of sab_kvcache8_attn, and nseq * ceil(max_pages * page_size / C) +
+ *   ceil(nseq / S) * P' / C < 2^31. */
+int sab_kvcache8_attn_shared(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
+                             const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
+                             const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq,
+                             int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h,
+                             int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale,
+                             void* workspace, int shared_prefix_len, void* stream);
 
 #ifdef __cplusplus
 }

@@ -93,6 +93,8 @@ EXPORTS = {
                                  [c_int, c_int, c_float, c_void_p, c_int, c_int, c_void_p]),
     "sab_kvcache8_prefill_window": (c_int, [c_void_p, c_int] + [c_void_p] * 10 + [c_int64] + [c_int] * 7 + [c_int64] * 4 +
                                     [c_int, c_int, c_float, c_int, c_int, c_void_p]),
+    "sab_kvcache8_attn_shared": (c_int, [c_void_p, c_int] + [c_void_p] * 10 + [c_int64] + [c_int] * 7 + [c_int64] * 4 +
+                                 [c_int, c_int, c_float, c_void_p, c_int, c_void_p]),
     "sab_block_stats": (c_int, [c_void_p, c_int, c_void_p, c_void_p] + [c_int] * 4 + [c_int64] * 3 + [c_int, c_void_p]),
     "sab_predict_block_mask": (c_int, [c_void_p] * 5 + [c_int] * 7 + [c_float] * 3 + [c_void_p]),
     "sab_block_stats_varlen": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 4 + [c_int64] * 2 + [c_int, c_void_p]),

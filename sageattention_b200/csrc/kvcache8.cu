@@ -9,6 +9,7 @@
 // Decode is bound by the bytes of the cache, so the kernels aim at one read of each K / V byte per chunk, not at tensor-core rate.
 //   kv8_prefill_kernel one CTA per (sequence, 128-row Q tile, Q head) for query chunks of any length (chunked prefill): the decode
 //                      numerics without chunks, on the warpgroup tensor cores (see its section below).
+#include <algorithm>
 #include <atomic>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -162,7 +163,15 @@ struct Kv8Params {
   float* o_part;        // [Tq, Hq, max_chunks, D]
   float2* ml_part;      // [Tq, Hq, max_chunks]: (running max in log2 units, sum of p)
   int window_left, window_right;   // kWindow: query i sees keys [i + off - left, i + off + right], off = Lk - Lq_b (-1: unbounded)
+  int nseq, shared_chunks, shared_seqs;   // kShared: chunks c < shared_chunks are shared; shared_seqs sequences per shared CTA
 };
+
+// kShared: chunk c of sequence b goes to a shared CTA iff every held row of b sees every key of the chunk (so no row has a masked
+// key in it): b has a query, and the chunk ends at or before Lk_b (non-causal) or the first row's diagonal key + 1 (causal).
+template <bool kCausal>
+__device__ __forceinline__ bool kv8_takes_shared(int Lqb, int Lk, int c) {
+  return Lqb >= 1 && int64_t(c + 1) * kChunk <= (kCausal ? int64_t(Lk) - Lqb + 1 : int64_t(Lk));
+}
 
 template <int D>
 struct Kv8Smem {
@@ -181,12 +190,24 @@ struct Kv8Smem {
 // CTA's first visible key are skipped (a tile in which a row sees nothing is an exact identity on its m, l and O), and keys left of
 // it are zero-filled without reading their table entry.  Three CTAs per SM (168 registers, no spill) as the D = 128 forms; the
 // D = 64 forms' 128 registers would spill here.  The minimum of 0 leaves the other forms as they were.
-template <typename T, int D, bool kCausal, bool kWindow = false>
+//
+// kShared: the shared-prefix form.  Grid x is nseq * max_chunks per-sequence CTAs, then ceil(nseq / shared_seqs) * shared_chunks
+// shared CTAs.  A per-sequence CTA runs as above, and exits at once when kv8_takes_shared gives its chunk to a shared CTA.  Shared
+// CTA (slice s, chunk c) holds the rows of sequences s * shared_seqs + m, member m's at rows m * G * max_seqlen_q + i * G + g, and
+// reads chunk c once, through table row 0, for all of them.  Every row it writes runs the per-row arithmetic above on the same
+// keys, unmasked as in its own sequence's CTA, so it writes the partial that CTA would have written.  The token of each query slot
+// r / G (-1: the row is not computed here) lives in shared memory past Kv8Smem.
+template <typename T, int D, bool kCausal, bool kWindow = false, bool kShared = false>
 __global__ void __launch_bounds__(kThreads, kWindow ? 3 : 0) kv8_attn_kernel(const Kv8Params p) {
   using S = Kv8Smem<D>;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   S& sm = *reinterpret_cast<S*>(smem_raw);
-  const int b = blockIdx.x / p.max_chunks, chunk = blockIdx.x % p.max_chunks, h = blockIdx.y;
+  int* const slot_tok = reinterpret_cast<int*>(smem_raw + sizeof(S));   // kShared: [kRows]
+  const int nper = p.nseq * p.max_chunks;                                 // kShared: the per-sequence CTAs
+  const bool shared_cta = kShared && int(blockIdx.x) >= nper;
+  const int slice = shared_cta ? (int(blockIdx.x) - nper) / p.shared_chunks : 0;
+  const int b = shared_cta ? 0 : blockIdx.x / p.max_chunks, h = blockIdx.y;   // a shared CTA reads table row 0
+  const int chunk = shared_cta ? (int(blockIdx.x) - nper) % p.shared_chunks : blockIdx.x % p.max_chunks;
   const int G = p.Hq / p.Hkv;
   const int q0 = p.cu_q[b];
   const int Lqb = p.cu_q[b + 1] - q0;   // the sequence's queries: the causal and window offsets are taken from it
@@ -194,9 +215,31 @@ __global__ void __launch_bounds__(kThreads, kWindow ? 3 : 0) kv8_attn_kernel(con
   const int Lk = min(p.seqused_k[b], p.max_pages * p.page_size);
   const int off = Lk - Lqb;             // query i's diagonal key is i + off
   const int kbeg = chunk * kChunk;
-  if (Lq <= 0 || kbeg >= Lk) return;
-  const int kend = min(Lk, kbeg + kChunk);
-  const int R = Lq * G;                 // rows r = i * G + g: query i, Q head h * G + g
+  if constexpr (kShared) {
+    if (!shared_cta && chunk < p.shared_chunks && kv8_takes_shared<kCausal>(Lqb, Lk, chunk)) return;
+  }
+  if (!shared_cta && (Lq <= 0 || kbeg >= Lk)) return;
+  const int kend = shared_cta ? kbeg + kChunk : min(Lk, kbeg + kChunk);
+  // rows r = i * G + g: query i, Q head h * G + g (shared CTA: query slot i of its members, max_seqlen_q per member)
+  const int R = shared_cta ? min(p.shared_seqs, p.nseq - slice * p.shared_seqs) * p.max_seqlen_q * G : Lq * G;
+  if constexpr (kShared) {
+    bool live = false;
+    if (threadIdx.x < kRows) {
+      const int u = threadIdx.x;
+      int tok = -1;
+      if (!shared_cta) {
+        if (u < Lq) tok = q0 + u;
+      } else if (u * G < R) {
+        const int bm = slice * p.shared_seqs + u / p.max_seqlen_q, i = u % p.max_seqlen_q;
+        const int qm = p.cu_q[bm], Lqm = p.cu_q[bm + 1] - qm;
+        if (i < min(Lqm, p.max_seqlen_q) && kv8_takes_shared<kCausal>(Lqm, min(p.seqused_k[bm], p.max_pages * p.page_size), chunk))
+          tok = qm + i;
+      }
+      slot_tok[u] = tok;
+      live = tok >= 0;
+    }
+    if (!__syncthreads_or(live)) return;   // a shared CTA none of whose members takes the chunk
+  }
   const int nM = (R + 15) / 16;
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32, g8 = lane / 4, c4 = lane % 4;
   const int32_t* table = p.table + int64_t(b) * p.table_stride;
@@ -252,10 +295,10 @@ __global__ void __launch_bounds__(kThreads, kWindow ? 3 : 0) kv8_attn_kernel(con
     for (int r = warp; r < nM * 16; r += 4) {
       uint32_t q8 = 0;
       float qc = 0.f;
-      if (r < R) {
+      if (kShared ? slot_tok[r / G] >= 0 : r < R) {
         const int i = r / G, hq = h * G + r % G;
         float x[E];
-        load_row<T, E>(q + int64_t(q0 + i) * p.q_st + int64_t(hq) * p.q_sh + lane * E, x);
+        load_row<T, E>(q + int64_t(kShared ? slot_tok[i] : q0 + i) * p.q_st + int64_t(hq) * p.q_sh + lane * E, x);
         const RowQuant rq(warp_amax<E>(x), 127.f);
         q8 = pack_s8<E>(x, rq);
         qc = __fmul_rn(rq.scale, p.scale_log2);
@@ -295,6 +338,7 @@ __global__ void __launch_bounds__(kThreads, kWindow ? 3 : 0) kv8_attn_kernel(con
     for (int j = 0; j < 2; ++j) {
       const int r = mt * 16 + g8 + 8 * j;
       if constexpr (kWindow) lim[mt][j] = r >= R ? kend : r / G + off - wl;
+      else if constexpr (kShared) lim[mt][j] = slot_tok[r / G] < 0 ? -1 : (kCausal && !shared_cta ? min(kend - 1, r / G + off) : kend - 1);
       else lim[mt][j] = r >= R ? -1 : (kCausal ? min(kend - 1, r / G + off) : kend - 1);
     }
 
@@ -438,8 +482,8 @@ __global__ void __launch_bounds__(kThreads, kWindow ? 3 : 0) kv8_attn_kernel(con
 #pragma unroll
     for (int j = 0; j < 2; ++j) {
       const int r = mt * 16 + g8 + 8 * j;
-      if (r >= R) continue;
-      const int64_t idx = (int64_t(q0 + r / G) * p.Hq + h * G + r % G) * p.max_chunks + chunk;
+      if (kShared ? slot_tok[r / G] < 0 : r >= R) continue;
+      const int64_t idx = (int64_t(kShared ? slot_tok[r / G] : q0 + r / G) * p.Hq + h * G + r % G) * p.max_chunks + chunk;
 #pragma unroll
       for (int nt = 0; nt < NO; ++nt)
         *reinterpret_cast<float2*>(p.o_part + idx * D + warp * (D / 4) + nt * 8 + 2 * c4) = make_float2(o[mt][nt][2 * j], o[mt][nt][2 * j + 1]);
@@ -837,10 +881,13 @@ int launch_write(const void* k, const void* v, const float* k_smooth, const int6
   return SAB_OK;
 }
 
-template <typename T, int D, bool kCausal, bool kWindow = false>
+// kShared: the per-sequence CTAs, then ceil(nseq / shared_seqs) slices x shared_chunks shared CTAs
+template <typename T, int D, bool kCausal, bool kWindow = false, bool kShared = false>
 int launch_attn_t(const Kv8Params& p, int nseq, cudaStream_t st) {
-  auto kern = kv8_attn_kernel<T, D, kCausal, kWindow>;
-  const int bytes = int(sizeof(Kv8Smem<D>));
+  auto kern = kv8_attn_kernel<T, D, kCausal, kWindow, kShared>;
+  const int bytes = int(sizeof(Kv8Smem<D>)) + (kShared ? kRows * int(sizeof(int)) : 0);
+  const int64_t grid_x = int64_t(nseq) * p.max_chunks +
+                         (kShared ? int64_t(nseq + p.shared_seqs - 1) / p.shared_seqs * p.shared_chunks : 0);
   // once per device, so a launch inside CUDA-graph capture makes no attribute call
   static std::atomic<uint64_t> configured{0};
   int dev = 0;
@@ -850,16 +897,18 @@ int launch_attn_t(const Kv8Params& p, int nseq, cudaStream_t st) {
     SAB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
     configured.fetch_or(bit);
   }
-  kern<<<dim3(unsigned(nseq * p.max_chunks), unsigned(p.Hkv)), kThreads, bytes, st>>>(p);
+  kern<<<dim3(unsigned(grid_x), unsigned(p.Hkv)), kThreads, bytes, st>>>(p);
   SAB_CUDA_OK(cudaGetLastError());
   return SAB_OK;
 }
 
-// window: the kWindow kernel, with the causal rule already folded into p.window_right
+// window: the kWindow kernel, with the causal rule already folded into p.window_right; p.shared_chunks > 0: the kShared kernel
 template <typename T, int D>
 int launch_attn(const Kv8Params& p, const Kv8CombineParams& c, int nseq, bool causal, bool window, cudaStream_t st) {
+  const bool shared = p.shared_chunks > 0;
   if (int r = window ? launch_attn_t<T, D, false, true>(p, nseq, st)
-                     : causal ? launch_attn_t<T, D, true>(p, nseq, st) : launch_attn_t<T, D, false>(p, nseq, st))
+              : shared ? (causal ? launch_attn_t<T, D, true, false, true>(p, nseq, st) : launch_attn_t<T, D, false, false, true>(p, nseq, st))
+                       : causal ? launch_attn_t<T, D, true>(p, nseq, st) : launch_attn_t<T, D, false>(p, nseq, st))
     return r;
   kv8_combine_kernel<T, D><<<dim3(unsigned(nseq * c.max_seqlen_q), unsigned(c.Hq)), D, 0, st>>>(c);
   SAB_CUDA_OK(cudaGetLastError());
@@ -931,13 +980,15 @@ extern "C" int sab_kvcache8_write(const void* k, const void* v, int dtype, const
                   : launch_write<__nv_bfloat16, 64>(k, v, k_smooth, slot_mapping, T, Hkv, k_stride_t, k_stride_h, v_stride_t, v_stride_h, k_pages, k_scale, v_pages, v_scale, ns, st);
 }
 
-// sab_kvcache8_attn and, with window, sab_kvcache8_attn_window (window_right with the causal rule folded in)
+// sab_kvcache8_attn and, with window, sab_kvcache8_attn_window (window_right with the causal rule folded in); with
+// shared_prefix_len >= one chunk, sab_kvcache8_attn_shared
 static int kvcache8_attn(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
                          const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
                          const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages, int nseq,
                          int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t, int64_t q_stride_h,
                          int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal, float sm_scale,
-                         void* workspace, bool window, int window_left, int window_right, void* stream) {
+                         void* workspace, bool window, int window_left, int window_right, int shared_prefix_len,
+                         void* stream) {
   SAB_REQUIRE(q && k_pages && k_scale && v_pages && v_scale && k_smooth && out && cu_seqlens_q && seqused_k && block_table && workspace,
               SAB_ERR_INVALID, "null pointer argument");
   if (int r = check_dtype_dim(dtype, D)) return r;
@@ -954,9 +1005,14 @@ static int kvcache8_attn(const void* q, int dtype, const int8_t* k_pages, const 
   SAB_REQUIRE(Hq <= 65535 && chunks * nseq < (int64_t(1) << 31) && int64_t(nseq) * max_seqlen_q < (int64_t(1) << 31),
               SAB_ERR_INVALID, "launch grid too large: need Hq <= 65535, nseq * chunks < 2^31 and nseq * max_seqlen_q < 2^31");
   SAB_REQUIRE(max_keys < (int64_t(1) << 31), SAB_ERR_INVALID, "max_pages * page_size must be < 2^31 keys");
+  // shared prefix: whole chunks only, at most the table's keys; shared_seqs sequences' rows fill one CTA's kRows
+  const int64_t shared_chunks = std::min(int64_t(shared_prefix_len), max_keys) / kChunk;
+  const int shared_seqs = kRows / (max_seqlen_q * (Hq / Hkv));
+  SAB_REQUIRE(chunks * nseq + (nseq + shared_seqs - 1) / shared_seqs * shared_chunks < (int64_t(1) << 31), SAB_ERR_INVALID,
+              "launch grid too large: need nseq * chunks + ceil(nseq / shared sequences per CTA) * shared chunks < 2^31");
   Kv8Params p{q, k_pages, k_scale, v_pages, v_scale, cu_seqlens_q, seqused_k, block_table, table_stride, max_pages, page_size, Hq, Hkv,
               int(chunks), max_seqlen_q, q_stride_t, q_stride_h, float(double(sm_scale) * 1.4426950408889634),
-              static_cast<float*>(workspace), nullptr, window_left, window_right};
+              static_cast<float*>(workspace), nullptr, window_left, window_right, nseq, int(shared_chunks), shared_seqs};
   p.ml_part = reinterpret_cast<float2*>(p.o_part + int64_t(Tq) * Hq * chunks * D);
   Kv8CombineParams c{q, k_smooth, cu_seqlens_q, seqused_k, p.o_part, p.ml_part, out, lse, Tq, Hq, Hkv, int(chunks), max_seqlen_q,
                      int(max_keys), q_stride_t, q_stride_h, o_stride_t, o_stride_h, sm_scale};
@@ -976,7 +1032,7 @@ extern "C" int sab_kvcache8_attn(const void* q, int dtype, const int8_t* k_pages
                                  void* workspace, void* stream) {
   return kvcache8_attn(q, dtype, k_pages, k_scale, v_pages, v_scale, k_smooth, out, lse, cu_seqlens_q, seqused_k, block_table,
                        table_stride, max_pages, nseq, Tq, Hq, Hkv, D, page_size, q_stride_t, q_stride_h, o_stride_t, o_stride_h,
-                       max_seqlen_q, is_causal, sm_scale, workspace, false, -1, -1, stream);
+                       max_seqlen_q, is_causal, sm_scale, workspace, false, -1, -1, 0, stream);
 }
 
 extern "C" int sab_kvcache8_attn_window(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
@@ -989,7 +1045,19 @@ extern "C" int sab_kvcache8_attn_window(const void* q, int dtype, const int8_t* 
   if (int r = window_args(window_left, window_right, is_causal, right)) return r;
   return kvcache8_attn(q, dtype, k_pages, k_scale, v_pages, v_scale, k_smooth, out, lse, cu_seqlens_q, seqused_k, block_table,
                        table_stride, max_pages, nseq, Tq, Hq, Hkv, D, page_size, q_stride_t, q_stride_h, o_stride_t, o_stride_h,
-                       max_seqlen_q, is_causal, sm_scale, workspace, true, window_left, right, stream);
+                       max_seqlen_q, is_causal, sm_scale, workspace, true, window_left, right, 0, stream);
+}
+
+extern "C" int sab_kvcache8_attn_shared(const void* q, int dtype, const int8_t* k_pages, const float* k_scale, const uint8_t* v_pages,
+                                        const float* v_scale, const float* k_smooth, void* out, float* lse, const int32_t* cu_seqlens_q,
+                                        const int32_t* seqused_k, const int32_t* block_table, int64_t table_stride, int max_pages,
+                                        int nseq, int Tq, int Hq, int Hkv, int D, int page_size, int64_t q_stride_t,
+                                        int64_t q_stride_h, int64_t o_stride_t, int64_t o_stride_h, int max_seqlen_q, int is_causal,
+                                        float sm_scale, void* workspace, int shared_prefix_len, void* stream) {
+  SAB_REQUIRE(shared_prefix_len >= 0, SAB_ERR_INVALID, "shared_prefix_len must be >= 0");
+  return kvcache8_attn(q, dtype, k_pages, k_scale, v_pages, v_scale, k_smooth, out, lse, cu_seqlens_q, seqused_k, block_table,
+                       table_stride, max_pages, nseq, Tq, Hq, Hkv, D, page_size, q_stride_t, q_stride_h, o_stride_t, o_stride_h,
+                       max_seqlen_q, is_causal, sm_scale, workspace, false, -1, -1, shared_prefix_len, stream);
 }
 
 // sab_kvcache8_prefill and, with window, sab_kvcache8_prefill_window (window_right with the causal rule folded in)

@@ -154,7 +154,7 @@ def _window_arg(window_size, block_table, cache):
 
 def sageattn_kvcache8(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_q: torch.Tensor, seqused_k: torch.Tensor,
                       block_table: torch.Tensor, max_seqlen_q: int, is_causal: bool = True, sm_scale: Optional[float] = None,
-                      return_lse: bool = False, window_size=(-1, -1)):
+                      return_lse: bool = False, window_size=(-1, -1), shared_prefix_len: int = 0):
     """Attention of packed queries against a PagedKVCache8, for decoding and speculative verification.
 
     q: packed [Tq, Hq, D] in the cache's dtype with cu_seqlens_q (int32 or int64, nseq + 1 offsets) and max_seqlen_q, as in
@@ -182,9 +182,26 @@ def sageattn_kvcache8(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_q: torch
     unbounded), and j <= i + off_b as well when is_causal.  Only keys j >= max(0, Lk_b - Lq_b - left) are ever loaded: their
     table entries, K / V bytes and scales are the only ones read, so the entries below that bound may name any page in
     [0, num_pages) (a shared null page, or pages reused for newer tokens).  Skipping keys left of the window changes no bit of what
-    a row computes, and (-1, -1) is the call without a window."""
+    a row computes, and (-1, -1) is the call without a window.
+
+    shared_prefix_len = P, an int >= 0 (ValueError otherwise, and together with a window, before any launch), reads a prefix
+    that every sequence shares once for many sequences instead of once per sequence: parallel sampling, beam search, requests
+    behind one system prompt.  P is clamped at max_pages * page_size, and only whole chunks are shared: P' = (P // C) * C with
+    C = ops.kvcache8_chunk_keys(); P < C is the call without a shared prefix.  The caller promises that keys j < P' of every
+    sequence are the same tokens, stored in the pages that block_table[0, :P' // page_size] names: row 0 is the only table row
+    read for a shared chunk, and the promise is trusted as table entries are.  Chunk c < P' / C of sequence b is computed for
+    up to 64 / (max_seqlen_q * Hq / Hkv) sequences at once when Lq_b >= 1 and (c + 1) * C <= Lk_b (causal: <= Lk_b - Lq_b + 1),
+    so no row of b has a masked key in it; its other chunks run as without a shared prefix.  Which chunks are shared is decided
+    on the device, so the call stays free of host synchronisation.  Where the promise holds, o and lse are bit for bit those of
+    the call with shared_prefix_len=0.  A batch with several shared prefixes can be split into one call per prefix group: a
+    sequence's bits do not depend on the batch."""
     Hq, D, cu_q = _attn_args(q, cache, cu_seqlens_q, seqused_k, block_table, max_seqlen_q)
     window = _window_arg(window_size, block_table, cache)
+    if isinstance(shared_prefix_len, bool) or not isinstance(shared_prefix_len, numbers.Integral) or shared_prefix_len < 0:
+        raise ValueError(f"shared_prefix_len must be an int >= 0, got {shared_prefix_len!r}")
+    if shared_prefix_len > 0 and window != (-1, -1):
+        raise ValueError("shared_prefix_len and window_size cannot be combined: use one or the other")
+    shared = min(int(shared_prefix_len), block_table.size(1) * cache.page_size)
     Hkv = cache.num_kv_heads
     if max_seqlen_q * (Hq // Hkv) > _ROW_LIMIT:
         raise ValueError(f"max_seqlen_q * Hq / Hkv = {max_seqlen_q * (Hq // Hkv)} exceeds the {_ROW_LIMIT} query rows the split-KV "
@@ -196,7 +213,12 @@ def sageattn_kvcache8(q: torch.Tensor, cache: PagedKVCache8, cu_seqlens_q: torch
         o = torch.empty(q.shape, dtype=q.dtype, device=cache.device)
         args = (q, cache.k_pages, cache.k_scale, cache.v_pages.view(torch.uint8), cache.v_scale, cache.k_smooth, o, cu_q.contiguous(),
                 seqused_k.contiguous(), block_table, int(max_seqlen_q), 1 if is_causal else 0, float(sm_scale), 1 if return_lse else 0)
-        lse = ops.kvcache8_attn(*args) if window == (-1, -1) else ops.kvcache8_attn_window(*args, *window)
+        if window != (-1, -1):
+            lse = ops.kvcache8_attn_window(*args, *window)
+        elif shared >= ops.kvcache8_chunk_keys():
+            lse = ops.kvcache8_attn_shared(*args, shared)
+        else:
+            lse = ops.kvcache8_attn(*args)
     return (o, lse) if return_lse else o
 
 

@@ -1238,3 +1238,33 @@ def _(q, k_pages, k_scale, v_pages, v_scale, k_smooth, output, cu_seqlens_q, seq
       sm_scale, return_lse, window_left, window_right):
     Tq, Hq, _ = q.shape
     return q.new_empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32)
+
+
+@torch.library.custom_op("sageattention_b200::kvcache8_attn_shared", mutates_args=("output",), device_types="cuda")
+def kvcache8_attn_shared(q: torch.Tensor, k_pages: torch.Tensor, k_scale: torch.Tensor, v_pages: torch.Tensor, v_scale: torch.Tensor,
+                         k_smooth: torch.Tensor, output: torch.Tensor, cu_seqlens_q: torch.Tensor, seqused_k: torch.Tensor,
+                         block_table: torch.Tensor, max_seqlen_q: int, is_causal: int, sm_scale: float, return_lse: int,
+                         shared_prefix_len: int) -> torch.Tensor:
+    """kvcache8_attn with the first shared_prefix_len keys (whole chunks) shared by every sequence through table row 0
+    (include/sageattn_b200.h, sab_kvcache8_attn_shared); shared_prefix_len int32, >= 0.  Returns the [Hq,Tq] natural-log LSE
+    when return_lse, else an empty tensor."""
+    Tq, Hq, D = q.shape
+    page_size, Hkv = k_pages.size(1), k_pages.size(2)
+    nseq, max_pages = block_table.shape
+    lse = torch.empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32, device=q.device)
+    with torch.cuda.device(q.device):
+        ws = torch.empty(lib().sab_kvcache8_workspace_bytes(Tq, Hq, D, max_pages * page_size), dtype=torch.uint8, device=q.device)
+        check(lib().sab_kvcache8_attn_shared(q.data_ptr(), _dt(q), k_pages.data_ptr(), k_scale.data_ptr(), v_pages.data_ptr(),
+                                             v_scale.data_ptr(), k_smooth.data_ptr(), output.data_ptr(),
+                                             lse.data_ptr() if return_lse else None, cu_seqlens_q.data_ptr(), seqused_k.data_ptr(),
+                                             block_table.data_ptr(), block_table.stride(0), max_pages, nseq, Tq, Hq, Hkv, D, page_size,
+                                             q.stride(0), q.stride(1), output.stride(0), output.stride(1), max_seqlen_q, is_causal,
+                                             float(sm_scale), ws.data_ptr(), shared_prefix_len, _stream(q)))
+    return lse
+
+
+@kvcache8_attn_shared.register_fake
+def _(q, k_pages, k_scale, v_pages, v_scale, k_smooth, output, cu_seqlens_q, seqused_k, block_table, max_seqlen_q, is_causal,
+      sm_scale, return_lse, shared_prefix_len):
+    Tq, Hq, _ = q.shape
+    return q.new_empty((Hq, Tq) if return_lse else (0,), dtype=torch.float32)

@@ -8,6 +8,10 @@ through a bit-identity with a form that is compared.
     counterpart of the same (D, per-thread K scales, dtype) is itself covered (the dense forms above, and for the per-sequence V
     forms the dense kernels of test_gpu_kernel_edges.INST_CASES and test_gpu_backward.ORACLE_CASES).
 
+The masked FP16-PV forward (attn_mask of sageattn_qk_int8_pv_fp16_triton, launch_attn<D, false, T, true, true>) is not a family
+of this module: tests/test_gpu_fp16pv_forward_edges.py compares it, and every other FP16-PV instantiation, element by element with
+attn_fp16pv_oracle's bound, and guards its own coverage of them the same way when it is imported.
+
 The check runs when the module is imported, so a new instantiation without a case, or a case list that loses one, fails the
 collection of every run, with or without a GPU."""
 import os
